@@ -1,8 +1,9 @@
 #!/usr/bin/env python
-"""Benchmark of the VisRAG-Ret hot path on B200 (contract: see the task statement / DESIGN.md §Measurement).
+"""Benchmark of the VisRAG-Ret hot path on an H100 (see DESIGN.md §Measurement).
 
   python bench.py --gpus N --steps K --warmup W            # our CUDA path (one JSON line from rank 0)
   python bench.py --impl reference --gpus N --steps K ...  # the reference algorithm on the host cores (oracle port)
+  python bench.py ... --dump-outputs DIR                   # also writes the last timed step's embeddings as DIR/page_reps.npy
 
 Workload = BASELINE.json configs[2]: full VisRAG-Ret (SigLIP-so400m 26 blocks + Resampler + MiniCPM-2B 40 layers,
 random-init weights of that architecture) encoding synthetic 448x448 pages, plus 1 k text queries scored top-10
@@ -34,27 +35,36 @@ def _env_int(name, default):
         return default
 
 
+H100_SXM_BF16_TFLOPS = 989.0   # NVIDIA H100 SXM data sheet, dense bf16 / fp16, card allowed up to 700 W
+H100_SXM_HBM_GBS = 3350.0      # same data sheet, HBM3
+
+
 def load_peaks():
+    """Peaks the roofline fractions are taken against: a MEASURED_PEAKS.json beside this file when there is one, else the
+    data-sheet figures (a power-limited card sustains less than those)."""
     p = os.path.join(ROOT, "MEASURED_PEAKS.json")
     if os.path.exists(p):
         d = json.load(open(p))
-        return d.get("bf16_tflops_sustained", 1429.0), d.get("hbm_gbs", 6585.8), "measured (MEASURED_PEAKS.json, sustained bf16)"
-    return 1400.0, 6650.0, "fallback (B200_PROFILING.md)"
+        return (d.get("bf16_tflops_sustained", H100_SXM_BF16_TFLOPS), d.get("hbm_gbs", H100_SXM_HBM_GBS),
+                "measured (MEASURED_PEAKS.json, sustained bf16)")
+    return H100_SXM_BF16_TFLOPS, H100_SXM_HBM_GBS, "NVIDIA H100 SXM data sheet (dense bf16, HBM3)"
 
 
 def burst_peak_tf():
     """Tensor peak for a kernel timed ALONE (the score filter): the burst figure; the sustained one is for the long step."""
     p = os.path.join(ROOT, "MEASURED_PEAKS.json")
     if os.path.exists(p):
-        return json.load(open(p)).get("bf16_tflops", 1693.1)
-    return 1700.0
+        return json.load(open(p)).get("bf16_tflops", H100_SXM_BF16_TFLOPS)
+    return H100_SXM_BF16_TFLOPS
 
 
 class ClockSampler:
-    """nvidia-smi sampling DURING the timed region (recipe in B200_PROFILING.md)."""
+    """nvidia-smi sampling (read-only queries) DURING the timed region."""
 
     def __init__(self, index):
-        self.index, self.proc, self.path = index, None, f"/tmp/vr_clocks_{os.getpid()}.csv"
+        import tempfile
+
+        self.index, self.proc, self.path = index, None, os.path.join(tempfile.gettempdir(), f"vr_clocks_{os.getpid()}.csv")
 
     def start(self):
         q = ("clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown,"
@@ -66,6 +76,7 @@ class ClockSampler:
             self.proc = None
 
     def stop(self):
+        """Ends the sampling process and removes its file; safe to call twice (the timed region calls it in a `finally`)."""
         if self.proc is None:
             return {"sm_mhz": None, "sm_max_mhz": None, "reasons": ["nvidia-smi unavailable"]}
         self.proc.terminate()
@@ -73,6 +84,17 @@ class ClockSampler:
             self.proc.wait(5)
         except subprocess.TimeoutExpired:
             self.proc.kill()
+            self.proc.wait()
+        self.proc = None
+        try:
+            return self._read()
+        finally:
+            try:
+                os.unlink(self.path)
+            except OSError:
+                pass
+
+    def _read(self):
         sm, mx, reasons = [], None, set()
         for line in open(self.path):
             f = [x.strip() for x in line.split(",")]
@@ -131,7 +153,7 @@ def run_ours(a):
     dev = f"cuda:{local}"
     if world > 1:
         # NCCL writes its "NCCL version ..." banner to STDOUT when the first communicator is created (whenever NCCL_DEBUG
-        # is set, as it is on the GPU boxes); stdout must carry exactly one JSON line, so the banner is sent to stderr
+        # is set); stdout must carry exactly one JSON line, so the banner is sent to stderr
         sys.stdout.flush()
         saved = os.dup(1)
         os.dup2(2, 1)
@@ -191,13 +213,21 @@ def run_ours(a):
         sampler.start()
     launches0 = L.LAUNCHES
     e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    e0.record()
-    for _ in range(a.steps):
-        reps = step_device()
-    e1.record()
-    barrier()
+    clocks = None
+    try:  # whatever happens in the timed loop, the sampling process must not outlive it
+        e0.record()
+        for _ in range(a.steps):
+            reps = step_device()
+        e1.record()
+        barrier()
+    finally:
+        if rank == 0:
+            clocks = sampler.stop()
     launches = L.LAUNCHES - launches0
-    clocks = sampler.stop() if rank == 0 else None
+    if a.dump_outputs and rank == 0:
+        # what a caller of the timed path receives from its last step: the [pages, hidden] fp32 embeddings
+        os.makedirs(a.dump_outputs, exist_ok=True)
+        np.save(os.path.join(a.dump_outputs, "page_reps.npy"), reps.float().cpu().numpy())
     ms_total = max_over_ranks(e0.elapsed_time(e1))
     value = world * a.steps * P / (ms_total / 1e3)
 
@@ -251,13 +281,9 @@ def run_ours(a):
         achieved = alg / (gemm_ms / 1e3) / 1e12
         # the single heaviest launch class (same kernel template, one shape + epilogue)
         top_k, (top_n, top_ms, top_fl) = max(gemm_classes.items(), key=lambda kv: kv[1][1])
-        traffic = None
-        tpath = os.path.join(ROOT, "profiles", "gemm_traffic.json")
-        if os.path.exists(tpath):
-            traffic = json.load(open(tpath)).get(top_k)
-        roofline = {"bound": "tensor", "kernel": "gemm_tcgen05_kernel (all launches of the step; epilogue variants bias/GELU/resid/RoPE/SwiGLU)",
+        roofline = {"bound": "tensor", "kernel": "gemm_wgmma_kernel (all launches of the step; epilogue variants bias/GELU/resid/RoPE/SwiGLU)",
                     "achieved": round(achieved, 1), "peak": peak_tf, "unit": "TFLOP/s", "frac": round(achieved / peak_tf, 4),
-                    "traffic": traffic, "peak_source": peak_src, "launches_per_step": gemm_n // 2,
+                    "peak_source": peak_src, "launches_per_step": gemm_n // 2,
                     "avg_launch_ms": round(gemm_ms / gemm_n, 4), "padded_tflops": round(gemm_padded_flops / (gemm_ms / 1e3) / 1e12, 1),
                     "heaviest_class": {"shape": top_k, "launches_per_step": top_n // 2, "avg_launch_ms": round(top_ms / top_n, 4),
                                        "tflops": round(top_fl / (top_ms / 1e3) / 1e12, 1), "share_of_gemm_time": round(top_ms / gemm_ms, 3)},
@@ -381,7 +407,7 @@ def run_ours(a):
                "index_build_ms": round(build_ms, 2), "ms_per_query_batch": round(big_ms, 3),
                "queries_per_s": round(a.big_queries / (big_ms / 1e3), 1), "stages_ms_rank0": stages,
                "filter_tflops_fp16_per_gpu": round(filt_tf, 1), "filter_frac_of_tensor_peak": round(filt_tf / burst_peak_tf(), 3),
-               "filter_peak": "burst dense bf16/fp16 figure of MEASURED_PEAKS.json (a kernel timed alone, not inside the encode step)",
+               "filter_peak": "dense bf16/fp16 tensor peak (a kernel timed alone, not inside the encode step)",
                "flagged": st.get("flagged"), "checked_queries_vs_torch_fp32": checked_big}
 
     # ---- (4c) the reference's own operating point (eval.sh: per-device batch 16) and the demo's single query, blocking API
@@ -458,7 +484,7 @@ def run_ours(a):
             "config": {"workload": workload_name(a), "queries": f"{nq} text queries top-10 over {nd * world} pages",
                        "size": a.model, "pages_per_step_per_gpu": P, "global_batch": P * world, "patches_per_page": n_patches,
                        "lm_tokens_per_page": lm_tokens, "parallelism": f"dp{world} (pages sharded, no encode collective)",
-                       "weights": "random-init, bf16", "l2": "working set (6.3 GB weights + >1 GB activations per step) >> 126 MB L2"},
+                       "weights": "random-init, bf16", "l2": "working set (6.3 GB weights + >1 GB activations per step) >> 50 MB L2"},
             "e2e": {"value": round(e2e_value, 2), "unit": UNIT, "h2d_bytes_per_step": h2d, "d2h_bytes_per_step": d2h,
                     "ms_per_step": round(e2e_ms / a.steps, 3), "batch_intervals_ms": intervals,
                     "api": "inference.encode_stream (loop body of distributed_parallel_embedding_inference) over DRModelForInference",
@@ -546,8 +572,8 @@ def pick_cpu_threads():
 # --------------------------------------------------------------------------------------------- reference arm
 def run_reference(a):
     """The reference's algorithm on the host cores. The reference itself is pure Python over PyTorch and cannot travel to
-    the GPU box (/root/reference is absent there), so this runs its oracle port (validated against the real reference in the
-    build container, tests/golden). Each step = ONE page through the full model; rank 0 only."""
+    a GPU machine without a checkout of it, so this runs its oracle port (validated against the real reference through
+    tests/golden). Each step = ONE page through the full model; rank 0 only."""
     rank = _env_int("RANK", 0)
     if rank != 0:
         return
@@ -571,7 +597,7 @@ def run_reference(a):
     rs = np.random.RandomState(1000)
     n = a.steps + a.warmup
     pages = [Image.fromarray(rs.randint(0, 256, (a.page_px, a.page_px, 3), dtype=np.uint8)) for _ in range(n)]
-    budget_s = 150.0  # the whole arm must end within a few minutes whatever K the driver passes
+    budget_s = 150.0  # the whole arm must end within a few minutes whatever K is passed
     t_w = time.time()
     for i in range(a.warmup):
         O.encode(sd, cfg, tok, [""], [pages[i]])
@@ -619,12 +645,17 @@ def main():
     ap.add_argument("--no-cpu-baseline", dest="cpu_baseline", action="store_false")
     ap.add_argument("--no-torch-baseline", dest="torch_baseline", action="store_false",
                     help="skip the stock-PyTorch-on-this-GPU context arm (N = 1 only)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the embeddings of the last timed step as DIR/page_reps.npy (float32 [pages, hidden]); the inputs are "
+                         "seeded, so two builds can be compared output for output")
     a = ap.parse_args()
     if a.warmup < 3 and a.impl == "ours":
         a.warmup = 3
     if a.big_corpus < 0:
         a.big_corpus = 125000 if a.gpus > 1 else 0
     if a.impl == "reference":
+        if a.dump_outputs:
+            ap.error("--dump-outputs applies to the CUDA path (--impl ours)")
         run_reference(a)
     else:
         run_ours(a)

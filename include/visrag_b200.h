@@ -1,5 +1,5 @@
 /*
- * visrag_b200 — C ABI of the B200-native VisRAG-Ret embedding + retrieval hot path.
+ * visrag_b200 — C ABI of the H100-native (sm_90a) VisRAG-Ret embedding + retrieval hot path.
  *
  * The reference (OpenBMB/VisRAG) is pure Python: it has no FFI for this path. The
  * drop-in boundary is the three Python call signatures of SURVEY.md §8(b); this C ABI
@@ -33,8 +33,8 @@ const char* vr_last_error(void);
 int vr_abi_version(void);
 
 /* ------------------------------------------------------------------------------------
- * Dense contraction  C[M,N] = A[M,K] * B[N,K]^T  on tcgen05 tensor cores (TMA-staged
- * 128B-swizzled tiles -> UMMA -> fp32 accumulators in TMEM -> fused epilogue).
+ * Dense contraction  C[M,N] = A[M,K] * B[N,K]^T  on wgmma tensor cores (TMA-staged
+ * 128B-swizzled tiles -> warpgroup MMA -> fp32 accumulators in registers -> fused epilogue).
  * Replaces every nn.Linear / Conv2d-as-GEMM the reference dispatches to cuBLAS/cuDNN:
  *   timm/layers/patch_embed.py:87 (patch conv), timm/models/vision_transformer.py:88,105
  *   (qkv, proj), timm/layers/mlp.py:41-49 (fc1+GELU, fc2), resampler.py:154,159-167,
@@ -68,15 +68,12 @@ typedef struct {
 int vr_gemm(const void* A, int64_t lda, const void* B, int64_t ldb, int32_t ab_dtype, int32_t M, int32_t N, int32_t K,
             const vr_gemm_epilogue* epi, void* stream);
 
-/* Same operation with the kernel variant chosen by the caller (benchmarks, parity tests of every variant):
- *   block_n = 0    what vr_gemm picks: the CTA-pair kernel when M > 128 and N >= 256, 128 x 64 tiles when M <= 128
- *                  (weight-streaming bound: more, narrower tiles), else 128-row tiles
- *   block_n = 2    CTA-pair kernel (tcgen05 cta_group::2, one 256x256 tile per pair of SMs, each CTA stages half of B);
- *                  LINEAR epilogues with N % 192 == 0, N % 256 != 0 and K <= 2304 (proj: N = K = 1152) use 256x192 tiles
- *   block_n = 4    CTA-pair kernel with 256x192 tiles forced (LINEAR epilogues only)
- *   block_n = 256 / 128 / 64   single-CTA kernel, token-major accumulator, 128 tokens x block_n features per tile
- *   block_n = 3    single-CTA kernel, feature-major accumulator (the weight tile is the MMA's M operand), LINEAR
- *                  epilogues only; its epilogue needs no shared-memory transpose */
+/* Same operation with the tile shape chosen by the caller (benchmarks, parity tests of every variant):
+ *   block_n = 0    what vr_gemm picks: 128 x 64 tiles when M <= 128 (weight-streaming bound: more, narrower tiles), else
+ *                  128 x 256, or 128 x 192 where 192 divides N and 256 does not (N = 1152), 128 x 128 for N < 256
+ *   block_n = 256 / 192 / 128 / 64   token-major accumulator, 128 tokens x block_n features per tile
+ *   block_n = 3    feature-major accumulator (the weight tile is the MMA's M operand, 128 tokens are its N), LINEAR
+ *                  epilogues only */
 int vr_gemm_tuned(const void* A, int64_t lda, const void* B, int64_t ldb, int32_t ab_dtype, int32_t M, int32_t N,
                   int32_t K, const vr_gemm_epilogue* epi, int32_t block_n, void* stream);
 
@@ -107,9 +104,9 @@ int vr_resample_u8(const uint8_t* src, int32_t src_pixel_bytes, int32_t n, int32
                    uint8_t* out, const int32_t* first_cell, int32_t cell_h, int32_t cell_w, void* stream);
 
 /* ------------------------------------------------------------------------------------
- * Fused softmax(Q K^T * scale) V on tcgen05. Sequences longer than 128 queries: two query tiles per CTA, S, P
- * (bf16, TS-MMA operand) and the O accumulator all live in TMEM, lazy rescaling. Up to 128 queries per sequence:
- * single-tile kernel, P re-staged through 128B-swizzled shared memory, running max/sum/O in registers.
+ * Fused softmax(Q K^T * scale) V on wgmma. S, P (bf16, register A operand of the second MMA), running max / sum and the
+ * O accumulator all live in registers. Sequences longer than 64 queries: two consumer warpgroups (128 queries) per CTA
+ * share one K/V stream; up to 64 queries per sequence: one warpgroup per CTA.
  * Replaces F.scaled_dot_product_attention in timm/models/vision_transformer.py:92-96 (ViT,
  * 16 heads x 72, no mask), modeling_minicpm.py:895-903 (MiniCPM, causal + right padding ->
  * here: packed var-len sequences, no padding rows at all) and nn.MultiheadAttention in
@@ -135,19 +132,13 @@ typedef struct {
 } vr_attn_params;
 
 /* The caller guarantees V[:, head_dim] == 1 for every head (head_dim == head_stride - 8; e.g. a bias of 1 in the zero
- * padding of the QKV projection). Kernels that can use it take the softmax denominator out of the P.V MMA (column
- * head_dim of the accumulator) instead of summing P in registers; the others ignore the column. Results are the same
- * up to fp32 summation order. */
+ * padding of the QKV projection). A kernel may then take the softmax denominator out of the P.V MMA (column head_dim of
+ * the accumulator) instead of summing P in registers; the sm_90a kernels sum P in registers (it is already there) and
+ * ignore the column. Results are the same up to fp32 summation order. */
 #define VR_ATTN_V_ONES_COLUMN 1
 
 int vr_attention(const vr_attn_params* p, void* stream);
-/* Dispatch: non-causal sequences longer than 128 queries (the ViT) run the persistent kernel of attention4.cuh (one CTA per
- * SM loops over (query-tile pair, head, sequence) items; P in its own TMEM buffer so Q.K^T of the next key block is issued
- * while the exps of the current one run); causal long sequences the two-tile kernel of attention2.cuh; everything else
- * the single-tile kernel.
- * test / benchmark hook (process-wide): 0 = default dispatch, 1 = always the one-tile-per-CTA kernel, 2 = attention2 wherever
- * attention4 is the default, 5 = two-tile kernel with Q in tensor memory as well (measured slower than the default; kept
- * as a tested alternative) */
+/* test / benchmark hook (process-wide): 0 = default dispatch, 1 = always the one-warpgroup (64 queries per CTA) kernel */
 void vr_attention_force_v1(int32_t variant);
 
 
@@ -193,7 +184,7 @@ int vr_pool_norm(const float* h, int64_t ldh, const float* gamma, float eps, con
  * Similarity + top-k: replaces `torch.matmul(Q, D^T)` + `torch.topk` of
  * retriever/dense_retriever.py:25-30 (fp32 scores) and the Python merge loop `:88-92`.
  * The [nq, nd] score matrix is never materialised:
- *   vr_score_filter  : tcgen05 fp16 GEMM on CTA pairs (256 queries x 256 docs per MMA tile) with a fused per-row running
+ *   vr_score_filter  : wgmma fp16 GEMM on CTA pairs (256 queries x 256 docs per tile, 128 queries per CTA) with a fused per-row running
  *                      top-16 per (query, doc range); writes `lists = 2*ranges` sorted 16-entry candidate lists per query into
  *                      cand_scores / cand_ids [nq, lists*16] (unused lists: score -inf, id -1; the first score of the LAST
  *                      list slot is scratch - the query's running threshold - and carries id -1);

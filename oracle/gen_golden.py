@@ -1,5 +1,5 @@
 """TEST INFRASTRUCTURE. Generates tests/golden/*.npz by running the REAL reference (through
-oracle/reference_shim.py) in the build container:   python -m oracle.gen_golden [--full]
+oracle/reference_shim.py) where a checkout of it is available (VISRAG_REFERENCE):   python -m oracle.gen_golden [--full]
 
 The .npz files hold everything needed to replay the case without the reference: the config, the weight seed
 (weights are re-drawn by visrag_b200.weights.random_state_dict), the page sizes + pixel seed (pages are
@@ -79,7 +79,7 @@ def gen_model_case(name, cfg, weight_seed, page_sizes, page_seed, n_queries, que
     print(name, "pages", p.shape, "queries", q.shape)
 
 
-REAL_PAGES = os.path.join(GOLDEN_DIR, "real_pages.npz")
+REAL_PAGES = [os.path.join(GOLDEN_DIR, n) for n in ("real_pages_parquet.npz", "real_pages_demo.npz")]  # each below 1 MB
 
 
 def gen_real_pages():
@@ -90,20 +90,21 @@ def gen_real_pages():
     from oracle.reference_shim import REF_ROOT
 
     t = pq.read_table(os.path.join(REF_ROOT, "examples", "training_data", "0.parquet"))
-    out, queries = {}, []
+    out, demo, queries = {}, {}, []
     for i in range(t.num_rows):
         out[f"parquet{i}"] = np.frombuffer(t.column("image")[i].as_py()["bytes"], dtype=np.uint8)
         queries.append(t.column("query")[i].as_py())
     for n in ("cat.jpeg", "dog.jpg"):
         with open(os.path.join(REF_ROOT, "visrag_scripts", "demo", "retriever", "test_image", n), "rb") as f:
-            out[n.split(".")[0]] = np.frombuffer(f.read(), dtype=np.uint8)
-    np.savez(REAL_PAGES, queries=np.asarray(queries), **out)
-    print("real pages:", {k: v.size for k, v in out.items()})
+            demo[n.split(".")[0]] = np.frombuffer(f.read(), dtype=np.uint8)
+    np.savez(REAL_PAGES[0], queries=np.asarray(queries), **out)
+    np.savez(REAL_PAGES[1], **demo)
+    print("real pages:", {k: v.size for k, v in dict(out, **demo).items()})
 
 
 def full_v2_spec():
     """>= 32 pages (>= 8 multi-slice + the reference's 4 real example images) and >= 8 queries: a corpus on which the
-    top-5 ranking is a real statement (VERDICT r01 'next' #1)."""
+    top-5 ranking is a real statement."""
     single = [(448, 448), (400, 500), (300, 600), (224, 224), (336, 336), (420, 420), (500, 390), (448, 448), (360, 540),
               (640, 300), (448, 448), (280, 280), (512, 384), (384, 512), (448, 448), (330, 600), (600, 330), (448, 440),
               (224, 224), (436, 452)]
@@ -149,16 +150,85 @@ def gen_spec_case(name, cfg, weight_seed, spec, n_queries, query_seed, topk, bat
     print(name, "pages", p.shape, "queries", q.shape, "min score gap inside top-(k+1):", gaps.min(), "median", np.median(gaps))
 
 
+def gen_reference_pins():
+    """What tests/test_oracle_vs_reference.py compares the oracle with: outputs of the reference on the test's own seeded
+    inputs (embeddings, hidden states, the other poolings on a ragged batch, `_retrieve_one_shard`, run files, MRR)."""
+    import pickle
+    import tempfile
+
+    import torch
+    from oracle import reference_shim as RS
+    from visrag_b200 import retriever as R
+    from visrag_b200.config import VisRAGConfig
+    from visrag_b200.tokenizer_stub import StubTokenizer
+    from visrag_b200.weights import random_state_dict
+
+    out = {}
+    cfg = VisRAGConfig.tiny()
+    tok = StubTokenizer(cfg.vocab)
+    sd = random_state_dict(cfg, 777)
+    model = RS.build_reference_model(cfg, sd, attn_implementation="sdpa")
+    pages = synth_pages([(300, 300), (1000, 600), (448, 448)], 21)
+    items = [{"id": str(i), "text": "doc text" if i == 1 else "", "image": im} for i, im in enumerate(pages)]
+    out["fresh_pages"] = RS.encode(model, tok, items, False)
+    qs = [QUERY_PREFIX + "what is shown", QUERY_PREFIX + "x"]
+    out["fresh_queries"] = RS.encode(model, tok, [{"id": f"q{i}", "text": t, "image": None} for i, t in enumerate(qs)], True)
+    hs, mask = RS.hidden_states(model, tok, [it["text"] for it in items], pages)
+    out["fresh_hidden"], out["fresh_mask"] = hs.astype(np.float32), mask.astype(np.int64)
+    sd = random_state_dict(cfg, 778)
+    page = synth_pages([(448, 448)], 5)[0]
+    texts = [QUERY_PREFIX + "a", QUERY_PREFIX + "a much longer query about the page content", ""]
+    items = [{"id": str(i), "text": t, "image": im} for i, (t, im) in enumerate(zip(texts, [None, None, page]))]
+    for pooling in ("lasttoken", "mean", "cls"):
+        model = RS.build_reference_model(cfg, sd, attn_implementation="sdpa", pooling=pooling)
+        out[f"pooling_{pooling}"] = RS.encode(model, tok, items, False)
+    # scoring side: the reference's shard reader + top-k, run-file writer / reader and MRR on the test's vectors
+    from openmatch import utils as ref_utils
+    from openmatch.retriever.dense_retriever import _retrieve_one_shard as ref_retrieve
+
+    rs = np.random.RandomState(12)
+    D = rs.randn(500, 64).astype(np.float32)
+    D /= np.linalg.norm(D, axis=1, keepdims=True)
+    Q = rs.randn(7, 64).astype(np.float32)
+    Q /= np.linalg.norm(Q, axis=1, keepdims=True)
+    lookup = [f"doc{i}" for i in range(len(D))]
+    with tempfile.TemporaryDirectory() as tmp:
+        shard = os.path.join(tmp, "embeddings.corpus.rank.0")
+        R.save_shard(shard, D, lookup)
+        s_ref, i_ref, look_ref = ref_retrieve(shard, torch.from_numpy(Q), 10, "cpu")
+        assert look_ref == lookup and pickle.load(open(shard, "rb"))[1] == lookup
+        s, i = s_ref.numpy(), i_ref.numpy()
+        run = {f"q{q}": {lookup[j]: float(s[q, r]) for r, j in enumerate(i[q])} for q in range(len(Q))}
+        qrel = {f"q{q}": {lookup[int(i[q, q % 10])]: 1} for q in range(len(Q))}
+        trec = os.path.join(tmp, "ref.trec")
+        ref_utils.save_as_trec(run, trec)
+        out["trec_text"] = np.asarray(open(trec).read())
+        from visrag_b200 import inference as I
+
+        ours = os.path.join(tmp, "ours.trec")
+        I.save_as_trec(run, ours)   # the reference's reader on OUR writer's file
+        assert ref_utils.load_from_trec(ours) == ref_utils.load_from_trec(trec)
+        out["trec_loaded"] = np.asarray(json.dumps(ref_utils.load_from_trec(trec), sort_keys=True))
+        out["mrr"] = np.asarray(json.dumps([ref_utils.eval_mrr(qrel, run, 10), ref_utils.eval_mrr(qrel, run, 3)], sort_keys=True))
+    out["topk_scores"], out["topk_indices"] = s, i
+    np.savez_compressed(os.path.join(GOLDEN_DIR, "reference_pins.npz"), **out)
+    print("reference pins:", {k: getattr(v, "shape", None) for k, v in out.items()})
+
+
 def main():
     ap = argparse.ArgumentParser()
+    ap.add_argument("--pins", action="store_true", help="only generate reference_pins.npz (tests/test_oracle_vs_reference.py)")
     ap.add_argument("--full", action="store_true", help="also generate the full-size (3.1 B parameter) case")
     ap.add_argument("--full-v2", action="store_true", help="only generate full_v2 (36 pages, 10 queries, top-5; ~15 min of CPU)")
     ap.add_argument("--tiny-v2", action="store_true", help="only generate tiny_v2 (same corpus as full_v2, tiny model)")
     a = ap.parse_args()
     from visrag_b200.config import VisRAGConfig as _C
 
+    if a.pins:
+        gen_reference_pins()
+        return
     if a.full_v2 or a.tiny_v2:
-        if not os.path.exists(REAL_PAGES):
+        if not all(os.path.exists(p) for p in REAL_PAGES):
             gen_real_pages()
         if a.tiny_v2:
             gen_spec_case("tiny_v2", _C.tiny(), 1234, full_v2_spec(), 8, 25, 5)

@@ -1,9 +1,9 @@
 """TEST INFRASTRUCTURE (oracle/) — never imported by the product path.
 
-Runs the UNMODIFIED reference implementation (``/root/reference``: timm_modified + src/openmatch) on CPU so
+Runs the UNMODIFIED reference implementation (a checkout of OpenBMB/VisRAG, ``VISRAG_REFERENCE``: timm_modified + src/openmatch) on CPU so
 that (1) the restatement in ``oracle/restated.py`` can be validated against it and (2) golden vectors can be
-generated (``oracle/gen_golden.py``). Only usable in the build container: ``/root/reference`` does not exist
-on the GPU box, so nothing under tests/ -m gpu, smoke() or bench.py touches this module.
+generated (``oracle/gen_golden.py``). Only usable where a checkout of the reference exists (``VISRAG_REFERENCE``), so nothing under
+tests/ -m gpu, smoke() or bench.py touches this module.
 
 Shims (SURVEY.md §8c; the reference pins transformers 4.40, this image has 5.x):
   1. ``transformers.utils.import_utils.is_torch_fx_available`` is gone -> provide ``lambda: False``

@@ -2,13 +2,13 @@
 __graft_entry__.smoke() and bench.py's cpu_baseline / --impl reference legs may call it.
 
 CPU fp32 restatement of the VisRAG-Ret embedding + retrieval hot path, written from the reference sources
-(paths relative to /root/reference; every function cites the lines it follows). The arithmetic is floating
+(paths relative to the reference checkout; every function cites the lines it follows). The arithmetic is floating
 point, so it is plain fp32 PyTorch-on-CPU / numpy (third-party primitives the reference itself calls:
 ``F.interpolate``, ``F.layer_norm``, ``erf``-GELU, ``softmax``, ``PIL.Image.resize``).
 
 Pinning: the reference has NO tests or golden vectors for this path (SURVEY.md §4, F11). This oracle is
-pinned against the reference *itself*, executed in the build container through ``oracle/reference_shim.py``
-(``tests/test_oracle_vs_reference.py``, skipped when /root/reference is absent) and against the golden
+pinned against the reference *itself*, executed through ``oracle/reference_shim.py``
+(``tests/test_oracle_vs_reference.py``, through stored reference outputs) and against the golden
 vectors generated from the real reference by ``oracle/gen_golden.py`` (``tests/golden/*.npz``,
 ``tests/test_oracle_golden.py`` — runs everywhere).
 

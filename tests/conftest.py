@@ -11,8 +11,8 @@ GOLDEN = os.path.join(ROOT, "tests", "golden")
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box with -m gpu)")
-    config.addinivalue_line("markers", "reference: needs /root/reference (build container only)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (an H100; select with -m gpu)")
+    config.addinivalue_line("markers", "reference: needs a checkout of the reference implementation (VISRAG_REFERENCE)")
 
 
 @pytest.fixture(scope="session")

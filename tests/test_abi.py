@@ -44,7 +44,7 @@ def test_missing_library_fails_loudly(monkeypatch, tmp_path):
 
 def test_score_plan_is_host_logic_and_bounded():
     """vr_score_ranges (the candidate-buffer sizing the caller needs before vr_score_filter) is pure host arithmetic: it must
-    answer without a GPU (148 SMs assumed) and stay within the rescoring kernel's list limit for any problem size."""
+    answer without a GPU (the 132 SMs of an H100 SXM assumed) and stay within the rescoring kernel's list limit for any problem size."""
     import ctypes as C
 
     from visrag_b200 import _lib as L
@@ -58,7 +58,7 @@ def test_score_plan_is_host_logic_and_bounded():
         assert 1 <= r <= 33, (nq, nd, r)
     assert lib.vr_score_ranges(10_000, 125_000) <= 8          # few lists per query where the rescoring cost matters
     # the work decomposition itself: every (query block, doc tile) is covered exactly once, the launch never exceeds the pairs
-    # of a 148-SM device, and the candidate buffers have a spare slot beyond the R real lists (the running threshold)
+    # of a 132-SM device, and the candidate buffers have a spare slot beyond the R real lists (the running threshold)
     import numpy as np
 
     for nq, nd in ((1, 256), (700, 33_333), (257, 70_001), (2600, 9000), (10_000, 125_000), (3, 300_000)):
@@ -66,7 +66,7 @@ def test_score_plan_is_host_logic_and_bounded():
         assert lib.vr_score_plan(nq, nd, out) == 0
         T, R, QB, items, pairs, lists = list(out)
         assert T == -(-nd // 256) and QB == -(-nq // 256) and 1 <= R <= min(T, 64) and items == R * QB
-        assert 1 <= pairs <= min(items, 74) and lists == 2 * lib.vr_score_ranges(nq, nd) and lists >= R + 1
+        assert 1 <= pairs <= min(items, 66) and lists == 2 * lib.vr_score_ranges(nq, nd) and lists >= R + 1
         cover = np.zeros((QB, T), dtype=np.int32)
         for i in range(items):
             b, r = i % QB, i // QB

@@ -1,4 +1,4 @@
-"""The drop-in classes under the REAL reference driver (build container only: needs /root/reference).
+"""The drop-in classes under the REAL reference driver (needs a checkout of the reference: VISRAG_REFERENCE).
 
 `src/openmatch/driver/eval.py` is imported unmodified; only the two names INTEGRATION.md §2.3 tells a maintainer to rebind are
 rebound: `DRModelForInference` (-> visrag_b200.modeling) and, for metrics, the absent `pytrec_eval` package (-> a shim over
@@ -8,7 +8,7 @@ visrag_b200.inference's restated measures). Then the driver's own functions run:
   the reference's distributed_parallel_embedding_inference (inference.py:53-172) drives the returned model with its own
                                     DataLoader / naive_collator / kwargs conventions and writes the pickle shards
   retrieve (eval.py:210-232)     -> the reference's CPU retrieval over those shards, save_as_trec, save_results
-There is no GPU in the build container, so the ONE thing replaced by test infrastructure is the device math: the model class
+This test runs without a GPU, so the ONE thing replaced by test infrastructure is the device math: the model class
 under test is a subclass of visrag_b200's whose `encode` computes the embeddings with the oracle (CPU). Everything else -
 checkpoint discovery and loading, config translation, the B2 call conventions the driver relies on (.to/.eval/forward(query=,
 passage=, **kwargs) -> .q_reps/.p_reps tensors) - is the shipped code. The same `build()` runs on real kernels in
@@ -26,7 +26,7 @@ import torch
 from oracle import reference_shim as RS
 from tests.helpers import synth_doc_pages
 
-pytestmark = pytest.mark.skipif(not RS.available(), reason="needs /root/reference (build container only)")
+pytestmark = pytest.mark.skipif(not RS.available(), reason="needs a checkout of the reference implementation (VISRAG_REFERENCE)")
 
 
 def _pytrec_eval_shim():

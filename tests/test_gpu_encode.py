@@ -1,4 +1,4 @@
-"""Encode-path parity on the B200: CUDA engine (through the C ABI and the reference-signature classes) against
+"""Encode-path parity on the H100: CUDA engine (through the C ABI and the reference-signature classes) against
   (1) golden embeddings produced by the REAL reference (tests/golden/*.npz), tiny and full-size model,
   (2) the oracle restatement on freshly seeded inputs, at the B1 (hidden states) and B2 (embeddings) boundaries.
 Stated tolerance (north_star: "within a stated fp tolerance"): cosine(embedding, fp32 reference) >= 0.9999 per vector

@@ -1,4 +1,4 @@
-"""Device image front-end on the B200 (SURVEY.md §8f.2): the CUDA resampler behind `vr_resample_u8` against PIL itself
+"""Device image front-end on the H100 (SURVEY.md §8f.2): the CUDA resampler behind `vr_resample_u8` against PIL itself
 (bit for bit), and the encode path with device-rendered slices against the same path with PIL-rendered slices
 (bit-identical embeddings)."""
 import numpy as np

@@ -1,4 +1,4 @@
-"""Kernel-level parity on the B200 (through the C ABI) against plain PyTorch fp32 references of the same op.
+"""Kernel-level parity on the H100 (through the C ABI) against plain PyTorch fp32 references of the same op.
 Tolerances: fp32-output paths 2e-3 relative to max|ref| (bf16 operands, fp32 accumulate); bf16-output paths 1e-2
 (one bf16 rounding of the result)."""
 import pytest
@@ -10,12 +10,12 @@ from tools import check_encode as CE  # noqa: E402
 from tools import check_gemm as CG  # noqa: E402
 
 
-@pytest.mark.parametrize("bn", [256, 128, 64, 3, 2, 4])  # 3 = feature-major accumulator kernel, 2 = CTA-pair kernel, 4 = pair, 192-wide tiles
+@pytest.mark.parametrize("bn", [256, 128, 64, 192, 3, 0])  # tile width; 3 = feature-major accumulator kernel, 0 = what vr_gemm picks
 def test_gemm_plain_shapes(bn):
     assert CG.case_basic(bn)
 
 
-@pytest.mark.parametrize("bn", [256, 128, 64, 3, 2, 4])
+@pytest.mark.parametrize("bn", [256, 128, 64, 192, 3, 0])
 def test_gemm_fused_epilogues(bn):
     assert CG.case_epilogues(bn)
 
@@ -25,16 +25,11 @@ def test_elementwise_kernels():
 
 
 def test_attention_three_shapes():
-    assert CE.stage_attention()          # two-tile ping-pong kernel wherever max_q > 128
+    assert CE.stage_attention()          # two-warpgroup (128 queries per CTA) kernel wherever max_q > 64
 
 
 def test_attention_three_shapes_single_tile_kernel():
     assert CE.stage_attention(force_v1=True)
-
-
-@pytest.mark.parametrize("variant", [2, 5])  # 2 = round-1 two-tile kernel (still the causal long-sequence kernel), 5 = the same with Q in tensor memory
-def test_attention_three_shapes_other_variants(variant):
-    assert CE.stage_attention(variant=variant)
 
 
 def test_gemm_rejects_bad_arguments():

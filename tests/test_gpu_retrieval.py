@@ -1,4 +1,4 @@
-"""Similarity + top-k on the B200 against the oracle's fp32 scan: ids bit-identical (tie rule: score desc, id asc),
+"""Similarity + top-k on the H100 against the oracle's fp32 scan: ids bit-identical (tie rule: score desc, id asc),
 scores within fp32 summation-order noise (2e-6 on unit vectors)."""
 import os
 from types import SimpleNamespace
@@ -189,7 +189,7 @@ def _nccl_worker(rank, world, port, out_q):
 
 
 def test_sharded_topk_under_nccl_equals_the_brute_force_scan():
-    """World-size-2 NCCL run on two real GPUs (skipped on a one-GPU box): query all-gather + partial-top-k all-gather +
+    """World-size-2 NCCL run on two real GPUs (skipped on a one-GPU machine): query all-gather + partial-top-k all-gather +
     merge kernel give exactly the ids of a brute-force fp32 scan of the unsharded corpus, on every rank."""
     if torch.cuda.device_count() < 2:
         pytest.skip("needs two GPUs")
@@ -211,7 +211,7 @@ def test_sharded_topk_under_nccl_equals_the_brute_force_scan():
 
 
 def test_engine_and_index_on_a_non_current_device():
-    """ADVICE r01: kernels must launch on the device that owns the buffers, not on the process's current device."""
+    """Kernels must launch on the device that owns the buffers, not on the process's current device."""
     if torch.cuda.device_count() < 2:
         pytest.skip("needs two GPUs")
     from tests.helpers import cosine_rows, synth_pages
@@ -239,7 +239,7 @@ def test_engine_and_index_on_a_non_current_device():
 
 
 def test_non_finite_and_out_of_fp16_range_inputs_fall_back_to_the_fp32_scan():
-    """ADVICE r01: |x| > 65504 or NaN would become inf/NaN in the fp16 copies; the rescoring kernel flags those queries (or
+    """|x| > 65504 or NaN would become inf/NaN in the fp16 copies; the rescoring kernel flags those queries (or
     every query when the corpus is affected) and the fp32 scan answers them."""
     rs = np.random.RandomState(3)
     D = rs.randn(8000, 256).astype(np.float32)

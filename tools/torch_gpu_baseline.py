@@ -1,6 +1,6 @@
-"""Stock-PyTorch-on-B200 context arm (VERDICT r1 item 10): the same encode path written the way a PyTorch user would run it
+"""Stock-PyTorch-on-the-same-GPU context arm: the same encode path written the way a PyTorch user would run it
 on the GPU today — bf16 modules, cuBLAS `F.linear`, `F.scaled_dot_product_attention` (flash / cuDNN kernels), `F.layer_norm`,
-batched over all pages — with none of this repo's kernels. It answers "how far are the hand-written sm_100a kernels ahead
+batched over all pages — with none of this repo's kernels. It answers "how far are the hand-written sm_90a kernels ahead
 of cuBLAS + library attention", which the CPU arm cannot. Same algorithm as the reference modules it restates
 (`timm/models/vision_transformer.py:86-107,682-692`, `resampler.py:146-168`, `modeling_minicpm.py:824-1004`,
 `dense_retrieval_model.py:170-225`); stronger than the reference's own loop, which runs the ViT page by page

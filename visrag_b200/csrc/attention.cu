@@ -1,100 +1,53 @@
 #include <string.h>
 #include "common.h"
 #include "attention.cuh"
-#include "attention2.cuh"
-#include "attention4.cuh"
 
 namespace vr {
 
 static int g_variant = 0;  // see vr_attention_force_v1()
 
-
-template <int HS, bool CAUSAL, bool V2>
+template <int HS, bool CAUSAL, int NWG>
 static int launch_attention(const vr_attn_params& p, cudaStream_t stream) {
-    using Cfg = AttCfg<HS>;
+    using Cfg = AttCfg<HS, NWG>;
     AttMaps maps;
     memset(&maps, 0, sizeof(maps));
     // TMA extents: all columns of the token matrices, rows = buffer rows (out-of-range rows read as zero)
     const uint64_t qcols = p.ldq, kcols = p.ldk, vcols = p.ldv;
-    if (int rc = make_tmap_2d(&maps.q64, p.q, p.q_rows, qcols, p.ldq, ATT_BM, 64, 128, true)) return rc;
+    if (int rc = make_tmap_2d(&maps.q64, p.q, p.q_rows, qcols, p.ldq, Cfg::BM, 64, 128, true)) return rc;
     if (int rc = make_tmap_2d(&maps.k64, p.k, p.kv_rows, kcols, p.ldk, ATT_BN, 64, 128, true)) return rc;
     if (int rc = make_tmap_2d(&maps.v64, p.v, p.kv_rows, vcols, p.ldv, ATT_BN, 64, 128, true)) return rc;
     if (Cfg::HAS16) {
-        if (int rc = make_tmap_2d(&maps.q16, p.q, p.q_rows, qcols, p.ldq, ATT_BM, 16, 32, true)) return rc;
+        if (int rc = make_tmap_2d(&maps.q16, p.q, p.q_rows, qcols, p.ldq, Cfg::BM, 16, 32, true)) return rc;
         if (int rc = make_tmap_2d(&maps.k16, p.k, p.kv_rows, kcols, p.ldk, ATT_BN, 16, 32, true)) return rc;
         if (int rc = make_tmap_2d(&maps.v16, p.v, p.kv_rows, vcols, p.ldv, ATT_BN, 16, 32, true)) return rc;
     }
     AttArgs a;
     a.q_col0 = p.q_col0; a.k_col0 = p.k_col0; a.v_col0 = p.v_col0;
     a.head_dim = p.head_dim; a.heads = p.heads; a.batch = p.batch;
-    a.cu_q = p.cu_q; a.cu_k = p.cu_k; a.max_q = p.max_q; a.causal = p.causal;
+    a.cu_q = p.cu_q; a.cu_k = p.cu_k; a.max_q = p.max_q;
     a.scale_log2 = p.scale * 1.4426950408889634f;
     a.out = reinterpret_cast<__nv_bfloat16*>(p.out);
     a.ldo = p.ldo;
-    a.q = reinterpret_cast<const __nv_bfloat16*>(p.q);
-    a.ldq = p.ldq;
-    a.tma_out = 0;
-    if constexpr (V2 && !CAUSAL) {
-        if (g_variant == 0) {
-            // default for long non-causal sequences (the ViT): persistent decoupled kernel, attention4.cuh
-            using Cfg4 = Att4Cfg<HS>;
-            const bool ones = (p.flags & VR_ATTN_V_ONES_COLUMN) != 0;
-            const int nqp = (p.max_q + 2 * ATT_BM - 1) / (2 * ATT_BM);
-            const long long items = static_cast<long long>(nqp) * p.heads * p.batch;
-            // output tile store: 128 rows x head_dim columns per (tile, head), plain row-major box (no swizzle)
-            if (p.cu_q && (reinterpret_cast<uintptr_t>(p.out) & 15) == 0 && p.head_dim % 8 == 0) {
-                if (int rc = make_tmap_2d(&maps.o, p.out, p.q_rows, p.ldo, p.ldo, ATT_BM, p.head_dim, 0, true)) return rc;
-                a.tma_out = 1;
-            }
-            auto kern = ones ? attention4_tcgen05_kernel<HS, true> : attention4_tcgen05_kernel<HS, false>;
-            static unsigned long long attr_set4[2] = {0, 0};
-            if (first_use_on_device(&attr_set4[ones]))
-                VR_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg4::SMEM_BYTES));
-            const int grid = static_cast<int>(items < num_sms() ? items : num_sms());
-            kern<<<grid, ATT4_THREADS, Cfg4::SMEM_BYTES, stream>>>(maps, a, static_cast<int>(items), nqp);
-            VR_CHECK_CUDA(cudaGetLastError());
-            return 0;
-        }
-    }
-    if constexpr (V2) {
-        {
-            // sequences longer than one query tile: two 128-query tiles per CTA in ping-pong, P and O in tensor memory
-            using Cfg2 = Att2Cfg<HS>;
-            // variant 5: Q in tensor memory as well (TS-MMA for Q.K^T). Measured SLOWER than Q in shared memory (1.20 vs
-            // 1.11 ms per ViT layer): the per-CTA prologue (row-wise global loads + tcgen05.st) and the extra TMEM reads
-            // cost more than the cheaper A operand saves. Needs 16-byte aligned Q rows.
-            const bool q_tmem = g_variant == 5 && p.ldq % 8 == 0 && p.q_col0 % 8 == 0 &&
-                                (reinterpret_cast<uintptr_t>(p.q) & 15) == 0;
-            auto kern = q_tmem ? attention2_tcgen05_kernel<HS, CAUSAL, true> : attention2_tcgen05_kernel<HS, CAUSAL, false>;
-            static unsigned long long attr_set[2] = {0, 0};
-            if (first_use_on_device(&attr_set[q_tmem]))
-                VR_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg2::SMEM_BYTES));
-            dim3 grid((p.max_q + 2 * ATT_BM - 1) / (2 * ATT_BM), p.heads, p.batch);
-            kern<<<grid, ATT2_THREADS, Cfg2::SMEM_BYTES, stream>>>(maps, a);
-        }
-    } else {
-        auto kern = attention_tcgen05_kernel<HS, CAUSAL>;
-        static unsigned long long attr_set = 0;
-        if (first_use_on_device(&attr_set))
-            VR_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES));
-        dim3 grid((p.max_q + ATT_BM - 1) / ATT_BM, p.heads, p.batch);
-        kern<<<grid, ATT_THREADS, Cfg::SMEM_BYTES, stream>>>(maps, a);
-    }
+    auto kern = attention_wgmma_kernel<HS, CAUSAL, NWG>;
+    static unsigned long long attr_set = 0;
+    if (first_use_on_device(&attr_set))
+        VR_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES));
+    dim3 grid((p.max_q + Cfg::BM - 1) / Cfg::BM, p.heads, p.batch);
+    kern<<<grid, Cfg::THREADS, Cfg::SMEM_BYTES, stream>>>(maps, a);
     VR_CHECK_CUDA(cudaGetLastError());
     return 0;
 }
 
+template <int HS>
+static int dispatch_attention(const vr_attn_params& p, cudaStream_t s) {
+    const bool two = p.max_q > 64 && g_variant != 1;  // more than one 64-query tile per sequence
+    if (p.causal) return two ? launch_attention<HS, true, 2>(p, s) : launch_attention<HS, true, 1>(p, s);
+    return two ? launch_attention<HS, false, 2>(p, s) : launch_attention<HS, false, 1>(p, s);
+}
+
 }  // namespace vr
 
-#if VR_A_TRACE
-extern "C" int vr_attention_trace_read(long long* out) {
-    return cudaMemcpyFromSymbol(out, vr::g_att_trace, sizeof(vr::g_att_trace)) == cudaSuccess ? 0 : 1;
-}
-#endif
-
-// test hook: 0 = default kernels, 1 = force the single-tile kernel for every shape, 2 = round-1 two-tile kernel (attention2)
-// where the persistent attention4 kernel is the default,
-// 5 = two-tile kernel with Q in tensor memory too (slower; kept as a measured alternative)
+// test hook: 0 = default dispatch, 1 = force the one-warpgroup (64 queries per CTA) kernel for every shape
 extern "C" void vr_attention_force_v1(int32_t variant) { vr::g_variant = variant; }
 
 extern "C" int vr_attention(const vr_attn_params* p, void* stream) {
@@ -107,18 +60,11 @@ extern "C" int vr_attention(const vr_attn_params* p, void* stream) {
     VR_REQUIRE(p->ldo % 8 == 0, "vr_attention: ldo must be a multiple of 8");
     VR_REQUIRE(!(p->flags & VR_ATTN_V_ONES_COLUMN) || p->head_dim == p->head_stride - 8,
                "vr_attention: VR_ATTN_V_ONES_COLUMN needs head_dim == head_stride - 8 (got %d / %d)", p->head_dim, p->head_stride);
-    VR_REQUIRE(static_cast<long long>(p->heads) * p->batch * ((p->max_q + 255) / 256) < (1ll << 31), "vr_attention: too many work items");
     cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
-    const bool c = p->causal != 0;
-    const bool v2 = p->max_q > ATT_BM && g_variant != 1;  // more than one query tile per sequence
     switch (p->head_stride) {
-        case 64:
-            if (v2) return c ? launch_attention<64, true, true>(*p, s) : launch_attention<64, false, true>(*p, s);
-            return c ? launch_attention<64, true, false>(*p, s) : launch_attention<64, false, false>(*p, s);
-        case 80:
-            if (v2) return c ? launch_attention<80, true, true>(*p, s) : launch_attention<80, false, true>(*p, s);
-            return c ? launch_attention<80, true, false>(*p, s) : launch_attention<80, false, false>(*p, s);
-        case 128: return c ? launch_attention<128, true, false>(*p, s) : launch_attention<128, false, false>(*p, s);
+        case 64: return dispatch_attention<64>(*p, s);
+        case 80: return dispatch_attention<80>(*p, s);
+        case 128: return dispatch_attention<128>(*p, s);
         default: set_error("vr_attention: head_stride must be 64, 80 or 128 (got %d)", p->head_stride); return 2;
     }
 }

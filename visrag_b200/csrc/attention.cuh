@@ -1,44 +1,44 @@
-// Flash-style attention on tcgen05 for the three attention shapes of VisRAG-Ret
+// Flash-style attention on wgmma for the three attention shapes of VisRAG-Ret
 // (ViT 16x72 non-causal, MiniCPM 36x64 causal var-len, Resampler 18x128 cross-attention).
 //
-// One CTA = one (128-query tile, head, sequence). 5 warps:
-//   warps 0-3 : softmax. Thread r owns query row r: it reads its row of S from TMEM
-//               (tcgen05.ld 32x32b -> no cross-thread reduction at all), keeps running max /
-//               sum / O in registers, and writes P (bf16) into 128B-swizzled shared memory.
-//   warp 4    : one lane issues every TMA load and every tcgen05.mma:
-//               S = Q K^T  (M128 x N128 x K=head_stride)      -> TMEM columns [0,128)
-//               PV = P V   (M128 x N=head_stride x K128)      -> TMEM columns [128, 128+HS)
-// K and V tiles of the next key block are prefetched as soon as the MMA that read the current
-// ones has retired. Two CTAs fit per SM for head_stride <= 80, so one CTA's softmax overlaps the
-// other's MMAs.
+// One CTA = one (64*NWG-query tile, head, sequence):
+//   warpgroup 0 (one lane) : TMA producer. Q once, then K and V tiles of 128 keys through two-stage rings.
+//   warpgroups 1..NWG      : each owns 64 query rows and walks the same K/V stream:
+//               S = Q K^T  (m64 x n128 x k=head_stride, operands from shared memory) -> fp32 registers
+//               softmax on the accumulator fragments (a row lives in the 4 lanes of a quad: two shuffles per
+//               reduction), running max / sum in registers
+//               O += P V   (P stays in registers: the accumulator fragment layout of S is the A-operand layout of
+//               the next MMA; V is read MN-major from the same swizzled tile TMA wrote)
+// With NWG = 2 one warpgroup's softmax overlaps the other's MMAs and every K/V tile is staged once for 128 queries;
+// NWG = 1 is the kernel for sequences of up to 64 queries (the resampler's 64 learned queries).
 //
 // Head dims that are not multiples of 64 (ViT: 72, stored padded to 80 with zero columns) are
 // split into a 64-wide 128B-swizzled chunk plus a 16-wide 32B-swizzled chunk, each with its own
-// TMA box and UMMA descriptor.
+// TMA box and MMA descriptor.
 #pragma once
 #include "ptx.cuh"
 #include "../../include/visrag_b200.h"
 
 namespace vr {
 
-constexpr int ATT_BM = 128;  // queries per CTA
 constexpr int ATT_BN = 128;  // keys per iteration
-constexpr int ATT_THREADS = 160;
+constexpr int ATT_STAGES = 2;
 
-template <int HS>
+template <int HS, int NWG>
 struct AttCfg {
+    static constexpr int BM = 64 * NWG;                 // queries per CTA
+    static constexpr int THREADS = 384;                 // producer + two more warpgroups (with NWG = 1 the third only donates registers)
     static constexpr int NCH = HS / 64;                 // 64-wide swizzle-128B chunks
     static constexpr bool HAS16 = (HS % 64) == 16;      // extra 16-wide swizzle-32B chunk
     static_assert(HS == 64 || HS == 80 || HS == 128, "head stride must be 64, 80 or 128");
-    static constexpr int TILE_BYTES = NCH * 16384 + (HAS16 ? 4096 : 0);  // 128 rows x HS x 2B
+    static constexpr int Q_CHUNK = BM * 128;            // one 64-column chunk of the Q tile
+    static constexpr int Q_BYTES = NCH * Q_CHUNK + (HAS16 ? BM * 32 : 0);
+    static constexpr int TILE_BYTES = NCH * 16384 + (HAS16 ? 4096 : 0);  // 128 keys x HS x 2B
     static constexpr int OFF_Q = 0;
-    static constexpr int OFF_K = TILE_BYTES;
-    static constexpr int OFF_V = 2 * TILE_BYTES;
-    static constexpr int OFF_P = 3 * TILE_BYTES;
-    static constexpr int OFF_BAR = OFF_P + 32768;
+    static constexpr int OFF_K = (Q_BYTES + 1023) & ~1023;
+    static constexpr int OFF_V = OFF_K + ATT_STAGES * TILE_BYTES;
+    static constexpr int OFF_BAR = OFF_V + ATT_STAGES * TILE_BYTES;
     static constexpr int SMEM_BYTES = OFF_BAR + 128 + 1024;
-    static constexpr int TMEM_COLS = 256;
-    static constexpr int O_COL = 128;
 };
 
 struct AttArgs {
@@ -48,40 +48,37 @@ struct AttArgs {
     const int* cu_q;
     const int* cu_k;
     int max_q;
-    int causal;
     float scale_log2;  // scale * log2(e)
     __nv_bfloat16* out;
     long long ldo;
-    const __nv_bfloat16* q;  // query matrix base (kernels that stage Q themselves instead of through TMA)
-    long long ldq;
-    int tma_out;             // attention4: maps.o is valid, full 128-row tiles leave through a bulk tensor store
 };
 
 struct AttMaps {
     CUtensorMap q64, q16, k64, k16, v64, v16;
-    CUtensorMap o;  // output [rows, ldo] with a 128-row x head_dim box (attention4's bulk-store epilogue); unused elsewhere
 };
 
-template <int HS, bool CAUSAL>
-__global__ void __launch_bounds__(ATT_THREADS, (HS <= 80) ? 2 : 1)
-attention_tcgen05_kernel(const __grid_constant__ AttMaps maps, const AttArgs a) {
-    using Cfg = AttCfg<HS>;
+template <int HS, bool CAUSAL, int NWG>
+// Register file: 384 threads x 168 as compiled; the producer warpgroup (and, with NWG = 1, the idle third one) hands its
+// share to the consumers: 40 / 232 / 232 resp. 40 / 232 / 40. The same block shape for both forms keeps every role
+// branch warpgroup-uniform with a known register budget.
+__global__ void __launch_bounds__(384, 1)
+attention_wgmma_kernel(const __grid_constant__ AttMaps maps, const AttArgs a) {
+    using Cfg = AttCfg<HS, NWG>;
+    constexpr int NCH = Cfg::NCH;
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
     uint8_t* sQ = smem + Cfg::OFF_Q;
     uint8_t* sK = smem + Cfg::OFF_K;
     uint8_t* sV = smem + Cfg::OFF_V;
-    uint8_t* sP = smem + Cfg::OFF_P;
     uint64_t* bars = reinterpret_cast<uint64_t*>(smem + Cfg::OFF_BAR);
     uint64_t* q_bar = bars + 0;
-    uint64_t* k_bar = bars + 1;
-    uint64_t* v_bar = bars + 2;
-    uint64_t* s_bar = bars + 3;  // S ready (MMA commit)
-    uint64_t* p_bar = bars + 4;  // P written, S consumed (128 softmax threads)
-    uint64_t* o_bar = bars + 5;  // PV ready (MMA commit)
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 6);
+    uint64_t* k_full = bars + 1;                   // [ATT_STAGES]
+    uint64_t* k_empty = k_full + ATT_STAGES;
+    uint64_t* v_full = k_empty + ATT_STAGES;
+    uint64_t* v_empty = v_full + ATT_STAGES;
 
-    const int warp = threadIdx.x >> 5;
+    const int wg = threadIdx.x >> 7;
+    const int warp = (threadIdx.x >> 5) & 3;
     const int lane = threadIdx.x & 31;
     const int qt = blockIdx.x, head = blockIdx.y, b = blockIdx.z;
 
@@ -89,217 +86,220 @@ attention_tcgen05_kernel(const __grid_constant__ AttMaps maps, const AttArgs a) 
     const int len_k = a.cu_k[b + 1] - k_begin;
     const int q_begin = a.cu_q ? a.cu_q[b] : 0;
     const int len_q = a.cu_q ? a.cu_q[b + 1] - q_begin : a.max_q;
-    const int q0 = qt * ATT_BM;
-    if (q0 >= len_q || len_k <= 0) return;  // uniform per CTA: nothing allocated yet
+    const int q0 = qt * Cfg::BM;
+    if (q0 >= len_q || len_k <= 0) return;  // uniform per CTA: nothing set up yet
 
     int nkt = (len_k + ATT_BN - 1) / ATT_BN;
     if (CAUSAL) {
         // keys visible to the last query row of this tile: index <= q + (len_k - len_q)
-        const int last_q = min(q0 + ATT_BM, len_q) - 1;
+        const int last_q = min(q0 + Cfg::BM, len_q) - 1;
         const int max_key = last_q + (len_k - len_q);
         nkt = min(nkt, max_key / ATT_BN + 1);
     }
 
     if (threadIdx.x == 0) {
         mbar_init(q_bar, 1);
-        mbar_init(k_bar, 1);
-        mbar_init(v_bar, 1);
-        mbar_init(s_bar, 1);
-        mbar_init(p_bar, 128);
-        mbar_init(o_bar, 1);
+        for (int i = 0; i < ATT_STAGES; ++i) {
+            mbar_init(&k_full[i], 1);
+            mbar_init(&v_full[i], 1);
+            mbar_init(&k_empty[i], NWG * 4);  // one arrival per consumer warp
+            mbar_init(&v_empty[i], NWG * 4);
+        }
         fence_mbar_init();
     }
-    if (warp == 4) tmem_alloc<Cfg::TMEM_COLS>(tmem_slot);
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
-    const uint32_t tmem_s = tmem_base;
-    const uint32_t tmem_o = tmem_base + Cfg::O_COL;
 
-    if (warp == 4) {
-        if (lane == 0) {
-            // ------------------------------------------------------------ issuer
-            auto load_tile = [&](const CUtensorMap* m64, const CUtensorMap* m16, uint64_t* bar, uint8_t* dst, int col,
-                                 int row) {
+    if (wg == 0 || wg > NWG) {
+        // ---------------------------------------------------------------- TMA producer (warpgroup 0)
+        setmaxnreg_dec<40>();
+        if (wg == 0 && warp == 0 && lane == 0) {
+            const int qcol = a.q_col0 + head * HS, kcol = a.k_col0 + head * HS, vcol = a.v_col0 + head * HS;
+            mbar_expect_tx(q_bar, Cfg::Q_BYTES);
+#pragma unroll
+            for (int c = 0; c < NCH; ++c) tma_load_2d(&maps.q64, q_bar, sQ + c * Cfg::Q_CHUNK, qcol + c * 64, q_begin + q0);
+            if (Cfg::HAS16) tma_load_2d(&maps.q16, q_bar, sQ + NCH * Cfg::Q_CHUNK, qcol + NCH * 64, q_begin + q0);
+            auto load_tile = [&](const CUtensorMap* m64, const CUtensorMap* m16, uint64_t* bar, uint8_t* dst, int col, int row) {
                 mbar_expect_tx(bar, Cfg::TILE_BYTES);
 #pragma unroll
-                for (int c = 0; c < Cfg::NCH; ++c) tma_load_2d(m64, bar, dst + c * 16384, col + c * 64, row);
-                if (Cfg::HAS16) tma_load_2d(m16, bar, dst + Cfg::NCH * 16384, col + Cfg::NCH * 64, row);
+                for (int c = 0; c < NCH; ++c) tma_load_2d(m64, bar, dst + c * 16384, col + c * 64, row);
+                if (Cfg::HAS16) tma_load_2d(m16, bar, dst + NCH * 16384, col + NCH * 64, row);
             };
-            const int qcol = a.q_col0 + head * HS, kcol = a.k_col0 + head * HS, vcol = a.v_col0 + head * HS;
-            load_tile(&maps.q64, &maps.q16, q_bar, sQ, qcol, q_begin + q0);
-            load_tile(&maps.k64, &maps.k16, k_bar, sK, kcol, k_begin);
-            load_tile(&maps.v64, &maps.v16, v_bar, sV, vcol, k_begin);
-
-            constexpr uint32_t idesc_qk = make_idesc_f16(128, 128, 1, 0, 0);
-            constexpr uint32_t idesc_pv64 = make_idesc_f16(128, 64, 1, 0, 1);  // B (=V) is MN-major
-            constexpr uint32_t idesc_pv16 = make_idesc_f16(128, 16, 1, 0, 1);
-            const uint32_t q_addr = smem_u32(sQ), k_addr = smem_u32(sK), v_addr = smem_u32(sV), p_addr = smem_u32(sP);
-
-            mbar_wait(q_bar, 0);
             for (int kt = 0; kt < nkt; ++kt) {
-                const uint32_t ph = kt & 1;
-                // ---- S = Q K^T
-                mbar_wait(k_bar, ph);
-                tc_fence_after();
-                {
-                    uint32_t acc = 0;
-#pragma unroll
-                    for (int c = 0; c < Cfg::NCH; ++c) {
-#pragma unroll
-                        for (int kk = 0; kk < 4; ++kk) {
-                            umma_f16_ss(tmem_s, make_smem_desc(q_addr + c * 16384 + kk * 32, 16, 1024, kLayoutSW128),
-                                        make_smem_desc(k_addr + c * 16384 + kk * 32, 16, 1024, kLayoutSW128), idesc_qk,
-                                        acc);
-                            acc = 1;
-                        }
-                    }
-                    if (Cfg::HAS16) {
-                        umma_f16_ss(tmem_s, make_smem_desc(q_addr + Cfg::NCH * 16384, 16, 256, kLayoutSW32),
-                                    make_smem_desc(k_addr + Cfg::NCH * 16384, 16, 256, kLayoutSW32), idesc_qk, acc);
-                    }
-                }
-                umma_commit(s_bar);
-                // K smem is free once the QK MMAs retired: prefetch the next key tile
-                mbar_wait(s_bar, ph);
-                if (kt + 1 < nkt) load_tile(&maps.k64, &maps.k16, k_bar, sK, kcol, k_begin + (kt + 1) * ATT_BN);
-                // ---- PV = P V   (P from the softmax warps)
-                mbar_wait(p_bar, ph);
-                mbar_wait(v_bar, ph);
-                tc_fence_after();
-#pragma unroll
-                for (int kk = 0; kk < ATT_BN / 16; ++kk) {
-                    const uint64_t pd =
-                        make_smem_desc(p_addr + (kk >> 2) * 16384 + (kk & 3) * 32, 16, 1024, kLayoutSW128);
-#pragma unroll
-                    for (int c = 0; c < Cfg::NCH; ++c) {
-                        // V chunk: [128 keys][64 dims], 128 B per key row -> MN-major, 8-key groups 1024 B apart
-                        umma_f16_ss(tmem_o + c * 64, pd,
-                                    make_smem_desc(v_addr + c * 16384 + kk * 2048, 16, 1024, kLayoutSW128), idesc_pv64,
-                                    kk != 0);
-                    }
-                    if (Cfg::HAS16) {
-                        // [128 keys][16 dims], 32 B per key row
-                        umma_f16_ss(tmem_o + Cfg::NCH * 64, pd,
-                                    make_smem_desc(v_addr + Cfg::NCH * 16384 + kk * 512, 16, 256, kLayoutSW32),
-                                    idesc_pv16, kk != 0);
-                    }
-                }
-                umma_commit(o_bar);
-                mbar_wait(o_bar, ph);  // V and P smem free again
-                if (kt + 1 < nkt) load_tile(&maps.v64, &maps.v16, v_bar, sV, vcol, k_begin + (kt + 1) * ATT_BN);
+                const int st = kt % ATT_STAGES;
+                const uint32_t ph = (kt / ATT_STAGES) & 1;
+                mbar_wait(&k_empty[st], ph ^ 1);
+                load_tile(&maps.k64, &maps.k16, &k_full[st], sK + st * Cfg::TILE_BYTES, kcol, k_begin + kt * ATT_BN);
+                mbar_wait(&v_empty[st], ph ^ 1);
+                load_tile(&maps.v64, &maps.v16, &v_full[st], sV + st * Cfg::TILE_BYTES, vcol, k_begin + kt * ATT_BN);
             }
         }
-    } else {
-        // ---------------------------------------------------------------- softmax warps
-        const int r = threadIdx.x;       // row in the tile == TMEM lane
-        const int q_idx = q0 + r;        // query index inside the sequence
-        const uint32_t lane_off = static_cast<uint32_t>(warp * 32) << 16;
-        const int causal_shift = len_k - len_q;
-        float m_run = -INFINITY, l_run = 0.f;
-        float o[HS];
-#pragma unroll
-        for (int j = 0; j < HS; ++j) o[j] = 0.f;
-        uint8_t* p_row = sP + (r >> 3) * 1024 + (r & 7) * 128;
-
-        for (int kt = 0; kt < nkt; ++kt) {
-            const uint32_t ph = kt & 1;
-            const int key0 = kt * ATT_BN;
-            int limit = len_k - key0;  // keys [0, limit) of this tile exist
-            if (CAUSAL) limit = min(limit, q_idx + causal_shift - key0 + 1);
-            mbar_wait(s_bar, ph);
-            tc_fence_after();
-            // pass 1: row max
-            float m_tile = -INFINITY;
-#pragma unroll 1
-            for (int c = 0; c < 4; ++c) {
-                uint32_t v[32];
-                tmem_ld_32x32(tmem_s + lane_off + c * 32, v);
-                tmem_ld_wait();
-#pragma unroll
-                for (int j = 0; j < 32; ++j)
-                    if (c * 32 + j < limit) m_tile = fmaxf(m_tile, __uint_as_float(v[j]));
-            }
-            const float m_new = fmaxf(m_run, m_tile);
-            const float m_use = (m_new == -INFINITY) ? 0.f : m_new;
-            const float alpha = exp2f((m_run - m_use) * a.scale_log2);  // m_run = -inf -> 0
-            // pass 2: p = exp2((s - m) * scale*log2e); write bf16 P into swizzled smem
-            float l_tile = 0.f;
-#pragma unroll 1
-            for (int c = 0; c < 4; ++c) {
-                uint32_t v[32];
-                tmem_ld_32x32(tmem_s + lane_off + c * 32, v);
-                tmem_ld_wait();
-                float p[32];
-#pragma unroll
-                for (int j = 0; j < 32; ++j) {
-                    const float s = __uint_as_float(v[j]);
-                    p[j] = (c * 32 + j < limit) ? exp2f((s - m_use) * a.scale_log2) : 0.f;
-                    l_tile += p[j];
-                }
-                uint8_t* dst = p_row + (c >> 1) * 16384;
-#pragma unroll
-                for (int i = 0; i < 4; ++i) {
-                    uint4 pk;
-                    pk.x = pack_bf16x2(p[i * 8 + 0], p[i * 8 + 1]);
-                    pk.y = pack_bf16x2(p[i * 8 + 2], p[i * 8 + 3]);
-                    pk.z = pack_bf16x2(p[i * 8 + 4], p[i * 8 + 5]);
-                    pk.w = pack_bf16x2(p[i * 8 + 6], p[i * 8 + 7]);
-                    const int piece = (c & 1) * 4 + i;  // 16-byte piece inside the 128-byte row
-                    *reinterpret_cast<uint4*>(dst + ((piece ^ (r & 7)) << 4)) = pk;
-                }
-            }
-            l_run = l_run * alpha + l_tile;
-            m_run = m_new;
-            // publish P to the async proxy (UMMA reads smem through it) and release S
-            fence_proxy_async_smem();
-            tc_fence_before();
-            mbar_arrive(p_bar);
-            // O = O * alpha + PV
-            mbar_wait(o_bar, ph);
-            tc_fence_after();
-#pragma unroll
-            for (int c = 0; c < HS / 32; ++c) {
-                uint32_t v[32];
-                tmem_ld_32x32(tmem_o + lane_off + c * 32, v);
-                tmem_ld_wait();
-#pragma unroll
-                for (int j = 0; j < 32; ++j) o[c * 32 + j] = o[c * 32 + j] * alpha + __uint_as_float(v[j]);
-            }
-            if (HS % 32 == 16) {
-                uint32_t v[16];
-                tmem_ld_32x16(tmem_o + lane_off + (HS / 32) * 32, v);
-                tmem_ld_wait();
-#pragma unroll
-                for (int j = 0; j < 16; ++j)
-                    o[(HS / 32) * 32 + j] = o[(HS / 32) * 32 + j] * alpha + __uint_as_float(v[j]);
-            }
-        }
-        // ---- write O / l  (head_dim columns; the zero pad columns of a 72->80 head are dropped)
-        if (q_idx < len_q) {
-            const float inv = 1.0f / l_run;
-            const long long row = a.cu_q ? (long long)(q_begin + q_idx) : (long long)b * a.max_q + q_idx;
-            __nv_bfloat16* dst = a.out + row * a.ldo + head * a.head_dim;
-#pragma unroll
-            for (int j8 = 0; j8 < HS / 8; ++j8) {
-                if (j8 * 8 < a.head_dim) {
-                    uint4 pk;
-                    pk.x = pack_bf16x2(o[j8 * 8 + 0] * inv, o[j8 * 8 + 1] * inv);
-                    pk.y = pack_bf16x2(o[j8 * 8 + 2] * inv, o[j8 * 8 + 3] * inv);
-                    pk.z = pack_bf16x2(o[j8 * 8 + 4] * inv, o[j8 * 8 + 5] * inv);
-                    pk.w = pack_bf16x2(o[j8 * 8 + 6] * inv, o[j8 * 8 + 7] * inv);
-                    *reinterpret_cast<uint4*>(dst + j8 * 8) = pk;
-                }
-            }
-        }
+        return;
     }
 
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 4) {
-        tc_fence_after();
-        tmem_dealloc<Cfg::TMEM_COLS>(tmem_base);
+    // -------------------------------------------------------------------- consumers
+    setmaxnreg_inc<232>();
+    const int cw = wg - 1;
+    const int g8 = lane >> 2, q4 = lane & 3;
+    const int row_a = q0 + cw * 64 + warp * 16 + g8;  // query index (inside the sequence) of accumulator rows g8 / g8 + 8
+    const int row_b = row_a + 8;
+    const int causal_shift = len_k - len_q;
+    const uint32_t q_addr = smem_u32(sQ) + cw * (64 * 128);
+    const uint32_t q16_addr = smem_u32(sQ) + NCH * Cfg::Q_CHUNK + cw * (64 * 32);
+
+    float o[NCH][32];
+    float o16[8];
+#pragma unroll
+    for (int c = 0; c < NCH; ++c)
+#pragma unroll
+        for (int j = 0; j < 32; ++j) o[c][j] = 0.f;
+#pragma unroll
+    for (int j = 0; j < 8; ++j) o16[j] = 0.f;
+    float m_a = -INFINITY, m_b = -INFINITY, l_a = 0.f, l_b = 0.f;
+
+    mbar_wait(q_bar, 0);
+    for (int kt = 0; kt < nkt; ++kt) {
+        const int st = kt % ATT_STAGES;
+        const uint32_t ph = (kt / ATT_STAGES) & 1;
+        const uint32_t k_addr = smem_u32(sK) + st * Cfg::TILE_BYTES, v_addr = smem_u32(sV) + st * Cfg::TILE_BYTES;
+        // ---- S = Q K^T
+        float s[64];
+        mbar_wait(&k_full[st], ph);
+        wgmma_fence();
+#pragma unroll
+        for (int c = 0; c < NCH; ++c) {
+#pragma unroll
+            for (int kk = 0; kk < 4; ++kk)
+                wgmma_ss<false, false>(s, make_smem_desc(q_addr + c * Cfg::Q_CHUNK + kk * 32, 16, 1024, kLayoutSW128),
+                                       make_smem_desc(k_addr + c * 16384 + kk * 32, 16, 1024, kLayoutSW128), (c | kk) != 0,
+                                       std::integral_constant<int, 128>());
+        }
+        if (Cfg::HAS16)
+            wgmma_ss<false, false>(s, make_smem_desc(q16_addr, 16, 256, kLayoutSW32),
+                                   make_smem_desc(k_addr + NCH * 16384, 16, 256, kLayoutSW32), 1, std::integral_constant<int, 128>());
+        wgmma_commit();
+        wgmma_wait<0>();
+        if (lane == 0) mbar_arrive(&k_empty[st]);
+        wgmma_touch(s);
+
+        // ---- softmax on the fragments: registers 4j+0/1 = row a, 4j+2/3 = row b, keys 8j + 2 q4 + 0/1
+        const int key0 = kt * ATT_BN;
+        int lim_a = len_k - key0, lim_b = lim_a;  // keys [0, lim) of this tile exist for the row
+        if (CAUSAL) {
+            lim_a = min(lim_a, row_a + causal_shift - key0 + 1);
+            lim_b = min(lim_b, row_b + causal_shift - key0 + 1);
+        }
+        float mt_a = -INFINITY, mt_b = -INFINITY;
+#pragma unroll
+        for (int j = 0; j < 16; ++j) {
+#pragma unroll
+            for (int e = 0; e < 2; ++e) {
+                const int key = j * 8 + q4 * 2 + e;
+                if (key < lim_a) mt_a = fmaxf(mt_a, s[4 * j + e]);
+                if (key < lim_b) mt_b = fmaxf(mt_b, s[4 * j + 2 + e]);
+            }
+        }
+        mt_a = fmaxf(mt_a, __shfl_xor_sync(0xffffffffu, mt_a, 1));
+        mt_a = fmaxf(mt_a, __shfl_xor_sync(0xffffffffu, mt_a, 2));
+        mt_b = fmaxf(mt_b, __shfl_xor_sync(0xffffffffu, mt_b, 1));
+        mt_b = fmaxf(mt_b, __shfl_xor_sync(0xffffffffu, mt_b, 2));
+        const float mn_a = fmaxf(m_a, mt_a), mn_b = fmaxf(m_b, mt_b);
+        const float mu_a = (mn_a == -INFINITY) ? 0.f : mn_a, mu_b = (mn_b == -INFINITY) ? 0.f : mn_b;
+        const float alpha_a = exp2f((m_a - mu_a) * a.scale_log2), alpha_b = exp2f((m_b - mu_b) * a.scale_log2);  // m = -inf -> 0
+        m_a = mn_a;
+        m_b = mn_b;
+        float lt_a = 0.f, lt_b = 0.f;  // this thread's part of the row sums (reduced over the quad at the end)
+#pragma unroll
+        for (int j = 0; j < 16; ++j) {
+#pragma unroll
+            for (int e = 0; e < 2; ++e) {
+                const int key = j * 8 + q4 * 2 + e;
+                const float pa = key < lim_a ? exp2f((s[4 * j + e] - mu_a) * a.scale_log2) : 0.f;
+                const float pb = key < lim_b ? exp2f((s[4 * j + 2 + e] - mu_b) * a.scale_log2) : 0.f;
+                s[4 * j + e] = pa;
+                s[4 * j + 2 + e] = pb;
+                lt_a += pa;
+                lt_b += pb;
+            }
+        }
+        l_a = l_a * alpha_a + lt_a;
+        l_b = l_b * alpha_b + lt_b;
+        // ---- O = O * alpha + P V
+#pragma unroll
+        for (int c = 0; c < NCH; ++c)
+#pragma unroll
+            for (int j = 0; j < 8; ++j) {
+                o[c][4 * j] *= alpha_a; o[c][4 * j + 1] *= alpha_a;
+                o[c][4 * j + 2] *= alpha_b; o[c][4 * j + 3] *= alpha_b;
+            }
+        if (Cfg::HAS16) {
+#pragma unroll
+            for (int j = 0; j < 2; ++j) {
+                o16[4 * j] *= alpha_a; o16[4 * j + 1] *= alpha_a;
+                o16[4 * j + 2] *= alpha_b; o16[4 * j + 3] *= alpha_b;
+            }
+        }
+        // P as the A operand: 16 keys = accumulator column blocks 2kk, 2kk+1 -> the four A registers of k step kk. All of
+        // them are written before the fence: register operands of an MMA must not change between fence and wait.
+        uint32_t pa[ATT_BN / 16][4];
+#pragma unroll
+        for (int kk = 0; kk < ATT_BN / 16; ++kk) {
+            pa[kk][0] = pack_bf16x2(s[8 * kk + 0], s[8 * kk + 1]);
+            pa[kk][1] = pack_bf16x2(s[8 * kk + 2], s[8 * kk + 3]);
+            pa[kk][2] = pack_bf16x2(s[8 * kk + 4], s[8 * kk + 5]);
+            pa[kk][3] = pack_bf16x2(s[8 * kk + 6], s[8 * kk + 7]);
+        }
+        mbar_wait(&v_full[st], ph);
+        wgmma_fence();
+#pragma unroll
+        for (int kk = 0; kk < ATT_BN / 16; ++kk) {
+#pragma unroll
+            for (int c = 0; c < NCH; ++c) {
+                // V chunk: [128 keys][64 dims], 128 B per key row -> MN-major, 8-key groups 1024 B apart
+                wgmma_rs_tb(o[c], pa[kk], make_smem_desc(v_addr + c * 16384 + kk * 2048, 16, 1024, kLayoutSW128), 1,
+                            std::integral_constant<int, 64>());
+            }
+            if (Cfg::HAS16) {
+                // [128 keys][16 dims], 32 B per key row
+                wgmma_rs_tb(o16, pa[kk], make_smem_desc(v_addr + NCH * 16384 + kk * 512, 16, 256, kLayoutSW32), 1,
+                            std::integral_constant<int, 16>());
+            }
+        }
+        wgmma_commit();
+        wgmma_wait<0>();
+        if (lane == 0) mbar_arrive(&v_empty[st]);
+#pragma unroll
+        for (int c = 0; c < NCH; ++c) wgmma_touch(o[c]);
+        wgmma_touch(o16);
+    }
+
+    // ---- write O / l  (head_dim columns; the zero pad columns of a 72->80 head are dropped)
+    l_a += __shfl_xor_sync(0xffffffffu, l_a, 1);
+    l_a += __shfl_xor_sync(0xffffffffu, l_a, 2);
+    l_b += __shfl_xor_sync(0xffffffffu, l_b, 1);
+    l_b += __shfl_xor_sync(0xffffffffu, l_b, 2);
+#pragma unroll
+    for (int half = 0; half < 2; ++half) {
+        const int q_idx = half ? row_b : row_a;
+        if (q_idx >= len_q) continue;
+        const float inv = 1.0f / (half ? l_b : l_a);
+        const long long row = a.cu_q ? (long long)(q_begin + q_idx) : (long long)b * a.max_q + q_idx;
+        __nv_bfloat16* dst = a.out + row * a.ldo + head * a.head_dim;
+#pragma unroll
+        for (int c = 0; c < NCH; ++c)
+#pragma unroll
+            for (int j = 0; j < 8; ++j) {
+                const int col = c * 64 + j * 8 + q4 * 2;
+                if (col < a.head_dim)
+                    *reinterpret_cast<uint32_t*>(dst + col) = pack_bf16x2(o[c][4 * j + 2 * half] * inv, o[c][4 * j + 2 * half + 1] * inv);
+            }
+        if (Cfg::HAS16) {
+#pragma unroll
+            for (int j = 0; j < 2; ++j) {
+                const int col = NCH * 64 + j * 8 + q4 * 2;
+                if (col < a.head_dim)
+                    *reinterpret_cast<uint32_t*>(dst + col) = pack_bf16x2(o16[4 * j + 2 * half] * inv, o16[4 * j + 2 * half + 1] * inv);
+            }
+        }
     }
 }
 

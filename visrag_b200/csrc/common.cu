@@ -26,7 +26,7 @@ int num_sms() {
     const int slot = (dev >= 0 && dev < 64) ? dev : 0;
     if (cached[slot] == 0) {
         int n = 0;
-        cached[slot] = (dev >= 0 && cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) == cudaSuccess && n > 0) ? n : 148;
+        cached[slot] = (dev >= 0 && cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) == cudaSuccess && n > 0) ? n : 132;  // no device (host-only planning): an H100 SXM
     }
     return cached[slot];
 }

@@ -86,8 +86,8 @@ im2col_norm_kernel(const uint8_t* __restrict__ px, int n_strips, int gw, int pat
 constexpr int IM2COL14_THREADS = 224;  // 7 warps: 14 pixel rows x 16 patches per round
 
 // BULK: the pixel rows are 16-byte multiples at 16-byte aligned addresses -> the strip is staged by 14 bulk (TMA) row
-// copies onto an mbarrier, double buffered: strip i+1 streams in while strip i is converted (the version with ordinary
-// loads was latency bound: ncu long_scoreboard 7.9 with 21 resident warps per SM).
+// copies onto an mbarrier, double buffered: strip i+1 streams in while strip i is converted (a version with ordinary
+// loads is latency bound: too few loads in flight per SM).
 template <bool BULK>
 __global__ void __launch_bounds__(IM2COL14_THREADS)
 im2col_norm14_kernel(const uint8_t* __restrict__ px, int n_strips, int gw, __nv_bfloat16* __restrict__ out, int ldo) {

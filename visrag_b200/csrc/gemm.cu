@@ -1,21 +1,17 @@
-#include <cstdio>
-#include <cstdlib>
 #include "common.h"
 #include "gemm.cuh"
-#include "gemm2.cuh"
 
 namespace vr {
 
-template <int BN, int MODE, bool OUT_F32, bool GELU, int AB_FMT, bool SWAP = false>
+template <int BN, int MODE, bool OUT_F32, bool GELU, bool SWAP = false>
 static int launch_gemm(const void* A, int64_t lda, const void* B, int64_t ldb, const GemmArgs& g, cudaStream_t stream) {
     using Cfg = GemmCfg<BN>;
     CUtensorMap ta, tb;
-    const bool bf16 = AB_FMT == 1;
-    // both operands use 128-row x 64-column boxes, so the maps are interchangeable: SWAP hands the weight to the MMA's
-    // M side (128 features per tile) and the activations to its N side (BN tokens per tile)
-    if (int rc = make_tmap_2d(SWAP ? &tb : &ta, A, g.M, g.K, lda, GEMM_BM, GEMM_BK, 128, bf16)) return rc;
-    if (int rc = make_tmap_2d(SWAP ? &ta : &tb, B, g.N, g.K, ldb, BN < 128 ? BN : 128, GEMM_BK, 128, bf16)) return rc;
-    auto kern = gemm_tcgen05_kernel<BN, MODE, OUT_F32, GELU, AB_FMT, SWAP>;
+    // the MMA's M operand is staged in 128-row boxes, its N operand in 64-row boxes: SWAP hands the weight to the M side
+    // (128 features per tile) and the activations to the N side (BN tokens per tile)
+    if (int rc = make_tmap_2d(SWAP ? &tb : &ta, A, g.M, g.K, lda, SWAP ? 64 : GEMM_BM, GEMM_BK, 128, true)) return rc;
+    if (int rc = make_tmap_2d(SWAP ? &ta : &tb, B, g.N, g.K, ldb, SWAP ? GEMM_BM : 64, GEMM_BK, 128, true)) return rc;
+    auto kern = gemm_wgmma_kernel<BN, MODE, OUT_F32, GELU, SWAP>;
     static unsigned long long attr_set = 0;  // per template instantiation, one bit per device
     if (first_use_on_device(&attr_set))
         VR_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES));
@@ -27,98 +23,17 @@ static int launch_gemm(const void* A, int64_t lda, const void* B, int64_t ldb, c
     return 0;
 }
 
-template <int MODE, bool OUT_F32, bool GELU, int BN = 256>
-static int launch_gemm2(const void* A, int64_t lda, const void* B, int64_t ldb, const GemmArgs& g, cudaStream_t stream) {
-    using Cfg = Gemm2CfgT<BN>;
-    CUtensorMap ta, tb;
-    if (int rc = make_tmap_2d(&ta, A, g.M, g.K, lda, GEMM_BM, GEMM_BK, 128, true)) return rc;
-    if (int rc = make_tmap_2d(&tb, B, g.N, g.K, ldb, BN / 2, GEMM_BK, 128, true)) return rc;
-    auto kern = gemm2_tcgen05_kernel<MODE, OUT_F32, GELU, BN>;
-    static unsigned long long attr_set = 0;
-    if (first_use_on_device(&attr_set))
-        VR_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES));
-    const int tiles = ((g.M + 2 * GEMM_BM - 1) / (2 * GEMM_BM)) * ((g.N + Cfg::BN - 1) / Cfg::BN);
-    // A persistent kernel must not launch more clusters than can be co-resident: GPCs with an odd number of usable SMs
-    // cannot pair all of them, and a cluster that has to wait for a free pair would run its whole tile list after the
-    // others finished (measured: 74 clusters requested -> about half the throughput). Ask the driver.
-    static int max_pairs_dev[64] = {};
-    const int dev_slot = (current_device() >= 0 && current_device() < 64) ? current_device() : 0;
-    int& max_pairs = max_pairs_dev[dev_slot];
-    if (max_pairs == 0) {
-        cudaLaunchConfig_t cfg = {};
-        cfg.gridDim = dim3(num_sms() / 2 * 2);
-        cfg.blockDim = dim3(GEMM_THREADS);
-        cfg.dynamicSmemBytes = Cfg::SMEM_BYTES;
-        cudaLaunchAttribute attr;
-        attr.id = cudaLaunchAttributeClusterDimension;
-        attr.val.clusterDim.x = 2; attr.val.clusterDim.y = 1; attr.val.clusterDim.z = 1;
-        cfg.attrs = &attr;
-        cfg.numAttrs = 1;
-        int n = 0;
-        VR_CHECK_CUDA(cudaOccupancyMaxActiveClusters(&n, kern, &cfg));
-        VR_REQUIRE(n > 0, "vr_gemm: the CTA-pair kernel cannot be scheduled on this device");
-        max_pairs = n;
-        if (getenv("VR_VERBOSE")) fprintf(stderr, "[visrag_b200] co-resident CTA pairs: %d of %d\n", n, num_sms() / 2);
-    }
-    const int pairs = max_pairs < num_sms() / 2 ? max_pairs : num_sms() / 2;
-    const int clusters = tiles < pairs ? tiles : pairs;
-    kern<<<2 * clusters, GEMM_THREADS, Cfg::SMEM_BYTES, stream>>>(ta, tb, g);
-    VR_CHECK_CUDA(cudaGetLastError());
-    return 0;
-}
-
-// CTA-pair kernel (block_n == 2: tile width chosen here; block_n == 4: 192-wide tiles forced)
-static int dispatch_mode2(const void* A, int64_t lda, const void* B, int64_t ldb, const GemmArgs& g, cudaStream_t s, bool force192,
-                          bool allow_narrow) {
-    const vr_gemm_epilogue& e = g.epi;
-    // 192-wide tiles where they tile N exactly and 256-wide ones do not (N = 1152), for SHORT main loops only. Measured in
-    // the bench step (1.42-1.45 GHz): proj (K = 1152) 791 -> 860 TFLOP/s, patch embed (K = 640) 419 -> 460, but fc2
-    // (K = 4304) 1246 -> 1174: an MMA costs a fixed ~34 cycles plus N/2, so with a long K loop the wider tile's better
-    // per-column rate outweighs the 10 % of zero padding it computes.
-    const bool narrow = force192 || (allow_narrow && e.mode == VR_EPI_LINEAR && g.N % 192 == 0 && g.N % 256 != 0 && g.K <= 2304);
-    if (narrow) {
-        VR_REQUIRE(e.mode == VR_EPI_LINEAR, "vr_gemm: 192-wide pair tiles (block_n=4) support LINEAR epilogues only");
-        if (e.out_dtype == VR_F32) {
-            VR_REQUIRE(!e.act_gelu, "vr_gemm: GELU epilogue writes bf16 only");
-            return launch_gemm2<VR_EPI_LINEAR, true, false, 192>(A, lda, B, ldb, g, s);
-        }
-        VR_REQUIRE(e.out_dtype == VR_BF16, "vr_gemm: out_dtype must be VR_BF16 or VR_F32");
-        if (e.act_gelu) return launch_gemm2<VR_EPI_LINEAR, false, true, 192>(A, lda, B, ldb, g, s);
-        return launch_gemm2<VR_EPI_LINEAR, false, false, 192>(A, lda, B, ldb, g, s);
-    }
-    switch (e.mode) {
-        case VR_EPI_LINEAR:
-            if (e.out_dtype == VR_F32) {
-                VR_REQUIRE(!e.act_gelu, "vr_gemm: GELU epilogue writes bf16 only");
-                return launch_gemm2<VR_EPI_LINEAR, true, false>(A, lda, B, ldb, g, s);
-            }
-            VR_REQUIRE(e.out_dtype == VR_BF16, "vr_gemm: out_dtype must be VR_BF16 or VR_F32");
-            if (e.act_gelu) return launch_gemm2<VR_EPI_LINEAR, false, true>(A, lda, B, ldb, g, s);
-            return launch_gemm2<VR_EPI_LINEAR, false, false>(A, lda, B, ldb, g, s);
-        case VR_EPI_ROPE:
-            VR_REQUIRE(e.positions && e.rope_cos && e.rope_sin, "vr_gemm: ROPE epilogue needs positions/cos/sin");
-            VR_REQUIRE(g.N % 64 == 0 && e.rope_cols % 64 == 0, "vr_gemm: ROPE needs N and rope_cols multiples of 64");
-            return launch_gemm2<VR_EPI_ROPE, false, false>(A, lda, B, ldb, g, s);
-        case VR_EPI_SWIGLU:
-            VR_REQUIRE(g.N % 64 == 0, "vr_gemm: SWIGLU needs N multiple of 64");
-            return launch_gemm2<VR_EPI_SWIGLU, false, false>(A, lda, B, ldb, g, s);
-        default:
-            set_error("vr_gemm: unknown epilogue mode %d", e.mode);
-            return 2;
-    }
-}
-
-// feature-major accumulator kernels (block_n == 3): LINEAR epilogues only
+// feature-major accumulator kernel (block_n == 3): LINEAR epilogues only
 static int dispatch_swapped(const void* A, int64_t lda, const void* B, int64_t ldb, const GemmArgs& g, cudaStream_t s) {
     const vr_gemm_epilogue& e = g.epi;
     VR_REQUIRE(e.mode == VR_EPI_LINEAR, "vr_gemm: block_n=3 (feature-major accumulator) supports LINEAR epilogues only");
     if (e.out_dtype == VR_F32) {
         VR_REQUIRE(!e.act_gelu, "vr_gemm: GELU epilogue writes bf16 only");
-        return launch_gemm<256, VR_EPI_LINEAR, true, false, 1, true>(A, lda, B, ldb, g, s);
+        return launch_gemm<128, VR_EPI_LINEAR, true, false, true>(A, lda, B, ldb, g, s);
     }
     VR_REQUIRE(e.out_dtype == VR_BF16, "vr_gemm: out_dtype must be VR_BF16 or VR_F32");
-    if (e.act_gelu) return launch_gemm<256, VR_EPI_LINEAR, false, true, 1, true>(A, lda, B, ldb, g, s);
-    return launch_gemm<256, VR_EPI_LINEAR, false, false, 1, true>(A, lda, B, ldb, g, s);
+    if (e.act_gelu) return launch_gemm<128, VR_EPI_LINEAR, false, true, true>(A, lda, B, ldb, g, s);
+    return launch_gemm<128, VR_EPI_LINEAR, false, false, true>(A, lda, B, ldb, g, s);
 }
 
 template <int BN>
@@ -128,18 +43,18 @@ static int dispatch_mode(const void* A, int64_t lda, const void* B, int64_t ldb,
         case VR_EPI_LINEAR:
             if (e.out_dtype == VR_F32) {
                 VR_REQUIRE(!e.act_gelu, "vr_gemm: GELU epilogue writes bf16 only");
-                return launch_gemm<BN, VR_EPI_LINEAR, true, false, 1>(A, lda, B, ldb, g, s);
+                return launch_gemm<BN, VR_EPI_LINEAR, true, false>(A, lda, B, ldb, g, s);
             }
             VR_REQUIRE(e.out_dtype == VR_BF16, "vr_gemm: out_dtype must be VR_BF16 or VR_F32");
-            if (e.act_gelu) return launch_gemm<BN, VR_EPI_LINEAR, false, true, 1>(A, lda, B, ldb, g, s);
-            return launch_gemm<BN, VR_EPI_LINEAR, false, false, 1>(A, lda, B, ldb, g, s);
+            if (e.act_gelu) return launch_gemm<BN, VR_EPI_LINEAR, false, true>(A, lda, B, ldb, g, s);
+            return launch_gemm<BN, VR_EPI_LINEAR, false, false>(A, lda, B, ldb, g, s);
         case VR_EPI_ROPE:
             VR_REQUIRE(e.positions && e.rope_cos && e.rope_sin, "vr_gemm: ROPE epilogue needs positions/cos/sin");
             VR_REQUIRE(g.N % 64 == 0 && e.rope_cols % 64 == 0, "vr_gemm: ROPE needs N and rope_cols multiples of 64");
-            return launch_gemm<BN, VR_EPI_ROPE, false, false, 1>(A, lda, B, ldb, g, s);
+            return launch_gemm<BN, VR_EPI_ROPE, false, false>(A, lda, B, ldb, g, s);
         case VR_EPI_SWIGLU:
             VR_REQUIRE(g.N % 64 == 0, "vr_gemm: SWIGLU needs N multiple of 64");
-            return launch_gemm<BN, VR_EPI_SWIGLU, false, false, 1>(A, lda, B, ldb, g, s);
+            return launch_gemm<BN, VR_EPI_SWIGLU, false, false>(A, lda, B, ldb, g, s);
         default:
             set_error("vr_gemm: unknown epilogue mode %d", e.mode);
             return 2;
@@ -161,40 +76,21 @@ extern "C" int vr_gemm_tuned(const void* A, int64_t lda, const void* B, int64_t 
                (long long)epi->ldo);
     GemmArgs g;
     g.M = M; g.N = N; g.K = K; g.epi = *epi;
-    // Residual L2 prefetch: worth it when the main loop of a tile is short (the epilogue's own loads then sit on the
-    // critical path); with a long K the lines are evicted again before the epilogue reads them (ncu: fc2, K = 4304,
-    // read 2.53 GB from DRAM instead of 1.73 GB) and the epilogue has time to spare anyway.
-    static int maxk = -1;
-    if (maxk < 0) {
-        const char* e = getenv("VR_GEMM_PREFETCH_MAXK");
-        maxk = e ? atoi(e) : 2304;
-    }
-    g.prefetch_resid = epi->resid != nullptr && epi->out_dtype == VR_F32 && (epi->ldo & 3) == 0 &&
-                       (reinterpret_cast<uintptr_t>(epi->resid) & 15) == 0 && K <= maxk;
     cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
     int bn = block_n;
     if (bn == 0) {
-        // CTA-pair kernel (tcgen05 cta_group::2) wherever a pair has a full 256-row tile to work on: each SM stages only
-        // half of B, which lifts the shared-memory/L2 feed limit of the single-CTA kernel (measured, in isolation: qkv
-        // 1585 vs 1334 TFLOP/s, fc2+resid 1290 vs 1094, LM down 1197 vs 1048). Small problems keep 128-row tiles.
         // M <= 128 (a few queries): one row tile, the kernel only streams the weight - 64-wide feature tiles spread that
-        // stream over 4x as many SMs as 256-wide ones (o_proj 2304x2304: 36 CTAs instead of 9)
-        bn = (M > 128 && N >= 256) ? 2 : (M <= 128 ? 64 : (N >= 256 ? 256 : 128));
-    }
-    if (bn == 2 || bn == 4) {
-        const bool force192 = bn == 4;
-        static int narrow_ok = -1;  // VR_GEMM_NARROW=0 keeps 256-wide tiles everywhere (A/B switch for measurements)
-        if (narrow_ok < 0) {
-            const char* e2 = getenv("VR_GEMM_NARROW");
-            narrow_ok = e2 ? atoi(e2) : 1;
-        }
-        return dispatch_mode2(A, lda, B, ldb, g, s, force192, narrow_ok != 0);
+        // stream over 4x as many SMs as 256-wide ones (o_proj 2304x2304: 36 CTAs instead of 9). Otherwise the widest tile
+        // (most reuse of the A rows per byte staged), except where 192 tiles N exactly and 256 does not (N = 1152:
+        // 6 x 192 instead of 4.5 x 256).
+        bn = M <= 128 ? 64 : (N < 256 ? 128 : ((N % 192 == 0 && N % 256 != 0) ? 192 : 256));
     }
     if (bn == 3) return dispatch_swapped(A, lda, B, ldb, g, s);
     if (bn == 256) return dispatch_mode<256>(A, lda, B, ldb, g, s);
+    if (bn == 192) return dispatch_mode<192>(A, lda, B, ldb, g, s);
     if (bn == 128) return dispatch_mode<128>(A, lda, B, ldb, g, s);
     if (bn == 64) return dispatch_mode<64>(A, lda, B, ldb, g, s);
-    set_error("vr_gemm: block_n must be 0 (auto), 64, 128, 256, 2 (CTA-pair kernel), 4 (CTA pair, 192-wide tiles) or 3 (feature-major accumulator)");
+    set_error("vr_gemm: block_n must be 0 (auto), 64, 128, 192, 256 or 3 (feature-major accumulator)");
     return 2;
 }
 

@@ -1,15 +1,15 @@
-// Persistent warp-specialised tcgen05 GEMM:  C[M,N] = A[M,K] * B[N,K]^T  (both K-major).
+// Persistent warp-specialised wgmma GEMM:  C[M,N] = A[M,K] * B[N,K]^T  (both K-major).
 //
-//   warp 0 (one lane)  TMA producer : A/B 128B-swizzled tiles -> 4-stage smem ring
-//   warp 1 (one lane)  MMA issuer   : tcgen05.mma 128 x BN x 16, fp32 accumulators in TMEM,
-//                                     two accumulator stages (2 x BN columns) so the epilogue
-//                                     of tile i overlaps the main loop of tile i+1
-//   warp 2             TMEM allocator
-//   warps 4..11        epilogue     : tcgen05.ld (thread = one output row, 32 columns per
-//                                     chunk) -> fused bias / GELU / residual / RoPE / SwiGLU
-//                                     -> 16-byte global stores
+//   warpgroup 0 (one lane)  TMA producer : A/B 128B-swizzled tiles -> multi-stage smem ring; the ring runs ahead
+//                                          into the next tile while the consumers are in their epilogue
+//   warpgroups 1, 2         consumers    : each owns 64 of the tile's 128 rows: wgmma m64 x BN x k16 from shared
+//                                          memory, fp32 accumulators in registers (BN/2 per thread), then the fused
+//                                          epilogue (bias / GELU / residual / RoPE / SwiGLU) straight from the
+//                                          accumulator fragments: a thread holds pairs of adjacent columns, so
+//                                          global accesses are 8-byte (fp32) or 4-byte (bf16) and a quad of lanes
+//                                          covers one 32-byte sector of a row.
 //
-// Three mbarrier pipelines: smem full/empty (TMA <-> MMA), TMEM full/empty (MMA <-> epilogue).
+// Two mbarrier arrays: smem full (TMA -> consumers, transaction bytes) and empty (8 consumer warps -> TMA).
 // Tiles are scheduled round-robin over a grid of min(#tiles, #SMs) CTAs, n-block fastest so
 // that CTAs running together share the same A rows in L2.
 #pragma once
@@ -20,23 +20,20 @@ namespace vr {
 
 constexpr int GEMM_BM = 128;
 constexpr int GEMM_BK = 64;  // 64 bf16 = 128 B = one swizzle-128B row
-constexpr int GEMM_EPI_WARPS = 8;
-constexpr int GEMM_THREADS = (4 + GEMM_EPI_WARPS) * 32;
+constexpr int GEMM_THREADS = 3 * 128;  // producer warpgroup + two consumer warpgroups
 
 template <int BN>
 struct GemmCfg {
-    static constexpr int STAGES = (BN == 256) ? 4 : (BN == 64 ? 7 : 6);
+    static_assert(BN % 64 == 0 && BN <= 256, "tile width: 64, 128, 192 or 256");
     static constexpr int A_BYTES = GEMM_BM * GEMM_BK * 2;
     static constexpr int B_BYTES = BN * GEMM_BK * 2;
     static constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
-    static constexpr int EPI_STAGE_BYTES = 4096;  // per epilogue warp: 32 rows x 128 B transpose buffer
-    static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + GEMM_EPI_WARPS * EPI_STAGE_BYTES + 1024 /*align slack*/ + 256 /*barriers*/;
-    static constexpr int TMEM_COLS = 2 * BN;  // 128, 256 or 512: power of two >= 32
+    static constexpr int STAGES = (192 * 1024) / STAGE_BYTES;  // 4 / 4 / 6 / 8 stages in 192 KB of the SM's 227 KB
+    static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + 1024 /*align slack*/ + 256 /*barriers*/;
 };
 
 struct GemmArgs {
     int M, N, K;
-    int prefetch_resid;  // 1: warp 3 pulls the fp32 residual tile into L2 ahead of the epilogue (set by the launcher)
     vr_gemm_epilogue epi;
 };
 
@@ -57,14 +54,10 @@ __device__ __forceinline__ float erf_as(float x) {
 }
 __device__ __forceinline__ float gelu_erf(float x) { return 0.5f * x * (1.0f + erf_as(x * 0.70710678118654752f)); }
 
-// two GELUs at once on the packed fp32x2 pipe (FFMA2): the fc1 epilogue is issue bound, this halves its FMA count
+// two independent GELUs side by side (instruction-level parallelism for the Horner chains)
 __device__ __forceinline__ void pk_fma(float& d0, float& d1, float a0, float a1, float b0, float b1, float c0, float c1) {
-    unsigned long long A, B, Cc, D;
-    asm("mov.b64 %0, {%1, %2};" : "=l"(A) : "f"(a0), "f"(a1));
-    asm("mov.b64 %0, {%1, %2};" : "=l"(B) : "f"(b0), "f"(b1));
-    asm("mov.b64 %0, {%1, %2};" : "=l"(Cc) : "f"(c0), "f"(c1));
-    asm("fma.rn.f32x2 %0, %1, %2, %3;" : "=l"(D) : "l"(A), "l"(B), "l"(Cc));
-    asm("mov.b64 {%0, %1}, %2;" : "=f"(d0), "=f"(d1) : "l"(D));
+    d0 = fmaf(a0, b0, c0);
+    d1 = fmaf(a1, b1, c1);
 }
 #ifndef VR_GELU_POLY
 #define VR_GELU_POLY 1
@@ -74,8 +67,7 @@ __device__ __forceinline__ void pk_fma(float& d0, float& d1, float a0, float a1,
 // near-minimax polynomial (Chebyshev fit of erf(z)/z, evaluated by Horner in the mapped variable so the coefficients stay
 // O(1) and nothing cancels). |erf error| <= 3.2e-6 in fp32 incl. the clamp (1 - erf(3.2) = 6e-6), |GELU error| <= 1.2e-5
 // absolute - two orders below the bf16 rounding of the result. The Abramowitz-Stegun form below needs two MUFU ops per
-// element (rcp + ex2): 65536 per 128x256 tile = 4096 SFU cycles, the largest serial piece of the fc1 epilogue, which
-// was longer than the K = 1152 main loop. This form is 10.5 FMA-pipe instructions per element (packed FFMA2) and no MUFU.
+// element (rcp + ex2): 65536 per 128x256 tile = 4096 SFU cycles on the critical path of the fc1 epilogue. This form is 14 FMA-pipe instructions per element and no MUFU.
 __device__ __forceinline__ void gelu_erf2(float& x0, float& x1) {
     constexpr float R2 = 0.70710678118654752f, ZMAX = 3.2f, A = 2.0f / (ZMAX * ZMAX);
     const float z0 = fminf(fmaxf(x0 * R2, -ZMAX), ZMAX), z1 = fminf(fmaxf(x1 * R2, -ZMAX), ZMAX);
@@ -129,305 +121,86 @@ __device__ __forceinline__ float silu(float x) {
 }
 
 // ---------------------------------------------------------------------------------------
-// Epilogue. tcgen05.ld hands every thread ONE output row (32 consecutive columns per chunk), which is the wrong shape
-// for global memory: a warp-wide 16-byte access would touch 32 different rows. Each epilogue warp therefore owns a 4 KB
-// shared-memory transpose buffer: values go thread-row -> smem -> row-contiguous 16-byte global accesses (8 lanes cover
-// one 128-byte row segment), and the fp32 residual comes in the opposite way. The buffer is XOR-swizzled in 16-byte
-// units so both directions are bank-conflict free.
-//   "wide" tile : 32 rows x 128 B (32 fp32, or 64 bf16)   unit u of row r lives at r*128 + ((u ^ (r&7)) << 4)
-//   "half" tile : 32 rows x  64 B (32 bf16)               unit u of row r lives at r*64  + ((u ^ ((r>>1)&3)) << 4)
+// Epilogue, per accumulator fragment pair (two adjacent columns of one row).
 // ---------------------------------------------------------------------------------------
-__device__ __forceinline__ uint32_t wide_off(int r, int u) { return r * 128 + ((u ^ (r & 7)) << 4); }
-__device__ __forceinline__ uint32_t half_off(int r, int u) { return r * 64 + ((u ^ ((r >> 1) & 3)) << 4); }
-
-// this thread's row (lane) -> smem, 8 x 16 B
-__device__ __forceinline__ void stage_put_wide(uint8_t* st, int lane, const uint32_t (&w)[32]) {
-#pragma unroll
-    for (int u = 0; u < 8; ++u)
-        *reinterpret_cast<uint4*>(st + wide_off(lane, u)) = make_uint4(w[u * 4], w[u * 4 + 1], w[u * 4 + 2], w[u * 4 + 3]);
-}
-__device__ __forceinline__ void stage_get_wide(const uint8_t* st, int lane, uint32_t (&w)[32]) {
-#pragma unroll
-    for (int u = 0; u < 8; ++u) {
-        const uint4 q = *reinterpret_cast<const uint4*>(st + wide_off(lane, u));
-        w[u * 4] = q.x; w[u * 4 + 1] = q.y; w[u * 4 + 2] = q.z; w[u * 4 + 3] = q.w;
-    }
-}
-// smem <-> global, row-contiguous: lane handles 16 B of row (i*4 + lane/8); `elems16` = elements per 16 bytes
-template <typename T>
-__device__ __forceinline__ void stage_store_wide(const uint8_t* st, int lane, T* gbase, long long ld, int row0, int rows_valid,
-                                                 int col0, int cols_valid) {
-    constexpr int E = 16 / sizeof(T);
-    const int u = lane & 7;
-    uint4 q[8];
-#pragma unroll
-    for (int i = 0; i < 8; ++i) q[i] = *reinterpret_cast<const uint4*>(st + wide_off(i * 4 + (lane >> 3), u));
-#pragma unroll
-    for (int i = 0; i < 8; ++i) {
-        const int r = i * 4 + (lane >> 3);
-        if (r < rows_valid && u * E < cols_valid)
-            *reinterpret_cast<uint4*>(gbase + static_cast<long long>(row0 + r) * ld + col0 + u * E) = q[i];
-    }
-}
-__device__ __forceinline__ void stage_load_wide_f32(uint8_t* st, int lane, const float* gbase, long long ld, int row0,
-                                                    int rows_valid, int col0, int cols_valid) {
-    const int u = lane & 7;
-    // all 8 global loads are issued before the first shared-memory store: the pointers may alias as far as the compiler
-    // knows, so interleaving load/store would serialise 8 full memory round trips per chunk
-    uint4 q[8];
-#pragma unroll
-    for (int i = 0; i < 8; ++i) {
-        const int r = i * 4 + (lane >> 3);
-        q[i] = make_uint4(0, 0, 0, 0);
-        if (r < rows_valid && u * 4 < cols_valid)
-            q[i] = *reinterpret_cast<const uint4*>(gbase + static_cast<long long>(row0 + r) * ld + col0 + u * 4);
-    }
-#pragma unroll
-    for (int i = 0; i < 8; ++i) {
-        const int r = i * 4 + (lane >> 3);
-        *reinterpret_cast<uint4*>(st + wide_off(r, u)) = q[i];
-    }
-}
-// The two halves of stage_load_wide_f32 as separate steps: the pair kernel issues a chunk's residual loads one chunk (for
-// the first chunk: one tile) ahead, so their latency is off the epilogue's critical path (epi_linear<.., PRE = true>).
-__device__ __forceinline__ void resid_issue(uint4 (&q)[8], int lane, const float* gbase, long long ld, int row0, int rows_valid,
-                                            int col0, int cols_valid) {
-    const int u = lane & 7;
-#pragma unroll
-    for (int i = 0; i < 8; ++i) {
-        const int r = i * 4 + (lane >> 3);
-        q[i] = make_uint4(0, 0, 0, 0);
-        if (r < rows_valid && u * 4 < cols_valid)
-            q[i] = *reinterpret_cast<const uint4*>(gbase + static_cast<long long>(row0 + r) * ld + col0 + u * 4);
-    }
-}
-__device__ __forceinline__ void resid_to_stage(uint8_t* st, int lane, const uint4 (&q)[8]) {
-    const int u = lane & 7;
-#pragma unroll
-    for (int i = 0; i < 8; ++i) *reinterpret_cast<uint4*>(st + wide_off(i * 4 + (lane >> 3), u)) = q[i];
-}
-__device__ __forceinline__ void stage_put_half(uint8_t* st, int lane, const uint32_t (&w)[16]) {
-#pragma unroll
-    for (int u = 0; u < 4; ++u)
-        *reinterpret_cast<uint4*>(st + half_off(lane, u)) = make_uint4(w[u * 4], w[u * 4 + 1], w[u * 4 + 2], w[u * 4 + 3]);
-}
-__device__ __forceinline__ void stage_store_half(const uint8_t* st, int lane, __nv_bfloat16* gbase, long long ld, int row0,
-                                                 int rows_valid, int col0, int cols_valid) {
-    const int u = lane & 3;
-    uint4 q[4];
-#pragma unroll
-    for (int i = 0; i < 4; ++i) q[i] = *reinterpret_cast<const uint4*>(st + half_off(i * 8 + (lane >> 2), u));
-#pragma unroll
-    for (int i = 0; i < 4; ++i) {
-        const int r = i * 8 + (lane >> 2);
-        if (r < rows_valid && u * 8 < cols_valid)
-            *reinterpret_cast<uint4*>(gbase + static_cast<long long>(row0 + r) * ld + col0 + u * 8) = q[i];
-    }
-}
-
-// LINEAR: out = [resid +] scale * gelu?(acc + bias) [+ rowadd[row % period]]   (one 32-column chunk of one warp)
-// The bias of the warp's COLS_PER_WARP (<= 128) columns is fetched ONCE per tile, before the wait for the accumulator
-// (epi_bias_prefetch: lane l holds columns 4l..4l+3 of the warp's span, zeros past N), and handed to the chunks by warp
-// shuffles. Loading it per chunk (8 x LDG.128 per thread) put an L1/L2 round trip on the critical path of every chunk:
-// 17 % of the fc1 kernel's stall samples sat on the bias FADDs.
-__device__ __forceinline__ float4 epi_bias_prefetch(const GemmArgs& g, int lane, int col_first, int cols_per_warp) {
-    float4 b = make_float4(0.f, 0.f, 0.f, 0.f);
-    const int c = col_first + lane * 4;
-    if (g.epi.bias && lane * 4 < cols_per_warp && c < g.N) b = *reinterpret_cast<const float4*>(g.epi.bias + c);  // N % 8 == 0
-    return b;
-}
-
-// PRE: the residual of this chunk was loaded into `q` beforehand (resid_issue); after it has been consumed, the loads of the
-// chunk at `next_col0` (< 0: none) are issued into the same registers, ahead of this chunk's output stores.
-template <bool OUT_F32, bool GELU, bool PRE = false>
-__device__ __forceinline__ void epi_linear(const GemmArgs& g, uint8_t* st, int lane, int row0, int col0, float (&x)[32],
-                                           const float4& bias4, int chunk, uint4 (*q)[8] = nullptr, int next_col0 = -1) {
-    const vr_gemm_epilogue& e = g.epi;
-    const int rows_valid = g.M - row0;          // may exceed 32
-    const int cols_valid = g.N - col0;          // may exceed 32; N % 8 == 0
-    if (e.bias) {  // shuffles are warp collective: before the (warp-uniform) early exit anyway
-#pragma unroll
-        for (int j4 = 0; j4 < 8; ++j4) {
-            const int src = chunk * 8 + j4;
-            x[j4 * 4] += __shfl_sync(0xffffffffu, bias4.x, src);
-            x[j4 * 4 + 1] += __shfl_sync(0xffffffffu, bias4.y, src);
-            x[j4 * 4 + 2] += __shfl_sync(0xffffffffu, bias4.z, src);
-            x[j4 * 4 + 3] += __shfl_sync(0xffffffffu, bias4.w, src);
-        }
-    }
-    if (rows_valid <= 0 || cols_valid <= 0) return;  // warp-uniform
-    if (GELU) {
-#pragma unroll
-        for (int j = 0; j < 32; j += 2) gelu_erf2(x[j], x[j + 1]);
-    }
-    if (e.scale != 1.0f) {
-#pragma unroll
-        for (int j = 0; j < 32; ++j) x[j] *= e.scale;
-    }
-    if (e.rowadd && lane < rows_valid) {
-        const float* p = e.rowadd + static_cast<long long>((row0 + lane) % e.rowadd_period) * g.N + col0;
-#pragma unroll
-        for (int j4 = 0; j4 < 8; ++j4) {
-            if (j4 * 4 < cols_valid) {
-                const float4 a4 = *reinterpret_cast<const float4*>(p + j4 * 4);
-                x[j4 * 4] += a4.x; x[j4 * 4 + 1] += a4.y; x[j4 * 4 + 2] += a4.z; x[j4 * 4 + 3] += a4.w;
-            }
-        }
-    }
-    if (e.resid) {
-        if (PRE) resid_to_stage(st, lane, *q);
-        else stage_load_wide_f32(st, lane, e.resid, e.ldo, row0, rows_valid, col0, cols_valid);
-        __syncwarp();
-        uint32_t w[32];
-        stage_get_wide(st, lane, w);
-#pragma unroll
-        for (int j = 0; j < 32; ++j) x[j] += __uint_as_float(w[j]);
-        __syncwarp();
-        if (PRE && next_col0 >= 0) resid_issue(*q, lane, e.resid, e.ldo, row0, rows_valid, next_col0, g.N - next_col0);
-    }
-    if (OUT_F32) {
-        uint32_t w[32];
-#pragma unroll
-        for (int j = 0; j < 32; ++j) w[j] = __float_as_uint(x[j]);
-        stage_put_wide(st, lane, w);
-        __syncwarp();
-        stage_store_wide<float>(st, lane, reinterpret_cast<float*>(e.out), e.ldo, row0, rows_valid, col0, cols_valid);
-    } else {
-        uint32_t w[16];
-#pragma unroll
-        for (int j = 0; j < 16; ++j) w[j] = pack_bf16x2(x[2 * j], x[2 * j + 1]);
-        stage_put_half(st, lane, w);
-        __syncwarp();
-        stage_store_half(st, lane, reinterpret_cast<__nv_bfloat16*>(e.out), e.ldo, row0, rows_valid, col0, cols_valid);
-    }
-    __syncwarp();
-}
-
-// LINEAR, feature-major accumulator (SWAP kernels: the WEIGHT tile is the MMA's M operand, 256 tokens are its N).
-// tcgen05.ld then hands every thread one output FEATURE and 32 consecutive tokens, which is already the shape global
-// memory wants: for a fixed token the 32 lanes hold 32 consecutive features = one 128-byte (fp32) row segment. No
-// shared-memory transpose, bias is a per-thread scalar, the residual comes in with the same coalesced pattern.
+// LINEAR: out = [resid +] scale * gelu?(acc + bias) [+ rowadd[row % period]]; columns col, col + 1 (col even, N % 8 == 0)
 template <bool OUT_F32, bool GELU>
-__device__ __forceinline__ void epi_linear_t(const GemmArgs& g, int lane, int f0, int tok0, float (&x)[32]) {
+__device__ __forceinline__ void epi_linear2(const GemmArgs& g, int row, int col, float x0, float x1) {
     const vr_gemm_epilogue& e = g.epi;
-    const int toks = g.M - tok0;                 // may exceed 32
-    if (toks <= 0 || f0 >= g.N) return;          // warp-uniform
-    const int f = f0 + lane;
-    const bool fv = f < g.N;
-    float r[32];
-    if (e.resid) {
-        // all residual loads first (independent, one 128-byte segment per warp instruction)
-        const float* rp = e.resid + static_cast<long long>(tok0) * e.ldo + f;
-#pragma unroll
-        for (int j = 0; j < 32; ++j) r[j] = (fv && j < toks) ? rp[static_cast<long long>(j) * e.ldo] : 0.0f;
-    }
+    if (row >= g.M || col >= g.N) return;
     if (e.bias) {
-        const float b = fv ? e.bias[f] : 0.0f;
-#pragma unroll
-        for (int j = 0; j < 32; ++j) x[j] += b;
+        const float2 b = *reinterpret_cast<const float2*>(e.bias + col);
+        x0 += b.x; x1 += b.y;
     }
-    if (GELU) {
-#pragma unroll
-        for (int j = 0; j < 32; j += 2) gelu_erf2(x[j], x[j + 1]);
-    }
-    if (e.scale != 1.0f) {
-#pragma unroll
-        for (int j = 0; j < 32; ++j) x[j] *= e.scale;
-    }
+    if (GELU) gelu_erf2(x0, x1);
+    if (e.scale != 1.0f) { x0 *= e.scale; x1 *= e.scale; }
     if (e.rowadd) {
-        int pr = tok0 % e.rowadd_period;
-#pragma unroll
-        for (int j = 0; j < 32; ++j) {
-            if (fv && j < toks) x[j] += e.rowadd[static_cast<long long>(pr) * g.N + f];
-            if (++pr == e.rowadd_period) pr = 0;
-        }
+        const float2 a2 = *reinterpret_cast<const float2*>(e.rowadd + static_cast<long long>(row % e.rowadd_period) * g.N + col);
+        x0 += a2.x; x1 += a2.y;
     }
+    const long long o = static_cast<long long>(row) * e.ldo + col;
     if (e.resid) {
-#pragma unroll
-        for (int j = 0; j < 32; ++j) x[j] += r[j];
+        const float2 r2 = *reinterpret_cast<const float2*>(e.resid + o);
+        x0 += r2.x; x1 += r2.y;
     }
-    if (OUT_F32) {
-        float* op = reinterpret_cast<float*>(e.out) + static_cast<long long>(tok0) * e.ldo + f;
-#pragma unroll
-        for (int j = 0; j < 32; ++j)
-            if (fv && j < toks) op[static_cast<long long>(j) * e.ldo] = x[j];
-    } else {
-        // lanes 2i / 2i+1 hold features f, f+1: the even lane takes token j, the odd lane token j+1, each storing one
-        // packed bf16x2 (features f..f+1) -> two 64-byte row segments per warp store
-        const bool odd = lane & 1;
-        uint32_t* ob = reinterpret_cast<uint32_t*>(reinterpret_cast<__nv_bfloat16*>(e.out) + (f & ~1));
-        const bool pv = fv;                      // N is even: both features of the pair are valid or neither
-#pragma unroll
-        for (int j = 0; j < 32; j += 2) {
-            const float send = odd ? x[j] : x[j + 1];
-            const float recv = __shfl_xor_sync(0xffffffffu, send, 1);
-            const uint32_t w = odd ? pack_bf16x2(recv, x[j + 1]) : pack_bf16x2(x[j], recv);
-            const int jj = j + (odd ? 1 : 0);
-            if (pv && jj < toks) ob[(static_cast<long long>(tok0 + jj) * e.ldo) >> 1] = w;
-        }
+    if (OUT_F32) *reinterpret_cast<float2*>(reinterpret_cast<float*>(e.out) + o) = make_float2(x0, x1);
+    else *reinterpret_cast<uint32_t*>(reinterpret_cast<__nv_bfloat16*>(e.out) + o) = pack_bf16x2(x0, x1);
+}
+
+// LINEAR, feature-major accumulator (SWAP kernels: the WEIGHT tile is the MMA's M operand, tokens are its N): one element
+template <bool OUT_F32, bool GELU>
+__device__ __forceinline__ void epi_linear_t(const GemmArgs& g, int tok, int f, float x) {
+    const vr_gemm_epilogue& e = g.epi;
+    if (tok >= g.M || f >= g.N) return;
+    if (e.bias) x += e.bias[f];
+    if (GELU) {
+        float y = x;
+        gelu_erf2(x, y);
     }
+    if (e.scale != 1.0f) x *= e.scale;
+    if (e.rowadd) x += e.rowadd[static_cast<long long>(tok % e.rowadd_period) * g.N + f];
+    const long long o = static_cast<long long>(tok) * e.ldo + f;
+    if (e.resid) x += e.resid[o];
+    if (OUT_F32) reinterpret_cast<float*>(e.out)[o] = x;
+    else reinterpret_cast<__nv_bfloat16*>(e.out)[o] = __float2bfloat16_rn(x);
 }
 
 // RoPE (modeling_minicpm.py:259-290): a head is 64 columns [lo(32) | hi(32)];
-//   lo' = lo*cos - hi*sin ; hi' = hi*cos + lo*sin   with cos/sin[pos, 0..31].  Writes 64 bf16 columns.
-__device__ __forceinline__ void epi_rope(const GemmArgs& g, uint8_t* st, int lane, int row0, int col0, float (&lo)[32],
-                                         float (&hi)[32]) {
+//   lo' = lo*cos - hi*sin ; hi' = hi*cos + lo*sin   with cos/sin[pos, 0..31].
+// (lo0, lo1) are columns head0 + c, head0 + c + 1 and (hi0, hi1) the columns 32 further, c even in [0, 32).
+__device__ __forceinline__ void epi_rope2(const GemmArgs& g, int row, int head0, int c, float lo0, float lo1, float hi0,
+                                          float hi1) {
     const vr_gemm_epilogue& e = g.epi;
-    const int rows_valid = g.M - row0;
-    if (rows_valid <= 0) return;
-    if (col0 < e.rope_cols && lane < rows_valid) {
-        const int pos = e.positions[row0 + lane];
-        const float* cs = e.rope_cos + static_cast<int64_t>(pos) * 32;
-        const float* sn = e.rope_sin + static_cast<int64_t>(pos) * 32;
-#pragma unroll
-        for (int j4 = 0; j4 < 8; ++j4) {
-            const float4 c4 = *reinterpret_cast<const float4*>(cs + j4 * 4);
-            const float4 s4 = *reinterpret_cast<const float4*>(sn + j4 * 4);
-            const float c[4] = {c4.x, c4.y, c4.z, c4.w};
-            const float s[4] = {s4.x, s4.y, s4.z, s4.w};
-#pragma unroll
-            for (int j = 0; j < 4; ++j) {
-                const float a = lo[j4 * 4 + j], b = hi[j4 * 4 + j];
-                lo[j4 * 4 + j] = a * c[j] - b * s[j];
-                hi[j4 * 4 + j] = b * c[j] + a * s[j];
-            }
-        }
+    if (row >= g.M || head0 >= g.N) return;
+    if (head0 < e.rope_cols) {
+        const long long pos = e.positions[row];
+        const float2 cs = *reinterpret_cast<const float2*>(e.rope_cos + pos * 32 + c);
+        const float2 sn = *reinterpret_cast<const float2*>(e.rope_sin + pos * 32 + c);
+        const float a0 = lo0, a1 = lo1, b0 = hi0, b1 = hi1;
+        lo0 = a0 * cs.x - b0 * sn.x; hi0 = b0 * cs.x + a0 * sn.x;
+        lo1 = a1 * cs.y - b1 * sn.y; hi1 = b1 * cs.y + a1 * sn.y;
     }
-    uint32_t w[32];
-#pragma unroll
-    for (int j = 0; j < 16; ++j) {
-        w[j] = pack_bf16x2(lo[2 * j], lo[2 * j + 1]);
-        w[16 + j] = pack_bf16x2(hi[2 * j], hi[2 * j + 1]);
-    }
-    stage_put_wide(st, lane, w);
-    __syncwarp();
-    stage_store_wide<__nv_bfloat16>(st, lane, reinterpret_cast<__nv_bfloat16*>(e.out), e.ldo, row0, rows_valid, col0, 64);
-    __syncwarp();
+    __nv_bfloat16* o = reinterpret_cast<__nv_bfloat16*>(e.out) + static_cast<long long>(row) * e.ldo + head0 + c;
+    *reinterpret_cast<uint32_t*>(o) = pack_bf16x2(lo0, lo1);
+    *reinterpret_cast<uint32_t*>(o + 32) = pack_bf16x2(hi0, hi1);
 }
 
-// SwiGLU (modeling_minicpm.py:333): accumulator columns [gate(32) | up(32)] -> 32 bf16 outputs at column col0/2.
-__device__ __forceinline__ void epi_swiglu(const GemmArgs& g, uint8_t* st, int lane, int row0, int col0, float (&gt)[32],
-                                           float (&up)[32]) {
+// SwiGLU (modeling_minicpm.py:333): accumulator columns [gate(32) | up(32)] -> 32 bf16 outputs at column blk0/2.
+__device__ __forceinline__ void epi_swiglu2(const GemmArgs& g, int row, int blk0, int c, float g0, float g1, float u0, float u1) {
     const vr_gemm_epilogue& e = g.epi;
-    const int rows_valid = g.M - row0;
-    if (rows_valid <= 0) return;
-    uint32_t w[16];
-#pragma unroll
-    for (int j = 0; j < 16; ++j) w[j] = pack_bf16x2(silu(gt[2 * j]) * up[2 * j], silu(gt[2 * j + 1]) * up[2 * j + 1]);
-    stage_put_half(st, lane, w);
-    __syncwarp();
-    stage_store_half(st, lane, reinterpret_cast<__nv_bfloat16*>(e.out), e.ldo, row0, rows_valid, col0 >> 1, 32);
-    __syncwarp();
+    if (row >= g.M || blk0 >= g.N) return;
+    __nv_bfloat16* o = reinterpret_cast<__nv_bfloat16*>(e.out) + static_cast<long long>(row) * e.ldo + (blk0 >> 1) + c;
+    *reinterpret_cast<uint32_t*>(o) = pack_bf16x2(silu(g0) * u0, silu(g1) * u1);
 }
 
 // ---------------------------------------------------------------------------------------
 // SWAP = true (LINEAR only): the host passes the WEIGHT map as tmap_a and the activation map as tmap_b; accumulator
 // rows are output features (128 per tile), accumulator columns are tokens (BN per tile). g keeps its meaning
-// (M tokens, N features). Feature blocks vary fastest so that co-running CTAs share one activation tile in L2.
-template <int BN, int MODE, bool OUT_F32, bool GELU, int AB_FMT /*0 f16, 1 bf16*/, bool SWAP = false>
+// (M tokens, N features). wgmma's M is fixed at 64 while its N goes down to 8, so this is the form for few tokens.
+// Feature blocks vary fastest so that co-running CTAs share one activation tile in L2.
+template <int BN, int MODE, bool OUT_F32, bool GELU, bool SWAP = false>
 __global__ void __launch_bounds__(GEMM_THREADS, 1)
-gemm_tcgen05_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b,
-                    const GemmArgs g) {
+gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b, const GemmArgs g) {
     using Cfg = GemmCfg<BN>;
     constexpr int STAGES = Cfg::STAGES;
 
@@ -435,16 +208,11 @@ gemm_tcgen05_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_con
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
     uint8_t* smem_a = smem;
     uint8_t* smem_b = smem + STAGES * Cfg::A_BYTES;
-    uint8_t* smem_stage = smem + STAGES * Cfg::STAGE_BYTES;
-    uint64_t* bars = reinterpret_cast<uint64_t*>(smem_stage + GEMM_EPI_WARPS * Cfg::EPI_STAGE_BYTES);
-    uint64_t* full_bar = bars;
-    uint64_t* empty_bar = bars + STAGES;
-    uint64_t* tfull_bar = bars + 2 * STAGES;
-    uint64_t* tempty_bar = bars + 2 * STAGES + 2;
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 2 * STAGES + 4);
-    volatile uint32_t* progress = tmem_slot + 1;  // tiles whose main loop has started (written by the MMA warp)
+    uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + STAGES * Cfg::STAGE_BYTES);
+    uint64_t* empty_bar = full_bar + STAGES;
 
-    const int warp = threadIdx.x >> 5;
+    const int wg = threadIdx.x >> 7;
+    const int warp = (threadIdx.x >> 5) & 3;  // inside the warpgroup
     const int lane = threadIdx.x & 31;
 
     static_assert(!SWAP || MODE == VR_EPI_LINEAR, "feature-major accumulators are implemented for LINEAR epilogues");
@@ -456,31 +224,21 @@ gemm_tcgen05_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_con
     auto tile_m0 = [&](int t) { return (SWAP ? t % tiles_m : t / tiles_n) * GEMM_BM; };
     auto tile_n0 = [&](int t) { return (SWAP ? t / tiles_m : t % tiles_n) * BN; };
 
-    if (warp == 0 && lane == 0) {
+    if (threadIdx.x == 0) {
         tma_prefetch_desc(&tmap_a);
         tma_prefetch_desc(&tmap_b);
-    }
-    if (warp == 1 && lane == 0) {
         for (int i = 0; i < STAGES; ++i) {
             mbar_init(&full_bar[i], 1);
-            mbar_init(&empty_bar[i], 1);
+            mbar_init(&empty_bar[i], 8);  // one arrival per consumer warp
         }
-        for (int i = 0; i < 2; ++i) {
-            mbar_init(&tfull_bar[i], 1);
-            mbar_init(&tempty_bar[i], GEMM_EPI_WARPS);
-        }
-        *progress = 0;
         fence_mbar_init();
     }
-    if (warp == 2) tmem_alloc<Cfg::TMEM_COLS>(tmem_slot);
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
 
-    if (warp == 0) {
+    if (wg == 0) {
         // ------------------------------------------------------------ TMA producer
-        if (lane == 0) {
+        setmaxnreg_dec<40>();
+        if (warp == 0 && lane == 0) {
             int stage = 0;
             uint32_t phase = 0;
             for (int t = blockIdx.x; t < num_tiles; t += gridDim.x) {
@@ -490,177 +248,85 @@ gemm_tcgen05_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_con
                     mbar_wait(&empty_bar[stage], phase ^ 1);
                     mbar_expect_tx(&full_bar[stage], Cfg::STAGE_BYTES);
                     tma_load_2d(&tmap_a, &full_bar[stage], smem_a + stage * Cfg::A_BYTES, kb * GEMM_BK, m0);
-                    if (BN == 256) {
-                        // a TMA box is at most 256 rows; keep boxes at 128 rows for both operands
-                        tma_load_2d(&tmap_b, &full_bar[stage], smem_b + stage * Cfg::B_BYTES, kb * GEMM_BK, n0);
-                        tma_load_2d(&tmap_b, &full_bar[stage], smem_b + stage * Cfg::B_BYTES + Cfg::B_BYTES / 2,
-                                    kb * GEMM_BK, n0 + 128);
-                    } else {
-                        tma_load_2d(&tmap_b, &full_bar[stage], smem_b + stage * Cfg::B_BYTES, kb * GEMM_BK, n0);
-                    }
+                    // B boxes are 64 rows (a box is at most 256 rows; 64 divides every tile width); rows past the
+                    // matrix read as zeros and still count their bytes
+#pragma unroll
+                    for (int h = 0; h < BN / 64; ++h)
+                        tma_load_2d(&tmap_b, &full_bar[stage], smem_b + stage * Cfg::B_BYTES + h * (64 * GEMM_BK * 2),
+                                    kb * GEMM_BK, n0 + h * 64);
                     if (++stage == STAGES) { stage = 0; phase ^= 1; }
                 }
             }
         }
-    } else if (warp == 1) {
-        // ------------------------------------------------------------ MMA issuer
-        // The WHOLE warp runs this loop with warp-uniform control flow (so stage / phase / descriptors live in uniform
-        // registers); one elected lane issues the tcgen05 instructions. A per-thread `if (lane == 0)` around the loop
-        // makes the compiler wrap every UTCHMMA in a uniformisation loop and the single issuing thread becomes the
-        // bottleneck (measured: 115 SASS instructions per k-block, tensor pipe 71 % busy).
-        constexpr uint32_t idesc = make_idesc_f16(GEMM_BM, BN, AB_FMT, 0, 0);
-        // descriptor = constant high word | (address >> 4); K-major SW128: LBO 16 B (unused), SBO 1024 B
+    } else {
+        // ------------------------------------------------------------ consumers: main loop + epilogue
+        setmaxnreg_inc<232>();
+        const int cw = wg - 1;  // rows [64 cw, 64 cw + 64) of the tile
+        // descriptor = constant high word | (address >> 4); K-major SW128: LBO unused, SBO 1024 B (8 rows)
         const uint64_t desc_hi = make_smem_desc(0, 16, 1024, kLayoutSW128);
-        const uint32_t a_lo0 = smem_u32(smem_a) >> 4, b_lo0 = smem_u32(smem_b) >> 4;
+        const uint32_t a_lo0 = (smem_u32(smem_a) + cw * (64 * GEMM_BK * 2)) >> 4, b_lo0 = smem_u32(smem_b) >> 4;
+        const int g8 = lane >> 2, q = lane & 3;
         int stage = 0;
         uint32_t phase = 0;
-        int it = 0;
-        for (int t = blockIdx.x; t < num_tiles; t += gridDim.x, ++it) {
-            const int acc = it & 1;
-            const uint32_t acc_phase = (it >> 1) & 1;
-            mbar_wait(&tempty_bar[acc], acc_phase ^ 1);
-            tc_fence_after();
-            if (lane == 0) *progress = static_cast<uint32_t>(it + 1);  // main loop of tile `it` starts (prefetcher pacing)
-            const uint32_t d_tmem = tmem_base + acc * BN;
+        for (int t = blockIdx.x; t < num_tiles; t += gridDim.x) {
+            float acc[BN / 2];
+            int prev = -1;
             for (int kb = 0; kb < num_kb; ++kb) {
                 mbar_wait(&full_bar[stage], phase);
-                tc_fence_after();
-                if (elect_one()) {
-                    const uint64_t ad = desc_hi | static_cast<uint64_t>(a_lo0 + stage * (Cfg::A_BYTES >> 4));
-                    const uint64_t bd = desc_hi | static_cast<uint64_t>(b_lo0 + stage * (Cfg::B_BYTES >> 4));
-                    // +32 B (= +2 in the >>4 address field) per 16-element K step inside the 128 B swizzle row
-                    umma_f16_ss(d_tmem, ad, bd, idesc, kb != 0 ? 1u : 0u);
-                    umma_f16_ss(d_tmem, ad + 2, bd + 2, idesc, 1u);
-                    umma_f16_ss(d_tmem, ad + 4, bd + 4, idesc, 1u);
-                    umma_f16_ss(d_tmem, ad + 6, bd + 6, idesc, 1u);
-                    umma_commit(&empty_bar[stage]);  // frees the smem slot when these MMAs retire
-                    if (kb == num_kb - 1) umma_commit(&tfull_bar[acc]);
+                const uint64_t ad = desc_hi | static_cast<uint64_t>(a_lo0 + stage * (Cfg::A_BYTES >> 4));
+                const uint64_t bd = desc_hi | static_cast<uint64_t>(b_lo0 + stage * (Cfg::B_BYTES >> 4));
+                wgmma_fence();
+                // +32 B (= +2 in the >>4 address field) per 16-element K step inside the 128 B swizzle row
+#pragma unroll
+                for (int kk = 0; kk < 4; ++kk)
+                    wgmma_ss<false, false>(acc, ad + 2 * kk, bd + 2 * kk, (kb | kk) != 0, std::integral_constant<int, BN>());
+                wgmma_commit();
+                if (prev >= 0) {
+                    wgmma_wait<1>();  // the MMAs of the previous k-block retired: hand its slot back
+                    if (lane == 0) mbar_arrive(&empty_bar[prev]);
                 }
-                __syncwarp();
+                prev = stage;
                 if (++stage == STAGES) { stage = 0; phase ^= 1; }
             }
-        }
-    } else if (warp == 3) {
-        // ------------------------------------------------------------ residual prefetcher
-        // The fp32 residual stream (604 MB per ViT layer at 128 pages) never survives in L2 between kernels, and the
-        // epilogue warps can only keep ~4 KB each in flight, so their residual reads were DRAM-latency bound. This warp
-        // pulls tile i's residual rows into L2 while tile i's main loop runs, one tile ahead of the epilogue. Pacing is
-        // a monotonic counter published by the MMA warp (not an mbarrier phase: a phase can be missed by a late
-        // waiter, a counter cannot), and a tile whose main loop is already over is skipped.
-        if (MODE == VR_EPI_LINEAR && OUT_F32 && g.prefetch_resid) {
-            int it = 0;
-            for (int t = blockIdx.x; t < num_tiles; t += gridDim.x, ++it) {
-                uint32_t started;
-                while ((started = *progress) < static_cast<uint32_t>(it + 1)) __nanosleep(256);
-                if (started > static_cast<uint32_t>(it + 1)) continue;  // too late to be useful
-                const int tok0 = SWAP ? tile_n0(t) : tile_m0(t);
-                const int f0 = SWAP ? tile_m0(t) : tile_n0(t);
-                constexpr int TOKS = SWAP ? BN : GEMM_BM, FEATS = SWAP ? GEMM_BM : BN;
-                const int cols = min(FEATS, g.N - f0) & ~3;  // bulk prefetch sizes are multiples of 16 bytes
-                if (cols == 0) continue;
-#pragma unroll
-                for (int r = lane; r < TOKS; r += 32) {
-                    if (tok0 + r < g.M)
-                        l2_prefetch_bulk(g.epi.resid + static_cast<int64_t>(tok0 + r) * g.epi.ldo + f0, cols * 4);
-                }
-            }
-        }
-    } else if (warp >= 4) {
-        // ------------------------------------------------------------ epilogue
-        const int ew = warp - 4;
-        const int quarter = warp & 3;          // TMEM lane quarter this warp may touch
-        const int half = ew >> 2;              // which half of the BN columns
-        constexpr int COLS_PER_WARP = BN / 2;  // 128, 64 or 32
-        int it = 0;
-        for (int t = blockIdx.x; t < num_tiles; t += gridDim.x, ++it) {
-            const int acc = it & 1;
-            const uint32_t acc_phase = (it >> 1) & 1;
-            const int m0 = tile_m0(t);
+            wgmma_wait<0>();
+            if (lane == 0) mbar_arrive(&empty_bar[prev]);
+            wgmma_touch(acc);
+
+            const int r0 = tile_m0(t) + cw * 64 + warp * 16 + g8;  // accumulator rows r0 and r0 + 8
             const int n0 = tile_n0(t);
-            const int row0 = m0 + quarter * 32;  // first of this warp's 32 rows
-            uint8_t* st = smem_stage + ew * Cfg::EPI_STAGE_BYTES;
-            float4 bias4 = make_float4(0.f, 0.f, 0.f, 0.f);
-            if (MODE == VR_EPI_LINEAR && !SWAP) bias4 = epi_bias_prefetch(g, lane, n0 + half * COLS_PER_WARP, COLS_PER_WARP);
-            mbar_wait(&tfull_bar[acc], acc_phase);
-            tc_fence_after();
-            const uint32_t taddr = tmem_base + (static_cast<uint32_t>(quarter * 32) << 16) + acc * BN + half * COLS_PER_WARP;
             if (MODE == VR_EPI_LINEAR) {
-#pragma unroll 1
-                for (int c = 0; c < COLS_PER_WARP / 32; ++c) {
-                    uint32_t r[32];
-                    tmem_ld_32x32(taddr + c * 32, r);
-                    tmem_ld_wait();
-                    if (c == COLS_PER_WARP / 32 - 1) {
-                        // all of this warp's TMEM reads for the tile are done: hand the stage back
-                        tc_fence_before();
-                        __syncwarp();
-                        if (lane == 0) mbar_arrive(&tempty_bar[acc]);
-                    }
-                    float v[32];
 #pragma unroll
-                    for (int j = 0; j < 32; ++j) v[j] = __uint_as_float(r[j]);
-                    if (SWAP) epi_linear_t<OUT_F32, GELU>(g, lane, row0, n0 + half * COLS_PER_WARP + c * 32, v);
-                    else epi_linear<OUT_F32, GELU>(g, st, lane, row0, n0 + half * COLS_PER_WARP + c * 32, v, bias4, c);
-                }
-            } else if (BN == 64) {
-                // one 64-column block (a RoPE head / a gate|up pair) per tile: the half-0 warps take it, the others only
-                // hand the accumulator stage back
-                if (half == 0) {
-                    uint32_t r0[32], r1[32];
-                    tmem_ld_32x32(taddr, r0);
-                    tmem_ld_32x32(taddr + 32, r1);
-                    tmem_ld_wait();
-                    tc_fence_before();
-                    __syncwarp();
-                    if (lane == 0) mbar_arrive(&tempty_bar[acc]);
-                    float a[32], b[32];
-#pragma unroll
-                    for (int j = 0; j < 32; ++j) {
-                        a[j] = __uint_as_float(r0[j]);
-                        b[j] = __uint_as_float(r1[j]);
+                for (int j = 0; j < BN / 8; ++j) {
+                    const int c = n0 + j * 8 + q * 2;
+                    if (SWAP) {
+                        epi_linear_t<OUT_F32, GELU>(g, c, r0, acc[4 * j]);
+                        epi_linear_t<OUT_F32, GELU>(g, c + 1, r0, acc[4 * j + 1]);
+                        epi_linear_t<OUT_F32, GELU>(g, c, r0 + 8, acc[4 * j + 2]);
+                        epi_linear_t<OUT_F32, GELU>(g, c + 1, r0 + 8, acc[4 * j + 3]);
+                    } else {
+                        epi_linear2<OUT_F32, GELU>(g, r0, c, acc[4 * j], acc[4 * j + 1]);
+                        epi_linear2<OUT_F32, GELU>(g, r0 + 8, c, acc[4 * j + 2], acc[4 * j + 3]);
                     }
-                    if (n0 < g.N) {
-                        if (MODE == VR_EPI_ROPE) epi_rope(g, st, lane, row0, n0, a, b);
-                        else epi_swiglu(g, st, lane, row0, n0, a, b);
-                    }
-                } else {
-                    tc_fence_before();
-                    __syncwarp();
-                    if (lane == 0) mbar_arrive(&tempty_bar[acc]);
                 }
             } else {
-#pragma unroll 1
-                for (int c = 0; c < COLS_PER_WARP / 64; ++c) {
-                    uint32_t r0[32], r1[32];
-                    tmem_ld_32x32(taddr + c * 64, r0);
-                    tmem_ld_32x32(taddr + c * 64 + 32, r1);
-                    tmem_ld_wait();
-                    if (c == COLS_PER_WARP / 64 - 1) {
-                        tc_fence_before();
-                        __syncwarp();
-                        if (lane == 0) mbar_arrive(&tempty_bar[acc]);
-                    }
-                    float a[32], b[32];
+                // 64-column blocks (a RoPE head / a gate|up pair): columns c and c + 32 sit in the same thread
 #pragma unroll
-                    for (int j = 0; j < 32; ++j) {
-                        a[j] = __uint_as_float(r0[j]);
-                        b[j] = __uint_as_float(r1[j]);
-                    }
-                    const int col0 = n0 + half * COLS_PER_WARP + c * 64;
-                    if (col0 < g.N) {
-                        if (MODE == VR_EPI_ROPE) epi_rope(g, st, lane, row0, col0, a, b);
-                        else epi_swiglu(g, st, lane, row0, col0, a, b);
+                for (int hb = 0; hb < BN / 64; ++hb) {
+#pragma unroll
+                    for (int j = 0; j < 4; ++j) {
+                        const int lo = 4 * (hb * 8 + j), hi = 4 * (hb * 8 + j + 4);
+                        const int blk0 = n0 + hb * 64, c = j * 8 + q * 2;
+                        if (MODE == VR_EPI_ROPE) {
+                            epi_rope2(g, r0, blk0, c, acc[lo], acc[lo + 1], acc[hi], acc[hi + 1]);
+                            epi_rope2(g, r0 + 8, blk0, c, acc[lo + 2], acc[lo + 3], acc[hi + 2], acc[hi + 3]);
+                        } else {
+                            epi_swiglu2(g, r0, blk0, c, acc[lo], acc[lo + 1], acc[hi], acc[hi + 1]);
+                            epi_swiglu2(g, r0 + 8, blk0, c, acc[lo + 2], acc[lo + 3], acc[hi + 2], acc[hi + 3]);
+                        }
                     }
                 }
             }
         }
-    }
-
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 2) {
-        tc_fence_after();
-        tmem_dealloc<Cfg::TMEM_COLS>(tmem_base);
     }
 }
 

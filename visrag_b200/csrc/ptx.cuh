@@ -1,5 +1,5 @@
-// Thin inline-PTX wrappers for the sm_100a features the kernels use:
-// mbarrier, TMA (cp.async.bulk.tensor), tcgen05 (alloc / mma / commit / ld), fences.
+// Thin inline-PTX wrappers for the sm_90a features the kernels use:
+// mbarrier, TMA (cp.async.bulk.tensor), wgmma (warpgroup MMA, fp32 accumulators in registers), fences, setmaxnreg.
 // No CUTLASS / CuTe: every instruction is spelled out here once.
 #pragma once
 #include <cuda.h>
@@ -7,6 +7,7 @@
 #include <cuda_bf16.h>
 #include <cuda_fp16.h>
 #include <stdint.h>
+#include <type_traits>
 
 namespace vr {
 
@@ -15,18 +16,6 @@ __device__ __forceinline__ uint32_t smem_u32(const void* p) {
 }
 
 __device__ __forceinline__ uint32_t lane_id() { return threadIdx.x & 31; }
-
-__device__ __forceinline__ bool elect_one() {
-    uint32_t pred = 0;
-    asm volatile(
-        "{\n\t"
-        ".reg .pred P;\n\t"
-        "elect.sync _|P, 0xffffffff;\n\t"
-        "selp.u32 %0, 1, 0, P;\n\t"
-        "}\n"
-        : "=r"(pred));
-    return pred != 0;
-}
 
 // ---------------------------------------------------------------- mbarrier
 __device__ __forceinline__ void mbar_init(uint64_t* bar, uint32_t count) {
@@ -55,7 +44,7 @@ __device__ __forceinline__ bool mbar_try_wait(uint32_t addr, uint32_t parity) {
         : "memory");
     return ok != 0;
 }
-// Spin on a phase parity. A pipeline bug must never hang the GPU box: after ~2 s of
+// Spin on a phase parity. A pipeline bug must never hang the GPU: after ~2 s of
 // spinning the kernel traps (the host then sees a launch failure instead of a hang).
 __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
     uint32_t addr = smem_u32(bar);
@@ -78,164 +67,8 @@ __device__ __forceinline__ uint32_t cluster_nctarank() {
     return r;
 }
 
-// 2-D tile store shared -> global through a tensor map (bulk async group of the issuing thread)
-__device__ __forceinline__ void tma_store_2d(const CUtensorMap* m, const void* smem_src, int c0, int c1) {
-    asm volatile("cp.async.bulk.tensor.2d.global.shared::cta.bulk_group [%0, {%2, %3}], [%1];" ::"l"(reinterpret_cast<uint64_t>(m)),
-                 "r"(smem_u32(smem_src)), "r"(c0), "r"(c1)
-                 : "memory");
-    asm volatile("cp.async.bulk.commit_group;" ::: "memory");
-}
-__device__ __forceinline__ void bulk_wait_read0() { asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory"); }
-__device__ __forceinline__ void bulk_wait0() { asm volatile("cp.async.bulk.wait_group 0;" ::: "memory"); }
 
-// ---------------------------------------------------------------- fences
-__device__ __forceinline__ void fence_proxy_async_smem() {
-    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-}
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-
-// ---------------------------------------------------------------- TMA
-// pull `bytes` (multiple of 16, 16-byte aligned address) of global memory into L2; no destination, no completion
-__device__ __forceinline__ void l2_prefetch_bulk(const void* gptr, uint32_t bytes) {
-    asm volatile("cp.async.bulk.prefetch.L2.global [%0], %1;" ::"l"(reinterpret_cast<uint64_t>(gptr)), "r"(bytes) : "memory");
-}
-__device__ __forceinline__ void tma_prefetch_desc(const CUtensorMap* m) {
-    asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(m)) : "memory");
-}
-// 2-D tiled load: coordinates are (c0 = innermost/contiguous dim, c1 = row).
-__device__ __forceinline__ void tma_load_2d(const CUtensorMap* m, uint64_t* bar, void* smem_dst, int c0, int c1) {
-    asm volatile(
-        "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];" ::"r"(
-            smem_u32(smem_dst)),
-        "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar)), "r"(c0), "r"(c1)
-        : "memory");
-}
-
-// ---------------------------------------------------------------- TMEM
-template <uint32_t kCols>
-__device__ __forceinline__ void tmem_alloc(uint32_t* smem_dst) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(smem_dst)),
-                 "n"(kCols)
-                 : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-template <uint32_t kCols>
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr) {
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "n"(kCols) : "memory");
-}
-
-// ---------------------------------------------------------------- UMMA
-// Shared-memory matrix descriptor (sm_100 format):
-//   [0,14)  start address >> 4      [16,30) leading byte offset >> 4
-//   [32,46) stride byte offset >> 4 [46,48) version = 1
-//   [49,52) base offset = 0         [61,64) layout type (0 none, 2 SW128, 4 SW64, 6 SW32)
-enum : uint64_t { kLayoutNone = 0, kLayoutSW128 = 2, kLayoutSW64 = 4, kLayoutSW32 = 6 };
-
-__device__ __forceinline__ uint64_t make_smem_desc(uint32_t smem_addr, uint32_t lbo_bytes, uint32_t sbo_bytes,
-                                                   uint64_t layout) {
-    uint64_t d = 0;
-    d |= static_cast<uint64_t>((smem_addr >> 4) & 0x3FFF);
-    d |= static_cast<uint64_t>((lbo_bytes >> 4) & 0x3FFF) << 16;
-    d |= static_cast<uint64_t>((sbo_bytes >> 4) & 0x3FFF) << 32;
-    d |= 1ull << 46;
-    d |= layout << 61;
-    return d;
-}
-
-// Instruction descriptor for kind::f16 (fp16/bf16 inputs, fp32 accumulate):
-//   [4,6) c_format (1 = f32)  [7,10) a_format  [10,13) b_format (0 = f16, 1 = bf16)
-//   [15] a_major [16] b_major (0 = K-major, 1 = MN-major)
-//   [17,23) N >> 3            [24,29) M >> 4
-__host__ __device__ constexpr uint32_t make_idesc_f16(uint32_t M, uint32_t N, uint32_t ab_format, uint32_t a_mn_major,
-                                                      uint32_t b_mn_major) {
-    return (1u << 4) | (ab_format << 7) | (ab_format << 10) | (a_mn_major << 15) | (b_mn_major << 16) |
-           ((N >> 3) << 17) | ((M >> 4) << 24);
-}
-
-// D[tmem] (+)= A[smem desc] * B[smem desc]; issued by ONE thread.
-__device__ __forceinline__ void umma_f16_ss(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc,
-                                            uint32_t accumulate) {
-    asm volatile(
-        "{\n\t"
-        ".reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t"
-        "}\n" ::"r"(tmem_d),
-        "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-        : "memory");
-}
-// A operand read from TMEM (used by attention: P lives in tensor memory).
-__device__ __forceinline__ void umma_f16_ts(uint32_t tmem_d, uint32_t tmem_a, uint64_t bdesc, uint32_t idesc,
-                                            uint32_t accumulate) {
-    asm volatile(
-        "{\n\t"
-        ".reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], [%1], %2, %3, p;\n\t"
-        "}\n" ::"r"(tmem_d),
-        "r"(tmem_a), "l"(bdesc), "r"(idesc), "r"(accumulate)
-        : "memory");
-}
-// Make all previously issued UMMAs arrive on an mbarrier when they complete
-// (implies tcgen05.fence::before_thread_sync).
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar))
-                 : "memory");
-}
-
-// TMEM -> registers: this warp's 32 lanes x 32 consecutive fp32 columns.
-__device__ __forceinline__ void tmem_ld_32x32(uint32_t taddr, uint32_t (&v)[32]) {
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-        : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]), "=r"(v[8]),
-          "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15]), "=r"(v[16]),
-          "=r"(v[17]), "=r"(v[18]), "=r"(v[19]), "=r"(v[20]), "=r"(v[21]), "=r"(v[22]), "=r"(v[23]), "=r"(v[24]),
-          "=r"(v[25]), "=r"(v[26]), "=r"(v[27]), "=r"(v[28]), "=r"(v[29]), "=r"(v[30]), "=r"(v[31])
-        : "r"(taddr)
-        : "memory");
-}
-__device__ __forceinline__ void tmem_ld_32x16(uint32_t taddr, uint32_t (&v)[16]) {
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-        : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]), "=r"(v[8]),
-          "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15])
-        : "r"(taddr)
-        : "memory");
-}
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-
-// registers -> TMEM (32 lanes x 32 columns of this warp)
-__device__ __forceinline__ void tmem_st_32x32(uint32_t taddr, const uint32_t (&v)[32]) {
-    asm volatile(
-        "tcgen05.st.sync.aligned.32x32b.x32.b32 [%0], "
-        "{%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, "
-        "%17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32};" ::"r"(taddr),
-        "r"(v[0]), "r"(v[1]), "r"(v[2]), "r"(v[3]), "r"(v[4]), "r"(v[5]), "r"(v[6]), "r"(v[7]), "r"(v[8]), "r"(v[9]),
-        "r"(v[10]), "r"(v[11]), "r"(v[12]), "r"(v[13]), "r"(v[14]), "r"(v[15]), "r"(v[16]), "r"(v[17]), "r"(v[18]),
-        "r"(v[19]), "r"(v[20]), "r"(v[21]), "r"(v[22]), "r"(v[23]), "r"(v[24]), "r"(v[25]), "r"(v[26]), "r"(v[27]),
-        "r"(v[28]), "r"(v[29]), "r"(v[30]), "r"(v[31])
-        : "memory");
-}
-__device__ __forceinline__ void tmem_st_32x16(uint32_t taddr, const uint32_t (&v)[16]) {
-    asm volatile(
-        "tcgen05.st.sync.aligned.32x32b.x16.b32 [%0], "
-        "{%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16};" ::"r"(taddr),
-        "r"(v[0]), "r"(v[1]), "r"(v[2]), "r"(v[3]), "r"(v[4]), "r"(v[5]), "r"(v[6]), "r"(v[7]), "r"(v[8]), "r"(v[9]),
-        "r"(v[10]), "r"(v[11]), "r"(v[12]), "r"(v[13]), "r"(v[14]), "r"(v[15])
-        : "memory");
-}
-__device__ __forceinline__ void tmem_st_32x8(uint32_t taddr, const uint32_t (&v)[8]) {
-    asm volatile("tcgen05.st.sync.aligned.32x32b.x8.b32 [%0], {%1, %2, %3, %4, %5, %6, %7, %8};" ::"r"(taddr), "r"(v[0]),
-                 "r"(v[1]), "r"(v[2]), "r"(v[3]), "r"(v[4]), "r"(v[5]), "r"(v[6]), "r"(v[7])
-                 : "memory");
-}
-__device__ __forceinline__ void tmem_st_wait() { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
-
-// ---------------------------------------------------------------- CTA pairs (cluster of 2, tcgen05 cta_group::2)
+// ---------------------------------------------------------------- clusters
 __device__ __forceinline__ uint32_t cluster_ctarank() {
     uint32_t r;
     asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
@@ -256,54 +89,129 @@ __device__ __forceinline__ float4 ld_shared_cluster_f4(uint32_t cluster_addr) {
     asm volatile("ld.shared::cluster.v4.f32 {%0, %1, %2, %3}, [%4];" : "=f"(v.x), "=f"(v.y), "=f"(v.z), "=f"(v.w) : "r"(cluster_addr) : "memory");
     return v;
 }
-__device__ __forceinline__ void st_shared_cluster_u32(uint32_t cluster_addr, uint32_t v) {
-    asm volatile("st.shared::cluster.u32 [%0], %1;" ::"r"(cluster_addr), "r"(v) : "memory");
+
+// ---------------------------------------------------------------- fences
+__device__ __forceinline__ void fence_proxy_async_smem() {
+    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
 }
-__device__ __forceinline__ void mbar_arrive_cluster(uint32_t cluster_addr) {
-    // .relaxed: a .release at cluster scope compiles to MEMBAR.ALL.GPU + ERRBAR (thousands of cycles per arrival). The
-    // callers have nothing to publish through memory: TMEM reads were completed with tcgen05.wait::ld beforehand.
-    asm volatile("mbarrier.arrive.relaxed.cluster.shared::cluster.b64 _, [%0];" ::"r"(cluster_addr) : "memory");
+
+// ---------------------------------------------------------------- TMA
+__device__ __forceinline__ void tma_prefetch_desc(const CUtensorMap* m) {
+    asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(m)) : "memory");
 }
-__device__ __forceinline__ void mbar_expect_tx_cluster(uint32_t cluster_addr, uint32_t bytes) {
-    // .relaxed for the same reason: the TMA bytes are tracked by complete_tx, the producer thread publishes nothing
-    asm volatile("mbarrier.arrive.expect_tx.relaxed.cluster.shared::cluster.b64 _, [%0], %1;" ::"r"(cluster_addr), "r"(bytes)
-                 : "memory");
-}
-// TMA load issued by either CTA of a pair; completes on the mbarrier at `bar_cluster_addr` (the leader's barrier)
-__device__ __forceinline__ void tma_load_2d_2sm(const CUtensorMap* m, uint32_t bar_cluster_addr, void* smem_dst, int c0, int c1) {
+// 2-D tiled load: coordinates are (c0 = innermost/contiguous dim, c1 = row).
+__device__ __forceinline__ void tma_load_2d(const CUtensorMap* m, uint64_t* bar, void* smem_dst, int c0, int c1) {
     asm volatile(
-        "cp.async.bulk.tensor.2d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];" ::"r"(
+        "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];" ::"r"(
             smem_u32(smem_dst)),
-        "l"(reinterpret_cast<uint64_t>(m)), "r"(bar_cluster_addr), "r"(c0), "r"(c1)
+        "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar)), "r"(c0), "r"(c1)
         : "memory");
 }
-template <uint32_t kCols>
-__device__ __forceinline__ void tmem_alloc_2sm(uint32_t* smem_dst) {
-    asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(smem_dst)), "n"(kCols)
-                 : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
+
+// ---------------------------------------------------------------- warpgroup MMA (wgmma)
+// Shared-memory matrix descriptor:
+//   [0,14)  start address >> 4      [16,30) leading byte offset >> 4
+//   [32,46) stride byte offset >> 4 [49,52) base offset = 0
+//   [62,64) swizzle (0 none, 1 128B, 2 64B, 3 32B)
+enum : uint64_t { kLayoutNone = 0, kLayoutSW128 = 1, kLayoutSW64 = 2, kLayoutSW32 = 3 };
+
+__device__ __forceinline__ uint64_t make_smem_desc(uint32_t smem_addr, uint32_t lbo_bytes, uint32_t sbo_bytes,
+                                                   uint64_t layout) {
+    uint64_t d = 0;
+    d |= static_cast<uint64_t>((smem_addr >> 4) & 0x3FFF);
+    d |= static_cast<uint64_t>((lbo_bytes >> 4) & 0x3FFF) << 16;
+    d |= static_cast<uint64_t>((sbo_bytes >> 4) & 0x3FFF) << 32;
+    d |= layout << 62;
+    return d;
 }
-template <uint32_t kCols>
-__device__ __forceinline__ void tmem_dealloc_2sm(uint32_t taddr) {
-    asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(taddr), "n"(kCols) : "memory");
+
+// Accumulator registers of other warpgroup-MMA groups may be touched only between fence and commit/wait.
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() {
+    asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory");
 }
-// D[tmem of both CTAs] (+)= A * B with M = 256 (128 rows per CTA), B's N split across the two CTAs; leader CTA only
-__device__ __forceinline__ void umma_f16_ss_2sm(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
-    asm volatile(
-        "{\n\t"
-        ".reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n\t"
-        "}\n" ::"r"(tmem_d),
-        "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-        : "memory");
+// keeps the compiler from moving reads of the accumulators above the wait
+template <int NR>
+__device__ __forceinline__ void wgmma_touch(float (&d)[NR]) {
+#pragma unroll
+    for (int i = 0; i < NR; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
-// arrive (when all prior MMAs of this thread retire) on the mbarrier at the same offset in every CTA of `mask`
-__device__ __forceinline__ void umma_commit_2sm(uint64_t* bar, uint16_t mask) {
-    asm volatile("tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;" ::"r"(
-                     smem_u32(bar)),
-                 "h"(mask)
-                 : "memory");
+
+// One m64nNk16 instruction, D (fp32, N/2 registers per thread) (+)= A * B. Register layout of D for thread t of the
+// warpgroup (warp w = t / 32, g = (t % 32) / 4, q = t % 4): d[4j + 0/1] = row 16w + g, columns 8j + 2q + 0/1;
+// d[4j + 2/3] = row 16w + g + 8, same columns.
+//   F16    : operands are fp16 (else bf16)
+//   TRANS_B: B tile is MN-major in shared memory (rows of the tile are K, N contiguous)
+// Inline asm cannot build "{%0, ..., %(N/2-1)}" from a template parameter: the operand lists below are spelled out
+// for every N the kernels use, and the overload is chosen by an integral_constant tag.
+#define VR_R4(d, i) "+f"(d[i]), "+f"(d[i + 1]), "+f"(d[i + 2]), "+f"(d[i + 3])
+#define VR_R8(d, i) VR_R4(d, i), VR_R4(d, i + 4)
+#define VR_R16(d, i) VR_R8(d, i), VR_R8(d, i + 8)
+#define VR_R32(d, i) VR_R16(d, i), VR_R16(d, i + 16)
+#define VR_R64(d, i) VR_R32(d, i), VR_R32(d, i + 32)
+
+// register-name lists "%0, %1, ..." of 8 / 32 / 64 / 96 / 128 entries
+#define VR_N8 "%0, %1, %2, %3, %4, %5, %6, %7"
+#define VR_N32 VR_N8 ", %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31"
+#define VR_N64 VR_N32 ", %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63"
+#define VR_N96 VR_N64 ", %64, %65, %66, %67, %68, %69, %70, %71, %72, %73, %74, %75, %76, %77, %78, %79, %80, %81, %82, %83, %84, %85, %86, %87, %88, %89, %90, %91, %92, %93, %94, %95"
+#define VR_N128 VR_N96 ", %96, %97, %98, %99, %100, %101, %102, %103, %104, %105, %106, %107, %108, %109, %110, %111, %112, %113, %114, %115, %116, %117, %118, %119, %120, %121, %122, %123, %124, %125, %126, %127"
+
+// A and B from shared memory
+#define VR_WGMMA_SS(NN, NREG, NAMES, REGS, A0, A1, A2)                                                                  \
+    template <bool F16, bool TRANS_B>                                                                                   \
+    __device__ __forceinline__ void wgmma_ss(float (&d)[NREG], uint64_t adesc, uint64_t bdesc, int accumulate,          \
+                                             std::integral_constant<int, NN>) {                                         \
+        if (F16)                                                                                                        \
+            asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %" #A2 ", 0;\n\t"                                         \
+                         "wgmma.mma_async.sync.aligned.m64n" #NN "k16.f32.f16.f16 {" NAMES "}, %" #A0 ", %" #A1          \
+                         ", p, 1, 1, 0, 0;\n\t}\n"                                                                      \
+                         : REGS(d, 0)                                                                                   \
+                         : "l"(adesc), "l"(bdesc), "r"(accumulate));                                                    \
+        else if (TRANS_B)                                                                                               \
+            asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %" #A2 ", 0;\n\t"                                         \
+                         "wgmma.mma_async.sync.aligned.m64n" #NN "k16.f32.bf16.bf16 {" NAMES "}, %" #A0 ", %" #A1        \
+                         ", p, 1, 1, 0, 1;\n\t}\n"                                                                      \
+                         : REGS(d, 0)                                                                                   \
+                         : "l"(adesc), "l"(bdesc), "r"(accumulate));                                                    \
+        else                                                                                                            \
+            asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %" #A2 ", 0;\n\t"                                         \
+                         "wgmma.mma_async.sync.aligned.m64n" #NN "k16.f32.bf16.bf16 {" NAMES "}, %" #A0 ", %" #A1        \
+                         ", p, 1, 1, 0, 0;\n\t}\n"                                                                      \
+                         : REGS(d, 0)                                                                                   \
+                         : "l"(adesc), "l"(bdesc), "r"(accumulate));                                                    \
+    }
+VR_WGMMA_SS(16, 8, VR_N8, VR_R8, 8, 9, 10)
+VR_WGMMA_SS(64, 32, VR_N32, VR_R32, 32, 33, 34)
+VR_WGMMA_SS(128, 64, VR_N64, VR_R64, 64, 65, 66)
+#define VR_R96(d, i) VR_R64(d, i), VR_R32(d, i + 64)
+VR_WGMMA_SS(192, 96, VR_N96, VR_R96, 96, 97, 98)
+#define VR_R128(d, i) VR_R64(d, i), VR_R64(d, i + 64)
+VR_WGMMA_SS(256, 128, VR_N128, VR_R128, 128, 129, 130)
+
+// A (bf16 pairs, the m16n8k16 A-fragment layout of each warp) from registers, B MN-major bf16 from shared memory
+#define VR_WGMMA_RS(NN, NREG, NAMES, REGS, A0, A1, A2, A3, B0, P0)                                                      \
+    __device__ __forceinline__ void wgmma_rs_tb(float (&d)[NREG], const uint32_t (&a)[4], uint64_t bdesc, int accumulate, \
+                                                std::integral_constant<int, NN>) {                                      \
+        asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %" #P0 ", 0;\n\t"                                             \
+                     "wgmma.mma_async.sync.aligned.m64n" #NN "k16.f32.bf16.bf16 {" NAMES "}, {%" #A0 ", %" #A1 ", %" #A2 \
+                     ", %" #A3 "}, %" #B0 ", p, 1, 1, 1;\n\t}\n"                                                        \
+                     : REGS(d, 0)                                                                                       \
+                     : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(bdesc), "r"(accumulate));                        \
+    }
+VR_WGMMA_RS(16, 8, VR_N8, VR_R8, 8, 9, 10, 11, 12, 13)
+VR_WGMMA_RS(64, 32, VR_N32, VR_R32, 32, 33, 34, 35, 36, 37)
+
+// register budget per warpgroup role (all warps of the warpgroup execute it)
+template <int R>
+__device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(R)); }
+template <int R>
+__device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(R)); }
+
+__device__ __forceinline__ void named_bar_sync(int id, int threads) {
+    asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(threads) : "memory");
 }
 
 // ---------------------------------------------------------------- misc

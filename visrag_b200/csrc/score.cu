@@ -2,9 +2,9 @@
 // retriever/dense_retriever.py:25-30), built so that the [nq, nd] score matrix never touches HBM and the
 // result is the EXACT fp32 top-k:
 //
-//  1. score_filter_kernel : tcgen05 GEMM on fp16 copies of Q and D (fp32 accumulate in TMEM). Each CTA owns a
-//     (128-query block, contiguous range of 256-doc tiles); its epilogue threads (one query row each) keep the 16
-//     best approximate scores of their row in registers across all tiles of the range. Output: per query
+//  1. score_filter_kernel : wgmma GEMM on fp16 copies of Q and D (fp32 accumulate in registers). Each CTA owns a
+//     (128-query block, contiguous range of 256-doc tiles); its MMA threads keep the 16 best approximate scores of
+//     their rows in registers across all tiles of the range. Output: per query
 //     `lists = ranges*2` sorted candidate lists of 16 (score, doc) pairs.
 //  2. rescore_topk_kernel : one CTA per query recomputes every candidate's score in fp32 on CUDA cores
 //     (q . d, 2304 FMAs each), selects the top-k by (score desc, doc id asc), and PROVES the selection: every
@@ -15,7 +15,7 @@
 //
 // Tie rule everywhere: higher score first, then lower doc id.
 #include "common.h"
-#include "gemm2.cuh"
+#include "gemm.cuh"
 #include <math.h>
 
 namespace vr {
@@ -24,13 +24,13 @@ constexpr int SC_KT = 16;    // candidates kept per list
 constexpr int SC_BN = 256;   // docs per tile
 constexpr int SC_MAX_RANGES = 64;  // doc ranges (= candidate lists per query) the filter may use
 
-// Work decomposition of the filter: the unit of work is one 256-query x 256-doc MMA tile (one CTA pair). The doc axis
+// Work decomposition of the filter: the unit of work is one 256-query x 256-doc tile (one CTA pair). The doc axis
 // is cut into R equal ranges; item i = r*QB + b (QB = 256-query blocks) is the sweep of query block b over doc range r,
 // and pair p runs items p, p+P, p+2P, ... Items have the same length and start together, so all pairs of a wave walk
 // their doc range in lockstep: at any moment the whole GPU reads at most ceil(P/QB)+1 distinct doc tiles and every doc
 // tile is fetched from HBM once and then served to the other query blocks from L2. (A contiguous "stream-K" split of
-// the b-major tile list balances perfectly but de-phases the pairs: measured 23 GB of DRAM reads instead of 0.6 GB
-// and 6.0 ms instead of the ~4 ms this layout takes at 10 k x 125 k.) R is chosen by the host to fill whole waves
+// the b-major tile list balances perfectly but de-phases the pairs, and every pair then streams its own doc tiles from
+// DRAM.) R is chosen by the host to fill whole waves
 // (score_plan); every item emits ONE 16-entry candidate list per query, so a query has R lists. Items of later waves
 // start from the threshold the finished items of the same query published (tau, see the epilogue).
 struct ScoreArgs {
@@ -48,12 +48,11 @@ struct ScoreArgs {
 
 struct Score2Cfg {
     static constexpr int STAGES = 6;
+    static constexpr int SUB_BN = 128;                      // docs per MMA sub-tile (a 256-doc tile is two of them)
     static constexpr int A_BYTES = GEMM_BM * GEMM_BK * 2;   // this CTA's 128 query rows
-    static constexpr int B_BYTES = 128 * GEMM_BK * 2;       // this CTA's half of the 256 docs
+    static constexpr int B_BYTES = SUB_BN * GEMM_BK * 2;
     static constexpr int STAGE_BYTES = A_BYTES + B_BYTES;   // 32 KB
-    static constexpr int MERGE_BYTES = 4 * SC_KT * 32 * 8;  // per quarter: 16 x 32 (score, id) pairs
-    static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + MERGE_BYTES + 1024 + 256;
-    static constexpr int TMEM_COLS = 512;
+    static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + 1024 + 256;
 };
 
 __device__ __forceinline__ void topk_insert(float (&sc)[SC_KT], int (&id)[SC_KT], float v, int i) {
@@ -72,15 +71,18 @@ __device__ __forceinline__ void topk_insert(float (&sc)[SC_KT], int (&id)[SC_KT]
     }
 }
 
-__device__ __forceinline__ void named_bar_sync(int id, int threads) {
-    asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(threads) : "memory");
+__device__ __forceinline__ float quad_max(float v) {
+    v = fmaxf(v, __shfl_xor_sync(0xffffffffu, v, 1));
+    return fmaxf(v, __shfl_xor_sync(0xffffffffu, v, 2));
 }
 
-// CTA pair (tcgen05 cta_group::2): 256 queries x 256 docs per MMA tile, fp16 operands, fp32 accumulators in the TMEM of
-// both CTAs (two stages). Roles as in gemm2.cuh; the epilogue threads (one query row each, the two column halves of a
-// row in two warps) keep a sorted top-16 in registers over all tiles of a piece, merge the halves through shared memory
-// (top-16 of the union: its tail bounds everything either half dropped) and write one list per (query, piece).
-__global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(GEMM_THREADS, 1)
+// A pair of CTAs (blocks 2p, 2p+1) shares one work item: 256 queries x a range of 256-doc tiles, 128 queries per CTA,
+// fp16 operands, fp32 wgmma accumulators in registers. Roles as in gemm.cuh: a TMA producer warpgroup and two consumer
+// warpgroups of 64 query rows each; a doc tile is computed as two 128-doc sub-tiles. A query row of the accumulator
+// lives in the 4 lanes of a quad (each lane holds a quarter of the columns), so every lane keeps a sorted top-16 of ITS
+// columns for each of its two rows over all tiles of the item; the four lists of a row are merged by shuffles at the end
+// of the item (top-16 of the union: its tail bounds everything any lane dropped) into one list per (query, doc range).
+__global__ void __launch_bounds__(GEMM_THREADS, 1)
 score_filter_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant__ CUtensorMap tmap_d,
                     const ScoreArgs g) {
     using Cfg = Score2Cfg;
@@ -89,17 +91,11 @@ score_filter_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_con
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
     uint8_t* smem_a = smem;
     uint8_t* smem_b = smem + STAGES * Cfg::A_BYTES;
-    float* merge_s = reinterpret_cast<float*>(smem + STAGES * Cfg::STAGE_BYTES);  // [4][SC_KT][32]
-    int* merge_i = reinterpret_cast<int*>(merge_s + 4 * SC_KT * 32);
-    uint64_t* bars = reinterpret_cast<uint64_t*>(smem + STAGES * Cfg::STAGE_BYTES + Cfg::MERGE_BYTES);
-    uint64_t* full_bar = bars;
-    uint64_t* empty_bar = bars + STAGES;
-    uint64_t* tfull_bar = bars + 2 * STAGES;
-    uint64_t* tempty_bar = bars + 2 * STAGES + 2;
-    uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 2 * STAGES + 4);
+    uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + STAGES * Cfg::STAGE_BYTES);
+    uint64_t* empty_bar = full_bar + STAGES;
 
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const uint32_t rank = cluster_ctarank();
+    const int wg = threadIdx.x >> 7, warp = (threadIdx.x >> 5) & 3, lane = threadIdx.x & 31;
+    const int rank = blockIdx.x & 1;
     const int pair = blockIdx.x >> 1;
     const int num_pairs = gridDim.x >> 1;
     const int num_kb = (g.dim + GEMM_BK - 1) / GEMM_BK;
@@ -108,191 +104,174 @@ score_filter_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_con
     auto item_t0 = [&](int item) { return static_cast<int>(static_cast<long long>(g.T) * (item / g.QB) / g.R); };
     auto item_t1 = [&](int item) { return static_cast<int>(static_cast<long long>(g.T) * (item / g.QB + 1) / g.R); };
 
-    if (warp == 0 && lane == 0) {
+    if (threadIdx.x == 0) {
         tma_prefetch_desc(&tmap_q);
         tma_prefetch_desc(&tmap_d);
-    }
-    if (warp == 1 && lane == 0) {
         for (int i = 0; i < STAGES; ++i) {
-            mbar_init(&full_bar[i], 2);   // one arrive.expect_tx per CTA (used in the leader only)
-            mbar_init(&empty_bar[i], 1);
-        }
-        for (int i = 0; i < 2; ++i) {
-            mbar_init(&tfull_bar[i], 1);
-            mbar_init(&tempty_bar[i], 2 * GEMM_EPI_WARPS);  // used in the leader only
+            mbar_init(&full_bar[i], 1);
+            mbar_init(&empty_bar[i], 8);  // one arrival per consumer warp
         }
         fence_mbar_init();
     }
-    cluster_sync_all();
-    if (warp == 2) tmem_alloc_2sm<Cfg::TMEM_COLS>(tmem_slot);
-    tc_fence_before();
-    cluster_sync_all();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
+    __syncthreads();
 
-    if (warp == 0) {
-        if (lane == 0) {
+    if (wg == 0) {
+        setmaxnreg_dec<40>();
+        if (warp == 0 && lane == 0) {
             int stage = 0;
             uint32_t phase = 0;
             for (int item = pair; item < g.items; item += num_pairs) {
-                const int m0 = item_b(item) * 2 * GEMM_BM + static_cast<int>(rank) * GEMM_BM;
+                const int m0 = item_b(item) * 2 * GEMM_BM + rank * GEMM_BM;
                 const int t1 = item_t1(item);
-                for (int t = item_t0(item); t < t1; ++t) {
-                    const int n0 = t * SC_BN + static_cast<int>(rank) * 128;
+                for (int u = 2 * item_t0(item); u < 2 * t1; ++u) {  // 128-doc sub-tiles
+                    const int n0 = u * Cfg::SUB_BN;
                     for (int kb = 0; kb < num_kb; ++kb) {
                         mbar_wait(&empty_bar[stage], phase ^ 1);
-                        const uint32_t lfull = mapa_u32(smem_u32(&full_bar[stage]), 0);
-                        mbar_expect_tx_cluster(lfull, Cfg::STAGE_BYTES);
-                        tma_load_2d_2sm(&tmap_q, lfull, smem_a + stage * Cfg::A_BYTES, kb * GEMM_BK, m0);
-                        tma_load_2d_2sm(&tmap_d, lfull, smem_b + stage * Cfg::B_BYTES, kb * GEMM_BK, n0);
+                        mbar_expect_tx(&full_bar[stage], Cfg::STAGE_BYTES);
+                        tma_load_2d(&tmap_q, &full_bar[stage], smem_a + stage * Cfg::A_BYTES, kb * GEMM_BK, m0);
+                        tma_load_2d(&tmap_d, &full_bar[stage], smem_b + stage * Cfg::B_BYTES, kb * GEMM_BK, n0);
                         if (++stage == STAGES) { stage = 0; phase ^= 1; }
                     }
                 }
             }
         }
-    } else if (warp == 1) {
-        if (rank == 0) {
-            // whole warp, warp-uniform control flow, one elected lane issues (see gemm.cuh)
-            constexpr uint32_t idesc = make_idesc_f16(2 * GEMM_BM, SC_BN, 0 /*fp16*/, 0, 0);
-            const uint64_t desc_hi = make_smem_desc(0, 16, 1024, kLayoutSW128);
-            const uint32_t a_lo0 = smem_u32(smem_a) >> 4, b_lo0 = smem_u32(smem_b) >> 4;
-            int stage = 0;
-            uint32_t phase = 0;
-            int units = 0;  // tiles this pair computes
-            for (int item = pair; item < g.items; item += num_pairs) units += item_t1(item) - item_t0(item);
-            for (int it = 0; it < units; ++it) {
-                const int acc = it & 1;
-                mbar_wait(&tempty_bar[acc], ((it >> 1) & 1) ^ 1);
-                tc_fence_after();
-                const uint32_t d_tmem = tmem_base + acc * SC_BN;
-                for (int kb = 0; kb < num_kb; ++kb) {
-                    mbar_wait(&full_bar[stage], phase);
-                    tc_fence_after();
-                    if (elect_one()) {
-                        const uint64_t ad = desc_hi | static_cast<uint64_t>(a_lo0 + stage * (Cfg::A_BYTES >> 4));
-                        const uint64_t bd = desc_hi | static_cast<uint64_t>(b_lo0 + stage * (Cfg::B_BYTES >> 4));
-                        umma_f16_ss_2sm(d_tmem, ad, bd, idesc, kb != 0 ? 1u : 0u);
-                        umma_f16_ss_2sm(d_tmem, ad + 2, bd + 2, idesc, 1u);
-                        umma_f16_ss_2sm(d_tmem, ad + 4, bd + 4, idesc, 1u);
-                        umma_f16_ss_2sm(d_tmem, ad + 6, bd + 6, idesc, 1u);
-                        umma_commit_2sm(&empty_bar[stage], 3);  // frees the slot in BOTH CTAs
-                        if (kb == num_kb - 1) umma_commit_2sm(&tfull_bar[acc], 3);
-                    }
-                    __syncwarp();
-                    if (++stage == STAGES) { stage = 0; phase ^= 1; }
-                }
-            }
+        return;
+    }
+
+    setmaxnreg_inc<232>();
+    const int cw = wg - 1;
+    const uint64_t desc_hi = make_smem_desc(0, 16, 1024, kLayoutSW128);
+    const uint32_t a_lo0 = (smem_u32(smem_a) + cw * (64 * GEMM_BK * 2)) >> 4, b_lo0 = smem_u32(smem_b) >> 4;
+    const int g8 = lane >> 2, q4 = lane & 3;
+    float sc[2][SC_KT];  // [accumulator row g8 / g8 + 8]
+    int id[2][SC_KT];
+    int stage = 0;
+    uint32_t phase = 0;
+    for (int item = pair; item < g.items; item += num_pairs) {
+        const int b = item_b(item), r = item / g.QB;
+        const int row0 = b * 2 * GEMM_BM + rank * GEMM_BM + cw * 64 + warp * 16 + g8;
+        // tau: a lower bound on what this query can still use, published by the items of this query that already
+        // finished (the 16th best score of their doc range). Dropping everything <= tau is covered by the proof: the
+        // rescoring kernel's bound is the maximum over all list tails, and tau is one of them.
+        float* tau_ptr[2];
+        float tau[2], thr[2];  // thr = max(tau, best tail of the quad's four lists: the merged list's tail is no lower)
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+            tau_ptr[h] = g.cand_scores + (static_cast<long long>(min(row0 + 8 * h, g.nq - 1)) * g.lists + g.lists - 1) * SC_KT;
+            thr[h] = tau[h] = __ldcg(tau_ptr[h]);
+#pragma unroll
+            for (int j = 0; j < SC_KT; ++j) { sc[h][j] = -INFINITY; id[h][j] = -1; }
         }
-    } else if (warp >= 4) {
-        const int quarter = warp & 3, half = (warp - 4) >> 2;
-        float sc[SC_KT];
-        int id[SC_KT];
+        const int t1 = item_t1(item);
+        for (int u = 2 * item_t0(item); u < 2 * t1; ++u) {
+            float acc[Cfg::SUB_BN / 2];
+            int prev = -1;
+            for (int kb = 0; kb < num_kb; ++kb) {
+                mbar_wait(&full_bar[stage], phase);
+                const uint64_t ad = desc_hi | static_cast<uint64_t>(a_lo0 + stage * (Cfg::A_BYTES >> 4));
+                const uint64_t bd = desc_hi | static_cast<uint64_t>(b_lo0 + stage * (Cfg::B_BYTES >> 4));
+                wgmma_fence();
 #pragma unroll
-        for (int j = 0; j < SC_KT; ++j) { sc[j] = -INFINITY; id[j] = -1; }
-        float* ms = merge_s + quarter * SC_KT * 32;
-        int* mi = merge_i + quarter * SC_KT * 32;
-        const uint32_t ltempty0 = mapa_u32(smem_u32(&tempty_bar[0]), 0);
-        const uint32_t ltempty1 = mapa_u32(smem_u32(&tempty_bar[1]), 0);
-        int it = 0;
-        for (int item = pair; item < g.items; item += num_pairs) {
-            const int b = item_b(item), r = item / g.QB;
-            const int row = b * 2 * GEMM_BM + static_cast<int>(rank) * GEMM_BM + quarter * 32 + lane;
-            // tau: a lower bound on what this query can still use, published by the items of this query that already
-            // finished (the 16th best score of their doc range). Dropping everything <= tau is covered by the proof: the
-            // rescoring kernel's bound is the maximum over all list tails, and tau is one of them.
-            float* tau_ptr = g.cand_scores + (static_cast<long long>(min(row, g.nq - 1)) * g.lists + g.lists - 1) * SC_KT;
-            const float tau = __ldcg(tau_ptr);
-            float thr = tau;  // max(tau, sc[SC_KT-1])
-            const int t1 = item_t1(item);
-            for (int t = item_t0(item); t < t1; ++t, ++it) {
-                const int acc = it & 1;
-                mbar_wait(&tfull_bar[acc], (it >> 1) & 1);
-                tc_fence_after();
-                const uint32_t taddr = tmem_base + (static_cast<uint32_t>(quarter * 32) << 16) + acc * SC_BN + half * 128;
-                const long long col_base = static_cast<long long>(t) * SC_BN + half * 128;
+                for (int kk = 0; kk < 4; ++kk)
+                    wgmma_ss<true, false>(acc, ad + 2 * kk, bd + 2 * kk, (kb | kk) != 0, std::integral_constant<int, Cfg::SUB_BN>());
+                wgmma_commit();
+                if (prev >= 0) {
+                    wgmma_wait<1>();
+                    if (lane == 0) mbar_arrive(&empty_bar[prev]);
+                }
+                prev = stage;
+                if (++stage == STAGES) { stage = 0; phase ^= 1; }
+            }
+            wgmma_wait<0>();
+            if (lane == 0) mbar_arrive(&empty_bar[prev]);
+            wgmma_touch(acc);
+
+            const long long col_base = static_cast<long long>(u) * Cfg::SUB_BN + q4 * 2;
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+                // this lane's 32 scores of the row: v[2j + e] = column 8j + 2 q4 + e of the sub-tile
+                uint32_t v[32];
+#pragma unroll
+                for (int j = 0; j < 16; ++j) {
+                    v[2 * j] = __float_as_uint(acc[4 * j + 2 * h]);
+                    v[2 * j + 1] = __float_as_uint(acc[4 * j + 2 * h + 1]);
+                }
+                // fast path: nothing of the 32 scores beats the threshold (the common case after the first tiles)
+                float mx = fmaxf(__uint_as_float(v[0]), __uint_as_float(v[1]));
+#pragma unroll
+                for (int j = 2; j < 32; j += 2) mx = fmaxf(mx, fmaxf(__uint_as_float(v[j]), __uint_as_float(v[j + 1])));
+                if (mx > thr[h]) {
+                    // slow path, ONE compact instance of the insertion code per row (a fully unrolled form - 32 inlined
+                    // insertions - would thrash the instruction cache)
+                    uint32_t mask = 0;
+#pragma unroll
+                    for (int j = 0; j < 32; ++j) mask |= (__uint_as_float(v[j]) > thr[h] ? 1u : 0u) << j;
 #pragma unroll 1
-                for (int c = 0; c < 4; ++c) {
-                    uint32_t v[32];
-                    tmem_ld_32x32(taddr + c * 32, v);
-                    tmem_ld_wait();
-                    if (c == 3) {
-                        tc_fence_before();
-                        __syncwarp();
-                        if (lane == 0) mbar_arrive_cluster(acc ? ltempty1 : ltempty0);
-                    }
-                    // fast path: nothing of the 32 scores beats the threshold (the common case after the first tiles)
-                    float mx = fmaxf(__uint_as_float(v[0]), __uint_as_float(v[1]));
+                    while (mask) {
+                        const int j = __ffs(mask) - 1;
+                        mask &= mask - 1;
+                        // v[j] with a run-time j: binary select tree over the register array
+                        uint32_t s16[16], s8[8], s4[4], s2[2];
 #pragma unroll
-                    for (int j = 2; j < 32; j += 2) mx = fmaxf(mx, fmaxf(__uint_as_float(v[j]), __uint_as_float(v[j + 1])));
-                    if (mx > thr) {
-                        // slow path, ONE compact instance of the insertion code (the fully unrolled form - 32 inlined
-                        // insertions per chunk - thrashed the instruction cache: ncu top stall "no_instruction")
-                        uint32_t mask = 0;
+                        for (int i = 0; i < 16; ++i) s16[i] = (j & 1) ? v[2 * i + 1] : v[2 * i];
 #pragma unroll
-                        for (int j = 0; j < 32; ++j) mask |= (__uint_as_float(v[j]) > thr ? 1u : 0u) << j;
-                        const long long c0 = col_base + c * 32;
-#pragma unroll 1
-                        while (mask) {
-                            const int j = __ffs(mask) - 1;
-                            mask &= mask - 1;
-                            // v[j] with a run-time j: binary select tree over the register array
-                            uint32_t s16[16], s8[8], s4[4], s2[2];
+                        for (int i = 0; i < 8; ++i) s8[i] = (j & 2) ? s16[2 * i + 1] : s16[2 * i];
 #pragma unroll
-                            for (int i = 0; i < 16; ++i) s16[i] = (j & 1) ? v[2 * i + 1] : v[2 * i];
+                        for (int i = 0; i < 4; ++i) s4[i] = (j & 4) ? s8[2 * i + 1] : s8[2 * i];
 #pragma unroll
-                            for (int i = 0; i < 8; ++i) s8[i] = (j & 2) ? s16[2 * i + 1] : s16[2 * i];
-#pragma unroll
-                            for (int i = 0; i < 4; ++i) s4[i] = (j & 4) ? s8[2 * i + 1] : s8[2 * i];
-#pragma unroll
-                            for (int i = 0; i < 2; ++i) s2[i] = (j & 8) ? s4[2 * i + 1] : s4[2 * i];
-                            const float sv = __uint_as_float((j & 16) ? s2[1] : s2[0]);
-                            if (sv > thr && c0 + j < g.nd) {
-                                topk_insert(sc, id, sv, static_cast<int>(c0 + j));
-                                thr = fmaxf(tau, sc[SC_KT - 1]);
-                            }
+                        for (int i = 0; i < 2; ++i) s2[i] = (j & 8) ? s4[2 * i + 1] : s4[2 * i];
+                        const float sv = __uint_as_float((j & 16) ? s2[1] : s2[0]);
+                        const long long col = col_base + (j >> 1) * 8 + (j & 1);
+                        if (sv > thr[h] && col < g.nd) {
+                            topk_insert(sc[h], id[h], sv, static_cast<int>(col));
+                            thr[h] = fmaxf(thr[h], sc[h][SC_KT - 1]);
                         }
                     }
                 }
+                thr[h] = fmaxf(thr[h], quad_max(sc[h][SC_KT - 1]));
             }
-            // one candidate list per (query row, doc range): merge the two column halves (top-16 of the union: its tail
-            // bounds everything either half dropped), write it, publish its tail as the query's new tau
-            if (half == 1) {
+        }
+        // one candidate list per (query row, doc range): merge the quad's four column subsets (after the two exchange
+        // steps every lane of the quad holds the top-16 of the union), write it, publish its tail as the query's new tau
 #pragma unroll
-                for (int j = 0; j < SC_KT; ++j) { ms[j * 32 + lane] = sc[j]; mi[j * 32 + lane] = id[j]; }
-            }
-            named_bar_sync(1 + quarter, 64);
-            if (half == 0) {
+        for (int h = 0; h < 2; ++h) {
+#pragma unroll
+            for (int step = 1; step <= 2; ++step) {
+                float os[SC_KT];
+                int oi[SC_KT];
+#pragma unroll
+                for (int j = 0; j < SC_KT; ++j) {
+                    os[j] = __shfl_xor_sync(0xffffffffu, sc[h][j], step);
+                    oi[j] = __shfl_xor_sync(0xffffffffu, id[h][j], step);
+                }
 #pragma unroll 1
                 for (int j = 0; j < SC_KT; ++j) {
-                    const float v2 = ms[j * 32 + lane];
-                    if (v2 > sc[SC_KT - 1]) topk_insert(sc, id, v2, mi[j * 32 + lane]);
+                    // os[j] with a run-time j (one compact instance of the insertion code)
+                    float v2 = os[0];
+                    int i2 = oi[0];
+#pragma unroll
+                    for (int i = 1; i < SC_KT; ++i)
+                        if (i == j) { v2 = os[i]; i2 = oi[i]; }
+                    if (v2 > sc[h][SC_KT - 1]) topk_insert(sc[h], id[h], v2, i2);
                 }
             }
-            named_bar_sync(1 + quarter, 64);
-            if (half == 0 && row < g.nq) {
+            const int row = row0 + 8 * h;
+            if (q4 == 0 && row < g.nq) {
                 const long long base = (static_cast<long long>(row) * g.lists + r) * SC_KT;
 #pragma unroll
                 for (int j4 = 0; j4 < SC_KT / 4; ++j4) {
                     *reinterpret_cast<float4*>(g.cand_scores + base + j4 * 4) =
-                        make_float4(sc[j4 * 4], sc[j4 * 4 + 1], sc[j4 * 4 + 2], sc[j4 * 4 + 3]);
+                        make_float4(sc[h][j4 * 4], sc[h][j4 * 4 + 1], sc[h][j4 * 4 + 2], sc[h][j4 * 4 + 3]);
                     *reinterpret_cast<int4*>(g.cand_ids + base + j4 * 4) =
-                        make_int4(id[j4 * 4], id[j4 * 4 + 1], id[j4 * 4 + 2], id[j4 * 4 + 3]);
+                        make_int4(id[h][j4 * 4], id[h][j4 * 4 + 1], id[h][j4 * 4 + 2], id[h][j4 * 4 + 3]);
                 }
-                const float tail = sc[SC_KT - 1];
-                if (tail > tau) {  // float max through the integer atomics (tail may be negative)
-                    if (tail >= 0.f) atomicMax(reinterpret_cast<int*>(tau_ptr), __float_as_int(tail));
-                    else atomicMin(reinterpret_cast<unsigned int*>(tau_ptr), __float_as_uint(tail));
+                const float tail = sc[h][SC_KT - 1];
+                if (tail > tau[h]) {  // float max through the integer atomics (tail may be negative)
+                    if (tail >= 0.f) atomicMax(reinterpret_cast<int*>(tau_ptr[h]), __float_as_int(tail));
+                    else atomicMin(reinterpret_cast<unsigned int*>(tau_ptr[h]), __float_as_uint(tail));
                 }
             }
-#pragma unroll
-            for (int j = 0; j < SC_KT; ++j) { sc[j] = -INFINITY; id[j] = -1; }
         }
-    }
-    tc_fence_before();
-    cluster_sync_all();  // the peer may still be arriving on this CTA's barriers until here
-    if (warp == 2) {
-        tc_fence_after();
-        tmem_dealloc_2sm<Cfg::TMEM_COLS>(tmem_base);
     }
 }
 
@@ -706,33 +685,8 @@ __global__ void score_init_lists_kernel(float* __restrict__ cand_scores, int* __
     }
 }
 
-// Co-resident CTA pairs of the filter kernel on the current device (GPCs with an odd number of usable SMs cannot pair
-// all of them; a persistent kernel must not launch more clusters than fit at once).
-static int score_pairs() {
-    static int cached[64] = {};
-    const int dev = current_device();
-    const int slot = (dev >= 0 && dev < 64) ? dev : 0;
-    if (cached[slot] == 0) {
-        int n = 0;
-        cudaLaunchConfig_t cfg = {};
-        cfg.gridDim = dim3(num_sms() / 2 * 2);
-        cfg.blockDim = dim3(GEMM_THREADS);
-        cfg.dynamicSmemBytes = Score2Cfg::SMEM_BYTES;
-        cudaLaunchAttribute attr;
-        attr.id = cudaLaunchAttributeClusterDimension;
-        attr.val.clusterDim.x = 2; attr.val.clusterDim.y = 1; attr.val.clusterDim.z = 1;
-        cfg.attrs = &attr;
-        cfg.numAttrs = 1;
-        if (dev < 0 ||
-            cudaFuncSetAttribute(score_filter_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, Score2Cfg::SMEM_BYTES) != cudaSuccess ||
-            cudaOccupancyMaxActiveClusters(&n, score_filter_kernel, &cfg) != cudaSuccess || n <= 0) {
-            cudaGetLastError();
-            n = num_sms() / 2;
-        }
-        cached[slot] = n < num_sms() / 2 ? n : num_sms() / 2;
-    }
-    return cached[slot];
-}
+// CTA pairs of the (persistent) filter kernel: one CTA per SM
+static int score_pairs() { return num_sms() / 2; }
 
 struct ScorePlan {
     int T, R, QB, items, lists, pairs;
@@ -743,12 +697,13 @@ static ScorePlan score_plan(int nq, long long nd) {
     p.QB = (nq + 2 * GEMM_BM - 1) / (2 * GEMM_BM);
     p.T = static_cast<int>((nd + SC_BN - 1) / SC_BN);
     const int P = score_pairs();
-    // time ~ waves * tiles per item, plus a quarter tile per item for the pipeline fill and the list write-out
+    // time ~ waves * tiles per item, plus half a tile per item for the pipeline fill, the merge of the quad's lists and
+    // the list write-out
     double best = 1e30;
     p.R = 1;
     for (int R = 1; R <= SC_MAX_RANGES && R <= p.T; ++R) {
         const long long waves = (static_cast<long long>(p.QB) * R + P - 1) / P;
-        const double cost = static_cast<double>(waves) * ((p.T + R - 1) / R + 0.25);
+        const double cost = static_cast<double>(waves) * ((p.T + R - 1) / R + 0.5);
         if (cost < best * 0.98) { best = cost; p.R = R; }  // a larger R must win by 2 %: fewer lists to rescore
     }
     p.items = p.QB * p.R;

@@ -1,4 +1,4 @@
-"""B200 engine for the VisRAG-Ret encode path: uint8 slices + packed tokens -> pooled fp32 embeddings.
+"""H100 engine for the VisRAG-Ret encode path: uint8 slices + packed tokens -> pooled fp32 embeddings.
 
 Replaces the GPU work of `VisRAG_Ret.forward` (`modeling_visrag_ret.py:86-126`), `get_vllm_embedding`
 (`modeling_minicpmv.py:124-171`), the timm ViT, the Resampler and `MiniCPMModel.forward`, plus the pooling of
@@ -6,7 +6,7 @@ Replaces the GPU work of `VisRAG_Ret.forward` (`modeling_visrag_ret.py:86-126`),
   * the ViT runs over ALL slices of a batch that share a geometry at once (the reference loops page by page
     with batch 1, `modeling_minicpmv.py:130-135`);
   * LM sequences are packed (cu_seqlens) instead of right-padded;
-  * the residual streams stay fp32 in HBM; every GEMM reads bf16 operands and accumulates in fp32 (TMEM).
+  * the residual streams stay fp32 in HBM; every GEMM reads bf16 operands and accumulates in fp32 (registers).
 Every kernel is a C-ABI call (visrag_b200/ops.py); torch only owns the buffers.
 """
 from __future__ import annotations
@@ -25,7 +25,7 @@ from .config import VisRAGConfig
 from .host import PreparedBatch, prepare_batch
 from .weights import sincos_2d
 
-VIT_HEAD_STRIDE = 80  # 72 padded to a multiple of 16 (UMMA K granularity); pad rows of Wqkv are zero
+VIT_HEAD_STRIDE = 80  # 72 padded to a multiple of 16 (the MMA K step); pad rows of Wqkv are zero
 
 # CUDA-graph path (small batches): eligibility and cache bounds
 GRAPH_MAX_VIT_TOKENS = 32 * 1024   # up to 32 slices of 448x448: beyond that the kernels are long enough to hide launches
@@ -105,8 +105,6 @@ class VisRAGEngine:
                 bpad = torch.zeros((3, nh, hs), device=wq.device)
                 wpad[:, :, :hd] = wq
                 bpad[:, :, :hd] = bq
-                bpad[2, :, hd] = 1.0  # V[:, 72] == 1 for every head: the attention kernel reads the softmax denominator
-                #                       out of the P.V accumulator (VR_ATTN_V_ONES_COLUMN); Q/K padding stays zero
                 self.blocks.append(dict(
                     n1w=_f32(sd[p + "norm1.weight"], dev), n1b=_f32(sd[p + "norm1.bias"], dev),
                     qkv_w=_bf16(wpad.reshape(3 * nh * hs, D), dev), qkv_b=_f32(bpad.reshape(-1), dev),
@@ -192,7 +190,7 @@ class VisRAGEngine:
             ops.gemm(y, blk["qkv_w"], bias=blk["qkv_b"], out=qkv)
             ops.attention(qkv, qkv, qkv, q_col0=0, k_col0=nh * VIT_HEAD_STRIDE, v_col0=2 * nh * VIT_HEAD_STRIDE,
                           head_stride=VIT_HEAD_STRIDE, head_dim=cfg.vit_head_dim, heads=nh, batch=S, cu_k=cu, max_k=N,
-                          cu_q=cu, max_q=N, causal=False, scale=scale, out=att, v_ones_column=True)
+                          cu_q=cu, max_q=N, causal=False, scale=scale, out=att)
             ops.gemm(att, blk["proj_w"], bias=blk["proj_b"], resid=x, out=x, out_dtype=torch.float32)
             y = ops.layernorm(x, blk["n2w"], blk["n2b"], cfg.ln_eps)
             y = ops.gemm(y, blk["fc1_w"], bias=blk["fc1_b"], gelu=True)

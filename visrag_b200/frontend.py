@@ -122,7 +122,7 @@ def page_pixels(image) -> np.ndarray:
     """uint8 pixels of a PIL RGB image for the device front-end, WITHOUT repacking when possible: Pillow stores mode "RGB"
     as RGBX rows (4 bytes per pixel) and exports that buffer zero-copy through the Arrow C data interface (Pillow >= 11.2),
     so the page can be copied straight into pinned memory as [H, W, 4]; `np.asarray(image)` instead goes through
-    `tobytes()`, which repacks to RGB under the GIL (0.2-0.45 ms per 448x448 page). Falls back to that ([H, W, 3]) when the
+    `tobytes()`, which repacks to RGB under the GIL. Falls back to that ([H, W, 3]) when the
     export is unavailable (older Pillow, no pyarrow, images stored in several blocks)."""
     if image.mode != "RGB":
         image = image.convert("RGB")

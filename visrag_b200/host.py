@@ -5,7 +5,7 @@ Mirrors, with the same results, the reference's
   * placeholder text        `modeling_visrag_ret.py:57-84`, `modeling_minicpmv.py:247-274,595-609`,
   * tokenisation + image_bound `modeling_minicpmv.py:173-216`,
 but produces *packed* (unpadded) sequences and uint8 slice tensors grouped by geometry, which is what the
-B200 engine consumes. The geometry is split into a pure integer planner (`plan_slices`) — testable against
+H100 engine consumes. The geometry is split into a pure integer planner (`plan_slices`) — testable against
 the reference's golden geometry without touching pixels — and the PIL resampling that executes a plan
 (PIL's bicubic filter stays on the host because Recall parity depends on pixel-exact inputs, SURVEY.md H3).
 """
@@ -248,7 +248,7 @@ def prepare_batch(texts: Sequence[str], images: Sequence, tokenizer, cfg: VisRAG
     items = list(zip(texts, images))
     # Threads only pay off when PIL resamples on the host (Image.resize releases the GIL; the reference uses
     # ThreadPoolExecutor(8) for the same reason). What is left with the device front-end - PIL's tobytes() behind
-    # np.asarray - holds the GIL: measured 55 ms per 128 pages on one thread, 72 ms on eight.
+    # np.asarray - holds the GIL, so eight threads are no faster than one.
     if n_img >= 8 and not device_frontend:
         # one persistent pool and one task per worker: creating a pool and 128 futures per batch cost more than the work
         n_chunks = min(_POOL_WORKERS, len(items))

@@ -61,9 +61,9 @@ def encode_stream(batches: Iterable[dict], model, model_additional_args: Optiona
     of batch i (asynchronous launches on the current stream) and the device->host copy of batch i-1 (pinned buffer +
     event instead of the reference's blocking `.cpu()`, `inference.py:98`). `ramp_parts` > 1 cuts the FIRST batch into
     pieces (re-joined before it is yielded) so that the GPU starts after a fraction of a batch has been prepared. That
-    paid off while host preparation cost ~55 ms per 128 pages; with the zero-copy RGBX page path it costs ~4 ms, and
-    differently sized pieces make the caching allocator re-carve its blocks (a synchronising cudaFree/cudaMalloc:
-    measured 70 ms on the first full-size batch), so the default is no ramp."""
+    pays off only when host preparation is slow (PIL resampling on the host); with the zero-copy RGBX page path it is a small
+    fraction of a step, and differently sized pieces make the caching allocator re-carve its blocks (a synchronising
+    cudaFree/cudaMalloc on the first full-size batch), so the default is no ramp."""
     from collections import deque
     from concurrent.futures import ThreadPoolExecutor
 

@@ -1,4 +1,4 @@
-"""Drop-in classes with the reference's call signatures (SURVEY.md §8b), backed by the B200 engine.
+"""Drop-in classes with the reference's call signatures (SURVEY.md §8b), backed by the H100 engine.
 
   B1  `VisRAGRetB200.forward(text, image, tokenizer, vision_hidden_states=None, max_inp_length=2048, **kw)`
       == `VisRAG_Ret.forward` (`modeling_visrag_ret/modeling_visrag_ret.py:86-126`): returns an object with

@@ -70,7 +70,7 @@ def gemm(
     rope_cols: int = 0,
     block_n: int = 0,
 ) -> torch.Tensor:
-    """``out = epilogue(a @ w.T)`` on tcgen05. ``a`` [M,K] bf16, ``w`` [N,K] bf16 (nn.Linear layout).
+    """``out = epilogue(a @ w.T)`` on wgmma. ``a`` [M,K] bf16, ``w`` [N,K] bf16 (nn.Linear layout).
 
     LINEAR: ``out = [resid +] scale * gelu?(a@w.T + bias) [+ rowadd[row % period]]``; bf16 or fp32 out.
     ROPE / SWIGLU: see include/visrag_b200.h.
@@ -121,7 +121,7 @@ def attention(
     head_dim: int, heads: int, batch: int, cu_k: torch.Tensor, max_k: int, cu_q: Optional[torch.Tensor], max_q: int,
     causal: bool, scale: float, out: torch.Tensor, v_ones_column: bool = False,
 ) -> torch.Tensor:
-    """softmax(QK^T*scale)V on tcgen05; q/k/v are bf16 token matrices (see include/visrag_b200.h)."""
+    """softmax(QK^T*scale)V on wgmma; q/k/v are bf16 token matrices (see include/visrag_b200.h)."""
     for t, n in ((q, "q"), (k, "k"), (v, "v"), (out, "out")):
         _bf16_2d(t, n)
     if cu_k.dtype != torch.int32 or (cu_q is not None and cu_q.dtype != torch.int32):

@@ -1,10 +1,10 @@
-"""Dense retrieval on the B200: drop-in for `src/openmatch/retriever/dense_retriever.py`.
+"""Dense retrieval on the H100: drop-in for `src/openmatch/retriever/dense_retriever.py`.
 
 Same call signatures and on-disk formats as the reference:
   * `_retrieve_one_shard(corpus_shard_path, encoded_queries_tensor, topk, device)` -> (scores, indices, lookup)
     (`dense_retriever.py:13-34`), shard file = `pickle((float32[n, d], List[str]))` (`inference/inference.py:126`);
   * `distributed_parallel_retrieve(args, topk)` -> {qid: {docid: score}} (`dense_retriever.py:37-97`).
-Underneath, `torch.matmul` + `torch.topk` are replaced by the fused tcgen05 filter + exact fp32 rescoring kernels
+Underneath, `torch.matmul` + `torch.topk` are replaced by the fused wgmma filter + exact fp32 rescoring kernels
 (csrc/score.cu): the returned scores are fp32 dot products and the top-k equals the fp32 scan's
 (order: score descending, then doc index ascending — `torch.topk` leaves tie order unspecified).
 
