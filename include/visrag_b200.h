@@ -70,8 +70,15 @@ int vr_gemm(const void* A, int64_t lda, const void* B, int64_t ldb, int32_t ab_d
 
 /* Same operation with the tile shape chosen by the caller (benchmarks, parity tests of every variant):
  *   block_n = 0    what vr_gemm picks: 128 x 64 tiles when M <= 128 (weight-streaming bound: more, narrower tiles), else
- *                  128 x 256, or 128 x 192 where 192 divides N and 256 does not (N = 1152), 128 x 128 for N < 256
- *   block_n = 256 / 192 / 128 / 64   token-major accumulator, 128 tokens x block_n features per tile
+ *                  the ping-pong kernel in CTA pairs (block_n = 4)
+ *   block_n = 2    ping-pong kernel: 128 x 128 tiles, each owned by one of two consumer warpgroups that take turns on the
+ *                  tensor cores, so one tile's epilogue runs under the next tile's MMAs; N tiles ordered in slices whose
+ *                  weight fits in L2
+ *   block_n = 4    the same in 2-CTA clusters: a pair takes two adjacent M tiles of one N tile and each CTA loads half of
+ *                  the B tile, multicast to both
+ *   block_n = 5    block_n = 2 with plain n-fastest tile order (measures what the L2 slices buy)
+ *   block_n = 256 / 192 / 128 / 64   cooperative kernel, token-major accumulator, 128 tokens x block_n features per tile
+ *                  (both consumer warpgroups share a tile and run its epilogue together)
  *   block_n = 3    feature-major accumulator (the weight tile is the MMA's M operand, 128 tokens are its N), LINEAR
  *                  epilogues only */
 int vr_gemm_tuned(const void* A, int64_t lda, const void* B, int64_t ldb, int32_t ab_dtype, int32_t M, int32_t N,

@@ -18,8 +18,9 @@ from visrag_b200 import retriever as R  # noqa: E402
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 PEAKS = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json"))) if os.path.exists(os.path.join(ROOT, "MEASURED_PEAKS.json")) else {}
-HBM = PEAKS.get("hbm_gbs_burst") or PEAKS.get("hbm_gbs") or 6586.0
-TF = PEAKS.get("bf16_tflops_burst") or PEAKS.get("bf16_tflops") or 1693.0
+# without measured peaks: the H100 SXM data sheet (3.35 TB/s HBM3, 989 TFLOP/s dense bf16, card allowed up to 700 W)
+HBM = PEAKS.get("hbm_gbs_burst") or PEAKS.get("hbm_gbs") or 3350.0
+TF = PEAKS.get("bf16_tflops_burst") or PEAKS.get("bf16_tflops") or 989.0
 
 
 def run(name, fn, bytes_alg, flops, a, flush):
@@ -33,7 +34,7 @@ def run(name, fn, bytes_alg, flops, a, flush):
         return
     tot = 0.0
     for _ in range(a.reps):
-        flush.add_(1.0)  # rewrites 256 MB: evicts the previous launch's lines from the 126 MB L2
+        flush.add_(1.0)  # rewrites 256 MB: evicts the previous launch's lines from the 50 MB L2
         e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
         e0.record()
         fn()

@@ -1,5 +1,5 @@
 """Device-resident step time of the full model for different batch shapes: pages per step x ViT sub-batch (tokens).
-Answers two layout questions with measurements: does a ViT sub-batch whose fp32 residual stream fits the 126 MB L2
+Answers two layout questions with measurements: does a ViT sub-batch whose fp32 residual stream fits the 50 MB L2
 beat the wave-quantisation loss of smaller GEMMs, and how much does a larger step amortise the LM tail.
   python tools/sweep_step.py [--pages 128,256] [--vit-tokens 16384,32768,65536,131072]"""
 import argparse

@@ -23,6 +23,46 @@ static int launch_gemm(const void* A, int64_t lda, const void* B, int64_t ldb, c
     return 0;
 }
 
+template <int MODE, bool OUT_F32, bool GELU, int CLUSTER>
+static int launch_pingpong(const void* A, int64_t lda, const void* B, int64_t ldb, const GemmArgs& g, bool l2_slices,
+                           cudaStream_t stream) {
+    CUtensorMap ta, tb;
+    if (int rc = make_tmap_2d(&ta, A, g.M, g.K, lda, GEMM_BM, GEMM_BK, 128, true)) return rc;
+    if (int rc = make_tmap_2d(&tb, B, g.N, g.K, ldb, 64, GEMM_BK, 128, true)) return rc;
+    auto kern = gemm_pingpong_kernel<MODE, OUT_F32, GELU, CLUSTER>;
+    cudaLaunchConfig_t cfg = {};
+    cudaLaunchAttribute attr[1];
+    cfg.blockDim = dim3(GEMM_THREADS);
+    cfg.dynamicSmemBytes = GEMM_PP_SMEM_BYTES;
+    cfg.stream = stream;
+    attr[0].id = cudaLaunchAttributeClusterDimension;
+    attr[0].val.clusterDim.x = CLUSTER;
+    attr[0].val.clusterDim.y = 1;
+    attr[0].val.clusterDim.z = 1;
+    cfg.attrs = attr;
+    cfg.numAttrs = 1;
+    // persistent grid: one CTA (pair) per resident slot, at most one per unit
+    static unsigned long long attr_set = 0;
+    static int max_clusters[64] = {};
+    const int dev = current_device(), dev_slot = dev >= 0 && dev < 64 ? dev : 0;
+    if (first_use_on_device(&attr_set)) {
+        VR_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, GEMM_PP_SMEM_BYTES));
+        int n = num_sms() / CLUSTER;
+        if (CLUSTER > 1) {
+            cfg.gridDim = dim3(num_sms() / CLUSTER * CLUSTER);
+            VR_CHECK_CUDA(cudaOccupancyMaxActiveClusters(&n, kern, &cfg));
+        }
+        max_clusters[dev_slot] = n;
+    }
+    const PPSched sch = pp_schedule(g.M, g.N, g.K, CLUSTER, l2_slices);
+    VR_REQUIRE(max_clusters[dev_slot] > 0, "vr_gemm: no %d-CTA cluster of the ping-pong kernel fits on this device", CLUSTER);
+    const int units = sch.num_units();
+    const int clusters = units < max_clusters[dev_slot] ? units : max_clusters[dev_slot];
+    cfg.gridDim = dim3(clusters * CLUSTER);
+    VR_CHECK_CUDA(cudaLaunchKernelEx(&cfg, kern, ta, tb, g, sch));
+    return 0;
+}
+
 // feature-major accumulator kernel (block_n == 3): LINEAR epilogues only
 static int dispatch_swapped(const void* A, int64_t lda, const void* B, int64_t ldb, const GemmArgs& g, cudaStream_t s) {
     const vr_gemm_epilogue& e = g.epi;
@@ -36,6 +76,15 @@ static int dispatch_swapped(const void* A, int64_t lda, const void* B, int64_t l
     return launch_gemm<128, VR_EPI_LINEAR, false, false, true>(A, lda, B, ldb, g, s);
 }
 
+// BN > 0: tile width of the cooperative kernel. BN < 0: the ping-pong kernel (128 x 128 tiles), as the block_n selector
+// -BN names it: PP (L2-sliced tile order), PP_NFAST (plain n-fastest order), PP_MC (CTA pairs with B multicast).
+constexpr int PP = 2, PP_MC = 4, PP_NFAST = 5;
+template <int BN, int MODE, bool OUT_F32, bool GELU>
+static int launch_any(const void* A, int64_t lda, const void* B, int64_t ldb, const GemmArgs& g, cudaStream_t s) {
+    if constexpr (BN < 0) return launch_pingpong<MODE, OUT_F32, GELU, -BN == PP_MC ? 2 : 1>(A, lda, B, ldb, g, -BN != PP_NFAST, s);
+    else return launch_gemm<BN, MODE, OUT_F32, GELU>(A, lda, B, ldb, g, s);
+}
+
 template <int BN>
 static int dispatch_mode(const void* A, int64_t lda, const void* B, int64_t ldb, const GemmArgs& g, cudaStream_t s) {
     const vr_gemm_epilogue& e = g.epi;
@@ -43,18 +92,18 @@ static int dispatch_mode(const void* A, int64_t lda, const void* B, int64_t ldb,
         case VR_EPI_LINEAR:
             if (e.out_dtype == VR_F32) {
                 VR_REQUIRE(!e.act_gelu, "vr_gemm: GELU epilogue writes bf16 only");
-                return launch_gemm<BN, VR_EPI_LINEAR, true, false>(A, lda, B, ldb, g, s);
+                return launch_any<BN, VR_EPI_LINEAR, true, false>(A, lda, B, ldb, g, s);
             }
             VR_REQUIRE(e.out_dtype == VR_BF16, "vr_gemm: out_dtype must be VR_BF16 or VR_F32");
-            if (e.act_gelu) return launch_gemm<BN, VR_EPI_LINEAR, false, true>(A, lda, B, ldb, g, s);
-            return launch_gemm<BN, VR_EPI_LINEAR, false, false>(A, lda, B, ldb, g, s);
+            if (e.act_gelu) return launch_any<BN, VR_EPI_LINEAR, false, true>(A, lda, B, ldb, g, s);
+            return launch_any<BN, VR_EPI_LINEAR, false, false>(A, lda, B, ldb, g, s);
         case VR_EPI_ROPE:
             VR_REQUIRE(e.positions && e.rope_cos && e.rope_sin, "vr_gemm: ROPE epilogue needs positions/cos/sin");
             VR_REQUIRE(g.N % 64 == 0 && e.rope_cols % 64 == 0, "vr_gemm: ROPE needs N and rope_cols multiples of 64");
-            return launch_gemm<BN, VR_EPI_ROPE, false, false>(A, lda, B, ldb, g, s);
+            return launch_any<BN, VR_EPI_ROPE, false, false>(A, lda, B, ldb, g, s);
         case VR_EPI_SWIGLU:
             VR_REQUIRE(g.N % 64 == 0, "vr_gemm: SWIGLU needs N multiple of 64");
-            return launch_gemm<BN, VR_EPI_SWIGLU, false, false>(A, lda, B, ldb, g, s);
+            return launch_any<BN, VR_EPI_SWIGLU, false, false>(A, lda, B, ldb, g, s);
         default:
             set_error("vr_gemm: unknown epilogue mode %d", e.mode);
             return 2;
@@ -80,17 +129,22 @@ extern "C" int vr_gemm_tuned(const void* A, int64_t lda, const void* B, int64_t 
     int bn = block_n;
     if (bn == 0) {
         // M <= 128 (a few queries): one row tile, the kernel only streams the weight - 64-wide feature tiles spread that
-        // stream over 4x as many SMs as 256-wide ones (o_proj 2304x2304: 36 CTAs instead of 9). Otherwise the widest tile
-        // (most reuse of the A rows per byte staged), except where 192 tiles N exactly and 256 does not (N = 1152:
-        // 6 x 192 instead of 4.5 x 256).
-        bn = M <= 128 ? 64 : (N < 256 ? 128 : ((N % 192 == 0 && N % 256 != 0) ? 192 : 256));
+        // stream over 4x as many SMs as 256-wide ones (o_proj 2304x2304: 36 CTAs instead of 9). Otherwise the ping-pong
+        // kernel in CTA pairs with the B tile multicast: one warpgroup's epilogue runs under the other's MMAs, and the
+        // pair reads 24 KB instead of 32 KB from L2 per stage. On H100 it was the fastest or tied on every GEMM class of
+        // the encode step (tools/bench_gemm.py); single-CTA ping-pong was slower than the cooperative kernel on
+        // mainloop-bound ones (gate|up, RoPE qkv).
+        bn = M <= 128 ? 64 : PP_MC;
     }
+    if (bn == PP) return dispatch_mode<-PP>(A, lda, B, ldb, g, s);
+    if (bn == PP_MC) return dispatch_mode<-PP_MC>(A, lda, B, ldb, g, s);
+    if (bn == PP_NFAST) return dispatch_mode<-PP_NFAST>(A, lda, B, ldb, g, s);
     if (bn == 3) return dispatch_swapped(A, lda, B, ldb, g, s);
     if (bn == 256) return dispatch_mode<256>(A, lda, B, ldb, g, s);
     if (bn == 192) return dispatch_mode<192>(A, lda, B, ldb, g, s);
     if (bn == 128) return dispatch_mode<128>(A, lda, B, ldb, g, s);
     if (bn == 64) return dispatch_mode<64>(A, lda, B, ldb, g, s);
-    set_error("vr_gemm: block_n must be 0 (auto), 64, 128, 192, 256 or 3 (feature-major accumulator)");
+    set_error("vr_gemm: block_n must be 0 (auto), 64, 128, 192, 256, 2 / 4 / 5 (ping-pong) or 3 (feature-major accumulator)");
     return 2;
 }
 

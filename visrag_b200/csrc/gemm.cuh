@@ -12,6 +12,10 @@
 // Two mbarrier arrays: smem full (TMA -> consumers, transaction bytes) and empty (8 consumer warps -> TMA).
 // Tiles are scheduled round-robin over a grid of min(#tiles, #SMs) CTAs, n-block fastest so
 // that CTAs running together share the same A rows in L2.
+//
+// gemm_pingpong_kernel (below) is the same pipeline with a different consumer schedule: each consumer warpgroup owns a
+// whole 128 x 128 tile and the two take turns on the tensor cores, so one tile's epilogue overlaps the next tile's
+// MMAs. vr_gemm uses it, in CTA pairs that share the B tile by multicast, for every problem with more than one row tile.
 #pragma once
 #include "ptx.cuh"
 #include "../../include/visrag_b200.h"
@@ -328,6 +332,266 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_const
             }
         }
     }
+}
+
+// ---------------------------------------------------------------------------------------
+// Ping-pong schedule: each consumer warpgroup owns a whole 128 x 128 tile (two m64n128k16 row halves per k16 step,
+// 128 accumulator registers per thread) and the CTA's tiles alternate between the two warpgroups (tile i of the CTA
+// goes to warpgroup 1 + i % 2). The producer fills one ring in tile order, so warpgroup w finds tile i's k-blocks at
+// ring position i * num_kb. The mainloops take turns through a named-barrier handoff: a warpgroup waits for its turn,
+// issues its whole k-loop, passes the turn on, and only then waits for its MMAs and runs its epilogue - so the epilogue
+// of one tile runs while the other warpgroup's MMAs of the next tile keep the tensor cores busy.
+constexpr int GEMM_PP_BN = 128;
+constexpr int GEMM_PP_A_BYTES = GEMM_BM * GEMM_BK * 2;
+constexpr int GEMM_PP_B_BYTES = GEMM_PP_BN * GEMM_BK * 2;
+constexpr int GEMM_PP_STAGE_BYTES = GEMM_PP_A_BYTES + GEMM_PP_B_BYTES;               // 32 KB
+constexpr int GEMM_PP_STAGES = (192 * 1024) / GEMM_PP_STAGE_BYTES;                    // 6
+constexpr int GEMM_PP_SMEM_BYTES = GEMM_PP_STAGES * GEMM_PP_STAGE_BYTES + 1024 + 256;  // + align slack + barriers
+constexpr int GEMM_PP_BAR_TURN = 1;  // named barriers 1 (warpgroup 1's turn) and 2 (warpgroup 2's turn); 0 is __syncthreads
+
+// Tile order. A wave of CTAs reads its weight tiles from L2 only if the weight columns it works on stay resident while
+// the wave sweeps down M. So the N tiles are cut into the fewest equal slices whose weight (128 rows x K bf16 per tile)
+// fits in GEMM_PP_L2_SLICE bytes - under half of the 50 MB L2, leaving room for the A rows in flight and the output
+// stream - and the tiles are ordered slice by slice, then by M row, N tile fastest. A wave then covers about
+// grid / slice_width M rows of one slice. Where the whole weight fits (all ViT GEMMs, LM o_proj) there is one slice
+// and this is plain n-fastest order; LM qkv (54 tiles) and down (18 tiles at K = 5760) take 2 slices, gate|up (90) 3,
+// so each weight tile is read from HBM about once per slice instead of once per M row of the wave.
+constexpr long long GEMM_PP_L2_SLICE = 20ll << 20;
+
+// The schedule works on units: a unit is CLUSTER vertically adjacent tiles of one N column (one tile without clusters,
+// the two tiles of a CTA pair with them). Computed on the host; slice_w = tiles_n gives plain n-fastest order.
+struct PPSched {
+    int units_m, tiles_n, slice_w;
+    __host__ __device__ int num_units() const { return units_m * tiles_n; }
+    // unit -> (M unit index, N tile index)
+    __device__ void coords(int u, int& um, int& tn) const {
+        const int slice_units = units_m * slice_w;
+        const int s = u / slice_units, r = u - s * slice_units;
+        const int w = min(slice_w, tiles_n - s * slice_w);  // the last slice may be narrower
+        um = r / w;
+        tn = s * slice_w + r % w;
+    }
+};
+
+inline PPSched pp_schedule(int M, int N, int K, int cluster, bool l2_slices) {
+    PPSched s;
+    s.units_m = ((M + GEMM_BM - 1) / GEMM_BM + cluster - 1) / cluster;
+    s.tiles_n = (N + GEMM_PP_BN - 1) / GEMM_PP_BN;
+    s.slice_w = s.tiles_n;
+    if (l2_slices) {
+        long long fit = GEMM_PP_L2_SLICE / (static_cast<long long>(GEMM_PP_BN) * K * 2);
+        if (fit < 1) fit = 1;
+        if (fit < s.tiles_n) {
+            const int slices = static_cast<int>((s.tiles_n + fit - 1) / fit);
+            s.slice_w = (s.tiles_n + slices - 1) / slices;
+        }
+    }
+    return s;
+}
+
+// LINEAR epilogue of one 64 x 128 row half, the same arithmetic as epi_linear2 in the same order. The output may be the
+// residual itself (in place), so the compiler cannot move a load above an earlier store: written pair by pair, every
+// fragment pair waits for a full memory round trip. Here the loads of PP_EPI_BATCH column groups (both rows) are
+// issued together before any of their stores - one round trip per batch.
+constexpr int PP_EPI_BATCH = 4;
+template <bool OUT_F32, bool GELU>
+__device__ __forceinline__ void pp_epilogue_linear(const GemmArgs& g, const float (&acc)[64], int r0, int n0, int q2) {
+    const vr_gemm_epilogue& e = g.epi;
+    const bool row_ok[2] = {r0 < g.M, r0 + 8 < g.M};
+    const long long o[2] = {static_cast<long long>(r0) * e.ldo, static_cast<long long>(r0 + 8) * e.ldo};
+    long long ra[2] = {0, 0};
+    if (e.rowadd) {
+        ra[0] = static_cast<long long>(r0 % e.rowadd_period) * g.N;
+        ra[1] = static_cast<long long>((r0 + 8) % e.rowadd_period) * g.N;
+    }
+#pragma unroll
+    for (int jb = 0; jb < GEMM_PP_BN / 8; jb += PP_EPI_BATCH) {
+        float2 bias[PP_EPI_BATCH], add[PP_EPI_BATCH][2], res[PP_EPI_BATCH][2];
+#pragma unroll
+        for (int j = 0; j < PP_EPI_BATCH; ++j) {
+            const int c = n0 + (jb + j) * 8 + q2;
+            const bool col_ok = c < g.N;
+            bias[j] = make_float2(0.0f, 0.0f);
+            if (e.bias && col_ok) bias[j] = __ldg(reinterpret_cast<const float2*>(e.bias + c));
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+                add[j][h] = res[j][h] = make_float2(0.0f, 0.0f);
+                if (e.rowadd && col_ok && row_ok[h]) add[j][h] = __ldg(reinterpret_cast<const float2*>(e.rowadd + ra[h] + c));
+                if (e.resid && col_ok && row_ok[h]) res[j][h] = *reinterpret_cast<const float2*>(e.resid + o[h] + c);
+            }
+        }
+#pragma unroll
+        for (int j = 0; j < PP_EPI_BATCH; ++j) {
+            const int c = n0 + (jb + j) * 8 + q2;
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+                if (!row_ok[h] || c >= g.N) continue;
+                float x0 = acc[4 * (jb + j) + 2 * h], x1 = acc[4 * (jb + j) + 2 * h + 1];
+                if (e.bias) { x0 += bias[j].x; x1 += bias[j].y; }
+                if (GELU) gelu_erf2(x0, x1);
+                if (e.scale != 1.0f) { x0 *= e.scale; x1 *= e.scale; }
+                if (e.rowadd) { x0 += add[j][h].x; x1 += add[j][h].y; }
+                if (e.resid) { x0 += res[j][h].x; x1 += res[j][h].y; }
+                if (OUT_F32) *reinterpret_cast<float2*>(reinterpret_cast<float*>(e.out) + o[h] + c) = make_float2(x0, x1);
+                else *reinterpret_cast<uint32_t*>(reinterpret_cast<__nv_bfloat16*>(e.out) + o[h] + c) = pack_bf16x2(x0, x1);
+            }
+        }
+    }
+}
+
+// epilogue of one 64 x 128 row half: accumulator rows r0 and r0 + 8, columns n0 + 8 j + q2 (+1), q2 = 2 (lane % 4)
+template <int MODE, bool OUT_F32, bool GELU>
+__device__ __forceinline__ void pp_epilogue(const GemmArgs& g, const float (&acc)[64], int r0, int n0, int q2) {
+    if (MODE == VR_EPI_LINEAR) {
+        pp_epilogue_linear<OUT_F32, GELU>(g, acc, r0, n0, q2);
+    } else {
+        // 64-column blocks (a RoPE head / a gate|up pair): columns c and c + 32 sit in the same thread
+#pragma unroll
+        for (int hb = 0; hb < GEMM_PP_BN / 64; ++hb) {
+#pragma unroll
+            for (int j = 0; j < 4; ++j) {
+                const int lo = 4 * (hb * 8 + j), hi = 4 * (hb * 8 + j + 4);
+                const int blk0 = n0 + hb * 64, c = j * 8 + q2;
+                if (MODE == VR_EPI_ROPE) {
+                    epi_rope2(g, r0, blk0, c, acc[lo], acc[lo + 1], acc[hi], acc[hi + 1]);
+                    epi_rope2(g, r0 + 8, blk0, c, acc[lo + 2], acc[lo + 3], acc[hi + 2], acc[hi + 3]);
+                } else {
+                    epi_swiglu2(g, r0, blk0, c, acc[lo], acc[lo + 1], acc[hi], acc[hi + 1]);
+                    epi_swiglu2(g, r0 + 8, blk0, c, acc[lo + 2], acc[lo + 3], acc[hi + 2], acc[hi + 3]);
+                }
+            }
+        }
+    }
+}
+
+// CLUSTER = 2: CTA pairs take M tiles 2u and 2u + 1 of the same N tile. Each CTA loads its own A box and one 64-row
+// half of the shared B tile, multicast to both CTAs, so each CTA stages its full 32 KB stage while it reads only 24 KB
+// from L2. A stage is refilled only when the consumers of BOTH CTAs are done with it (the partner's producer writes
+// into it too): every consumer warp arrives on the empty barrier of both CTAs. Both CTAs walk the same unit sequence,
+// so their rings stay in step. With an odd number of M tiles the last pair's second tile lies past M: TMA fills it
+// with zeros (the bytes still count) and the epilogue's row guard drops it.
+template <int MODE, bool OUT_F32, bool GELU, int CLUSTER>
+__global__ void __launch_bounds__(GEMM_THREADS, 1)
+gemm_pingpong_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b, const GemmArgs g,
+                     const PPSched sch) {
+    static_assert(CLUSTER == 1 || CLUSTER == 2, "CTA pairs at most");
+    constexpr int STAGES = GEMM_PP_STAGES;
+    extern __shared__ uint8_t smem_raw[];
+    uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
+    uint8_t* smem_a = smem;
+    uint8_t* smem_b = smem + STAGES * GEMM_PP_A_BYTES;
+    uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + STAGES * GEMM_PP_STAGE_BYTES);
+    uint64_t* empty_bar = full_bar + STAGES;
+
+    const int wg = threadIdx.x >> 7;
+    const int warp = (threadIdx.x >> 5) & 3;
+    const int lane = threadIdx.x & 31;
+    const int num_kb = (g.K + GEMM_BK - 1) / GEMM_BK;
+    const int rank = CLUSTER == 1 ? 0 : static_cast<int>(cluster_ctarank());
+    const int unit0 = blockIdx.x / CLUSTER, unit_step = gridDim.x / CLUSTER;  // the pair's units: unit0 + k unit_step
+    const int num_units = sch.num_units();
+
+    if (threadIdx.x == 0) {
+        tma_prefetch_desc(&tmap_a);
+        tma_prefetch_desc(&tmap_b);
+        for (int i = 0; i < STAGES; ++i) {
+            mbar_init(&full_bar[i], 1);
+            mbar_init(&empty_bar[i], 4 * CLUSTER);  // each warp of the owning warpgroup, in every CTA of the cluster
+        }
+        fence_mbar_init();  // release at cluster scope: the partner arrives on these barriers and multicasts into them
+    }
+    if (CLUSTER == 1) __syncthreads();
+    else cluster_sync_all();  // both CTAs' barriers are initialised before either issues a multicast or remote arrive
+
+    if (wg == 0) {
+        // ------------------------------------------------------------ TMA producer: the CTA's tiles in order
+        setmaxnreg_dec<40>();
+        if (warp == 0 && lane == 0) {
+            int stage = 0;
+            uint32_t phase = 0;
+            for (int u = unit0; u < num_units; u += unit_step) {
+                int um, tn;
+                sch.coords(u, um, tn);
+                const int m0 = (um * CLUSTER + rank) * GEMM_BM, n0 = tn * GEMM_PP_BN;
+                for (int kb = 0; kb < num_kb; ++kb) {
+                    mbar_wait(&empty_bar[stage], phase ^ 1);
+                    mbar_expect_tx(&full_bar[stage], GEMM_PP_STAGE_BYTES);
+                    // rows past the matrix (A or B) read as zeros and count their bytes
+                    tma_load_2d(&tmap_a, &full_bar[stage], smem_a + stage * GEMM_PP_A_BYTES, kb * GEMM_BK, m0);
+                    uint8_t* b_dst = smem_b + stage * GEMM_PP_B_BYTES;
+                    if (CLUSTER == 1) {
+#pragma unroll
+                        for (int h = 0; h < GEMM_PP_BN / 64; ++h)
+                            tma_load_2d(&tmap_b, &full_bar[stage], b_dst + h * (64 * GEMM_BK * 2), kb * GEMM_BK, n0 + h * 64);
+                    } else {
+                        tma_load_2d_multicast(&tmap_b, &full_bar[stage], b_dst + rank * (64 * GEMM_BK * 2), kb * GEMM_BK,
+                                              n0 + rank * 64, 0x3);
+                    }
+                    if (++stage == STAGES) { stage = 0; phase ^= 1; }
+                }
+            }
+        }
+    } else {
+        // ------------------------------------------------------------ consumers: tiles i = wg - 1, wg + 1, ...
+        setmaxnreg_inc<232>();
+        const int me = wg - 1;
+        const uint64_t desc_hi = make_smem_desc(0, 16, 1024, kLayoutSW128);
+        const uint32_t a_lo0 = smem_u32(smem_a) >> 4, b_lo0 = smem_u32(smem_b) >> 4;
+        constexpr uint32_t HALF = (64 * GEMM_BK * 2) >> 4;  // rows 64..127 of the A stage
+        const int g8 = lane >> 2, q = lane & 3;
+        // release a stage: one arrival per warp on the empty barrier of every CTA of the cluster
+        auto release = [&](int s) {
+            if (lane != 0) return;
+            if (CLUSTER == 1) {
+                mbar_arrive(&empty_bar[s]);
+            } else {
+#pragma unroll
+                for (int r = 0; r < CLUSTER; ++r) mbar_arrive_cluster(&empty_bar[s], r);
+            }
+        };
+        for (int i = me, u = unit0 + me * unit_step; u < num_units; i += 2, u += 2 * unit_step) {
+            const int pos = i * num_kb;  // ring position of this tile's first k-block
+            int stage = pos % STAGES;
+            uint32_t phase = (pos / STAGES) & 1;
+            if (i > 0) named_bar_sync(GEMM_PP_BAR_TURN + me, 256);  // the previous tile's MMAs are all issued
+            float acc0[64], acc1[64];  // rows 0..63 and 64..127 of the tile
+            int prev = -1;
+            for (int kb = 0; kb < num_kb; ++kb) {
+                mbar_wait(&full_bar[stage], phase);
+                const uint64_t ad = desc_hi | static_cast<uint64_t>(a_lo0 + stage * (GEMM_PP_A_BYTES >> 4));
+                const uint64_t bd = desc_hi | static_cast<uint64_t>(b_lo0 + stage * (GEMM_PP_B_BYTES >> 4));
+                wgmma_fence();
+#pragma unroll
+                for (int kk = 0; kk < 4; ++kk) {
+                    wgmma_ss<false, false>(acc0, ad + 2 * kk, bd + 2 * kk, (kb | kk) != 0, std::integral_constant<int, 128>());
+                    wgmma_ss<false, false>(acc1, ad + HALF + 2 * kk, bd + 2 * kk, (kb | kk) != 0,
+                                           std::integral_constant<int, 128>());
+                }
+                wgmma_commit();
+                if (prev >= 0) {
+                    wgmma_wait<1>();
+                    release(prev);
+                }
+                prev = stage;
+                if (++stage == STAGES) { stage = 0; phase ^= 1; }
+            }
+            // pass the turn on only if the CTA has a next tile: every arrive then meets exactly one bar.sync
+            if (u + unit_step < num_units) named_bar_arrive(GEMM_PP_BAR_TURN + (me ^ 1), 256);
+            wgmma_wait<0>();
+            release(prev);
+            wgmma_touch(acc0);
+            wgmma_touch(acc1);
+
+            int um, tn;
+            sch.coords(u, um, tn);
+            const int m0 = (um * CLUSTER + rank) * GEMM_BM, n0 = tn * GEMM_PP_BN;
+            pp_epilogue<MODE, OUT_F32, GELU>(g, acc0, m0 + warp * 16 + g8, n0, q * 2);
+            pp_epilogue<MODE, OUT_F32, GELU>(g, acc1, m0 + 64 + warp * 16 + g8, n0, q * 2);
+        }
+    }
+    // The partner may still multicast into this CTA's ring or arrive on its barriers until it has drained its own
+    // work: neither CTA exits before both are done.
+    if (CLUSTER == 2) cluster_sync_all();
 }
 
 }  // namespace vr

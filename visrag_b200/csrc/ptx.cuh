@@ -108,6 +108,23 @@ __device__ __forceinline__ void tma_load_2d(const CUtensorMap* m, uint64_t* bar,
         : "memory");
 }
 
+// Same load written to the same smem offset of every CTA in cta_mask (bit r = cluster rank r); each destination CTA's
+// mbarrier at `bar`'s offset receives the box's bytes.
+__device__ __forceinline__ void tma_load_2d_multicast(const CUtensorMap* m, uint64_t* bar, void* smem_dst, int c0, int c1,
+                                                      uint16_t cta_mask) {
+    asm volatile(
+        "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes.multicast::cluster"
+        " [%0], [%1, {%3, %4}], [%2], %5;" ::"r"(smem_u32(smem_dst)),
+        "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "h"(cta_mask)
+        : "memory");
+}
+// arrive on the mbarrier at `bar`'s offset in CTA `rank` of the cluster. Default (CTA-scope release) semantics: the
+// arrivals that use it hand back a shared-memory stage whose only readers were retired wgmma instructions, so there
+// is no generic-proxy write to publish, and a cluster-scope release would cost a GPU-wide fence per arrival.
+__device__ __forceinline__ void mbar_arrive_cluster(uint64_t* bar, uint32_t rank) {
+    asm volatile("mbarrier.arrive.shared::cluster.b64 _, [%0];" ::"r"(mapa_u32(smem_u32(bar), rank)) : "memory");
+}
+
 // ---------------------------------------------------------------- warpgroup MMA (wgmma)
 // Shared-memory matrix descriptor:
 //   [0,14)  start address >> 4      [16,30) leading byte offset >> 4
@@ -212,6 +229,10 @@ __device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.
 
 __device__ __forceinline__ void named_bar_sync(int id, int threads) {
     asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(threads) : "memory");
+}
+// signal a named barrier without waiting on it (the other side of a one-way handoff does bar.sync)
+__device__ __forceinline__ void named_bar_arrive(int id, int threads) {
+    asm volatile("bar.arrive %0, %1;" ::"r"(id), "r"(threads) : "memory");
 }
 
 // ---------------------------------------------------------------- misc
