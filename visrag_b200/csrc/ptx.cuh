@@ -236,6 +236,13 @@ __device__ __forceinline__ void named_bar_arrive(int id, int threads) {
 }
 
 // ---------------------------------------------------------------- misc
+// 2^x on the MUFU, one instruction (exp2f is the non-ftz form: a range test and two scalings around the same MUFU.EX2).
+// Results below 2^-126 flush to zero; relative error 2^-22 as for exp2f.
+__device__ __forceinline__ float ex2_ftz(float x) {
+    float y;
+    asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
+    return y;
+}
 __device__ __forceinline__ uint32_t pack_bf16x2(float lo, float hi) {
     __nv_bfloat162 v = __floats2bfloat162_rn(lo, hi);
     return *reinterpret_cast<uint32_t*>(&v);
