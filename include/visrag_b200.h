@@ -113,7 +113,8 @@ int vr_resample_u8(const uint8_t* src, int32_t src_pixel_bytes, int32_t n, int32
 /* ------------------------------------------------------------------------------------
  * Fused softmax(Q K^T * scale) V on wgmma. S, P (bf16, register A operand of the second MMA), running max / sum and the
  * O accumulator all live in registers. Sequences longer than 64 queries: two consumer warpgroups (128 queries) per CTA
- * share one K/V stream; up to 64 queries per sequence: one warpgroup per CTA.
+ * share one K/V stream; up to 64 queries per sequence: one warpgroup per CTA. Both forms (and vr_attention_force_v1)
+ * give a sequence the same output bits: it does not depend on max_q, on the other sequences of the batch or on the form.
  * Replaces F.scaled_dot_product_attention in timm/models/vision_transformer.py:92-96 (ViT,
  * 16 heads x 72, no mask), modeling_minicpm.py:895-903 (MiniCPM, causal + right padding ->
  * here: packed var-len sequences, no padding rows at all) and nn.MultiheadAttention in
@@ -182,7 +183,8 @@ int vr_build_lm_input(const int32_t* src, int32_t tokens, int32_t dim, const voi
  * per packed sequence b (rows cu[b]..cu[b+1]) of h [tokens, dim] fp32 -> reps [batch, dim] fp32.
  * pooling: 0 wmean (w_t = t+1), 1 mean, 2 lasttoken, 3 cls. normalise: x / max(||x||, 1e-12).
  * One thread-block cluster of 8 (or 4) CTAs per sequence, every row read once; h, gamma and reps 16-byte aligned; any
- * sequence length (no per-length shared memory), dim <= 4096. */
+ * sequence length (no per-length shared memory), dim <= 4096. A sequence's sums run in one fixed order whatever the
+ * cluster size, so its output bits do not depend on the batch size or on the other sequences of the batch. */
 int vr_pool_norm(const float* h, int64_t ldh, const float* gamma, float eps, const int32_t* cu, int32_t batch, int32_t dim,
                  int32_t pooling, int32_t normalize, float* reps, void* stream);
 
@@ -215,7 +217,8 @@ int vr_score_filter(const void* q_f16, int32_t nq, const void* d_f16, int64_t nd
 int vr_score_rescore(const float* q_f32, int32_t nq, const float* d_f32, int64_t nd, int32_t dim, int32_t ranges,
                      const float* cand_scores, const int32_t* cand_ids, const float* max_doc_norm, int32_t k,
                      int64_t id_offset, float* out_scores, int64_t* out_ids, int32_t* flags, void* stream);
-/* plain fp32 scan (small problems, flagged queries): scores [nq, nd] */
+/* plain fp32 scan (small problems, flagged queries): scores [nq, nd], any nq. A score has the same bits as the one
+ * vr_score_rescore computes for the same (query, doc) pair (same FMA order and reduction). */
 int vr_score_exact(const float* q_f32, int32_t nq, const float* d_f32, int64_t nd, int32_t dim, float* scores, void* stream);
 /* top-k of every row of scores [rows, cols]; ids == NULL -> column index (+ id_offset), else ids[row, col]
  * (negative ids are skipped): also the k-way merge of per-shard / per-rank partial top-k lists. */

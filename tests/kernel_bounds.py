@@ -305,6 +305,71 @@ def build_lm_input_ref(src, embed, scale_emb, vision):
 
 
 # ----------------------------------------------------------------------------------------------------------------------
+# Final RMSNorm + pooling + L2 normalise (elementwise.cu pool_norm_kernel), per sequence over its weighted rows t:
+#   ss_t:   sum of squares as in the norms: a lane sums ceil(D/128) float4 groups (x^2 + y^2) + (z^2 + w^2) serially, then
+#           the 5-level shuffle tree: depth ceil(D/128) + 8 with the products, so ss^ = ss (1 + d), |d| <= G U.
+#   r_t:    rsqrtf(ss / D + eps): the division and the add round once each, rsqrt.approx adds 2^-22 (PTX). With
+#           rho = (ss/D) / (ss/D + eps) only the ss part of the argument carries d:
+#           dr/r <= rho (G + 1) U / 2 + U / 2 + 2^-22  (half the argument's relative error, plus rsqrt's own).
+#   sc_t:   w_t r_t, w_t = t + 1 (wmean) or 1, an integer exact in fp32: one more U.
+#   A:      sum_t sc_t x_t. A warp adds its rows serially (one product and one add per row, or one FMA), ceil(n/32) rows
+#           at most; then 3 adds over the CTA's 4 warps and 8 over the virtual ranks (0 + the first is exact):
+#           |dA_c| <= sum_t |sc_t x_tc| (dsc_t + U) + (ceil(n/32) + 11) U sum_t |sc_t x_tc|,  dsc_t = dr_t/r_t + U.
+#   p:      A_c gamma_c / W: a product and an IEEE division (2 U |p|). W = sum w_t is exact in fp32 for n <= 5792
+#           (n (n + 1) < 2^25 and even).
+#   norm:   sq = sum_c p_c^2 per thread over ceil(D/512) float4 groups, the shuffle tree and 4 warps serially: depth
+#           ceil(D/512) + 11 (G2 U relative), plus 2 sum_c |p_c| |dp_c| from p's error; sqrtf and 1 / max(., 1e-12) are
+#           IEEE (U each), so 1/N^ is off by sum|p||dp| / N^2 + (G2 / 2 + 2) U relative; the product p / N rounds once more.
+#           y = p / N moves by |dp_c| / N + |y_c| (relative error of 1/N). Second-order terms are covered by 1e-3 of slack.
+#   An empty sequence is written as zeros, and an all-zero one pools to p = 0 and y = 0 (the max(N, 1e-12) guard).
+# ----------------------------------------------------------------------------------------------------------------------
+POOL_VRANKS = 8
+
+
+def pool_norm_ref(h, gamma, eps, cu, pooling, normalize):
+    """ops.pool_norm in float64: h [T, D] fp32 (any row pitch), gamma [D], cu [B + 1]. Returns (ref, e) [B, D]."""
+    D = gamma.numel()
+    g = gamma.double()
+    eps32 = float(np.float32(eps))
+    G = -(-D // 128) + 8
+    G2 = -(-D // 512) + 11
+    cu = [int(c) for c in cu.tolist()]
+    B = len(cu) - 1
+    ref = torch.zeros(B, D, dtype=torch.float64, device=h.device)
+    err = torch.zeros_like(ref)
+    for b in range(B):
+        n = cu[b + 1] - cu[b]
+        if n <= 0:
+            continue
+        t_lo, t_hi = {"lasttoken": (n - 1, n), "cls": (0, 1)}.get(pooling, (0, n))
+        X = h[cu[b] + t_lo:cu[b] + t_hi, :D].double()
+        m = t_hi - t_lo
+        w = torch.arange(t_lo + 1, t_hi + 1, dtype=torch.float64, device=h.device) if pooling == "wmean" else \
+            torch.ones(m, dtype=torch.float64, device=h.device)
+        ms = (X * X).sum(1) / D
+        r = torch.rsqrt(ms + eps32)
+        rho = ms / (ms + eps32)
+        dsc = rho * (G + 1) * U / 2 + U / 2 + 2.0 ** -22 + U          # + U: the product w r
+        Y = (w * r)[:, None] * X
+        aY = Y.abs()
+        eA = (aY * (dsc + U)[:, None]).sum(0) + (-(-m // 32) + 11) * U * aY.sum(0)
+        W = float(w.sum())
+        p = Y.sum(0) * g / W
+        ep = g.abs() * eA / W + 2 * U * p.abs()
+        if not normalize:
+            ref[b], err[b] = p, ep * (1 + 1e-3)
+            continue
+        N = float(p.norm())
+        if N == 0.0:
+            continue
+        y = p / max(N, 1e-12)
+        dinv = float((p.abs() * ep).sum()) / N ** 2 + (G2 / 2 + 2) * U
+        ref[b] = y
+        err[b] = (ep / N + y.abs() * (dinv + U)) * (1 + 1e-3)
+    return ref, err
+
+
+# ----------------------------------------------------------------------------------------------------------------------
 # The checker
 # ----------------------------------------------------------------------------------------------------------------------
 

@@ -168,21 +168,53 @@ def test_vision_tower_and_resampler_against_oracle():
             assert close(out, O.resampler_forward(sd, cfg, want, gh, gw), 3e-2), s.shape
 
 
+def _short_queries(n):
+    words = ["cat", "tax", "map", "2020", "dog", "sofa", "chart", "x"]
+    return [" ".join(words[(i + j) % len(words)] for j in range(1 + i % 5)) for i in range(n)]
+
+
 def test_batch_composition_does_not_change_results():
-    """Same item alone vs inside a mixed batch: bit-identical (no padding, no cross-sequence leakage)."""
+    """Same item alone vs inside a mixed batch: bit-identical (no padding, no cross-sequence leakage). The batch decides
+    which attention kernel runs (longest sequence <= 64 or not), the cluster size of the final pooling (more than
+    5 x #SMs / 8 sequences or not) and whether a CUDA graph replays; none of that may change an embedding."""
     from visrag_b200.config import VisRAGConfig
     from visrag_b200.encoder import VisRAGEngine
     from visrag_b200.tokenizer_stub import StubTokenizer
     from visrag_b200.weights import random_state_dict
 
     cfg = VisRAGConfig.tiny()
-    eng = VisRAGEngine(cfg, random_state_dict(cfg, 5))
+    sd = random_state_dict(cfg, 5)
+    eng = VisRAGEngine(cfg, sd)
+    eager = VisRAGEngine(cfg, sd, cuda_graphs=False)
     tok = StubTokenizer(cfg.vocab)
     pages = synth_pages([(448, 448), (700, 900), (448, 448)], 9)
     alone = eng.encode([""], [pages[1]], tok)
     mixed = eng.encode(["", "", "query text", ""], [pages[0], pages[1], None, pages[2]], tok)
     assert torch.equal(alone[0], mixed[1])
     assert eng.encode([], [], tok).shape == (0, cfg.hidden)
+    # short text queries (<= 64 LM tokens, prefix included): alone, next to a longer query, next to pages
+    short = ["cat", QUERY_PREFIX + "tax", "revenue table 2020", QUERY_PREFIX + "2020"]
+    assert all(len(tok.encode(q)) < 64 for q in short)
+    long_q = QUERY_PREFIX + " ".join(["word"] * 30)
+    assert len(tok.encode(long_q)) > 64
+    for e in (eng, eager):
+        for qi, q in enumerate(short):
+            alone = e.encode([q], [None], tok)[0]
+            with_long = e.encode([long_q, q], [None, None], tok)[1]
+            with_pages = e.encode(["", q, ""], [pages[0], None, pages[2]], tok)[1]
+            assert torch.equal(alone, with_long) and torch.equal(alone, with_pages), (q, e.cuda_graphs)
+    # 128 pages in one batch (eager: more LM tokens than a graph takes) and in batches of 16
+    many = synth_pages([(224, 224)] * 128, 10)
+    whole = eng.encode([""] * 128, many, tok)
+    parts = torch.cat([eng.encode([""] * 16, many[i:i + 16], tok) for i in range(0, 128, 16)])
+    assert torch.equal(whole, parts), (whole - parts).abs().max().item()
+    # 128 short queries in one batch (small enough for a CUDA graph) and in batches of 16, graphs on and off
+    qs = _short_queries(128)
+    for e in (eng, eager):
+        whole = e.encode(qs, [None] * 128, tok)
+        parts = torch.cat([e.encode(qs[i:i + 16], [None] * 16, tok) for i in range(0, 128, 16)])
+        assert torch.equal(whole, parts), (e.cuda_graphs, (whole - parts).abs().max().item())
+    assert eng.graph_stats["captured"] + eng.graph_stats["replayed"] > 0
 
 
 def test_encode_stream_equals_blocking_calls():
@@ -214,6 +246,12 @@ def test_encode_stream_equals_blocking_calls():
     assert [len(ids) for ids, _ in out] == [17, 2] and out[0][0] == [d["id"] for d in big[:17]]
     want = model(passage=I.naive_collator(big[:17]), **kw).p_reps.cpu().numpy()
     assert np.array_equal(out[0][1], want)
+    # queries, first batch of 100 (above the 5 x #SMs / 8 sequences where pooling changes cluster size) cut in 4 pieces
+    qs = [{"id": f"q{i}", "text": t, "image": None} for i, t in enumerate(_short_queries(130))]
+    out = list(I.encode_stream(I._batches(qs, 100), model, kw, ramp_parts=4))
+    assert [len(ids) for ids, _ in out] == [100, 30]
+    for (ids, got), batch in zip(out, I._batches(qs, 100)):
+        assert np.array_equal(got, model(query=batch, **kw).q_reps.cpu().numpy())
 
 
 def test_config1_pipeline_encode_shards_retrieve_trec_metrics(tmp_path):

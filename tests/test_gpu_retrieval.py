@@ -289,3 +289,103 @@ def test_filter_candidate_lists_cover_every_query_block_piece(nq, nd, d):
         kth = np.sort(approx[r])[-kt]
         must = set(np.nonzero(approx[r] > kth + 1e-4)[0].tolist())  # clear members of the approximate top-16
         assert must <= have
+
+
+# ------------------------------------------------------------------------------------------------------------------------
+# The top-k does not depend on the path that answers it (tensor-core filter + exact rescoring, or the plain fp32 scan), on
+# the other queries of the batch, or on how the corpus is sharded: the same scores and ids, bit for bit. The rescoring
+# kernel and the fp32 scan sum a dot product in the same lane-strided FMA order and the same butterfly.
+
+
+def _topk(Q, idx, k, **kw):
+    return R.score_topk(torch.from_numpy(Q).cuda() if isinstance(Q, np.ndarray) else Q, idx, k, **kw)
+
+
+def _assert_same(a, b, what):
+    (sa, ia), (sb, ib) = a, b
+    assert torch.equal(ia, ib), (what, int((ia != ib).sum()))
+    assert torch.equal(sa, sb), (what, float((sa - sb).abs().max()))
+
+
+def _corpora():
+    rs = np.random.RandomState(31)
+    yield "random", _unit(rs, 1000, 2304), _unit(rs, 10000, 2304), [10]
+    base = _unit(rs, 3000, 128)
+    yield "exact duplicates", _unit(rs, 2000, 128), np.concatenate([base, base[:500]]), [10]
+    D = _unit(rs, 40000, 128)
+    Q = _unit(rs, 1500, 128)
+    for qi in range(5):                               # the clustered corpus: the filter flags these, the fp32 scan answers
+        pert = Q[qi] + rs.randn(40, 128).astype(np.float32) * 1e-4
+        D[5000 + 300 * qi: 5040 + 300 * qi] = pert / np.linalg.norm(pert, axis=1, keepdims=True)
+    yield "clustered", Q, D, [10]
+    yield "k 17 to 300", _unit(rs, 500, 256), _unit(rs, 20000, 256), [17, 64, 300]
+    D = rs.randn(8000, 256).astype(np.float32)
+    Q = rs.randn(700, 256).astype(np.float32)
+    Q[5] *= 1e6
+    yield "fp16-overflow query", Q, D, [10]
+    Dbig = D.copy()
+    Dbig[17] *= 1e6
+    yield "fp16-overflow document", Q, Dbig, [10]
+
+
+def test_filter_path_equals_the_exact_scan_bit_for_bit():
+    for name, Q, D, ks in _corpora():
+        idx = R.build_index(D)
+        for k in ks:
+            stats = {}
+            got = _topk(Q, idx, k, stats=stats)
+            assert stats["path"] == "filter+rescore", (name, stats)
+            _assert_same(got, _topk(Q, idx, k, force_exact=True), f"{name} k={k}")
+
+
+def test_one_query_alone_equals_the_same_query_in_a_batch():
+    """Alone, one query over 20000 docs takes the fp32 scan with the chunked top-k; in a batch of 2000 it takes the filter."""
+    rs = np.random.RandomState(12)
+    Q, D = _unit(rs, 2000, 256), _unit(rs, 20000, 256)
+    idx = R.build_index(D)
+    batch = _topk(Q, idx, 10)
+    for r in (0, 777, 1999):
+        _assert_same(_topk(Q[r:r + 1], idx, 10), (batch[0][r:r + 1], batch[1][r:r + 1]), f"query {r}")
+
+
+def test_three_shards_merged_equal_the_unsharded_index():
+    """sharded_topk on one GPU: each shard's top-k with its global id offset, then merge_topk."""
+    rs = np.random.RandomState(13)
+    Q, D = _unit(rs, 500, 256), _unit(rs, 30001, 256)
+    D[20000] = D[3]                                   # a tie across shards: the lower global id wins
+    q = torch.from_numpy(Q).cuda()
+    want = _topk(q, R.build_index(D), 10)
+    parts = []
+    for r in range(3):
+        lo, hi = R.shard_range(len(D), r, 3)
+        parts.append(_topk(q, R.build_index(D[lo:hi]), 10, id_offset=lo))
+    got = R.merge_topk(torch.cat([p[0] for p in parts], 1), torch.cat([p[1] for p in parts], 1), 10)
+    _assert_same(got, want, "3 shards")
+
+
+def test_knowledge_base_one_query_equals_a_batch_of_100(tmp_path):
+    from visrag_b200 import knowledge_base as KBase
+
+    rs = np.random.RandomState(14)
+    D = _unit(rs, 50000, 256)
+    KBase.save_knowledge_base(str(tmp_path), D, [f"p{i}.png" for i in range(len(D))])
+    kb = KBase.KnowledgeBase(str(tmp_path))
+    Q = _unit(rs, 100, 256)
+    s, i = kb.search(Q, 7)
+    for r in (0, 42, 99):
+        _assert_same(kb.search(Q[r:r + 1], 7), (s[r:r + 1], i[r:r + 1]), f"query {r}")
+
+
+def test_exact_scan_takes_more_than_65535_query_blocks():
+    """8 x 65535 + 9 queries: more query blocks of the fp32 scan than one launch's grid.y holds. The index needs a
+    dimension divisible by 8; with 3 docs this is 17 MB of queries."""
+    nq = 8 * 65535 + 9
+    g = torch.Generator(device="cuda").manual_seed(15)
+    q = torch.randn(nq, 8, device="cuda", generator=g)
+    idx = R.build_index(torch.randn(3, 8, device="cuda", generator=g))
+    stats = {}
+    whole = _topk(q, idx, 2, stats=stats)
+    assert stats["path"] == "exact"
+    h = nq // 2
+    a, b = _topk(q[:h].contiguous(), idx, 2), _topk(q[h:].contiguous(), idx, 2)
+    _assert_same(whole, (torch.cat([a[0], b[0]]), torch.cat([a[1], b[1]])), "two halves")

@@ -368,3 +368,140 @@ def test_bf16_cell_is_the_rounding_interval():
     eps = g.double().abs() * 2.0 ** -20          # above fp32 resolution: the nudged values are exact in fp32
     assert torch.equal((lo + eps).float().bfloat16(), g) and torch.equal((hi - eps).float().bfloat16(), g)
     assert ((lo - eps).float().bfloat16() != g).all() and ((hi + eps).float().bfloat16() != g).all()
+
+
+# ---------------------------------------------------------------------------------------------------------- pool_norm
+
+
+def _butterfly(v):
+    """warp_sum over the last axis (32 lanes): xor-shuffle tree, fp32."""
+    lanes = np.arange(32)
+    for off in (16, 8, 4, 2, 1):
+        v = (v + v[..., lanes ^ off]).astype(np.float32)
+    return v[..., 0]
+
+
+def _sum_sq_f32(x, per_lane):
+    """Sum of squares of the rows of x [m, D] as the kernel's lanes take it: float4 f = lane + 32 * per_lane_index
+    (pool rows: 32 lanes; the final norm: 128 threads = 4 warps), each float4 as (x^2 + y^2) + (z^2 + w^2), serially."""
+    m, D = x.shape
+    threads = 32 * per_lane
+    steps = -(-D // (4 * threads))
+    xp = np.zeros((m, steps * threads * 4), np.float32)
+    xp[:, :D] = x
+    q = (xp * xp).reshape(m, steps, threads, 4)
+    grp = ((q[..., 0] + q[..., 1]).astype(np.float32) + (q[..., 2] + q[..., 3]).astype(np.float32)).astype(np.float32)
+    acc = np.zeros((m, threads), np.float32)
+    for i in range(steps):
+        acc = (acc + grp[:, i]).astype(np.float32)
+    return acc.reshape(m, per_lane, 32)
+
+
+def emu_pool_norm(h, gamma, eps, cu, pooling, normalize, mut=None):
+    """pool_norm_kernel in fp32, in its order: 8 virtual ranks of 4 warps, warp slot 4v + w takes rows t_lo + 4v + w + 32k."""
+    h, g = h.numpy().astype(np.float32), gamma.numpy().astype(np.float32)
+    D = g.size
+    eps32 = np.float32(eps)
+    out = np.zeros((len(cu) - 1, D), np.float32)
+    with np.errstate(divide="ignore", invalid="ignore"):     # the mutants' 1/0 and 0/0 become inf / NaN, as on the GPU
+        for b in range(len(cu) - 1):
+            out[b] = _emu_pool_seq(h, g, eps32, int(cu[b]), int(cu[b + 1]), pooling, normalize, mut)
+    return torch.from_numpy(out)
+
+
+def _emu_pool_seq(h, g, eps32, r0, r1, pooling, normalize, mut):
+    D = g.size
+    n = r1 - r0
+    if n <= 0:
+        return np.zeros(D, np.float32)
+    t_lo, t_hi = {"lasttoken": (n - 1, n), "cls": (0, 1)}.get(pooling, (0, n))
+    if mut == "lasttoken reads row len - 2" and pooling == "lasttoken":
+        t_lo, t_hi = n - 2, n - 1
+    X = h[r0 + t_lo:r0 + t_hi, :D]
+    m = X.shape[0]
+    ss = _butterfly(_sum_sq_f32(X, 1)[:, 0])
+    ms = (ss / np.float32(D)).astype(np.float32)
+    if mut != "eps omitted":
+        ms = (ms + eps32).astype(np.float32)
+    r = (1.0 / np.sqrt(ms.astype(np.float64))).astype(np.float32)
+    t = np.arange(t_lo, t_hi)
+    w = (t + (0 if mut == "weights t instead of t + 1" else 1)).astype(np.float32) if pooling == "wmean" else np.ones(m, np.float32)
+    sc = (w * r).astype(np.float32)
+    Y = np.zeros((-(-m // 32) * 32, D), np.float32)
+    Y[:m] = (sc[:, None] * X).astype(np.float32)
+    acc = np.zeros((32, D), np.float32)
+    for k in range(Y.shape[0] // 32):
+        acc = (acc + Y[32 * k:32 * k + 32]).astype(np.float32)
+        if mut == "accumulator rounded to bf16":
+            acc = torch.from_numpy(acc).bfloat16().float().numpy()
+    total = np.zeros(D, np.float32)
+    for v in range(KB.POOL_VRANKS):
+        part = acc[4 * v]
+        for wv in range(1, 4):
+            part = (part + acc[4 * v + wv]).astype(np.float32)
+        if not (mut == "one virtual rank's partial dropped" and v == KB.POOL_VRANKS - 1):
+            total = (total + part).astype(np.float32)
+    nf = np.float32(m)
+    W = (np.float32(0.5) * nf * (nf + np.float32(1))).astype(np.float32) if pooling == "wmean" else nf
+    if mut == "sum of weights off by one":
+        W = np.float32(W + 1)
+    p = ((total * g).astype(np.float32) / W).astype(np.float32)
+    inv = np.float32(1)
+    if normalize:
+        warps = _butterfly(_sum_sq_f32(p[None], 4)[0])
+        sq = np.float32(0)
+        for s in warps:
+            sq = np.float32(sq + s)
+        nrm = np.float32(np.sqrt(sq))
+        inv = np.float32(1) / (nrm if mut == "norm guard removed" else max(nrm, np.float32(1e-12)))
+    return (p * inv).astype(np.float32)
+
+
+POOL_EPS = 1e-5
+POOL_LENS = [0, 1, 2, 17, 33, 300, 40]
+
+
+def _pool_data(D):
+    """Rows of the LM's last residual stream: O(1) rows, rows with mean square ~ eps next to them (so a missing or doubled
+    eps changes their weight against the others; a uniform scale error would cancel in the L2 normalisation), |h| ~ 1e3
+    rows, and one all-zero sequence (the last)."""
+    T = sum(POOL_LENS)
+    x = _randn(T, D, seed=D)
+    x[1::3] *= POOL_EPS ** 0.5
+    x[2::7] = _randn(len(range(2, T, 7)), D, scale=1e3, seed=D + 1)
+    x[T - POOL_LENS[-1]:] = 0.0
+    cu = torch.tensor([0] + list(np.cumsum(POOL_LENS)), dtype=torch.int32)
+    return x, _randn(D, seed=D + 2), cu
+
+
+POOL_MUTANTS = [
+    ("eps omitted", "wmean", True),
+    ("weights t instead of t + 1", "wmean", True),
+    ("sum of weights off by one", "mean", False),
+    ("lasttoken reads row len - 2", "lasttoken", True),
+    ("one virtual rank's partial dropped", "mean", True),
+    ("accumulator rounded to bf16", "wmean", True),
+    ("norm guard removed", "wmean", True),
+]
+
+
+@pytest.mark.parametrize("D", [64, 576, 2304])
+@pytest.mark.parametrize("normalize", [True, False], ids=["l2", "raw"])
+@pytest.mark.parametrize("pooling", ["wmean", "mean", "lasttoken", "cls"])
+def test_pool_norm_faithful_emulation_passes(pooling, normalize, D):
+    x, g, cu = _pool_data(D)
+    _check(f"pool_norm {pooling} {normalize} D={D}", emu_pool_norm(x, g, POOL_EPS, cu, pooling, normalize),
+           *KB.pool_norm_ref(x, g, POOL_EPS, cu, pooling, normalize))
+
+
+@pytest.mark.parametrize("D", [64, 2304])
+@pytest.mark.parametrize("mut,pooling,normalize", POOL_MUTANTS, ids=[m for m, _, _ in POOL_MUTANTS])
+def test_pool_norm_mutant_fails(mut, pooling, normalize, D):
+    x, g, cu = _pool_data(D)
+    got = emu_pool_norm(x, g, POOL_EPS, cu, pooling, normalize, mut)
+    ref, e = KB.pool_norm_ref(x, g, POOL_EPS, cu, pooling, normalize)
+    fin = torch.isfinite(got).all(1)
+    need = (got.double() - ref)[fin].abs()
+    frac = float(torch.where(need == 0, torch.zeros_like(need), need / e[fin].clamp_min(1e-300)).max())
+    print(f"pool_norm mutant '{mut}' D={D}: {frac:.3g} x the bound on finite rows, {int((~fin).sum())} non-finite rows")
+    _fails(lambda: _check(f"pool_norm {mut}", got, ref, e))

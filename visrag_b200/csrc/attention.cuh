@@ -20,6 +20,9 @@
 // At head stride 128 (no caller in the model has more than 64 queries there), O, S and P of this form would not fit the
 // register budget together, so that stride keeps the sequential per-tile loop for both warpgroups.
 // NWG = 1 is the kernel for sequences of up to 64 queries (the resampler's 64 learned queries).
+// Both loops run the same arithmetic per query row: the same S MMAs, the same masked att_softmax_tile, O rescaled by alpha
+// before P V is added, and the same store. Key tiles past a row's causal limit change nothing (alpha = 1, p = 0). So a
+// sequence's output does not depend on which form ran it, and hence not on max_q or on the other sequences of the batch.
 //
 // Head dims that are not multiples of 64 (ViT: 72, stored padded to 80 with zero columns) are
 // split into a 64-wide 128B-swizzled chunk plus a 16-wide 32B-swizzled chunk, each with its own
@@ -413,48 +416,25 @@ attention_wgmma_kernel(const __grid_constant__ AttMaps maps, const AttArgs a) {
             if (lane == 0) mbar_arrive(&k_empty[st]);
             wgmma_touch(s);
 
-            // ---- softmax on the fragments: registers 4j+0/1 = row a, 4j+2/3 = row b, keys 8j + 2 q4 + 0/1
+            // ---- softmax on the fragments: masked scores -> -inf, then the same arithmetic as the pipelined form, so a
+            // sequence gets the same bits from either form (and from either side of the max_q <= 64 dispatch)
             const int key0 = kt * ATT_BN;
             int lim_a = len_k - key0, lim_b = lim_a;  // keys [0, lim) of this tile exist for the row
             if (CAUSAL) {
                 lim_a = min(lim_a, row_a + causal_shift - key0 + 1);
                 lim_b = min(lim_b, row_b + causal_shift - key0 + 1);
             }
-            float mt_a = -INFINITY, mt_b = -INFINITY;
 #pragma unroll
             for (int j = 0; j < 16; ++j) {
 #pragma unroll
                 for (int e = 0; e < 2; ++e) {
                     const int key = j * 8 + q4 * 2 + e;
-                    if (key < lim_a) mt_a = fmaxf(mt_a, s[4 * j + e]);
-                    if (key < lim_b) mt_b = fmaxf(mt_b, s[4 * j + 2 + e]);
+                    s[4 * j + e] = key < lim_a ? s[4 * j + e] : -INFINITY;
+                    s[4 * j + 2 + e] = key < lim_b ? s[4 * j + 2 + e] : -INFINITY;
                 }
             }
-            mt_a = fmaxf(mt_a, __shfl_xor_sync(0xffffffffu, mt_a, 1));
-            mt_a = fmaxf(mt_a, __shfl_xor_sync(0xffffffffu, mt_a, 2));
-            mt_b = fmaxf(mt_b, __shfl_xor_sync(0xffffffffu, mt_b, 1));
-            mt_b = fmaxf(mt_b, __shfl_xor_sync(0xffffffffu, mt_b, 2));
-            const float mn_a = fmaxf(m_a, mt_a), mn_b = fmaxf(m_b, mt_b);
-            const float mu_a = (mn_a == -INFINITY) ? 0.f : mn_a, mu_b = (mn_b == -INFINITY) ? 0.f : mn_b;
-            const float alpha_a = exp2f((m_a - mu_a) * a.scale_log2), alpha_b = exp2f((m_b - mu_b) * a.scale_log2);  // m = -inf -> 0
-            m_a = mn_a;
-            m_b = mn_b;
-            float lt_a = 0.f, lt_b = 0.f;  // this thread's part of the row sums (reduced over the quad at the end)
-#pragma unroll
-            for (int j = 0; j < 16; ++j) {
-#pragma unroll
-                for (int e = 0; e < 2; ++e) {
-                    const int key = j * 8 + q4 * 2 + e;
-                    const float pa = key < lim_a ? exp2f((s[4 * j + e] - mu_a) * a.scale_log2) : 0.f;
-                    const float pb = key < lim_b ? exp2f((s[4 * j + 2 + e] - mu_b) * a.scale_log2) : 0.f;
-                    s[4 * j + e] = pa;
-                    s[4 * j + 2 + e] = pb;
-                    lt_a += pa;
-                    lt_b += pb;
-                }
-            }
-            l_a = l_a * alpha_a + lt_a;
-            l_b = l_b * alpha_b + lt_b;
+            float alpha_a, alpha_b;
+            att_softmax_tile(s, a.scale_log2, m_a, m_b, l_a, l_b, alpha_a, alpha_b);
             // ---- O = O * alpha + P V
 #pragma unroll
             for (int c = 0; c < NCH; ++c)

@@ -325,22 +325,28 @@ __global__ void build_lm_input_kernel(const int* __restrict__ src, int tokens, i
 
 // ---------------------------------------------------------------------------------------------
 // Final RMSNorm + pooling + L2 normalise: one thread-block CLUSTER of 8 (or 4) CTAs per sequence, every row read from HBM once.
-//   phase 1: the cluster's warps take the weighted rows round-robin; a warp holds its row in registers (VPL float4
-//            per lane), computes 1/rms and adds w_t/rms_t * x_t into its private register accumulator;
-//   phase 2: the 4 warps of a CTA are summed through shared memory (fixed order -> deterministic);
-//   phase 3: after a cluster barrier CTA 0 sums the partial vectors over distributed shared memory, applies
-//            gamma / sum(w), reduces the squared norm, normalises and writes the embedding.
+// The sum order is fixed by 8 virtual ranks of 4 warps each, whatever the cluster size: warp w of virtual rank v takes
+// the weighted rows t_lo + 4v + w + 32k in increasing k. An 8-CTA cluster runs virtual rank v in CTA v; a 4-CTA cluster
+// runs virtual ranks r and r + 4 in CTA r, one after the other, into two partial vectors. So the embedding's bits do
+// not depend on the cluster size, i.e. on the batch size, nor on which other sequences share the launch.
+//   phase 1: a warp holds one row in registers (VPL float4 per lane), computes 1/rms and adds w_t/rms_t * x_t into its
+//            accumulator (its shared-memory staging row), one row after the other;
+//   phase 2: the virtual rank's partial = ((warp 0 + warp 1) + warp 2) + warp 3, per column through shared memory;
+//   phase 3: after a cluster barrier CTA 0 sums the 8 partials in virtual-rank order over distributed shared memory,
+//            applies gamma / sum(w), reduces the squared norm, normalises and writes the embedding.
 // pooling: 0 = wmean (w_t = t+1), 1 = mean, 2 = lasttoken, 3 = cls (dense_retrieval_model.py:170-218).
 // ---------------------------------------------------------------------------------------------
 constexpr int POOL_THREADS = 128;  // 4 warps x ~164 registers: three CTAs per SM (256 threads left one)
 constexpr int POOL_WARPS = POOL_THREADS / 32;
-constexpr int POOL_MAX_CLUSTER = 8;  // CTAs per sequence: 8, or 4 when that lets every cluster be resident at once
+constexpr int POOL_VRANKS = 8;  // virtual ranks per sequence; the cluster has 8 CTAs, or 4 when that lets every cluster be resident at once
 
 template <int VPL, bool EXACT>
 __global__ void __launch_bounds__(POOL_THREADS, VPL <= 18 ? 5 : 2)
 pool_norm_kernel(const float* __restrict__ h, long long ldh, const float* __restrict__ gamma, float eps,
                  const int* __restrict__ cu, int dim, int pooling, int normalize, float* __restrict__ reps) {
-    extern __shared__ __align__(16) float pool_smem[];  // [POOL_WARPS][VPL*128] staging, reused as the CTA's partial vector
+    // [POOL_WARPS][VPL*128] staging, reused as the partial of the CTA's last virtual rank; with 4 CTAs one more [VPL*128]
+    // holds the partial of its first
+    extern __shared__ __align__(16) float pool_smem[];
     __shared__ float red[POOL_WARPS];
     __shared__ float total;
     constexpr int COLS = VPL * 128;
@@ -362,39 +368,45 @@ pool_norm_kernel(const float* __restrict__ h, long long ldh, const float* __rest
     // the warp's accumulator lives in its shared-memory staging row (registers hold one input row: ~100 per thread,
     // five CTAs per SM; with a register accumulator it was 164 and three)
     float4* stage = reinterpret_cast<float4*>(pool_smem) + warp * (COLS / 4);
+    float4* first = reinterpret_cast<float4*>(pool_smem) + POOL_WARPS * (COLS / 4);  // 4-CTA cluster: partial of virtual rank `rank`
+    for (int v = static_cast<int>(rank); v < POOL_VRANKS; v += static_cast<int>(csize)) {
+        const bool last = v + static_cast<int>(csize) >= POOL_VRANKS;
 #pragma unroll
-    for (int i = 0; i < VPL; ++i) stage[lane + i * 32] = make_float4(0.f, 0.f, 0.f, 0.f);
-    for (int t = t_lo + static_cast<int>(rank) * POOL_WARPS + warp; t < t_hi; t += static_cast<int>(csize) * POOL_WARPS) {
-        const float4* xr = reinterpret_cast<const float4*>(h + static_cast<long long>(begin + t) * ldh);
-        float4 v[VPL];
+        for (int i = 0; i < VPL; ++i) stage[lane + i * 32] = make_float4(0.f, 0.f, 0.f, 0.f);
+        for (int t = t_lo + v * POOL_WARPS + warp; t < t_hi; t += POOL_VRANKS * POOL_WARPS) {
+            const float4* xr = reinterpret_cast<const float4*>(h + static_cast<long long>(begin + t) * ldh);
+            float4 x[VPL];
 #pragma unroll
-        for (int i = 0; i < VPL; ++i) {
-            const int c = lane + i * 32;
-            v[i] = (EXACT || c < nvec) ? __ldcs(xr + c) : make_float4(0.f, 0.f, 0.f, 0.f);
+            for (int i = 0; i < VPL; ++i) {
+                const int c = lane + i * 32;
+                x[i] = (EXACT || c < nvec) ? __ldcs(xr + c) : make_float4(0.f, 0.f, 0.f, 0.f);
+            }
+            float ss = 0.f;
+#pragma unroll
+            for (int i = 0; i < VPL; ++i) ss += (x[i].x * x[i].x + x[i].y * x[i].y) + (x[i].z * x[i].z + x[i].w * x[i].w);
+            ss = warp_sum(ss);
+            const float w = (pooling == 0) ? static_cast<float>(t + 1) : 1.0f;
+            const float sc = w * rsqrtf(ss / static_cast<float>(dim) + eps);
+#pragma unroll
+            for (int i = 0; i < VPL; ++i) {
+                float4 a = stage[lane + i * 32];
+                a.x += sc * x[i].x; a.y += sc * x[i].y; a.z += sc * x[i].z; a.w += sc * x[i].w;
+                stage[lane + i * 32] = a;
+            }
         }
-        float ss = 0.f;
+        __syncthreads();
+        // partial of virtual rank v: column-wise sum over the warps, written over warp 0's staging area (last) or `first`
+        float4* dst = last ? reinterpret_cast<float4*>(pool_smem) : first;
+        for (int c = threadIdx.x; c < COLS / 4; c += POOL_THREADS) {
+            float4 s4 = reinterpret_cast<const float4*>(pool_smem)[c];
 #pragma unroll
-        for (int i = 0; i < VPL; ++i) ss += (v[i].x * v[i].x + v[i].y * v[i].y) + (v[i].z * v[i].z + v[i].w * v[i].w);
-        ss = warp_sum(ss);
-        const float w = (pooling == 0) ? static_cast<float>(t + 1) : 1.0f;
-        const float sc = w * rsqrtf(ss / static_cast<float>(dim) + eps);
-#pragma unroll
-        for (int i = 0; i < VPL; ++i) {
-            float4 a = stage[lane + i * 32];
-            a.x += sc * v[i].x; a.y += sc * v[i].y; a.z += sc * v[i].z; a.w += sc * v[i].w;
-            stage[lane + i * 32] = a;
+            for (int wv = 1; wv < POOL_WARPS; ++wv) {
+                const float4 o = reinterpret_cast<const float4*>(pool_smem)[wv * (COLS / 4) + c];
+                s4.x += o.x; s4.y += o.y; s4.z += o.z; s4.w += o.w;
+            }
+            dst[c] = s4;  // column c of warp 0's area is read only by this thread
         }
-    }
-    __syncthreads();
-    // CTA partial: column-wise sum over the warps, written over warp 0's staging area
-    for (int c = threadIdx.x; c < COLS / 4; c += POOL_THREADS) {
-        float4 s4 = reinterpret_cast<const float4*>(pool_smem)[c];
-#pragma unroll
-        for (int wv = 1; wv < POOL_WARPS; ++wv) {
-            const float4 o = reinterpret_cast<const float4*>(pool_smem)[wv * (COLS / 4) + c];
-            s4.x += o.x; s4.y += o.y; s4.z += o.z; s4.w += o.w;
-        }
-        reinterpret_cast<float4*>(pool_smem)[c] = s4;  // column c of warp 0's area is read only by this thread
+        if (!last) __syncthreads();  // the staging rows are zeroed again for the next virtual rank
     }
     cluster_sync_all();
     if (rank == 0) {
@@ -409,8 +421,9 @@ pool_norm_kernel(const float* __restrict__ h, long long ldh, const float* __rest
             const int c = threadIdx.x + k * POOL_THREADS;
             float4 s4 = make_float4(0.f, 0.f, 0.f, 0.f);
             if (c < nvec) {
-                for (unsigned r = 0; r < csize; ++r) {
-                    const float4 o = ld_shared_cluster_f4(mapa_u32(my + c * 16, r));
+                for (unsigned v = 0; v < POOL_VRANKS; ++v) {  // virtual rank v's partial: CTA v % csize, `first` unless it is that CTA's last
+                    const uint32_t off = v + csize >= POOL_VRANKS ? 0u : POOL_WARPS * COLS * 4u;
+                    const float4 o = ld_shared_cluster_f4(mapa_u32(my + off + c * 16, v % csize));
                     s4.x += o.x; s4.y += o.y; s4.z += o.z; s4.w += o.w;
                 }
                 const float4 g = reinterpret_cast<const float4*>(gamma)[c];
@@ -557,8 +570,9 @@ extern "C" int vr_pool_norm(const float* h, int64_t ldh, const float* gamma, flo
                "vr_pool_norm: h, gamma and reps must be 16-byte aligned");
     cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
     // 8 CTAs per sequence while all clusters fit on the GPU at once (5 CTAs per SM), else 4: one wave of longer CTAs beats
-    // a second wave of whole clusters (the kernel is a latency chain: load rows -> CTA sum -> cluster sum -> normalise)
-    const unsigned csize = static_cast<long long>(batch) * POOL_MAX_CLUSTER <= static_cast<long long>(num_sms()) * 5 ? POOL_MAX_CLUSTER : 4;
+    // a second wave of whole clusters (the kernel is a latency chain: load rows -> CTA sum -> cluster sum -> normalise).
+    // Both sum in the same order (virtual ranks), so the choice does not change the result.
+    const unsigned csize = static_cast<long long>(batch) * POOL_VRANKS <= static_cast<long long>(num_sms()) * 5 ? POOL_VRANKS : POOL_VRANKS / 2;
     cudaLaunchConfig_t cfg = {};
     cfg.gridDim = dim3(static_cast<unsigned>(batch) * csize);
     cfg.blockDim = dim3(POOL_THREADS);
@@ -570,11 +584,12 @@ extern "C" int vr_pool_norm(const float* h, int64_t ldh, const float* gamma, flo
     cfg.numAttrs = 1;
 #define VR_POOL_LAUNCH(VPL, EXACT)                                                                                        \
     do {                                                                                                                  \
-        const int smem = POOL_WARPS * (VPL) * 128 * static_cast<int>(sizeof(float));                                      \
+        const int row_bytes = (VPL) * 128 * static_cast<int>(sizeof(float));                                              \
         static unsigned long long configured = 0;                                                                         \
         if (first_use_on_device(&configured))                                                                             \
-            VR_CHECK_CUDA(cudaFuncSetAttribute(pool_norm_kernel<VPL, EXACT>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem)); \
-        cfg.dynamicSmemBytes = smem;                                                                                      \
+            VR_CHECK_CUDA(cudaFuncSetAttribute(pool_norm_kernel<VPL, EXACT>, cudaFuncAttributeMaxDynamicSharedMemorySize,  \
+                                               (POOL_WARPS + 1) * row_bytes));                                            \
+        cfg.dynamicSmemBytes = (POOL_WARPS + (csize < POOL_VRANKS ? 1 : 0)) * row_bytes;                                  \
         VR_CHECK_CUDA(cudaLaunchKernelEx(&cfg, pool_norm_kernel<VPL, EXACT>, h, static_cast<long long>(ldh), gamma, eps, cu, dim, \
                                          pooling, normalize, reps));                                                      \
     } while (0)

@@ -804,21 +804,29 @@ extern "C" int vr_score_exact(const float* q_f32, int32_t nq, const float* d_f32
     long long bx = (nd + 8 * EX_DW - 1) / (8 * EX_DW);
     const long long cap = static_cast<long long>(num_sms()) * 3;
     if (bx > cap) bx = cap;
-    dim3 grid(static_cast<unsigned>(bx), (nq + NQ - 1) / NQ);
     cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+    // grid.y is one query block of NQ; past 65535 blocks the queries go in several launches (a query's scores do not
+    // depend on which launch, or which block, computes them)
+    const int chunk = 65535 * NQ;
+    for (int q0 = 0; q0 < nq; q0 += chunk) {
+        const int n = nq - q0 < chunk ? nq - q0 : chunk;
+        const float* q = q_f32 + static_cast<long long>(q0) * dim;
+        float* out = scores + static_cast<long long>(q0) * nd;
+        dim3 grid(static_cast<unsigned>(bx), (n + NQ - 1) / NQ);
 #define VR_EXACT_LAUNCH(N)                                                                                               \
     do {                                                                                                                 \
         static unsigned long long attr_set = 0;                                                                          \
         if (smem > 48 * 1024 && first_use_on_device(&attr_set))                                                          \
             VR_CHECK_CUDA(cudaFuncSetAttribute(exact_scores_kernel<N>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024)); \
-        exact_scores_kernel<N><<<grid, 256, smem, st>>>(q_f32, nq, d_f32, nd, dim, scores);                              \
+        exact_scores_kernel<N><<<grid, 256, smem, st>>>(q, n, d_f32, nd, dim, out);                                      \
     } while (0)
-    if (NQ == EX_QB) VR_EXACT_LAUNCH(EX_QB);
-    else if (NQ == 4) VR_EXACT_LAUNCH(4);
-    else if (NQ == 2) VR_EXACT_LAUNCH(2);
-    else VR_EXACT_LAUNCH(1);
+        if (NQ == EX_QB) VR_EXACT_LAUNCH(EX_QB);
+        else if (NQ == 4) VR_EXACT_LAUNCH(4);
+        else if (NQ == 2) VR_EXACT_LAUNCH(2);
+        else VR_EXACT_LAUNCH(1);
 #undef VR_EXACT_LAUNCH
-    VR_CHECK_CUDA(cudaGetLastError());
+        VR_CHECK_CUDA(cudaGetLastError());
+    }
     return 0;
 }
 
