@@ -39,18 +39,23 @@ int vr_abi_version(void);
  *   timm/layers/patch_embed.py:87 (patch conv), timm/models/vision_transformer.py:88,105
  *   (qkv, proj), timm/layers/mlp.py:41-49 (fc1+GELU, fc2), resampler.py:154,159-167,
  *   modeling_minicpm.py:850-852,908 (q,k,v,o), modeling_minicpm.py:333 (SwiGLU MLP).
- * A and B are bf16 (VR_BF16) or fp16 (VR_F16); K*2 bytes and lda/ldb*2 bytes must be
- * multiples of 16 (TMA); N must be a multiple of 8.
+ * A and B are both bf16 (ab_dtype = VR_BF16) or both fp16 (VR_F16); K*2 bytes and lda/ldb*2 bytes must be
+ * multiples of 16 (TMA); N must be a multiple of 8. Every block_n selector runs both operand types; the accumulator,
+ * bias, residual, row add and RoPE tables are fp32 either way. Output types:
+ *   bf16 operands: LINEAR writes VR_BF16 or VR_F32 (out_dtype); ROPE / SWIGLU write bf16 (out_dtype is not read);
+ *   fp16 operands: LINEAR writes VR_F16 or VR_F32; ROPE / SWIGLU write fp16 and need out_dtype = VR_F16;
+ *   GELU writes the operands' 16-bit type only. Any other combination is refused before any CUDA call.
+ * An fp16 output rounds to nearest with no clamp: a value beyond 65504 is stored as inf.
  * ---------------------------------------------------------------------------------- */
 typedef enum {
     VR_EPI_LINEAR = 0, /* out = [resid +] scale*(gelu?(acc + bias)) [+ rowadd[row % period]] */
-    VR_EPI_ROPE = 1,   /* MiniCPM q|k|v: rotate-half RoPE on 64-wide heads in columns < rope_cols; bf16 out */
-    VR_EPI_SWIGLU = 2  /* B rows interleaved [32 gate | 32 up] per 64: out[:, j] = silu(g_j)*u_j; bf16, N/2 cols */
+    VR_EPI_ROPE = 1,   /* MiniCPM q|k|v: rotate-half RoPE on 64-wide heads in columns < rope_cols; 16-bit out */
+    VR_EPI_SWIGLU = 2  /* B rows interleaved [32 gate | 32 up] per 64: out[:, j] = silu(g_j)*u_j; 16-bit, N/2 cols */
 } vr_epi_mode;
 
 typedef struct {
     int32_t mode;          /* vr_epi_mode */
-    int32_t out_dtype;     /* VR_BF16 or VR_F32 (LINEAR); others write bf16 */
+    int32_t out_dtype;     /* LINEAR: VR_F32 or the operands' type; ROPE / SWIGLU: VR_F16 with fp16 operands, else unread */
     int32_t act_gelu;      /* LINEAR: exact erf-GELU applied to (acc + bias) */
     float scale;           /* LINEAR: multiplies the activation before the residual add */
     const float* bias;     /* [N] fp32 or NULL */
@@ -119,7 +124,7 @@ int vr_resample_u8(const uint8_t* src, int32_t src_pixel_bytes, int32_t n, int32
  * 16 heads x 72, no mask), modeling_minicpm.py:895-903 (MiniCPM, causal + right padding ->
  * here: packed var-len sequences, no padding rows at all) and nn.MultiheadAttention in
  * resampler.py:159-163 (64 learned queries x N keys, 18 heads x 128).
- * q/k/v are bf16 row-major token matrices; head h starts at column *_col0 + h*head_stride
+ * q/k/v are bf16 (or, with VR_ATTN_F16, fp16) row-major token matrices; head h starts at column *_col0 + h*head_stride
  * (head_stride = head_dim rounded up to a multiple of 16; pad columns must hold zeros).
  * ---------------------------------------------------------------------------------- */
 typedef struct {
@@ -135,7 +140,7 @@ typedef struct {
     int32_t max_q, max_k;     /* longest query / key sequence (grid sizing) */
     int32_t causal;
     float scale;
-    void* out; int64_t ldo;   /* bf16; row = cu_q ? cu_q[b]+i : b*max_q+i ; head h at column h*head_dim */
+    void* out; int64_t ldo;   /* bf16 (fp16 with VR_ATTN_F16); row = cu_q ? cu_q[b]+i : b*max_q+i ; head h at column h*head_dim */
     int32_t flags;            /* VR_ATTN_* */
 } vr_attn_params;
 
@@ -144,6 +149,11 @@ typedef struct {
  * the accumulator) instead of summing P in registers; the sm_90a kernels sum P in registers (it is already there) and
  * ignore the column. Results are the same up to fp32 summation order. */
 #define VR_ATTN_V_ONES_COLUMN 1
+/* q, k, v and out are fp16 instead of bf16. P (the softmax numerators, <= 1) is rounded to fp16 for the P.V MMA with
+ * round-to-nearest and no flush: p below 2^-14 become fp16 subnormals, not zeros. S, the running max / sum, alpha and the
+ * O accumulator stay fp32 and run the same arithmetic as the bf16 form, so the batch-invariance statement above holds for
+ * fp16 too (the same bits from either form and any batch). */
+#define VR_ATTN_F16 2
 
 int vr_attention(const vr_attn_params* p, void* stream);
 /* test / benchmark hook (process-wide): 0 = default dispatch, 1 = always the one-warpgroup (64 queries per CTA) kernel */
@@ -162,15 +172,26 @@ void vr_attention_force_v1(int32_t variant);
  * pixel rows must fit 200 KB of shared memory (w up to ~4800 for patch 14). */
 int vr_im2col_norm(const uint8_t* pixels, int32_t n_slices, int32_t h, int32_t w, int32_t patch, void* out, int64_t ldo,
                    void* stream);
+/* The same with the output type chosen: out_dtype = VR_BF16 (what vr_im2col_norm writes) or VR_F16, where
+ * fp16(fma(u, 2/255, -1)) is likewise bit-identical to fp16((u/255 - 0.5)/0.5) for all 256 byte values. */
+int vr_im2col_norm_ex(const uint8_t* pixels, int32_t n_slices, int32_t h, int32_t w, int32_t patch, void* out, int64_t ldo,
+                      int32_t out_dtype, void* stream);
 
 /* LayerNorm over the last dim (timm vision_transformer.py:142,155,525; resampler.py:155,166): fp32 in -> bf16 out.
  * If out2 != NULL also writes out2 = LN(x) + add[row % add_period] (bf16) — the resampler's K input (kv + pos). */
 int vr_layernorm(const float* x, int64_t ldx, const float* gamma, const float* beta, float eps, int32_t rows, int32_t dim,
                  void* out, int64_t ldo, void* out2, const float* add, int32_t add_period, void* stream);
+/* vr_layernorm with out and out2 written as out_dtype = VR_BF16 (vr_layernorm) or VR_F16; mean, variance and the add of
+ * out2 stay fp32, and only the stores round. */
+int vr_layernorm_ex(const float* x, int64_t ldx, const float* gamma, const float* beta, float eps, int32_t rows, int32_t dim,
+                    void* out, int64_t ldo, void* out2, const float* add, int32_t add_period, int32_t out_dtype, void* stream);
 
 /* RMSNorm (modeling_minicpm.py:119-123): fp32 in -> bf16 out. */
 int vr_rmsnorm(const float* x, int64_t ldx, const float* gamma, float eps, int32_t rows, int32_t dim, void* out, int64_t ldo,
                void* stream);
+/* vr_rmsnorm with out written as out_dtype = VR_BF16 (vr_rmsnorm) or VR_F16; statistics in fp32. */
+int vr_rmsnorm_ex(const float* x, int64_t ldx, const float* gamma, float eps, int32_t rows, int32_t dim, void* out, int64_t ldo,
+                  int32_t out_dtype, void* stream);
 
 /* LM input assembly (modeling_minicpmv.py:139-166): for packed token t,
  *   src[t] >= 0 : h[t] = vision[src[t]]            (resampler output row, fp32)
@@ -178,6 +199,10 @@ int vr_rmsnorm(const float* x, int64_t ldx, const float* gamma, float eps, int32
  * h: [tokens, dim] fp32. */
 int vr_build_lm_input(const int32_t* src, int32_t tokens, int32_t dim, const void* embed_bf16, float scale_emb,
                       const float* vision, int64_t ldv, float* h, int64_t ldh, void* stream);
+/* vr_build_lm_input with the embedding table's type given: embed_dtype = VR_BF16 (vr_build_lm_input) or VR_F16. Either is
+ * widened to fp32 exactly and multiplied by scale_emb in fp32; h is fp32. */
+int vr_build_lm_input_ex(const int32_t* src, int32_t tokens, int32_t dim, const void* embed, int32_t embed_dtype,
+                         float scale_emb, const float* vision, int64_t ldv, float* h, int64_t ldh, void* stream);
 
 /* Final RMSNorm + pooling + L2 normalise (modeling_minicpm.py:1280; dense_retrieval_model.py:170-223):
  * per packed sequence b (rows cu[b]..cu[b+1]) of h [tokens, dim] fp32 -> reps [batch, dim] fp32.

@@ -56,6 +56,7 @@ class AttnParams(C.Structure):
 
 
 VR_ATTN_V_ONES_COLUMN = 1
+VR_ATTN_F16 = 2  # q / k / v / out are fp16
 
 _lib: Optional[C.CDLL] = None
 
@@ -76,12 +77,20 @@ def _declare(lib: C.CDLL) -> None:
     lib.vr_attention_force_v1.argtypes = [i32]
     lib.vr_im2col_norm.restype = i32
     lib.vr_im2col_norm.argtypes = [vp, i32, i32, i32, i32, vp, i64, vp]
+    lib.vr_im2col_norm_ex.restype = i32
+    lib.vr_im2col_norm_ex.argtypes = [vp, i32, i32, i32, i32, vp, i64, i32, vp]
     lib.vr_layernorm.restype = i32
     lib.vr_layernorm.argtypes = [vp, i64, vp, vp, f32, i32, i32, vp, i64, vp, vp, i32, vp]
+    lib.vr_layernorm_ex.restype = i32
+    lib.vr_layernorm_ex.argtypes = [vp, i64, vp, vp, f32, i32, i32, vp, i64, vp, vp, i32, i32, vp]
     lib.vr_rmsnorm.restype = i32
     lib.vr_rmsnorm.argtypes = [vp, i64, vp, f32, i32, i32, vp, i64, vp]
+    lib.vr_rmsnorm_ex.restype = i32
+    lib.vr_rmsnorm_ex.argtypes = [vp, i64, vp, f32, i32, i32, vp, i64, i32, vp]
     lib.vr_build_lm_input.restype = i32
     lib.vr_build_lm_input.argtypes = [vp, i32, i32, vp, f32, vp, i64, vp, i64, vp]
+    lib.vr_build_lm_input_ex.restype = i32
+    lib.vr_build_lm_input_ex.argtypes = [vp, i32, i32, vp, i32, f32, vp, i64, vp, i64, vp]
     lib.vr_score_ranges.restype = i32
     lib.vr_score_ranges.argtypes = [i32, i64]
     lib.vr_score_list_len.restype = i32

@@ -61,7 +61,7 @@ struct AttArgs {
     const int* cu_k;
     int max_q;
     float scale_log2;  // scale * log2(e)
-    __nv_bfloat16* out;
+    void* out;         // bf16, or fp16 when the kernel's F16 is set
     long long ldo;
 };
 
@@ -71,7 +71,7 @@ struct AttMaps {
 
 // Write O / l for the two accumulator rows of this thread (head_dim columns; the zero pad columns of a 72->80 head are
 // dropped). l_a / l_b are this thread's partial row sums; the quad reduces them here.
-template <int NCH, bool HAS16>
+template <bool F16, int NCH, bool HAS16>
 __device__ __forceinline__ void att_store(const AttArgs& a, const float (&o)[NCH][32], const float (&o16)[8], float l_a, float l_b,
                                           int row_a, int len_q, int q_begin, int b, int head, int q4) {
     l_a += __shfl_xor_sync(0xffffffffu, l_a, 1);
@@ -84,21 +84,21 @@ __device__ __forceinline__ void att_store(const AttArgs& a, const float (&o)[NCH
         if (q_idx >= len_q) continue;
         const float inv = 1.0f / (half ? l_b : l_a);
         const long long row = a.cu_q ? (long long)(q_begin + q_idx) : (long long)b * a.max_q + q_idx;
-        __nv_bfloat16* dst = a.out + row * a.ldo + head * a.head_dim;
+        half16_t<F16>* dst = reinterpret_cast<half16_t<F16>*>(a.out) + row * a.ldo + head * a.head_dim;
 #pragma unroll
         for (int c = 0; c < NCH; ++c)
 #pragma unroll
             for (int j = 0; j < 8; ++j) {
                 const int col = c * 64 + j * 8 + q4 * 2;
                 if (col < a.head_dim)
-                    *reinterpret_cast<uint32_t*>(dst + col) = pack_bf16x2(o[c][4 * j + 2 * half] * inv, o[c][4 * j + 2 * half + 1] * inv);
+                    *reinterpret_cast<uint32_t*>(dst + col) = pack16x2<F16>(o[c][4 * j + 2 * half] * inv, o[c][4 * j + 2 * half + 1] * inv);
             }
         if (HAS16) {
 #pragma unroll
             for (int j = 0; j < 2; ++j) {
                 const int col = NCH * 64 + j * 8 + q4 * 2;
                 if (col < a.head_dim)
-                    *reinterpret_cast<uint32_t*>(dst + col) = pack_bf16x2(o16[4 * j + 2 * half] * inv, o16[4 * j + 2 * half + 1] * inv);
+                    *reinterpret_cast<uint32_t*>(dst + col) = pack16x2<F16>(o16[4 * j + 2 * half] * inv, o16[4 * j + 2 * half + 1] * inv);
             }
         }
     }
@@ -142,7 +142,9 @@ __device__ __forceinline__ void att_softmax_tile(float (&s)[64], float c, float&
     l_b = l_b * alpha_b + lt_b;
 }
 
-template <int HS, bool CAUSAL, int NWG>
+// F16: Q, K, V, P and the output are fp16 (else bf16). P is rounded to nearest with no flush, so p below 2^-14 enter the
+// P V MMA as fp16 subnormals instead of zeros. The softmax and everything kept in fp32 are the same in both types.
+template <int HS, bool CAUSAL, int NWG, bool F16>
 // Register file: 384 threads x 168 as compiled; the producer warpgroup (and, with NWG = 1, the idle third one) hands its
 // share to the consumers: 40 / 232 / 232 resp. 40 / 232 / 40. The same block shape for both forms keeps every role
 // branch warpgroup-uniform with a known register budget.
@@ -243,7 +245,7 @@ attention_wgmma_kernel(const __grid_constant__ AttMaps maps, const AttArgs a) {
         for (int j = 0; j < 8; ++j) o16[j] = 0.f;
         float m_a = -INFINITY, m_b = -INFINITY, l_a = 0.f, l_b = 0.f, alpha_a, alpha_b;
         float s[64];
-        uint32_t pa[ATT_BN / 16][4];  // P in bf16 as the A operand: k step kk = accumulator column blocks 2kk, 2kk+1
+        uint32_t pa[ATT_BN / 16][4];  // P in bf16 / fp16 as the A operand: k step kk = accumulator column blocks 2kk, 2kk+1
 
         auto issue_s = [&](int kt) {  // S = Q K_kt^T
             const uint32_t k_addr = smem_u32(sK) + (kt % ATT_STAGES) * Cfg::TILE_BYTES;
@@ -251,12 +253,12 @@ attention_wgmma_kernel(const __grid_constant__ AttMaps maps, const AttArgs a) {
             for (int cc = 0; cc < NCH; ++cc) {
 #pragma unroll
                 for (int kk = 0; kk < 4; ++kk)
-                    wgmma_ss<false, false>(s, make_smem_desc(q_addr + cc * Cfg::Q_CHUNK + kk * 32, 16, 1024, kLayoutSW128),
+                    wgmma_ss<F16, false>(s, make_smem_desc(q_addr + cc * Cfg::Q_CHUNK + kk * 32, 16, 1024, kLayoutSW128),
                                            make_smem_desc(k_addr + cc * 16384 + kk * 32, 16, 1024, kLayoutSW128), (cc | kk) != 0,
                                            std::integral_constant<int, 128>());
             }
             if (Cfg::HAS16)
-                wgmma_ss<false, false>(s, make_smem_desc(q16_addr, 16, 256, kLayoutSW32),
+                wgmma_ss<F16, false>(s, make_smem_desc(q16_addr, 16, 256, kLayoutSW32),
                                        make_smem_desc(k_addr + NCH * 16384, 16, 256, kLayoutSW32), 1, std::integral_constant<int, 128>());
             wgmma_commit();
         };
@@ -266,10 +268,10 @@ attention_wgmma_kernel(const __grid_constant__ AttMaps maps, const AttArgs a) {
             for (int kk = 0; kk < ATT_BN / 16; ++kk) {
 #pragma unroll
                 for (int cc = 0; cc < NCH; ++cc)  // V chunk: [128 keys][64 dims], 128 B per key row -> MN-major
-                    wgmma_rs_tb(o[cc], pa[kk], make_smem_desc(v_addr + cc * 16384 + kk * 2048, 16, 1024, kLayoutSW128), 1,
+                    wgmma_rs_tb<F16>(o[cc], pa[kk], make_smem_desc(v_addr + cc * 16384 + kk * 2048, 16, 1024, kLayoutSW128), 1,
                                 std::integral_constant<int, 64>());
                 if (Cfg::HAS16)  // [128 keys][16 dims], 32 B per key row
-                    wgmma_rs_tb(o16, pa[kk], make_smem_desc(v_addr + NCH * 16384 + kk * 512, 16, 256, kLayoutSW32), 1,
+                    wgmma_rs_tb<F16>(o16, pa[kk], make_smem_desc(v_addr + NCH * 16384 + kk * 512, 16, 256, kLayoutSW32), 1,
                                 std::integral_constant<int, 16>());
             }
             wgmma_commit();
@@ -301,10 +303,10 @@ attention_wgmma_kernel(const __grid_constant__ AttMaps maps, const AttArgs a) {
         auto pack_p = [&] {
 #pragma unroll
             for (int kk = 0; kk < ATT_BN / 16; ++kk) {
-                pa[kk][0] = pack_bf16x2(s[8 * kk + 0], s[8 * kk + 1]);
-                pa[kk][1] = pack_bf16x2(s[8 * kk + 2], s[8 * kk + 3]);
-                pa[kk][2] = pack_bf16x2(s[8 * kk + 4], s[8 * kk + 5]);
-                pa[kk][3] = pack_bf16x2(s[8 * kk + 6], s[8 * kk + 7]);
+                pa[kk][0] = pack16x2<F16>(s[8 * kk + 0], s[8 * kk + 1]);
+                pa[kk][1] = pack16x2<F16>(s[8 * kk + 2], s[8 * kk + 3]);
+                pa[kk][2] = pack16x2<F16>(s[8 * kk + 4], s[8 * kk + 5]);
+                pa[kk][3] = pack16x2<F16>(s[8 * kk + 6], s[8 * kk + 7]);
             }
         };
         auto rescale_o = [&] {
@@ -379,7 +381,7 @@ attention_wgmma_kernel(const __grid_constant__ AttMaps maps, const AttArgs a) {
             wgmma_touch(o16);
         }
         if (cw == 0) turn_wait();
-        att_store<NCH, Cfg::HAS16>(a, o, o16, l_a, l_b, row_a, len_q, q_begin, b, head, q4);
+        att_store<F16, NCH, Cfg::HAS16>(a, o, o16, l_a, l_b, row_a, len_q, q_begin, b, head, q4);
     } else {  // NWG = 1, and NWG = 2 at head stride 128: each warpgroup takes each key tile in turn
         float o[NCH][32];
         float o16[8];
@@ -404,12 +406,12 @@ attention_wgmma_kernel(const __grid_constant__ AttMaps maps, const AttArgs a) {
             for (int c = 0; c < NCH; ++c) {
 #pragma unroll
                 for (int kk = 0; kk < 4; ++kk)
-                    wgmma_ss<false, false>(s, make_smem_desc(q_addr + c * Cfg::Q_CHUNK + kk * 32, 16, 1024, kLayoutSW128),
+                    wgmma_ss<F16, false>(s, make_smem_desc(q_addr + c * Cfg::Q_CHUNK + kk * 32, 16, 1024, kLayoutSW128),
                                            make_smem_desc(k_addr + c * 16384 + kk * 32, 16, 1024, kLayoutSW128), (c | kk) != 0,
                                            std::integral_constant<int, 128>());
             }
             if (Cfg::HAS16)
-                wgmma_ss<false, false>(s, make_smem_desc(q16_addr, 16, 256, kLayoutSW32),
+                wgmma_ss<F16, false>(s, make_smem_desc(q16_addr, 16, 256, kLayoutSW32),
                                        make_smem_desc(k_addr + NCH * 16384, 16, 256, kLayoutSW32), 1, std::integral_constant<int, 128>());
             wgmma_commit();
             wgmma_wait<0>();
@@ -455,10 +457,10 @@ attention_wgmma_kernel(const __grid_constant__ AttMaps maps, const AttArgs a) {
             uint32_t pa[ATT_BN / 16][4];
 #pragma unroll
             for (int kk = 0; kk < ATT_BN / 16; ++kk) {
-                pa[kk][0] = pack_bf16x2(s[8 * kk + 0], s[8 * kk + 1]);
-                pa[kk][1] = pack_bf16x2(s[8 * kk + 2], s[8 * kk + 3]);
-                pa[kk][2] = pack_bf16x2(s[8 * kk + 4], s[8 * kk + 5]);
-                pa[kk][3] = pack_bf16x2(s[8 * kk + 6], s[8 * kk + 7]);
+                pa[kk][0] = pack16x2<F16>(s[8 * kk + 0], s[8 * kk + 1]);
+                pa[kk][1] = pack16x2<F16>(s[8 * kk + 2], s[8 * kk + 3]);
+                pa[kk][2] = pack16x2<F16>(s[8 * kk + 4], s[8 * kk + 5]);
+                pa[kk][3] = pack16x2<F16>(s[8 * kk + 6], s[8 * kk + 7]);
             }
             mbar_wait(&v_full[st], ph);
             wgmma_fence();
@@ -467,12 +469,12 @@ attention_wgmma_kernel(const __grid_constant__ AttMaps maps, const AttArgs a) {
 #pragma unroll
                 for (int c = 0; c < NCH; ++c) {
                     // V chunk: [128 keys][64 dims], 128 B per key row -> MN-major, 8-key groups 1024 B apart
-                    wgmma_rs_tb(o[c], pa[kk], make_smem_desc(v_addr + c * 16384 + kk * 2048, 16, 1024, kLayoutSW128), 1,
+                    wgmma_rs_tb<F16>(o[c], pa[kk], make_smem_desc(v_addr + c * 16384 + kk * 2048, 16, 1024, kLayoutSW128), 1,
                                 std::integral_constant<int, 64>());
                 }
                 if (Cfg::HAS16) {
                     // [128 keys][16 dims], 32 B per key row
-                    wgmma_rs_tb(o16, pa[kk], make_smem_desc(v_addr + NCH * 16384 + kk * 512, 16, 256, kLayoutSW32), 1,
+                    wgmma_rs_tb<F16>(o16, pa[kk], make_smem_desc(v_addr + NCH * 16384 + kk * 512, 16, 256, kLayoutSW32), 1,
                                 std::integral_constant<int, 16>());
                 }
             }
@@ -484,7 +486,7 @@ attention_wgmma_kernel(const __grid_constant__ AttMaps maps, const AttArgs a) {
             wgmma_touch(o16);
         }
 
-        att_store<NCH, Cfg::HAS16>(a, o, o16, l_a, l_b, row_a, len_q, q_begin, b, head, q4);
+        att_store<F16, NCH, Cfg::HAS16>(a, o, o16, l_a, l_b, row_a, len_q, q_begin, b, head, q4);
     }
 }
 

@@ -20,12 +20,14 @@ __device__ __forceinline__ float warp_sum(float v) {
 // then every thread builds 8 consecutive output columns (col = c*p*p + ky*p + kx) of one patch from shared memory and
 // writes them with one 16-byte store (a warp writes 512 contiguous bytes). ToTensor + Normalize(0.5, 0.5) is one
 // FFMA: bf16(fma(u, 2/255, -1)) == bf16((u/255 - 0.5)/0.5) for all 256 byte values (tests/test_gpu_kernels.py checks
-// every value), so the division of the fp32 reference is not needed for a bit-identical bf16 result.
+// every value), so the division of the fp32 reference is not needed for a bit-identical bf16 result. The same holds for
+// fp16 (F16): fp16(fma(u, 2/255, -1)) == fp16((u/255 - 0.5)/0.5) for all 256 values (tests/test_fp16_host.py).
 // ---------------------------------------------------------------------------------------------
 constexpr int IM2COL_THREADS = 256;
 
+template <bool F16>
 __global__ void __launch_bounds__(IM2COL_THREADS)
-im2col_norm_kernel(const uint8_t* __restrict__ px, int n_strips, int gw, int patch, __nv_bfloat16* __restrict__ out,
+im2col_norm_kernel(const uint8_t* __restrict__ px, int n_strips, int gw, int patch, half16_t<F16>* __restrict__ out,
                    long long ldo) {
     extern __shared__ __align__(16) uint8_t strip[];  // [patch][w*3] + offset table [groups*8] (uint16)
     const int w3 = gw * patch * 3;
@@ -58,7 +60,7 @@ im2col_norm_kernel(const uint8_t* __restrict__ px, int n_strips, int gw, int pat
             for (int i = threadIdx.x; i < strip_bytes; i += IM2COL_THREADS) strip[i] = __ldg(src + i);
         }
         __syncthreads();
-        __nv_bfloat16* orow0 = out + static_cast<long long>(sidx) * gw * ldo;
+        half16_t<F16>* orow0 = out + static_cast<long long>(sidx) * gw * ldo;
         const int items = gw * groups;
         for (int it = threadIdx.x; it < items; it += IM2COL_THREADS) {
             const int p = it / groups, g = it - p * groups;
@@ -72,7 +74,7 @@ im2col_norm_kernel(const uint8_t* __restrict__ px, int n_strips, int gw, int pat
                 const uint32_t aa = (oa >> 8) * w3 + (oa & 0xFFu), ab = (ob >> 8) * w3 + (ob & 0xFFu);
                 const float va = oa == 0xFFFFu ? 0.f : fmaf(static_cast<float>(base[aa]), 2.0f / 255.0f, -1.0f);
                 const float vb = ob == 0xFFFFu ? 0.f : fmaf(static_cast<float>(base[ab]), 2.0f / 255.0f, -1.0f);
-                pk[j] = pack_bf16x2(va, vb);
+                pk[j] = pack16x2<F16>(va, vb);
             }
             *reinterpret_cast<uint4*>(orow0 + static_cast<long long>(p) * ldo + g * 8) = make_uint4(pk[0], pk[1], pk[2], pk[3]);
         }
@@ -88,9 +90,9 @@ constexpr int IM2COL14_THREADS = 224;  // 7 warps: 14 pixel rows x 16 patches pe
 // BULK: the pixel rows are 16-byte multiples at 16-byte aligned addresses -> the strip is staged by 14 bulk (TMA) row
 // copies onto an mbarrier, double buffered: strip i+1 streams in while strip i is converted (a version with ordinary
 // loads is latency bound: too few loads in flight per SM).
-template <bool BULK>
+template <bool BULK, bool F16>
 __global__ void __launch_bounds__(IM2COL14_THREADS)
-im2col_norm14_kernel(const uint8_t* __restrict__ px, int n_strips, int gw, __nv_bfloat16* __restrict__ out, int ldo) {
+im2col_norm14_kernel(const uint8_t* __restrict__ px, int n_strips, int gw, half16_t<F16>* __restrict__ out, int ldo) {
     constexpr int P = 14, RUN = P * 3;  // 42 bytes per (patch, pixel row)
     constexpr int NBUF = BULK ? 2 : 1;
     extern __shared__ __align__(16) uint8_t smem14[];
@@ -100,13 +102,13 @@ im2col_norm14_kernel(const uint8_t* __restrict__ px, int n_strips, int gw, __nv_
     // (consecutive lanes) start in different banks (w3 itself is 1344 B = 16 banks apart for 448-pixel slices)
     const int pitch = (((w3 + 15) >> 4) | 1) << 4;
     const int in_bytes = P * pitch + 16;  // + 16: the last item's 12-word window reads past its 42 bytes
-    uint8_t* tile = smem14 + NBUF * in_bytes;  // [gw][ldo] bf16, exactly the layout of the strip's output rows
+    uint8_t* tile = smem14 + NBUF * in_bytes;  // [gw][ldo] 16-bit, exactly the layout of the strip's output rows
     const int tile_bytes = gw * ldo * 2;
     const int strip_bytes = P * w3;
     // zero the padding columns once: they are never written again
     for (int i = threadIdx.x; i < gw * (ldo - 3 * P * P); i += IM2COL14_THREADS) {
         const int p = i / (ldo - 3 * P * P), c = i - p * (ldo - 3 * P * P);
-        reinterpret_cast<__nv_bfloat16*>(tile)[p * ldo + 3 * P * P + c] = __float2bfloat16(0.f);
+        reinterpret_cast<half16_t<F16>*>(tile)[p * ldo + 3 * P * P + c] = to_half16<F16>(0.f);
     }
     for (int i = threadIdx.x; i < NBUF * in_bytes / 4; i += IM2COL14_THREADS) reinterpret_cast<uint32_t*>(smem14)[i] = 0;
     if (BULK && threadIdx.x == 0) {
@@ -166,14 +168,14 @@ im2col_norm14_kernel(const uint8_t* __restrict__ px, int n_strips, int gw, __nv_
                     const int k0 = (2 * i) * 3 + c, k1 = (2 * i + 1) * 3 + c;  // byte index of pixel 2i / 2i+1, channel c
                     const float f0 = __uint_as_float(__byte_perm(w[k0 >> 2], 0x4B000000u, 0x7540 | (k0 & 3))) - 8388608.0f;
                     const float f1 = __uint_as_float(__byte_perm(w[k1 >> 2], 0x4B000000u, 0x7540 | (k1 & 3))) - 8388608.0f;
-                    dst[c * (P * P / 2) + i] = pack_bf16x2(fmaf(f0, 2.0f / 255.0f, -1.0f), fmaf(f1, 2.0f / 255.0f, -1.0f));
+                    dst[c * (P * P / 2) + i] = pack16x2<F16>(fmaf(f0, 2.0f / 255.0f, -1.0f), fmaf(f1, 2.0f / 255.0f, -1.0f));
                 }
             }
         }
         fence_proxy_async_smem();  // generic-proxy writes -> visible to the bulk copy engine
         __syncthreads();
         if (threadIdx.x == 0) {
-            __nv_bfloat16* gdst = out + static_cast<long long>(sidx) * gw * ldo;
+            half16_t<F16>* gdst = out + static_cast<long long>(sidx) * gw * ldo;
             asm volatile("cp.async.bulk.global.shared::cta.bulk_group [%0], [%1], %2;" ::"l"(gdst), "r"(smem_u32(tile)),
                          "r"(tile_bytes)
                          : "memory");
@@ -184,12 +186,12 @@ im2col_norm14_kernel(const uint8_t* __restrict__ px, int n_strips, int gw, __nv_
 }
 
 // ---------------------------------------------------------------------------------------------
-// LayerNorm / RMSNorm: one warp per row, dim % 4 == 0.
+// LayerNorm / RMSNorm: one warp per row, dim % 4 == 0. Statistics in fp32; the output is stored as bf16 or (F16) fp16.
 // ---------------------------------------------------------------------------------------------
-template <bool RMS>
+template <bool RMS, bool F16>
 __global__ void norm_kernel(const float* __restrict__ x, long long ldx, const float* __restrict__ gamma,
                             const float* __restrict__ beta, float eps, int rows, int dim,
-                            __nv_bfloat16* __restrict__ out, long long ldo, __nv_bfloat16* __restrict__ out2,
+                            half16_t<F16>* __restrict__ out, long long ldo, half16_t<F16>* __restrict__ out2,
                             const float* __restrict__ add, int add_period) {
     const int warps_per_block = blockDim.x >> 5;
     const int lane = threadIdx.x & 31;
@@ -212,8 +214,8 @@ __global__ void norm_kernel(const float* __restrict__ x, long long ldx, const fl
             ss += (a * a + b * b) + (c * c + d * d);
         }
         const float rstd = rsqrtf(warp_sum(ss) / static_cast<float>(dim) + eps);
-        __nv_bfloat16* orow = out + static_cast<long long>(row) * ldo;
-        __nv_bfloat16* orow2 = out2 ? out2 + static_cast<long long>(row) * ldo : nullptr;
+        half16_t<F16>* orow = out + static_cast<long long>(row) * ldo;
+        half16_t<F16>* orow2 = out2 ? out2 + static_cast<long long>(row) * ldo : nullptr;
         const float* arow = add ? add + static_cast<long long>(row % add_period) * dim : nullptr;
         for (int i = lane; i < nvec; i += 32) {
             const float4 v = xr[i];
@@ -225,14 +227,14 @@ __global__ void norm_kernel(const float* __restrict__ x, long long ldx, const fl
                 y0 += bb.x; y1 += bb.y; y2 += bb.z; y3 += bb.w;
             }
             uint2 pk;
-            pk.x = pack_bf16x2(y0, y1);
-            pk.y = pack_bf16x2(y2, y3);
+            pk.x = pack16x2<F16>(y0, y1);
+            pk.y = pack16x2<F16>(y2, y3);
             reinterpret_cast<uint2*>(orow)[i] = pk;
             if (orow2) {
                 const float4 aa = reinterpret_cast<const float4*>(arow)[i];
                 uint2 pk2;
-                pk2.x = pack_bf16x2(y0 + aa.x, y1 + aa.y);
-                pk2.y = pack_bf16x2(y2 + aa.z, y3 + aa.w);
+                pk2.x = pack16x2<F16>(y0 + aa.x, y1 + aa.y);
+                pk2.y = pack16x2<F16>(y2 + aa.z, y3 + aa.w);
                 reinterpret_cast<uint2*>(orow2)[i] = pk2;
             }
         }
@@ -240,10 +242,10 @@ __global__ void norm_kernel(const float* __restrict__ x, long long ldx, const fl
 }
 
 // Register-resident variant for dim == VPL * 128 (1152 -> VPL 9, 2304 -> VPL 18): the row is read from HBM exactly once.
-template <bool RMS, int VPL>
+template <bool RMS, int VPL, bool F16>
 __global__ void __launch_bounds__(256)
 norm_kernel_reg(const float* __restrict__ x, long long ldx, const float* __restrict__ gamma, const float* __restrict__ beta,
-                float eps, int rows, __nv_bfloat16* __restrict__ out, long long ldo, __nv_bfloat16* __restrict__ out2,
+                float eps, int rows, half16_t<F16>* __restrict__ out, long long ldo, half16_t<F16>* __restrict__ out2,
                 const float* __restrict__ add, int add_period) {
     constexpr int DIM = VPL * 128;
     const int warps_per_block = blockDim.x >> 5;
@@ -281,14 +283,14 @@ norm_kernel_reg(const float* __restrict__ x, long long ldx, const float* __restr
                 y0 += bb.x; y1 += bb.y; y2 += bb.z; y3 += bb.w;
             }
             uint2 pk;
-            pk.x = pack_bf16x2(y0, y1);
-            pk.y = pack_bf16x2(y2, y3);
+            pk.x = pack16x2<F16>(y0, y1);
+            pk.y = pack16x2<F16>(y2, y3);
             orow[c] = pk;
             if (orow2) {
                 const float4 aa = arow[c];
                 uint2 pk2;
-                pk2.x = pack_bf16x2(y0 + aa.x, y1 + aa.y);
-                pk2.y = pack_bf16x2(y2 + aa.z, y3 + aa.w);
+                pk2.x = pack16x2<F16>(y0 + aa.x, y1 + aa.y);
+                pk2.y = pack16x2<F16>(y2 + aa.z, y3 + aa.w);
                 orow2[c] = pk2;
             }
         }
@@ -298,8 +300,9 @@ norm_kernel_reg(const float* __restrict__ x, long long ldx, const float* __restr
 // ---------------------------------------------------------------------------------------------
 // LM input assembly: one warp per token row.
 // ---------------------------------------------------------------------------------------------
+template <bool F16>
 __global__ void build_lm_input_kernel(const int* __restrict__ src, int tokens, int dim,
-                                      const __nv_bfloat16* __restrict__ embed, float scale_emb,
+                                      const half16_t<F16>* __restrict__ embed, float scale_emb,
                                       const float* __restrict__ vision, long long ldv, float* __restrict__ h,
                                       long long ldh) {
     const int warps_per_block = blockDim.x >> 5;
@@ -314,10 +317,8 @@ __global__ void build_lm_input_kernel(const int* __restrict__ src, int tokens, i
             const uint2* e = reinterpret_cast<const uint2*>(embed + static_cast<long long>(-(s + 1)) * dim);
             for (int i = lane; i < (dim >> 2); i += 32) {
                 const uint2 raw = e[i];
-                const __nv_bfloat162 a = *reinterpret_cast<const __nv_bfloat162*>(&raw.x);
-                const __nv_bfloat162 b = *reinterpret_cast<const __nv_bfloat162*>(&raw.y);
-                dst[i] = make_float4(__low2float(a) * scale_emb, __high2float(a) * scale_emb,
-                                     __low2float(b) * scale_emb, __high2float(b) * scale_emb);
+                const float2 a = unpack16x2<F16>(raw.x), b = unpack16x2<F16>(raw.y);  // exact
+                dst[i] = make_float4(a.x * scale_emb, a.y * scale_emb, b.x * scale_emb, b.y * scale_emb);
             }
         }
     }
@@ -460,22 +461,13 @@ static int grid_for(long long work_items, int per_block) {
     return static_cast<int>(blocks);
 }
 
-}  // namespace vr
-
-using namespace vr;
-
-extern "C" int vr_im2col_norm(const uint8_t* pixels, int32_t n_slices, int32_t h, int32_t w, int32_t patch, void* out,
-                              int64_t ldo, void* stream) {
-    VR_REQUIRE(pixels && out, "vr_im2col_norm: null pointer");
-    VR_REQUIRE(n_slices > 0 && h > 0 && w > 0 && patch > 0 && h % patch == 0 && w % patch == 0,
-               "vr_im2col_norm: bad geometry n=%d h=%d w=%d patch=%d", n_slices, h, w, patch);
-    VR_REQUIRE(ldo % 8 == 0 && ldo >= 3 * patch * patch, "vr_im2col_norm: ldo=%lld must be a multiple of 8 and >= %d",
-               (long long)ldo, 3 * patch * patch);
-    VR_REQUIRE(patch <= 85, "vr_im2col_norm: patch=%d exceeds 85", patch);
+template <bool F16>
+static int im2col_norm_impl(const uint8_t* pixels, int32_t n_slices, int32_t h, int32_t w, int32_t patch, void* out, int64_t ldo,
+                            cudaStream_t st) {
     const int gw = w / patch;
     const long long n_strips = static_cast<long long>(n_slices) * (h / patch);
     VR_REQUIRE(n_strips < (1ll << 31), "vr_im2col_norm: too many patch rows");
-    cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+    half16_t<F16>* o = reinterpret_cast<half16_t<F16>*>(out);
     long long blocks = n_strips;
     if (patch == 14 && (reinterpret_cast<uintptr_t>(out) & 15) == 0 && (reinterpret_cast<uintptr_t>(pixels) & 3) == 0 && (ldo & 7) == 0) {
         const size_t pitch14 = static_cast<size_t>((((w * 3 + 15) >> 4) | 1) << 4);
@@ -484,18 +476,18 @@ extern "C" int vr_im2col_norm(const uint8_t* pixels, int32_t n_slices, int32_t h
         if (smem14 <= 200 * 1024) {
             static unsigned long long configured14 = 0;
             if (first_use_on_device(&configured14)) {
-                VR_CHECK_CUDA(cudaFuncSetAttribute(im2col_norm14_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
-                VR_CHECK_CUDA(cudaFuncSetAttribute(im2col_norm14_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
+                VR_CHECK_CUDA(cudaFuncSetAttribute(im2col_norm14_kernel<true, F16>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
+                VR_CHECK_CUDA(cudaFuncSetAttribute(im2col_norm14_kernel<false, F16>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
             }
             const long long per_sm = (200 * 1024) / static_cast<long long>(smem14) < 4 ? (200 * 1024) / static_cast<long long>(smem14) : 4;
             const long long cap14 = static_cast<long long>(num_sms()) * (per_sm < 1 ? 1 : per_sm);
             if (blocks > cap14) blocks = cap14;
             if (bulk)
-                im2col_norm14_kernel<true><<<static_cast<int>(blocks), IM2COL14_THREADS, smem14, st>>>(
-                    pixels, static_cast<int>(n_strips), gw, reinterpret_cast<__nv_bfloat16*>(out), static_cast<int>(ldo));
+                im2col_norm14_kernel<true, F16><<<static_cast<int>(blocks), IM2COL14_THREADS, smem14, st>>>(
+                    pixels, static_cast<int>(n_strips), gw, o, static_cast<int>(ldo));
             else
-                im2col_norm14_kernel<false><<<static_cast<int>(blocks), IM2COL14_THREADS, smem14, st>>>(
-                    pixels, static_cast<int>(n_strips), gw, reinterpret_cast<__nv_bfloat16*>(out), static_cast<int>(ldo));
+                im2col_norm14_kernel<false, F16><<<static_cast<int>(blocks), IM2COL14_THREADS, smem14, st>>>(
+                    pixels, static_cast<int>(n_strips), gw, o, static_cast<int>(ldo));
             VR_CHECK_CUDA(cudaGetLastError());
             return 0;
         }
@@ -504,59 +496,108 @@ extern "C" int vr_im2col_norm(const uint8_t* pixels, int32_t n_slices, int32_t h
     VR_REQUIRE(smem <= 200 * 1024, "vr_im2col_norm: a %d-pixel-wide slice does not fit the %d-row strip buffer", w, patch);
     static unsigned long long configured = 0;
     if (first_use_on_device(&configured))
-        VR_CHECK_CUDA(cudaFuncSetAttribute(im2col_norm_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
+        VR_CHECK_CUDA(cudaFuncSetAttribute(im2col_norm_kernel<F16>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
     const long long cap = static_cast<long long>(num_sms()) * 8;
     if (blocks > cap) blocks = cap;
-    im2col_norm_kernel<<<static_cast<int>(blocks), IM2COL_THREADS, smem, st>>>(
-        pixels, static_cast<int>(n_strips), gw, patch, reinterpret_cast<__nv_bfloat16*>(out), ldo);
+    im2col_norm_kernel<F16><<<static_cast<int>(blocks), IM2COL_THREADS, smem, st>>>(pixels, static_cast<int>(n_strips), gw, patch, o, ldo);
     VR_CHECK_CUDA(cudaGetLastError());
     return 0;
+}
+
+template <bool RMS, bool F16>
+static int norm_impl(const float* x, int64_t ldx, const float* gamma, const float* beta, float eps, int32_t rows, int32_t dim,
+                     void* out, int64_t ldo, void* out2, const float* add, int32_t add_period, cudaStream_t s) {
+    half16_t<F16>* o = reinterpret_cast<half16_t<F16>*>(out);
+    half16_t<F16>* o2 = reinterpret_cast<half16_t<F16>*>(out2);
+    if (dim == 2304)
+        norm_kernel_reg<RMS, 18, F16><<<grid_for(rows, 8), 256, 0, s>>>(x, ldx, gamma, beta, eps, rows, o, ldo, o2, add, add_period);
+    else if (!RMS && dim == 1152)
+        norm_kernel_reg<RMS, 9, F16><<<grid_for(rows, 8), 256, 0, s>>>(x, ldx, gamma, beta, eps, rows, o, ldo, o2, add, add_period);
+    else
+        norm_kernel<RMS, F16><<<grid_for(rows, 8), 256, 0, s>>>(x, ldx, gamma, beta, eps, rows, dim, o, ldo, o2, add, add_period);
+    VR_CHECK_CUDA(cudaGetLastError());
+    return 0;
+}
+
+}  // namespace vr
+
+using namespace vr;
+
+extern "C" int vr_im2col_norm_ex(const uint8_t* pixels, int32_t n_slices, int32_t h, int32_t w, int32_t patch, void* out,
+                                 int64_t ldo, int32_t out_dtype, void* stream) {
+    VR_REQUIRE(pixels && out, "vr_im2col_norm: null pointer");
+    VR_REQUIRE(n_slices > 0 && h > 0 && w > 0 && patch > 0 && h % patch == 0 && w % patch == 0,
+               "vr_im2col_norm: bad geometry n=%d h=%d w=%d patch=%d", n_slices, h, w, patch);
+    VR_REQUIRE(ldo % 8 == 0 && ldo >= 3 * patch * patch, "vr_im2col_norm: ldo=%lld must be a multiple of 8 and >= %d",
+               (long long)ldo, 3 * patch * patch);
+    VR_REQUIRE(patch <= 85, "vr_im2col_norm: patch=%d exceeds 85", patch);
+    VR_REQUIRE(out_dtype == VR_BF16 || out_dtype == VR_F16, "vr_im2col_norm: out_dtype must be VR_BF16 or VR_F16 (got %d)", out_dtype);
+    cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+    return out_dtype == VR_F16 ? im2col_norm_impl<true>(pixels, n_slices, h, w, patch, out, ldo, st)
+                               : im2col_norm_impl<false>(pixels, n_slices, h, w, patch, out, ldo, st);
+}
+
+extern "C" int vr_im2col_norm(const uint8_t* pixels, int32_t n_slices, int32_t h, int32_t w, int32_t patch, void* out,
+                              int64_t ldo, void* stream) {
+    return vr_im2col_norm_ex(pixels, n_slices, h, w, patch, out, ldo, VR_BF16, stream);
+}
+
+extern "C" int vr_layernorm_ex(const float* x, int64_t ldx, const float* gamma, const float* beta, float eps, int32_t rows,
+                               int32_t dim, void* out, int64_t ldo, void* out2, const float* add, int32_t add_period,
+                               int32_t out_dtype, void* stream) {
+    VR_REQUIRE(x && gamma && beta && out, "vr_layernorm: null pointer");
+    VR_REQUIRE(rows > 0 && dim > 0 && dim % 4 == 0 && ldx % 4 == 0 && ldo % 4 == 0, "vr_layernorm: bad shape rows=%d dim=%d",
+               rows, dim);
+    VR_REQUIRE(!out2 || (add && add_period > 0), "vr_layernorm: out2 needs add/add_period");
+    VR_REQUIRE(out_dtype == VR_BF16 || out_dtype == VR_F16, "vr_layernorm: out_dtype must be VR_BF16 or VR_F16 (got %d)", out_dtype);
+    cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
+    return out_dtype == VR_F16 ? norm_impl<false, true>(x, ldx, gamma, beta, eps, rows, dim, out, ldo, out2, add, add_period, s)
+                               : norm_impl<false, false>(x, ldx, gamma, beta, eps, rows, dim, out, ldo, out2, add, add_period, s);
 }
 
 extern "C" int vr_layernorm(const float* x, int64_t ldx, const float* gamma, const float* beta, float eps, int32_t rows,
                             int32_t dim, void* out, int64_t ldo, void* out2, const float* add, int32_t add_period,
                             void* stream) {
-    VR_REQUIRE(x && gamma && beta && out, "vr_layernorm: null pointer");
-    VR_REQUIRE(rows > 0 && dim > 0 && dim % 4 == 0 && ldx % 4 == 0 && ldo % 4 == 0, "vr_layernorm: bad shape rows=%d dim=%d",
+    return vr_layernorm_ex(x, ldx, gamma, beta, eps, rows, dim, out, ldo, out2, add, add_period, VR_BF16, stream);
+}
+
+extern "C" int vr_rmsnorm_ex(const float* x, int64_t ldx, const float* gamma, float eps, int32_t rows, int32_t dim, void* out,
+                             int64_t ldo, int32_t out_dtype, void* stream) {
+    VR_REQUIRE(x && gamma && out, "vr_rmsnorm: null pointer");
+    VR_REQUIRE(rows > 0 && dim > 0 && dim % 4 == 0 && ldx % 4 == 0 && ldo % 4 == 0, "vr_rmsnorm: bad shape rows=%d dim=%d",
                rows, dim);
-    VR_REQUIRE(!out2 || (add && add_period > 0), "vr_layernorm: out2 needs add/add_period");
+    VR_REQUIRE(out_dtype == VR_BF16 || out_dtype == VR_F16, "vr_rmsnorm: out_dtype must be VR_BF16 or VR_F16 (got %d)", out_dtype);
     cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
-    __nv_bfloat16* o = reinterpret_cast<__nv_bfloat16*>(out);
-    __nv_bfloat16* o2 = reinterpret_cast<__nv_bfloat16*>(out2);
-    if (dim == 1152)
-        norm_kernel_reg<false, 9><<<grid_for(rows, 8), 256, 0, s>>>(x, ldx, gamma, beta, eps, rows, o, ldo, o2, add, add_period);
-    else if (dim == 2304)
-        norm_kernel_reg<false, 18><<<grid_for(rows, 8), 256, 0, s>>>(x, ldx, gamma, beta, eps, rows, o, ldo, o2, add, add_period);
-    else
-        norm_kernel<false><<<grid_for(rows, 8), 256, 0, s>>>(x, ldx, gamma, beta, eps, rows, dim, o, ldo, o2, add, add_period);
-    VR_CHECK_CUDA(cudaGetLastError());
-    return 0;
+    return out_dtype == VR_F16 ? norm_impl<true, true>(x, ldx, gamma, nullptr, eps, rows, dim, out, ldo, nullptr, nullptr, 1, s)
+                               : norm_impl<true, false>(x, ldx, gamma, nullptr, eps, rows, dim, out, ldo, nullptr, nullptr, 1, s);
 }
 
 extern "C" int vr_rmsnorm(const float* x, int64_t ldx, const float* gamma, float eps, int32_t rows, int32_t dim, void* out,
                           int64_t ldo, void* stream) {
-    VR_REQUIRE(x && gamma && out, "vr_rmsnorm: null pointer");
-    VR_REQUIRE(rows > 0 && dim > 0 && dim % 4 == 0 && ldx % 4 == 0 && ldo % 4 == 0, "vr_rmsnorm: bad shape rows=%d dim=%d",
-               rows, dim);
+    return vr_rmsnorm_ex(x, ldx, gamma, eps, rows, dim, out, ldo, VR_BF16, stream);
+}
+
+extern "C" int vr_build_lm_input_ex(const int32_t* src, int32_t tokens, int32_t dim, const void* embed, int32_t embed_dtype,
+                                    float scale_emb, const float* vision, int64_t ldv, float* h, int64_t ldh, void* stream) {
+    VR_REQUIRE(src && embed && h, "vr_build_lm_input: null pointer");
+    VR_REQUIRE(tokens > 0 && dim % 4 == 0 && ldh % 4 == 0 && (vision == nullptr || ldv % 4 == 0),
+               "vr_build_lm_input: bad shape tokens=%d dim=%d", tokens, dim);
+    VR_REQUIRE(embed_dtype == VR_BF16 || embed_dtype == VR_F16, "vr_build_lm_input: embed_dtype must be VR_BF16 or VR_F16 (got %d)",
+               embed_dtype);
     cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
-    __nv_bfloat16* o = reinterpret_cast<__nv_bfloat16*>(out);
-    if (dim == 2304)
-        norm_kernel_reg<true, 18><<<grid_for(rows, 8), 256, 0, s>>>(x, ldx, gamma, nullptr, eps, rows, o, ldo, nullptr, nullptr, 1);
+    if (embed_dtype == VR_F16)
+        build_lm_input_kernel<true><<<grid_for(tokens, 8), 256, 0, s>>>(src, tokens, dim, reinterpret_cast<const __half*>(embed),
+                                                                        scale_emb, vision, ldv, h, ldh);
     else
-        norm_kernel<true><<<grid_for(rows, 8), 256, 0, s>>>(x, ldx, gamma, nullptr, eps, rows, dim, o, ldo, nullptr, nullptr, 1);
+        build_lm_input_kernel<false><<<grid_for(tokens, 8), 256, 0, s>>>(
+            src, tokens, dim, reinterpret_cast<const __nv_bfloat16*>(embed), scale_emb, vision, ldv, h, ldh);
     VR_CHECK_CUDA(cudaGetLastError());
     return 0;
 }
 
 extern "C" int vr_build_lm_input(const int32_t* src, int32_t tokens, int32_t dim, const void* embed_bf16, float scale_emb,
                                  const float* vision, int64_t ldv, float* h, int64_t ldh, void* stream) {
-    VR_REQUIRE(src && embed_bf16 && h, "vr_build_lm_input: null pointer");
-    VR_REQUIRE(tokens > 0 && dim % 4 == 0 && ldh % 4 == 0 && (vision == nullptr || ldv % 4 == 0),
-               "vr_build_lm_input: bad shape tokens=%d dim=%d", tokens, dim);
-    build_lm_input_kernel<<<grid_for(tokens, 8), 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(
-        src, tokens, dim, reinterpret_cast<const __nv_bfloat16*>(embed_bf16), scale_emb, vision, ldv, h, ldh);
-    VR_CHECK_CUDA(cudaGetLastError());
-    return 0;
+    return vr_build_lm_input_ex(src, tokens, dim, embed_bf16, VR_BF16, scale_emb, vision, ldv, h, ldh, stream);
 }
 
 extern "C" int vr_pool_norm(const float* h, int64_t ldh, const float* gamma, float eps, const int32_t* cu, int32_t batch,

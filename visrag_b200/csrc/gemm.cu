@@ -3,15 +3,15 @@
 
 namespace vr {
 
-template <int BN, int MODE, bool OUT_F32, bool GELU, bool SWAP = false>
+template <bool F16, int BN, int MODE, bool OUT_F32, bool GELU, bool SWAP = false>
 static int launch_gemm(const void* A, int64_t lda, const void* B, int64_t ldb, const GemmArgs& g, cudaStream_t stream) {
     using Cfg = GemmCfg<BN>;
     CUtensorMap ta, tb;
     // the MMA's M operand is staged in 128-row boxes, its N operand in 64-row boxes: SWAP hands the weight to the M side
     // (128 features per tile) and the activations to the N side (BN tokens per tile)
-    if (int rc = make_tmap_2d(SWAP ? &tb : &ta, A, g.M, g.K, lda, SWAP ? 64 : GEMM_BM, GEMM_BK, 128, true)) return rc;
-    if (int rc = make_tmap_2d(SWAP ? &ta : &tb, B, g.N, g.K, ldb, SWAP ? GEMM_BM : 64, GEMM_BK, 128, true)) return rc;
-    auto kern = gemm_wgmma_kernel<BN, MODE, OUT_F32, GELU, SWAP>;
+    if (int rc = make_tmap_2d(SWAP ? &tb : &ta, A, g.M, g.K, lda, SWAP ? 64 : GEMM_BM, GEMM_BK, 128, !F16)) return rc;
+    if (int rc = make_tmap_2d(SWAP ? &ta : &tb, B, g.N, g.K, ldb, SWAP ? GEMM_BM : 64, GEMM_BK, 128, !F16)) return rc;
+    auto kern = gemm_wgmma_kernel<F16, BN, MODE, OUT_F32, GELU, SWAP>;
     static unsigned long long attr_set = 0;  // per template instantiation, one bit per device
     if (first_use_on_device(&attr_set))
         VR_CHECK_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES));
@@ -23,13 +23,13 @@ static int launch_gemm(const void* A, int64_t lda, const void* B, int64_t ldb, c
     return 0;
 }
 
-template <int MODE, bool OUT_F32, bool GELU, int CLUSTER>
+template <bool F16, int MODE, bool OUT_F32, bool GELU, int CLUSTER>
 static int launch_pingpong(const void* A, int64_t lda, const void* B, int64_t ldb, const GemmArgs& g, bool l2_slices,
                            cudaStream_t stream) {
     CUtensorMap ta, tb;
-    if (int rc = make_tmap_2d(&ta, A, g.M, g.K, lda, GEMM_BM, GEMM_BK, 128, true)) return rc;
-    if (int rc = make_tmap_2d(&tb, B, g.N, g.K, ldb, 64, GEMM_BK, 128, true)) return rc;
-    auto kern = gemm_pingpong_kernel<MODE, OUT_F32, GELU, CLUSTER>;
+    if (int rc = make_tmap_2d(&ta, A, g.M, g.K, lda, GEMM_BM, GEMM_BK, 128, !F16)) return rc;
+    if (int rc = make_tmap_2d(&tb, B, g.N, g.K, ldb, 64, GEMM_BK, 128, !F16)) return rc;
+    auto kern = gemm_pingpong_kernel<F16, MODE, OUT_F32, GELU, CLUSTER>;
     cudaLaunchConfig_t cfg = {};
     cudaLaunchAttribute attr[1];
     cfg.blockDim = dim3(GEMM_THREADS);
@@ -63,51 +63,86 @@ static int launch_pingpong(const void* A, int64_t lda, const void* B, int64_t ld
     return 0;
 }
 
+// Output types: F16 = false (bf16 operands) writes bf16 or fp32, F16 = true (fp16 operands) fp16 or fp32. Checked before
+// any CUDA call; the bf16 messages are the ones the bf16-only library gave.
+template <bool F16>
+static int check_out_dtype(const vr_gemm_epilogue& e) {
+    if (F16) {
+        if (e.mode == VR_EPI_LINEAR && e.out_dtype == VR_F32) {
+            VR_REQUIRE(!e.act_gelu, "vr_gemm: GELU epilogue writes fp16 only (fp16 operands)");
+            return 0;
+        }
+        if (e.mode == VR_EPI_LINEAR)
+            VR_REQUIRE(e.out_dtype == VR_F16, "vr_gemm: with fp16 operands out_dtype must be VR_F16 or VR_F32");
+        else
+            VR_REQUIRE(e.out_dtype == VR_F16, "vr_gemm: with fp16 operands ROPE / SWIGLU write fp16: out_dtype must be VR_F16");
+        return 0;
+    }
+    if (e.mode != VR_EPI_LINEAR) return 0;  // ROPE / SWIGLU write bf16 whatever out_dtype says
+    if (e.out_dtype == VR_F32) {
+        VR_REQUIRE(!e.act_gelu, "vr_gemm: GELU epilogue writes bf16 only");
+        return 0;
+    }
+    VR_REQUIRE(e.out_dtype == VR_BF16, "vr_gemm: out_dtype must be VR_BF16 or VR_F32");
+    return 0;
+}
+
 // feature-major accumulator kernel (block_n == 3): LINEAR epilogues only
+template <bool F16>
 static int dispatch_swapped(const void* A, int64_t lda, const void* B, int64_t ldb, const GemmArgs& g, cudaStream_t s) {
     const vr_gemm_epilogue& e = g.epi;
     VR_REQUIRE(e.mode == VR_EPI_LINEAR, "vr_gemm: block_n=3 (feature-major accumulator) supports LINEAR epilogues only");
-    if (e.out_dtype == VR_F32) {
-        VR_REQUIRE(!e.act_gelu, "vr_gemm: GELU epilogue writes bf16 only");
-        return launch_gemm<128, VR_EPI_LINEAR, true, false, true>(A, lda, B, ldb, g, s);
-    }
-    VR_REQUIRE(e.out_dtype == VR_BF16, "vr_gemm: out_dtype must be VR_BF16 or VR_F32");
-    if (e.act_gelu) return launch_gemm<128, VR_EPI_LINEAR, false, true, true>(A, lda, B, ldb, g, s);
-    return launch_gemm<128, VR_EPI_LINEAR, false, false, true>(A, lda, B, ldb, g, s);
+    if (int rc = check_out_dtype<F16>(e)) return rc;
+    if (e.out_dtype == VR_F32) return launch_gemm<F16, 128, VR_EPI_LINEAR, true, false, true>(A, lda, B, ldb, g, s);
+    if (e.act_gelu) return launch_gemm<F16, 128, VR_EPI_LINEAR, false, true, true>(A, lda, B, ldb, g, s);
+    return launch_gemm<F16, 128, VR_EPI_LINEAR, false, false, true>(A, lda, B, ldb, g, s);
 }
 
 // BN > 0: tile width of the cooperative kernel. BN < 0: the ping-pong kernel (128 x 128 tiles), as the block_n selector
 // -BN names it: PP (L2-sliced tile order), PP_NFAST (plain n-fastest order), PP_MC (CTA pairs with B multicast).
 constexpr int PP = 2, PP_MC = 4, PP_NFAST = 5;
-template <int BN, int MODE, bool OUT_F32, bool GELU>
+template <bool F16, int BN, int MODE, bool OUT_F32, bool GELU>
 static int launch_any(const void* A, int64_t lda, const void* B, int64_t ldb, const GemmArgs& g, cudaStream_t s) {
-    if constexpr (BN < 0) return launch_pingpong<MODE, OUT_F32, GELU, -BN == PP_MC ? 2 : 1>(A, lda, B, ldb, g, -BN != PP_NFAST, s);
-    else return launch_gemm<BN, MODE, OUT_F32, GELU>(A, lda, B, ldb, g, s);
+    if constexpr (BN < 0) return launch_pingpong<F16, MODE, OUT_F32, GELU, -BN == PP_MC ? 2 : 1>(A, lda, B, ldb, g, -BN != PP_NFAST, s);
+    else return launch_gemm<F16, BN, MODE, OUT_F32, GELU>(A, lda, B, ldb, g, s);
 }
 
-template <int BN>
+template <bool F16, int BN>
 static int dispatch_mode(const void* A, int64_t lda, const void* B, int64_t ldb, const GemmArgs& g, cudaStream_t s) {
     const vr_gemm_epilogue& e = g.epi;
     switch (e.mode) {
         case VR_EPI_LINEAR:
-            if (e.out_dtype == VR_F32) {
-                VR_REQUIRE(!e.act_gelu, "vr_gemm: GELU epilogue writes bf16 only");
-                return launch_any<BN, VR_EPI_LINEAR, true, false>(A, lda, B, ldb, g, s);
-            }
-            VR_REQUIRE(e.out_dtype == VR_BF16, "vr_gemm: out_dtype must be VR_BF16 or VR_F32");
-            if (e.act_gelu) return launch_any<BN, VR_EPI_LINEAR, false, true>(A, lda, B, ldb, g, s);
-            return launch_any<BN, VR_EPI_LINEAR, false, false>(A, lda, B, ldb, g, s);
+            if (int rc = check_out_dtype<F16>(e)) return rc;
+            if (e.out_dtype == VR_F32) return launch_any<F16, BN, VR_EPI_LINEAR, true, false>(A, lda, B, ldb, g, s);
+            if (e.act_gelu) return launch_any<F16, BN, VR_EPI_LINEAR, false, true>(A, lda, B, ldb, g, s);
+            return launch_any<F16, BN, VR_EPI_LINEAR, false, false>(A, lda, B, ldb, g, s);
         case VR_EPI_ROPE:
             VR_REQUIRE(e.positions && e.rope_cos && e.rope_sin, "vr_gemm: ROPE epilogue needs positions/cos/sin");
             VR_REQUIRE(g.N % 64 == 0 && e.rope_cols % 64 == 0, "vr_gemm: ROPE needs N and rope_cols multiples of 64");
-            return launch_any<BN, VR_EPI_ROPE, false, false>(A, lda, B, ldb, g, s);
+            if (int rc = check_out_dtype<F16>(e)) return rc;
+            return launch_any<F16, BN, VR_EPI_ROPE, false, false>(A, lda, B, ldb, g, s);
         case VR_EPI_SWIGLU:
             VR_REQUIRE(g.N % 64 == 0, "vr_gemm: SWIGLU needs N multiple of 64");
-            return launch_any<BN, VR_EPI_SWIGLU, false, false>(A, lda, B, ldb, g, s);
+            if (int rc = check_out_dtype<F16>(e)) return rc;
+            return launch_any<F16, BN, VR_EPI_SWIGLU, false, false>(A, lda, B, ldb, g, s);
         default:
             set_error("vr_gemm: unknown epilogue mode %d", e.mode);
             return 2;
     }
+}
+
+template <bool F16>
+static int dispatch_block_n(const void* A, int64_t lda, const void* B, int64_t ldb, const GemmArgs& g, int bn, cudaStream_t s) {
+    if (bn == PP) return dispatch_mode<F16, -PP>(A, lda, B, ldb, g, s);
+    if (bn == PP_MC) return dispatch_mode<F16, -PP_MC>(A, lda, B, ldb, g, s);
+    if (bn == PP_NFAST) return dispatch_mode<F16, -PP_NFAST>(A, lda, B, ldb, g, s);
+    if (bn == 3) return dispatch_swapped<F16>(A, lda, B, ldb, g, s);
+    if (bn == 256) return dispatch_mode<F16, 256>(A, lda, B, ldb, g, s);
+    if (bn == 192) return dispatch_mode<F16, 192>(A, lda, B, ldb, g, s);
+    if (bn == 128) return dispatch_mode<F16, 128>(A, lda, B, ldb, g, s);
+    if (bn == 64) return dispatch_mode<F16, 64>(A, lda, B, ldb, g, s);
+    set_error("vr_gemm: block_n must be 0 (auto), 64, 128, 192, 256, 2 / 4 / 5 (ping-pong) or 3 (feature-major accumulator)");
+    return 2;
 }
 
 }  // namespace vr
@@ -117,7 +152,7 @@ extern "C" int vr_gemm_tuned(const void* A, int64_t lda, const void* B, int64_t 
     using namespace vr;
     VR_REQUIRE(A && B && epi && epi->out, "vr_gemm: null pointer argument");
     VR_REQUIRE(M > 0 && N > 0 && K > 0, "vr_gemm: empty problem M=%d N=%d K=%d", M, N, K);
-    VR_REQUIRE(ab_dtype == VR_BF16, "vr_gemm: only bf16 operands are instantiated (got dtype %d)", ab_dtype);
+    VR_REQUIRE(ab_dtype == VR_BF16 || ab_dtype == VR_F16, "vr_gemm: operands must be bf16 or fp16 (got dtype %d)", ab_dtype);
     VR_REQUIRE(N % 8 == 0, "vr_gemm: N=%d must be a multiple of 8", N);
     VR_REQUIRE(K % 8 == 0, "vr_gemm: K=%d must be a multiple of 8 (16-byte TMA rows)", K);
     const int64_t out_cols = epi->mode == VR_EPI_SWIGLU ? N / 2 : N;
@@ -136,16 +171,7 @@ extern "C" int vr_gemm_tuned(const void* A, int64_t lda, const void* B, int64_t 
         // mainloop-bound ones (gate|up, RoPE qkv).
         bn = M <= 128 ? 64 : PP_MC;
     }
-    if (bn == PP) return dispatch_mode<-PP>(A, lda, B, ldb, g, s);
-    if (bn == PP_MC) return dispatch_mode<-PP_MC>(A, lda, B, ldb, g, s);
-    if (bn == PP_NFAST) return dispatch_mode<-PP_NFAST>(A, lda, B, ldb, g, s);
-    if (bn == 3) return dispatch_swapped(A, lda, B, ldb, g, s);
-    if (bn == 256) return dispatch_mode<256>(A, lda, B, ldb, g, s);
-    if (bn == 192) return dispatch_mode<192>(A, lda, B, ldb, g, s);
-    if (bn == 128) return dispatch_mode<128>(A, lda, B, ldb, g, s);
-    if (bn == 64) return dispatch_mode<64>(A, lda, B, ldb, g, s);
-    set_error("vr_gemm: block_n must be 0 (auto), 64, 128, 192, 256, 2 / 4 / 5 (ping-pong) or 3 (feature-major accumulator)");
-    return 2;
+    return ab_dtype == VR_F16 ? dispatch_block_n<true>(A, lda, B, ldb, g, bn, s) : dispatch_block_n<false>(A, lda, B, ldb, g, bn, s);
 }
 
 extern "C" int vr_gemm(const void* A, int64_t lda, const void* B, int64_t ldb, int32_t ab_dtype, int32_t M, int32_t N,

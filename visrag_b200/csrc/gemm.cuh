@@ -6,7 +6,7 @@
 //                                          memory, fp32 accumulators in registers (BN/2 per thread), then the fused
 //                                          epilogue (bias / GELU / residual / RoPE / SwiGLU) straight from the
 //                                          accumulator fragments: a thread holds pairs of adjacent columns, so
-//                                          global accesses are 8-byte (fp32) or 4-byte (bf16) and a quad of lanes
+//                                          global accesses are 8-byte (fp32) or 4-byte (bf16 / fp16) and a quad of lanes
 //                                          covers one 32-byte sector of a row.
 //
 // Two mbarrier arrays: smem full (TMA -> consumers, transaction bytes) and empty (8 consumer warps -> TMA).
@@ -23,7 +23,7 @@
 namespace vr {
 
 constexpr int GEMM_BM = 128;
-constexpr int GEMM_BK = 64;  // 64 bf16 = 128 B = one swizzle-128B row
+constexpr int GEMM_BK = 64;  // 64 bf16 / fp16 = 128 B = one swizzle-128B row
 constexpr int GEMM_THREADS = 3 * 128;  // producer warpgroup + two consumer warpgroups
 
 template <int BN>
@@ -129,8 +129,9 @@ __device__ __forceinline__ float silu(float x) {
 // ---------------------------------------------------------------------------------------
 // Epilogue, per accumulator fragment pair (two adjacent columns of one row).
 // ---------------------------------------------------------------------------------------
+// F16: the operands are fp16 and every 16-bit output is fp16 (else bf16); the fp32 arithmetic does not change.
 // LINEAR: out = [resid +] scale * gelu?(acc + bias) [+ rowadd[row % period]]; columns col, col + 1 (col even, N % 8 == 0)
-template <bool OUT_F32, bool GELU>
+template <bool F16, bool OUT_F32, bool GELU>
 __device__ __forceinline__ void epi_linear2(const GemmArgs& g, int row, int col, float x0, float x1) {
     const vr_gemm_epilogue& e = g.epi;
     if (row >= g.M || col >= g.N) return;
@@ -150,11 +151,11 @@ __device__ __forceinline__ void epi_linear2(const GemmArgs& g, int row, int col,
         x0 += r2.x; x1 += r2.y;
     }
     if (OUT_F32) *reinterpret_cast<float2*>(reinterpret_cast<float*>(e.out) + o) = make_float2(x0, x1);
-    else *reinterpret_cast<uint32_t*>(reinterpret_cast<__nv_bfloat16*>(e.out) + o) = pack_bf16x2(x0, x1);
+    else *reinterpret_cast<uint32_t*>(reinterpret_cast<half16_t<F16>*>(e.out) + o) = pack16x2<F16>(x0, x1);
 }
 
 // LINEAR, feature-major accumulator (SWAP kernels: the WEIGHT tile is the MMA's M operand, tokens are its N): one element
-template <bool OUT_F32, bool GELU>
+template <bool F16, bool OUT_F32, bool GELU>
 __device__ __forceinline__ void epi_linear_t(const GemmArgs& g, int tok, int f, float x) {
     const vr_gemm_epilogue& e = g.epi;
     if (tok >= g.M || f >= g.N) return;
@@ -168,12 +169,13 @@ __device__ __forceinline__ void epi_linear_t(const GemmArgs& g, int tok, int f, 
     const long long o = static_cast<long long>(tok) * e.ldo + f;
     if (e.resid) x += e.resid[o];
     if (OUT_F32) reinterpret_cast<float*>(e.out)[o] = x;
-    else reinterpret_cast<__nv_bfloat16*>(e.out)[o] = __float2bfloat16_rn(x);
+    else reinterpret_cast<half16_t<F16>*>(e.out)[o] = to_half16<F16>(x);
 }
 
 // RoPE (modeling_minicpm.py:259-290): a head is 64 columns [lo(32) | hi(32)];
 //   lo' = lo*cos - hi*sin ; hi' = hi*cos + lo*sin   with cos/sin[pos, 0..31].
 // (lo0, lo1) are columns head0 + c, head0 + c + 1 and (hi0, hi1) the columns 32 further, c even in [0, 32).
+template <bool F16>
 __device__ __forceinline__ void epi_rope2(const GemmArgs& g, int row, int head0, int c, float lo0, float lo1, float hi0,
                                           float hi1) {
     const vr_gemm_epilogue& e = g.epi;
@@ -186,17 +188,18 @@ __device__ __forceinline__ void epi_rope2(const GemmArgs& g, int row, int head0,
         lo0 = a0 * cs.x - b0 * sn.x; hi0 = b0 * cs.x + a0 * sn.x;
         lo1 = a1 * cs.y - b1 * sn.y; hi1 = b1 * cs.y + a1 * sn.y;
     }
-    __nv_bfloat16* o = reinterpret_cast<__nv_bfloat16*>(e.out) + static_cast<long long>(row) * e.ldo + head0 + c;
-    *reinterpret_cast<uint32_t*>(o) = pack_bf16x2(lo0, lo1);
-    *reinterpret_cast<uint32_t*>(o + 32) = pack_bf16x2(hi0, hi1);
+    half16_t<F16>* o = reinterpret_cast<half16_t<F16>*>(e.out) + static_cast<long long>(row) * e.ldo + head0 + c;
+    *reinterpret_cast<uint32_t*>(o) = pack16x2<F16>(lo0, lo1);
+    *reinterpret_cast<uint32_t*>(o + 32) = pack16x2<F16>(hi0, hi1);
 }
 
-// SwiGLU (modeling_minicpm.py:333): accumulator columns [gate(32) | up(32)] -> 32 bf16 outputs at column blk0/2.
+// SwiGLU (modeling_minicpm.py:333): accumulator columns [gate(32) | up(32)] -> 32 16-bit outputs at column blk0/2.
+template <bool F16>
 __device__ __forceinline__ void epi_swiglu2(const GemmArgs& g, int row, int blk0, int c, float g0, float g1, float u0, float u1) {
     const vr_gemm_epilogue& e = g.epi;
     if (row >= g.M || blk0 >= g.N) return;
-    __nv_bfloat16* o = reinterpret_cast<__nv_bfloat16*>(e.out) + static_cast<long long>(row) * e.ldo + (blk0 >> 1) + c;
-    *reinterpret_cast<uint32_t*>(o) = pack_bf16x2(silu(g0) * u0, silu(g1) * u1);
+    half16_t<F16>* o = reinterpret_cast<half16_t<F16>*>(e.out) + static_cast<long long>(row) * e.ldo + (blk0 >> 1) + c;
+    *reinterpret_cast<uint32_t*>(o) = pack16x2<F16>(silu(g0) * u0, silu(g1) * u1);
 }
 
 // ---------------------------------------------------------------------------------------
@@ -204,7 +207,7 @@ __device__ __forceinline__ void epi_swiglu2(const GemmArgs& g, int row, int blk0
 // rows are output features (128 per tile), accumulator columns are tokens (BN per tile). g keeps its meaning
 // (M tokens, N features). wgmma's M is fixed at 64 while its N goes down to 8, so this is the form for few tokens.
 // Feature blocks vary fastest so that co-running CTAs share one activation tile in L2.
-template <int BN, int MODE, bool OUT_F32, bool GELU, bool SWAP = false>
+template <bool F16, int BN, int MODE, bool OUT_F32, bool GELU, bool SWAP = false>
 __global__ void __launch_bounds__(GEMM_THREADS, 1)
 gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b, const GemmArgs g) {
     using Cfg = GemmCfg<BN>;
@@ -285,7 +288,7 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_const
                 // +32 B (= +2 in the >>4 address field) per 16-element K step inside the 128 B swizzle row
 #pragma unroll
                 for (int kk = 0; kk < 4; ++kk)
-                    wgmma_ss<false, false>(acc, ad + 2 * kk, bd + 2 * kk, (kb | kk) != 0, std::integral_constant<int, BN>());
+                    wgmma_ss<F16, false>(acc, ad + 2 * kk, bd + 2 * kk, (kb | kk) != 0, std::integral_constant<int, BN>());
                 wgmma_commit();
                 if (prev >= 0) {
                     wgmma_wait<1>();  // the MMAs of the previous k-block retired: hand its slot back
@@ -305,13 +308,13 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_const
                 for (int j = 0; j < BN / 8; ++j) {
                     const int c = n0 + j * 8 + q * 2;
                     if (SWAP) {
-                        epi_linear_t<OUT_F32, GELU>(g, c, r0, acc[4 * j]);
-                        epi_linear_t<OUT_F32, GELU>(g, c + 1, r0, acc[4 * j + 1]);
-                        epi_linear_t<OUT_F32, GELU>(g, c, r0 + 8, acc[4 * j + 2]);
-                        epi_linear_t<OUT_F32, GELU>(g, c + 1, r0 + 8, acc[4 * j + 3]);
+                        epi_linear_t<F16, OUT_F32, GELU>(g, c, r0, acc[4 * j]);
+                        epi_linear_t<F16, OUT_F32, GELU>(g, c + 1, r0, acc[4 * j + 1]);
+                        epi_linear_t<F16, OUT_F32, GELU>(g, c, r0 + 8, acc[4 * j + 2]);
+                        epi_linear_t<F16, OUT_F32, GELU>(g, c + 1, r0 + 8, acc[4 * j + 3]);
                     } else {
-                        epi_linear2<OUT_F32, GELU>(g, r0, c, acc[4 * j], acc[4 * j + 1]);
-                        epi_linear2<OUT_F32, GELU>(g, r0 + 8, c, acc[4 * j + 2], acc[4 * j + 3]);
+                        epi_linear2<F16, OUT_F32, GELU>(g, r0, c, acc[4 * j], acc[4 * j + 1]);
+                        epi_linear2<F16, OUT_F32, GELU>(g, r0 + 8, c, acc[4 * j + 2], acc[4 * j + 3]);
                     }
                 }
             } else {
@@ -323,11 +326,11 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_const
                         const int lo = 4 * (hb * 8 + j), hi = 4 * (hb * 8 + j + 4);
                         const int blk0 = n0 + hb * 64, c = j * 8 + q * 2;
                         if (MODE == VR_EPI_ROPE) {
-                            epi_rope2(g, r0, blk0, c, acc[lo], acc[lo + 1], acc[hi], acc[hi + 1]);
-                            epi_rope2(g, r0 + 8, blk0, c, acc[lo + 2], acc[lo + 3], acc[hi + 2], acc[hi + 3]);
+                            epi_rope2<F16>(g, r0, blk0, c, acc[lo], acc[lo + 1], acc[hi], acc[hi + 1]);
+                            epi_rope2<F16>(g, r0 + 8, blk0, c, acc[lo + 2], acc[lo + 3], acc[hi + 2], acc[hi + 3]);
                         } else {
-                            epi_swiglu2(g, r0, blk0, c, acc[lo], acc[lo + 1], acc[hi], acc[hi + 1]);
-                            epi_swiglu2(g, r0 + 8, blk0, c, acc[lo + 2], acc[lo + 3], acc[hi + 2], acc[hi + 3]);
+                            epi_swiglu2<F16>(g, r0, blk0, c, acc[lo], acc[lo + 1], acc[hi], acc[hi + 1]);
+                            epi_swiglu2<F16>(g, r0 + 8, blk0, c, acc[lo + 2], acc[lo + 3], acc[hi + 2], acc[hi + 3]);
                         }
                     }
                 }
@@ -396,7 +399,7 @@ inline PPSched pp_schedule(int M, int N, int K, int cluster, bool l2_slices) {
 // fragment pair waits for a full memory round trip. Here the loads of PP_EPI_BATCH column groups (both rows) are
 // issued together before any of their stores - one round trip per batch.
 constexpr int PP_EPI_BATCH = 4;
-template <bool OUT_F32, bool GELU>
+template <bool F16, bool OUT_F32, bool GELU>
 __device__ __forceinline__ void pp_epilogue_linear(const GemmArgs& g, const float (&acc)[64], int r0, int n0, int q2) {
     const vr_gemm_epilogue& e = g.epi;
     const bool row_ok[2] = {r0 < g.M, r0 + 8 < g.M};
@@ -435,17 +438,17 @@ __device__ __forceinline__ void pp_epilogue_linear(const GemmArgs& g, const floa
                 if (e.rowadd) { x0 += add[j][h].x; x1 += add[j][h].y; }
                 if (e.resid) { x0 += res[j][h].x; x1 += res[j][h].y; }
                 if (OUT_F32) *reinterpret_cast<float2*>(reinterpret_cast<float*>(e.out) + o[h] + c) = make_float2(x0, x1);
-                else *reinterpret_cast<uint32_t*>(reinterpret_cast<__nv_bfloat16*>(e.out) + o[h] + c) = pack_bf16x2(x0, x1);
+                else *reinterpret_cast<uint32_t*>(reinterpret_cast<half16_t<F16>*>(e.out) + o[h] + c) = pack16x2<F16>(x0, x1);
             }
         }
     }
 }
 
 // epilogue of one 64 x 128 row half: accumulator rows r0 and r0 + 8, columns n0 + 8 j + q2 (+1), q2 = 2 (lane % 4)
-template <int MODE, bool OUT_F32, bool GELU>
+template <bool F16, int MODE, bool OUT_F32, bool GELU>
 __device__ __forceinline__ void pp_epilogue(const GemmArgs& g, const float (&acc)[64], int r0, int n0, int q2) {
     if (MODE == VR_EPI_LINEAR) {
-        pp_epilogue_linear<OUT_F32, GELU>(g, acc, r0, n0, q2);
+        pp_epilogue_linear<F16, OUT_F32, GELU>(g, acc, r0, n0, q2);
     } else {
         // 64-column blocks (a RoPE head / a gate|up pair): columns c and c + 32 sit in the same thread
 #pragma unroll
@@ -455,11 +458,11 @@ __device__ __forceinline__ void pp_epilogue(const GemmArgs& g, const float (&acc
                 const int lo = 4 * (hb * 8 + j), hi = 4 * (hb * 8 + j + 4);
                 const int blk0 = n0 + hb * 64, c = j * 8 + q2;
                 if (MODE == VR_EPI_ROPE) {
-                    epi_rope2(g, r0, blk0, c, acc[lo], acc[lo + 1], acc[hi], acc[hi + 1]);
-                    epi_rope2(g, r0 + 8, blk0, c, acc[lo + 2], acc[lo + 3], acc[hi + 2], acc[hi + 3]);
+                    epi_rope2<F16>(g, r0, blk0, c, acc[lo], acc[lo + 1], acc[hi], acc[hi + 1]);
+                    epi_rope2<F16>(g, r0 + 8, blk0, c, acc[lo + 2], acc[lo + 3], acc[hi + 2], acc[hi + 3]);
                 } else {
-                    epi_swiglu2(g, r0, blk0, c, acc[lo], acc[lo + 1], acc[hi], acc[hi + 1]);
-                    epi_swiglu2(g, r0 + 8, blk0, c, acc[lo + 2], acc[lo + 3], acc[hi + 2], acc[hi + 3]);
+                    epi_swiglu2<F16>(g, r0, blk0, c, acc[lo], acc[lo + 1], acc[hi], acc[hi + 1]);
+                    epi_swiglu2<F16>(g, r0 + 8, blk0, c, acc[lo + 2], acc[lo + 3], acc[hi + 2], acc[hi + 3]);
                 }
             }
         }
@@ -472,7 +475,7 @@ __device__ __forceinline__ void pp_epilogue(const GemmArgs& g, const float (&acc
 // into it too): every consumer warp arrives on the empty barrier of both CTAs. Both CTAs walk the same unit sequence,
 // so their rings stay in step. With an odd number of M tiles the last pair's second tile lies past M: TMA fills it
 // with zeros (the bytes still count) and the epilogue's row guard drops it.
-template <int MODE, bool OUT_F32, bool GELU, int CLUSTER>
+template <bool F16, int MODE, bool OUT_F32, bool GELU, int CLUSTER>
 __global__ void __launch_bounds__(GEMM_THREADS, 1)
 gemm_pingpong_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b, const GemmArgs g,
                      const PPSched sch) {
@@ -565,8 +568,8 @@ gemm_pingpong_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_co
                 wgmma_fence();
 #pragma unroll
                 for (int kk = 0; kk < 4; ++kk) {
-                    wgmma_ss<false, false>(acc0, ad + 2 * kk, bd + 2 * kk, (kb | kk) != 0, std::integral_constant<int, 128>());
-                    wgmma_ss<false, false>(acc1, ad + HALF + 2 * kk, bd + 2 * kk, (kb | kk) != 0,
+                    wgmma_ss<F16, false>(acc0, ad + 2 * kk, bd + 2 * kk, (kb | kk) != 0, std::integral_constant<int, 128>());
+                    wgmma_ss<F16, false>(acc1, ad + HALF + 2 * kk, bd + 2 * kk, (kb | kk) != 0,
                                            std::integral_constant<int, 128>());
                 }
                 wgmma_commit();
@@ -587,8 +590,8 @@ gemm_pingpong_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_co
             int um, tn;
             sch.coords(u, um, tn);
             const int m0 = (um * CLUSTER + rank) * GEMM_BM, n0 = tn * GEMM_PP_BN;
-            pp_epilogue<MODE, OUT_F32, GELU>(g, acc0, m0 + warp * 16 + g8, n0, q * 2);
-            pp_epilogue<MODE, OUT_F32, GELU>(g, acc1, m0 + 64 + warp * 16 + g8, n0, q * 2);
+            pp_epilogue<F16, MODE, OUT_F32, GELU>(g, acc0, m0 + warp * 16 + g8, n0, q * 2);
+            pp_epilogue<F16, MODE, OUT_F32, GELU>(g, acc1, m0 + 64 + warp * 16 + g8, n0, q * 2);
         }
     }
     // The partner may still multicast into this CTA's ring or arrive on its barriers until it has drained its own

@@ -208,15 +208,24 @@ VR_WGMMA_SS(192, 96, VR_N96, VR_R96, 96, 97, 98)
 #define VR_R128(d, i) VR_R64(d, i), VR_R64(d, i + 64)
 VR_WGMMA_SS(256, 128, VR_N128, VR_R128, 128, 129, 130)
 
-// A (bf16 pairs, the m16n8k16 A-fragment layout of each warp) from registers, B MN-major bf16 from shared memory
+// A (16-bit pairs, the m16n8k16 A-fragment layout of each warp) from registers, B MN-major from shared memory;
+// F16: both operands fp16 (else bf16)
 #define VR_WGMMA_RS(NN, NREG, NAMES, REGS, A0, A1, A2, A3, B0, P0)                                                      \
+    template <bool F16>                                                                                                 \
     __device__ __forceinline__ void wgmma_rs_tb(float (&d)[NREG], const uint32_t (&a)[4], uint64_t bdesc, int accumulate, \
                                                 std::integral_constant<int, NN>) {                                      \
-        asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %" #P0 ", 0;\n\t"                                             \
-                     "wgmma.mma_async.sync.aligned.m64n" #NN "k16.f32.bf16.bf16 {" NAMES "}, {%" #A0 ", %" #A1 ", %" #A2 \
-                     ", %" #A3 "}, %" #B0 ", p, 1, 1, 1;\n\t}\n"                                                        \
-                     : REGS(d, 0)                                                                                       \
-                     : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(bdesc), "r"(accumulate));                        \
+        if (F16)                                                                                                        \
+            asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %" #P0 ", 0;\n\t"                                         \
+                         "wgmma.mma_async.sync.aligned.m64n" #NN "k16.f32.f16.f16 {" NAMES "}, {%" #A0 ", %" #A1 ", %" #A2 \
+                         ", %" #A3 "}, %" #B0 ", p, 1, 1, 1;\n\t}\n"                                                    \
+                         : REGS(d, 0)                                                                                   \
+                         : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(bdesc), "r"(accumulate));                    \
+        else                                                                                                            \
+            asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %" #P0 ", 0;\n\t"                                         \
+                         "wgmma.mma_async.sync.aligned.m64n" #NN "k16.f32.bf16.bf16 {" NAMES "}, {%" #A0 ", %" #A1 ", %" #A2 \
+                         ", %" #A3 "}, %" #B0 ", p, 1, 1, 1;\n\t}\n"                                                    \
+                         : REGS(d, 0)                                                                                   \
+                         : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(bdesc), "r"(accumulate));                    \
     }
 VR_WGMMA_RS(16, 8, VR_N8, VR_R8, 8, 9, 10, 11, 12, 13)
 VR_WGMMA_RS(64, 32, VR_N32, VR_R32, 32, 33, 34, 35, 36, 37)
@@ -247,9 +256,29 @@ __device__ __forceinline__ uint32_t pack_bf16x2(float lo, float hi) {
     __nv_bfloat162 v = __floats2bfloat162_rn(lo, hi);
     return *reinterpret_cast<uint32_t*>(&v);
 }
+// round to nearest even, no flush: results below 2^-14 become fp16 subnormals; beyond 65504 they become inf
 __device__ __forceinline__ uint32_t pack_f16x2(float lo, float hi) {
     __half2 v = __floats2half2_rn(lo, hi);
     return *reinterpret_cast<uint32_t*>(&v);
+}
+
+// The kernels of the encode path store their 16-bit activations as bf16 or, with F16, as fp16 (one engine, one type).
+template <bool F16>
+using half16_t = typename std::conditional<F16, __half, __nv_bfloat16>::type;
+template <bool F16>
+__device__ __forceinline__ uint32_t pack16x2(float lo, float hi) {
+    return F16 ? pack_f16x2(lo, hi) : pack_bf16x2(lo, hi);
+}
+template <bool F16>
+__device__ __forceinline__ half16_t<F16> to_half16(float x) {
+    if constexpr (F16) return __float2half_rn(x);
+    else return __float2bfloat16_rn(x);
+}
+// two 16-bit values of one 32-bit word -> fp32 (exact)
+template <bool F16>
+__device__ __forceinline__ float2 unpack16x2(uint32_t w) {
+    if constexpr (F16) return __half22float2(*reinterpret_cast<const __half2*>(&w));
+    else return __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(&w));
 }
 
 }  // namespace vr

@@ -6,7 +6,10 @@ Replaces the GPU work of `VisRAG_Ret.forward` (`modeling_visrag_ret.py:86-126`),
   * the ViT runs over ALL slices of a batch that share a geometry at once (the reference loops page by page
     with batch 1, `modeling_minicpmv.py:130-135`);
   * LM sequences are packed (cu_seqlens) instead of right-padded;
-  * the residual streams stay fp32 in HBM; every GEMM reads bf16 operands and accumulates in fp32 (registers).
+  * the residual streams stay fp32 in HBM; every GEMM reads 16-bit operands and accumulates in fp32 (registers).
+    The 16-bit type is the engine's `dtype`: bf16 (the default) or fp16, the type of the reference's evaluation
+    (`--dtype float16`). It applies to the weights and to every activation stored in 16 bits; the residual streams, biases,
+    norm and softmax statistics, RoPE tables, pooling and the embeddings stay fp32 in both.
 Every kernel is a C-ABI call (visrag_b200/ops.py); torch only owns the buffers.
 """
 from __future__ import annotations
@@ -38,8 +41,8 @@ class _GraphEntry:
     __slots__ = ("graph", "groups", "src", "pos", "cu", "reps", "launches")
 
 
-def _bf16(t: torch.Tensor, dev) -> torch.Tensor:
-    return t.to(device=dev, dtype=torch.bfloat16).contiguous()
+def _half(t: torch.Tensor, dev, dtype: torch.dtype) -> torch.Tensor:
+    return t.to(device=dev, dtype=dtype).contiguous()
 
 
 def _f32(t: torch.Tensor, dev) -> torch.Tensor:
@@ -59,13 +62,18 @@ def _on_own_device(fn):
 
 class VisRAGEngine:
     """Holds device weights in kernel-ready layouts and runs the encode pipeline. Every public method makes the engine's
-    own device current for its launches, so an engine on cuda:1 works while cuda:0 is the process's current device."""
+    own device current for its launches, so an engine on cuda:1 works while cuda:0 is the process's current device.
+    `dtype` (torch.bfloat16 or torch.float16) is the type of the weights and of every 16-bit activation."""
 
     def __init__(self, cfg: VisRAGConfig, state_dict: Dict[str, torch.Tensor], device: str = "cuda:0",
-                 max_vit_tokens: int = 131072, device_frontend: bool = True, cuda_graphs: Optional[bool] = None):
+                 max_vit_tokens: int = 131072, device_frontend: bool = True, cuda_graphs: Optional[bool] = None,
+                 dtype: torch.dtype = torch.bfloat16):
         cfg.validate()
+        if dtype not in ops.HALF_DTYPES:
+            raise ValueError(f"VisRAGEngine: dtype must be torch.bfloat16 or torch.float16, got {dtype}")
         L.lib()  # fail loudly if the CUDA library is missing
         self.cfg = cfg
+        self.dtype = dtype
         # True: pages travel as raw RGB and are resampled / cut into slices on the GPU (bit-identical to PIL,
         # frontend.py); False: PIL renders the slices on the host as the reference does
         self.device_frontend = device_frontend
@@ -81,7 +89,7 @@ class VisRAGEngine:
             self._load(cfg, state_dict)
 
     def _load(self, cfg: VisRAGConfig, state_dict: Dict[str, torch.Tensor]) -> None:
-        sd, dev = state_dict, self.device
+        sd, dev, dt = state_dict, self.device, self.dtype
         D, E, H, I = cfg.vit_dim, cfg.hidden, cfg.hidden, cfg.inter
         nh, hd, hs = cfg.vit_heads, cfg.vit_head_dim, VIT_HEAD_STRIDE
         with torch.no_grad():
@@ -91,7 +99,7 @@ class VisRAGEngine:
             pw = sd["vpm.patch_embed.proj.weight"].float().reshape(D, P2)
             w = torch.zeros((D, self.patch_k), dtype=torch.float32, device=pw.device)
             w[:, :P2] = pw
-            self.patch_w = _bf16(w, dev)
+            self.patch_w = _half(w, dev, dt)
             self.patch_b = _f32(sd["vpm.patch_embed.proj.bias"], dev)
             self.pos_embed = sd["vpm.pos_embed"].float().cpu()
             self._pos_cache: Dict[Tuple[int, int], torch.Tensor] = {}
@@ -107,29 +115,29 @@ class VisRAGEngine:
                 bpad[:, :, :hd] = bq
                 self.blocks.append(dict(
                     n1w=_f32(sd[p + "norm1.weight"], dev), n1b=_f32(sd[p + "norm1.bias"], dev),
-                    qkv_w=_bf16(wpad.reshape(3 * nh * hs, D), dev), qkv_b=_f32(bpad.reshape(-1), dev),
-                    proj_w=_bf16(sd[p + "attn.proj.weight"], dev), proj_b=_f32(sd[p + "attn.proj.bias"], dev),
+                    qkv_w=_half(wpad.reshape(3 * nh * hs, D), dev, dt), qkv_b=_f32(bpad.reshape(-1), dev),
+                    proj_w=_half(sd[p + "attn.proj.weight"], dev, dt), proj_b=_f32(sd[p + "attn.proj.bias"], dev),
                     n2w=_f32(sd[p + "norm2.weight"], dev), n2b=_f32(sd[p + "norm2.bias"], dev),
-                    fc1_w=_bf16(sd[p + "mlp.fc1.weight"], dev), fc1_b=_f32(sd[p + "mlp.fc1.bias"], dev),
-                    fc2_w=_bf16(sd[p + "mlp.fc2.weight"], dev), fc2_b=_f32(sd[p + "mlp.fc2.bias"], dev),
+                    fc1_w=_half(sd[p + "mlp.fc1.weight"], dev, dt), fc1_b=_f32(sd[p + "mlp.fc1.bias"], dev),
+                    fc2_w=_half(sd[p + "mlp.fc2.weight"], dev, dt), fc2_b=_f32(sd[p + "mlp.fc2.bias"], dev),
                 ))
             self.vnorm_w, self.vnorm_b = _f32(sd["vpm.norm.weight"], dev), _f32(sd["vpm.norm.bias"], dev)
             # ---- Resampler
-            self.rs_kv_w = _bf16(sd["resampler.kv_proj.weight"], dev)
+            self.rs_kv_w = _half(sd["resampler.kv_proj.weight"], dev, dt)
             self.rs_lnkv = (_f32(sd["resampler.ln_kv.weight"], dev), _f32(sd["resampler.ln_kv.bias"], dev))
             self.rs_lnpost = (_f32(sd["resampler.ln_post.weight"], dev), _f32(sd["resampler.ln_post.bias"], dev))
             Win, bin_ = sd["resampler.attn.in_proj_weight"].float(), sd["resampler.attn.in_proj_bias"].float()
-            self.rs_wk, self.rs_bk = _bf16(Win[E:2 * E], dev), _f32(bin_[E:2 * E], dev)
-            self.rs_wv, self.rs_bv = _bf16(Win[2 * E:], dev), _f32(bin_[2 * E:], dev)
-            self.rs_wo, self.rs_bo = _bf16(sd["resampler.attn.out_proj.weight"], dev), _f32(sd["resampler.attn.out_proj.bias"], dev)
-            self.rs_projT = _bf16(sd["resampler.proj"].float().t(), dev)  # y = x @ proj  ->  B operand = proj^T
+            self.rs_wk, self.rs_bk = _half(Win[E:2 * E], dev, dt), _f32(bin_[E:2 * E], dev)
+            self.rs_wv, self.rs_bv = _half(Win[2 * E:], dev, dt), _f32(bin_[2 * E:], dev)
+            self.rs_wo, self.rs_bo = _half(sd["resampler.attn.out_proj.weight"], dev, dt), _f32(sd["resampler.attn.out_proj.bias"], dev)
+            self.rs_projT = _half(sd["resampler.proj"].float().t(), dev, dt)  # y = x @ proj  ->  B operand = proj^T
             # the query side is input independent (`resampler.py:158-160`): Q = Wq (LN_q(query) + pos_8x8) + bq, once
             q_in = ops.layernorm(_f32(sd["resampler.query"], dev), _f32(sd["resampler.ln_q.weight"], dev),
-                                 _f32(sd["resampler.ln_q.bias"], dev), 1e-6, add=_f32(sd["resampler.pos_embed"], dev))[1]
-            self.rs_q = torch.zeros((128, E), dtype=torch.bfloat16, device=dev)  # padded to one 128-row query tile
-            ops.gemm(q_in, _bf16(Win[:E], dev), bias=_f32(bin_[:E], dev), out=self.rs_q[: cfg.query_num])
+                                 _f32(sd["resampler.ln_q.bias"], dev), 1e-6, add=_f32(sd["resampler.pos_embed"], dev), dtype=dt)[1]
+            self.rs_q = torch.zeros((128, E), dtype=dt, device=dev)  # padded to one 128-row query tile
+            ops.gemm(q_in, _half(Win[:E], dev, dt), bias=_f32(bin_[:E], dev), out=self.rs_q[: cfg.query_num])
             # ---- MiniCPM
-            self.embed = _bf16(sd["llm.model.embed_tokens.weight"], dev)
+            self.embed = _half(sd["llm.model.embed_tokens.weight"], dev, dt)
             self.layers = []
             for i in range(cfg.layers):
                 p = f"llm.model.layers.{i}."
@@ -139,8 +147,8 @@ class VisRAGEngine:
                 wgu = torch.stack([wg.reshape(I // 32, 32, H), wu.reshape(I // 32, 32, H)], dim=1).reshape(2 * I, H)
                 self.layers.append(dict(
                     in_w=_f32(sd[p + "input_layernorm.weight"], dev), post_w=_f32(sd[p + "post_attention_layernorm.weight"], dev),
-                    qkv_w=_bf16(wqkv, dev), o_w=_bf16(sd[p + "self_attn.o_proj.weight"], dev),
-                    gu_w=_bf16(wgu, dev), down_w=_bf16(sd[p + "mlp.down_proj.weight"], dev),
+                    qkv_w=_half(wqkv, dev, dt), o_w=_half(sd[p + "self_attn.o_proj.weight"], dev, dt),
+                    gu_w=_half(wgu, dev, dt), down_w=_half(sd[p + "mlp.down_proj.weight"], dev, dt),
                 ))
             self.final_w = _f32(sd["llm.model.norm.weight"], dev)
             inv = 1.0 / (cfg.rope_theta ** (torch.arange(0, cfg.head_dim, 2).float() / cfg.head_dim))
@@ -173,45 +181,45 @@ class VisRAGEngine:
     # ------------------------------------------------------------------------------------------ vision
     @_on_own_device
     def vit_tokens(self, pixels: torch.Tensor) -> torch.Tensor:
-        """uint8 [S,h,w,3] (device) -> final-LayerNorm ViT tokens bf16 [S*N, D]."""
-        cfg = self.cfg
+        """uint8 [S,h,w,3] (device) -> final-LayerNorm ViT tokens [S*N, D] in the engine's dtype."""
+        cfg, dt = self.cfg, self.dtype
         S, h, w, _ = pixels.shape
         gh, gw = h // cfg.patch_size, w // cfg.patch_size
         N, D, nh = gh * gw, cfg.vit_dim, cfg.vit_heads
         M = S * N
-        a = ops.im2col_norm(pixels, cfg.patch_size, self.patch_k)
+        a = ops.im2col_norm(pixels, cfg.patch_size, self.patch_k, dt)
         x = ops.gemm(a, self.patch_w, bias=self.patch_b, rowadd=self._pos_table(gh, gw), out_dtype=torch.float32)
         cu = torch.arange(0, (S + 1) * N, N, dtype=torch.int32, device=self.device)
-        qkv = torch.empty((M, 3 * nh * VIT_HEAD_STRIDE), dtype=torch.bfloat16, device=self.device)
-        att = torch.empty((M, D), dtype=torch.bfloat16, device=self.device)
+        qkv = torch.empty((M, 3 * nh * VIT_HEAD_STRIDE), dtype=dt, device=self.device)
+        att = torch.empty((M, D), dtype=dt, device=self.device)
         scale = cfg.vit_head_dim ** -0.5
         for blk in self.blocks:
-            y = ops.layernorm(x, blk["n1w"], blk["n1b"], cfg.ln_eps)
+            y = ops.layernorm(x, blk["n1w"], blk["n1b"], cfg.ln_eps, dtype=dt)
             ops.gemm(y, blk["qkv_w"], bias=blk["qkv_b"], out=qkv)
             ops.attention(qkv, qkv, qkv, q_col0=0, k_col0=nh * VIT_HEAD_STRIDE, v_col0=2 * nh * VIT_HEAD_STRIDE,
                           head_stride=VIT_HEAD_STRIDE, head_dim=cfg.vit_head_dim, heads=nh, batch=S, cu_k=cu, max_k=N,
                           cu_q=cu, max_q=N, causal=False, scale=scale, out=att)
             ops.gemm(att, blk["proj_w"], bias=blk["proj_b"], resid=x, out=x, out_dtype=torch.float32)
-            y = ops.layernorm(x, blk["n2w"], blk["n2b"], cfg.ln_eps)
+            y = ops.layernorm(x, blk["n2w"], blk["n2b"], cfg.ln_eps, dtype=dt)
             y = ops.gemm(y, blk["fc1_w"], bias=blk["fc1_b"], gelu=True)
             ops.gemm(y, blk["fc2_w"], bias=blk["fc2_b"], resid=x, out=x, out_dtype=torch.float32)
-        return ops.layernorm(x, self.vnorm_w, self.vnorm_b, cfg.ln_eps)
+        return ops.layernorm(x, self.vnorm_w, self.vnorm_b, cfg.ln_eps, dtype=dt)
 
     @_on_own_device
     def resample(self, tokens: torch.Tensor, S: int, gh: int, gw: int, out: torch.Tensor) -> None:
-        """ViT tokens bf16 [S*N, D] -> 64 query tokens per slice, written to fp32 `out` [S*64, E]."""
-        cfg = self.cfg
+        """ViT tokens [S*N, D] (engine dtype) -> 64 query tokens per slice, written to fp32 `out` [S*64, E]."""
+        cfg, dt = self.cfg, self.dtype
         E, N, nh = cfg.hidden, gh * gw, cfg.rs_heads
         kv = ops.gemm(tokens, self.rs_kv_w, out_dtype=torch.float32)
-        v_in, k_in = ops.layernorm(kv, self.rs_lnkv[0], self.rs_lnkv[1], 1e-6, add=self._sincos_table(gh, gw))
+        v_in, k_in = ops.layernorm(kv, self.rs_lnkv[0], self.rs_lnkv[1], 1e-6, add=self._sincos_table(gh, gw), dtype=dt)
         k = ops.gemm(k_in, self.rs_wk, bias=self.rs_bk)
         v = ops.gemm(v_in, self.rs_wv, bias=self.rs_bv)
         cu = torch.arange(0, (S + 1) * N, N, dtype=torch.int32, device=self.device)
-        att = torch.empty((S * cfg.query_num, E), dtype=torch.bfloat16, device=self.device)
+        att = torch.empty((S * cfg.query_num, E), dtype=dt, device=self.device)
         ops.attention(self.rs_q, k, v, q_col0=0, k_col0=0, v_col0=0, head_stride=128, head_dim=128, heads=nh, batch=S,
                       cu_k=cu, max_k=N, cu_q=None, max_q=cfg.query_num, causal=False, scale=128 ** -0.5, out=att)
         o = ops.gemm(att, self.rs_wo, bias=self.rs_bo, out_dtype=torch.float32)
-        o = ops.layernorm(o, self.rs_lnpost[0], self.rs_lnpost[1], 1e-6)
+        o = ops.layernorm(o, self.rs_lnpost[0], self.rs_lnpost[1], 1e-6, dtype=dt)
         ops.gemm(o, self.rs_projT, out=out, out_dtype=torch.float32)
 
     @_on_own_device
@@ -237,22 +245,22 @@ class VisRAGEngine:
     def lm_hidden(self, token_src: torch.Tensor, positions: torch.Tensor, cu: torch.Tensor, max_len: int,
                   vision: Optional[torch.Tensor]) -> torch.Tensor:
         """Packed decoder: returns the fp32 residual stream BEFORE the final RMSNorm, [T, H]."""
-        cfg = self.cfg
+        cfg, dt = self.cfg, self.dtype
         H, nh = cfg.hidden, cfg.heads
         B = cu.shape[0] - 1
         h = ops.build_lm_input(token_src, self.embed, cfg.scale_emb, vision)
         T = h.shape[0]
-        qkv = torch.empty((T, 3 * H), dtype=torch.bfloat16, device=self.device)
-        att = torch.empty((T, H), dtype=torch.bfloat16, device=self.device)
+        qkv = torch.empty((T, 3 * H), dtype=dt, device=self.device)
+        att = torch.empty((T, H), dtype=dt, device=self.device)
         s = cfg.depth_scale
         for lyr in self.layers:
-            a = ops.rmsnorm(h, lyr["in_w"], cfg.rms_eps)
+            a = ops.rmsnorm(h, lyr["in_w"], cfg.rms_eps, dt)
             ops.gemm(a, lyr["qkv_w"], mode=L.VR_EPI_ROPE, positions=positions, rope_cos=self.rope_cos,
                      rope_sin=self.rope_sin, rope_cols=2 * H, out=qkv)
             ops.attention(qkv, qkv, qkv, q_col0=0, k_col0=H, v_col0=2 * H, head_stride=64, head_dim=64, heads=nh, batch=B,
                           cu_k=cu, max_k=max_len, cu_q=cu, max_q=max_len, causal=True, scale=cfg.head_dim ** -0.5, out=att)
             ops.gemm(att, lyr["o_w"], resid=h, out=h, scale=s, out_dtype=torch.float32)
-            a = ops.rmsnorm(h, lyr["post_w"], cfg.rms_eps)
+            a = ops.rmsnorm(h, lyr["post_w"], cfg.rms_eps, dt)
             a = ops.gemm(a, lyr["gu_w"], mode=L.VR_EPI_SWIGLU)
             ops.gemm(a, lyr["down_w"], resid=h, out=h, scale=s, out_dtype=torch.float32)
         return h

@@ -94,20 +94,31 @@ def load_checkpoint(path: str) -> Dict[str, torch.Tensor]:
     return sd
 
 
-class VisRAGRetB200:
-    """B1 boundary: the backbone (`lm_q`)."""
+def is_float16(dtype) -> bool:
+    """True for the reference's fp16 setting: torch.float16 (`torch_dtype=`) or "float16" (`--dtype float16`, what
+    `DRModel.build` maps to torch.float16, `dense_retrieval_model.py:301-309`)."""
+    return dtype is torch.float16 or dtype in ("float16", "fp16", "half", "torch.float16")
 
-    def __init__(self, cfg: VisRAGConfig, state_dict: Dict[str, torch.Tensor], device: str = "cuda:0"):
+
+class VisRAGRetB200:
+    """B1 boundary: the backbone (`lm_q`). `dtype` is the engine's 16-bit type: torch.bfloat16 (default) or torch.float16."""
+
+    def __init__(self, cfg: VisRAGConfig, state_dict: Dict[str, torch.Tensor], device: str = "cuda:0",
+                 dtype: torch.dtype = torch.bfloat16):
         self.config = cfg
-        self.engine = VisRAGEngine(cfg, state_dict, device)
+        self.engine = VisRAGEngine(cfg, state_dict, device, dtype=dtype)
         self.device = self.engine.device
-        self.dtype = torch.bfloat16
+        self.dtype = self.engine.dtype
         self.training = False
 
     @classmethod
     def from_pretrained(cls, path: str, config=None, torch_dtype=None, attn_implementation=None, device: str = "cuda:0", **_):
+        """torch_dtype=torch.float16 builds an fp16 engine (weights and 16-bit activations in fp16). Anything else -
+        None, torch.bfloat16, torch.float32 - builds the bf16 engine: there is no fp32 encode path, so float32 runs bf16."""
         with open(os.path.join(path, "config.json")) as f:
             cfg = config_from_hf(json.load(f))
+        if is_float16(torch_dtype):
+            return cls(cfg, load_checkpoint(path), device, dtype=torch.float16)
         return cls(cfg, load_checkpoint(path), device)
 
     def eval(self):
@@ -129,7 +140,7 @@ class VisRAGRetB200:
         groups, src, pos, cu = eng.upload(pb)
         vision = eng.encode_vision(groups, pb.group_row0, pb.n_slices)
         h = eng.lm_hidden(src, pos, cu, int(pb.seq_lens.max()), vision)
-        hn = ops.rmsnorm(h, eng.final_w, self.config.rms_eps)  # final norm (`modeling_minicpm.py:1280`)
+        hn = ops.rmsnorm(h, eng.final_w, self.config.rms_eps, eng.dtype)  # final norm (`modeling_minicpm.py:1280`)
         B, Lmax = pb.n_items, int(pb.seq_lens.max())
         out = torch.zeros((B, Lmax, self.config.hidden), dtype=hn.dtype, device=self.device)
         mask = torch.zeros((B, Lmax), dtype=torch.int8, device=self.device)
@@ -156,8 +167,13 @@ class DRModelForInference:
 
     @classmethod
     def build(cls, model_args, cache_dir=None, device: str = "cuda:0", **_):
-        """`DRModel.build` (`dense_retrieval_model.py:233-366`) for a VisRAG-Ret checkpoint directory."""
-        lm = VisRAGRetB200.from_pretrained(model_args.model_name_or_path, device=device)
+        """`DRModel.build` (`dense_retrieval_model.py:233-366`) for a VisRAG-Ret checkpoint directory. `model_args.dtype`
+        "float16" (the reference evaluation's `--dtype float16`) builds an fp16 engine; "bfloat16", "float32" or no dtype
+        build the bf16 one (float32 runs bf16: there is no fp32 encode path)."""
+        if is_float16(getattr(model_args, "dtype", None)):
+            lm = VisRAGRetB200.from_pretrained(model_args.model_name_or_path, torch_dtype=torch.float16, device=device)
+        else:
+            lm = VisRAGRetB200.from_pretrained(model_args.model_name_or_path, device=device)
         return cls(lm_q=lm, feature=getattr(model_args, "feature", "last_hidden_state"), pooling=model_args.pooling,
                    attention=getattr(model_args, "attention", "causal"), normalize=model_args.normalize, model_args=model_args)
 

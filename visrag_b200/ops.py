@@ -46,10 +46,30 @@ def _launch(kind: str, flops: float, fn, *args) -> None:
     _PROF.append((kind, e0, e1, flops))
 
 
-def _bf16_2d(t: torch.Tensor, name: str) -> None:
-    if t.dtype != torch.bfloat16 or t.dim() != 2 or t.stride(1) != 1 or not t.is_cuda:
-        raise ValueError(f"{name}: expected a CUDA bf16 matrix with unit inner stride, got {t.dtype} {tuple(t.shape)}")
-    L.check_device(t)
+HALF_DTYPES = (torch.bfloat16, torch.float16)  # the 16-bit types of the kernels' operands and activations
+_VR_DTYPE = {torch.bfloat16: L.VR_BF16, torch.float16: L.VR_F16, torch.float32: L.VR_F32}
+
+
+def _half_operands(**named: torch.Tensor) -> torch.dtype:
+    """The named tensors are all bf16 or all fp16 CUDA matrices with unit inner stride; returns their dtype. The dtype
+    checks run first, over all of them, before anything looks at a device."""
+    dtype = next(iter(named.values())).dtype
+    for name, t in named.items():
+        if t.dtype not in HALF_DTYPES:
+            raise ValueError(f"{name}: expected a bf16 or fp16 matrix, got {t.dtype} {tuple(t.shape)}")
+        if t.dtype != dtype:
+            raise ValueError(f"{name}: is {t.dtype} but the other operands are {dtype}: bf16 and fp16 operands do not mix")
+    for name, t in named.items():
+        if t.dim() != 2 or t.stride(1) != 1 or not t.is_cuda:
+            raise ValueError(f"{name}: expected a CUDA {t.dtype} matrix with unit inner stride, got {tuple(t.shape)}")
+        L.check_device(t)
+    return dtype
+
+
+def _half_dtype(dtype: torch.dtype, name: str) -> int:
+    if dtype not in HALF_DTYPES:
+        raise ValueError(f"{name}: the 16-bit output type must be bf16 or fp16, got {dtype}")
+    return _VR_DTYPE[dtype]
 
 
 def gemm(
@@ -62,7 +82,7 @@ def gemm(
     resid: Optional[torch.Tensor] = None,
     rowadd: Optional[torch.Tensor] = None,
     out: Optional[torch.Tensor] = None,
-    out_dtype: torch.dtype = torch.bfloat16,
+    out_dtype: Optional[torch.dtype] = None,
     mode: int = L.VR_EPI_LINEAR,
     positions: Optional[torch.Tensor] = None,
     rope_cos: Optional[torch.Tensor] = None,
@@ -70,20 +90,21 @@ def gemm(
     rope_cols: int = 0,
     block_n: int = 0,
 ) -> torch.Tensor:
-    """``out = epilogue(a @ w.T)`` on wgmma. ``a`` [M,K] bf16, ``w`` [N,K] bf16 (nn.Linear layout).
+    """``out = epilogue(a @ w.T)`` on wgmma. ``a`` [M,K], ``w`` [N,K] (nn.Linear layout), both bf16 or both fp16.
 
-    LINEAR: ``out = [resid +] scale * gelu?(a@w.T + bias) [+ rowadd[row % period]]``; bf16 or fp32 out.
-    ROPE / SWIGLU: see include/visrag_b200.h.
+    LINEAR: ``out = [resid +] scale * gelu?(a@w.T + bias) [+ rowadd[row % period]]``; out in the operands' type (the
+    default) or fp32. ROPE / SWIGLU write the operands' type; see include/visrag_b200.h.
     """
-    _bf16_2d(a, "a")
-    _bf16_2d(w, "w")
+    _half_operands(a=a, w=w)
     M, K = a.shape
     N, K2 = w.shape
     if K != K2:
         raise ValueError(f"gemm: K mismatch {K} vs {K2}")
     out_cols = N // 2 if mode == L.VR_EPI_SWIGLU else N
-    if mode != L.VR_EPI_LINEAR:
-        out_dtype = torch.bfloat16
+    if mode != L.VR_EPI_LINEAR or out_dtype is None:
+        out_dtype = a.dtype
+    if out_dtype not in (a.dtype, torch.float32):
+        raise ValueError(f"gemm: {a.dtype} operands write {a.dtype} or float32, not {out_dtype}")
     if out is None:
         out = torch.empty((M, out_cols), dtype=out_dtype, device=a.device)
     if out.dtype != out_dtype or out.shape != (M, out_cols) or out.stride(1) != 1:
@@ -95,7 +116,7 @@ def gemm(
         raise ValueError("gemm: resid must match out (shape and row pitch)")
     e = L.GemmEpilogue()
     e.mode = mode
-    e.out_dtype = L.VR_F32 if out_dtype == torch.float32 else L.VR_BF16
+    e.out_dtype = _VR_DTYPE[out_dtype]
     e.act_gelu = int(gelu)
     e.scale = float(scale)
     e.bias = L.ptr(bias)
@@ -110,8 +131,8 @@ def gemm(
     e.ldo = out.stride(0)
     kind = "gemm" if _PROF is None else f"gemm:{M}x{N}x{K}:" + ("rope" if mode == L.VR_EPI_ROPE else "swiglu" if mode == L.VR_EPI_SWIGLU
                                                                else ("gelu" if gelu else "") + ("+resid" if resid is not None else "") +
-                                                               ("f32" if out_dtype == torch.float32 else "bf16"))
-    _launch(kind, 2.0 * M * N * K, L.lib().vr_gemm_tuned, a.data_ptr(), a.stride(0), w.data_ptr(), w.stride(0), L.VR_BF16,
+                                                               ("f32" if out_dtype == torch.float32 else "bf16" if out_dtype == torch.bfloat16 else "f16"))
+    _launch(kind, 2.0 * M * N * K, L.lib().vr_gemm_tuned, a.data_ptr(), a.stride(0), w.data_ptr(), w.stride(0), _VR_DTYPE[a.dtype],
             M, N, K, C.byref(e), block_n, L.stream_ptr())
     return out
 
@@ -121,9 +142,9 @@ def attention(
     head_dim: int, heads: int, batch: int, cu_k: torch.Tensor, max_k: int, cu_q: Optional[torch.Tensor], max_q: int,
     causal: bool, scale: float, out: torch.Tensor, v_ones_column: bool = False,
 ) -> torch.Tensor:
-    """softmax(QK^T*scale)V on wgmma; q/k/v are bf16 token matrices (see include/visrag_b200.h)."""
-    for t, n in ((q, "q"), (k, "k"), (v, "v"), (out, "out")):
-        _bf16_2d(t, n)
+    """softmax(QK^T*scale)V on wgmma; q/k/v/out are bf16 or fp16 token matrices, all of one type (see
+    include/visrag_b200.h)."""
+    _half_operands(q=q, k=k, v=v, out=out)
     if cu_k.dtype != torch.int32 or (cu_q is not None and cu_q.dtype != torch.int32):
         raise ValueError("attention: cu_seqlens must be int32")
     p = L.AttnParams()
@@ -136,47 +157,55 @@ def attention(
     p.max_q, p.max_k = max_q, max_k
     p.causal, p.scale = int(causal), float(scale)
     p.out, p.ldo = out.data_ptr(), out.stride(0)
-    p.flags = L.VR_ATTN_V_ONES_COLUMN if v_ones_column else 0
+    p.flags = (L.VR_ATTN_V_ONES_COLUMN if v_ones_column else 0) | (L.VR_ATTN_F16 if q.dtype == torch.float16 else 0)
     _launch("attention", 0.0, L.lib().vr_attention, C.byref(p), L.stream_ptr())
     return out
 
 
-def im2col_norm(pixels: torch.Tensor, patch: int, ld_out: int) -> torch.Tensor:
-    """uint8 [S,h,w,3] -> bf16 patch matrix [S*(h/p)*(w/p), ld_out] (normalised, zero padded columns)."""
+def im2col_norm(pixels: torch.Tensor, patch: int, ld_out: int, dtype: torch.dtype = torch.bfloat16) -> torch.Tensor:
+    """uint8 [S,h,w,3] -> bf16 / fp16 patch matrix [S*(h/p)*(w/p), ld_out] (normalised, zero padded columns)."""
+    vr_dtype = _half_dtype(dtype, "im2col_norm")
     if pixels.dtype != torch.uint8 or pixels.dim() != 4 or pixels.shape[3] != 3 or not pixels.is_contiguous():
         raise ValueError("im2col_norm: expected contiguous uint8 [S,h,w,3]")
     L.check_device(pixels)
     S, h, w, _ = pixels.shape
-    out = torch.empty((S * (h // patch) * (w // patch), ld_out), dtype=torch.bfloat16, device=pixels.device)
-    _launch("im2col", 0.0, L.lib().vr_im2col_norm, pixels.data_ptr(), S, h, w, patch, out.data_ptr(), ld_out, L.stream_ptr())
+    out = torch.empty((S * (h // patch) * (w // patch), ld_out), dtype=dtype, device=pixels.device)
+    _launch("im2col", 0.0, L.lib().vr_im2col_norm_ex, pixels.data_ptr(), S, h, w, patch, out.data_ptr(), ld_out, vr_dtype,
+            L.stream_ptr())
     return out
 
 
-def layernorm(x: torch.Tensor, gamma: torch.Tensor, beta: torch.Tensor, eps: float, *, add: Optional[torch.Tensor] = None):
-    """fp32 [M,D] -> bf16 LN(x); with ``add`` [P,D] also returns LN(x)+add[row % P] (bf16)."""
+def layernorm(x: torch.Tensor, gamma: torch.Tensor, beta: torch.Tensor, eps: float, *, add: Optional[torch.Tensor] = None,
+              dtype: torch.dtype = torch.bfloat16):
+    """fp32 [M,D] -> LN(x) in `dtype` (bf16 or fp16); with ``add`` [P,D] also returns LN(x)+add[row % P] (same dtype)."""
+    vr_dtype = _half_dtype(dtype, "layernorm")
     M, D = x.shape
     L.check_device(x)
-    out = torch.empty((M, D), dtype=torch.bfloat16, device=x.device)
+    out = torch.empty((M, D), dtype=dtype, device=x.device)
     out2 = torch.empty_like(out) if add is not None else None
-    _launch("norm", 0.0, L.lib().vr_layernorm, x.data_ptr(), x.stride(0), gamma.data_ptr(), beta.data_ptr(), eps, M, D,
-            out.data_ptr(), out.stride(0), L.ptr(out2), L.ptr(add), 0 if add is None else add.shape[0], L.stream_ptr())
+    _launch("norm", 0.0, L.lib().vr_layernorm_ex, x.data_ptr(), x.stride(0), gamma.data_ptr(), beta.data_ptr(), eps, M, D,
+            out.data_ptr(), out.stride(0), L.ptr(out2), L.ptr(add), 0 if add is None else add.shape[0], vr_dtype, L.stream_ptr())
     return out if add is None else (out, out2)
 
 
-def rmsnorm(x: torch.Tensor, gamma: torch.Tensor, eps: float) -> torch.Tensor:
+def rmsnorm(x: torch.Tensor, gamma: torch.Tensor, eps: float, dtype: torch.dtype = torch.bfloat16) -> torch.Tensor:
+    """fp32 [M,D] -> RMSNorm(x) in `dtype` (bf16 or fp16)."""
+    vr_dtype = _half_dtype(dtype, "rmsnorm")
     M, D = x.shape
     L.check_device(x)
-    out = torch.empty((M, D), dtype=torch.bfloat16, device=x.device)
-    _launch("norm", 0.0, L.lib().vr_rmsnorm, x.data_ptr(), x.stride(0), gamma.data_ptr(), eps, M, D, out.data_ptr(),
-            out.stride(0), L.stream_ptr())
+    out = torch.empty((M, D), dtype=dtype, device=x.device)
+    _launch("norm", 0.0, L.lib().vr_rmsnorm_ex, x.data_ptr(), x.stride(0), gamma.data_ptr(), eps, M, D, out.data_ptr(),
+            out.stride(0), vr_dtype, L.stream_ptr())
     return out
 
 
 def build_lm_input(src: torch.Tensor, embed: torch.Tensor, scale_emb: float, vision: Optional[torch.Tensor]) -> torch.Tensor:
+    """Packed LM input rows (fp32) from the vision rows and a bf16 or fp16 embedding table."""
+    vr_dtype = _half_dtype(embed.dtype, "build_lm_input")
     T, D = src.shape[0], embed.shape[1]
     L.check_device(embed)
     h = torch.empty((T, D), dtype=torch.float32, device=embed.device)
-    _launch("other", 0.0, L.lib().vr_build_lm_input, src.data_ptr(), T, D, embed.data_ptr(), scale_emb, L.ptr(vision),
+    _launch("other", 0.0, L.lib().vr_build_lm_input_ex, src.data_ptr(), T, D, embed.data_ptr(), vr_dtype, scale_emb, L.ptr(vision),
             0 if vision is None else vision.stride(0), h.data_ptr(), h.stride(0), L.stream_ptr())
     return h
 
