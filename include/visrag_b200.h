@@ -46,6 +46,7 @@ int vr_abi_version(void);
  *   fp16 operands: LINEAR writes VR_F16 or VR_F32; ROPE / SWIGLU write fp16 and need out_dtype = VR_F16;
  *   GELU writes the operands' 16-bit type only. Any other combination is refused before any CUDA call.
  * An fp16 output rounds to nearest with no clamp: a value beyond 65504 is stored as inf.
+ * A LINEAR out must be 16-byte aligned (refused before any CUDA call otherwise); with ldo % 8 == 0 every row then is.
  * ---------------------------------------------------------------------------------- */
 typedef enum {
     VR_EPI_LINEAR = 0, /* out = [resid +] scale*(gelu?(acc + bias)) [+ rowadd[row % period]] */

@@ -7,7 +7,7 @@ at its exact shape and epilogue. The arms alternate in one process over several 
   pp_mc     ping-pong kernel in CTA pairs with the B tile multicast (block_n = 4): pp -> pp_mc is the multicast step
 with plain cuBLAS (torch.matmul, bf16 out, no epilogue) beside them for context.
 
-    python tools/bench_gemm.py [--rounds 5] [--only lm]
+    python tools/bench_gemm.py [--rounds 5] [--only lm] [--match KEY] [--arms auto]
 
 Prints the card name, power limit and SM clocks (read-only nvidia-smi query) first, then one JSON line per class:
 median ms and TFLOP/s of each arm, their spread over rounds ((max - min) / median), and max |arm - old| on the same
@@ -23,8 +23,10 @@ sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 
 # (class key as bench.py's roofline pass names it, launches per step, epilogue arguments)
 CLASSES = [
-    ("131072x4304x1152:gelubf16", 26, {"bias": True, "gelu": True}),          # ViT fc1
-    ("131072x1152x4304:+residf32", 26, {"bias": True, "resid": True}),        # ViT fc2
+    ("131072x4352x1152:gelubf16", 26, {"bias": True, "gelu": True}),          # ViT fc1 (MLP width 4304 padded to 4352)
+    ("131072x1152x4352:+residf32", 26, {"bias": True, "resid": True}),        # ViT fc2
+    ("131072x4304x1152:gelubf16", 0, {"bias": True, "gelu": True}),           # the unpadded fc1 / fc2, for comparison:
+    ("131072x1152x4304:+residf32", 0, {"bias": True, "resid": True}),         #   not in the step
     ("131072x3840x1152:bf16", 26, {"bias": True}),                            # ViT qkv
     ("131072x1152x1152:+residf32", 26, {"bias": True, "resid": True}),        # ViT proj
     ("8704x11520x2304:swiglu", 40, {"swiglu": True}),                         # LM gate|up
@@ -115,6 +117,8 @@ def main():
     ap.add_argument("--only", choices=["vit", "lm"], default=None, help="ViT-side (M = 131072) or LM (M = 8704) classes")
     ap.add_argument("--match", default=None, help="only the classes whose key contains this string")
     ap.add_argument("--no-cublas", dest="cublas", action="store_false")
+    ap.add_argument("--arms", default=None, help="comma-separated subset of old,auto,pp_nfast,pp,pp_mc (old always runs: "
+                                                  "it is the reference of max_abs_diff_vs_old)")
     a = ap.parse_args()
 
     import torch
@@ -129,6 +133,8 @@ def main():
         A, W, run, fresh = make_case(M, N, K, kw, 100 + ci)
         arm_bn = {"old": old_bn, "auto": 0}
         arm_bn.update(PP_ARMS)
+        if a.arms:
+            arm_bn = {k: v for k, v in arm_bn.items() if k == "old" or k in a.arms.split(",")}
         ref = fresh(old_bn)
         diff = {}
         for k, bn in arm_bn.items():

@@ -158,6 +158,9 @@ extern "C" int vr_gemm_tuned(const void* A, int64_t lda, const void* B, int64_t 
     const int64_t out_cols = epi->mode == VR_EPI_SWIGLU ? N / 2 : N;
     VR_REQUIRE(epi->ldo >= out_cols && epi->ldo % 8 == 0, "vr_gemm: ldo=%lld too small or not a multiple of 8",
                (long long)epi->ldo);
+    // the ping-pong kernel stores a 16-bit LINEAR output 16 bytes at a time (ldo % 8 == 0 keeps every row aligned)
+    VR_REQUIRE(epi->mode != VR_EPI_LINEAR || (reinterpret_cast<uintptr_t>(epi->out) & 15) == 0,
+               "vr_gemm: a LINEAR out must be 16-byte aligned (out=%p)", epi->out);
     GemmArgs g;
     g.M = M; g.N = N; g.K = K; g.epi = *epi;
     cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);

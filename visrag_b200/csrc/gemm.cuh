@@ -16,6 +16,7 @@
 // gemm_pingpong_kernel (below) is the same pipeline with a different consumer schedule: each consumer warpgroup owns a
 // whole 128 x 128 tile and the two take turns on the tensor cores, so one tile's epilogue overlaps the next tile's
 // MMAs. vr_gemm uses it, in CTA pairs that share the B tile by multicast, for every problem with more than one row tile.
+// Its LINEAR epilogue stores a 16-bit output 16 bytes per thread after a transpose across each quad of lanes.
 #pragma once
 #include "ptx.cuh"
 #include "../../include/visrag_b200.h"
@@ -394,6 +395,19 @@ inline PPSched pp_schedule(int M, int N, int K, int cluster, bool l2_slices) {
     return s;
 }
 
+// 4 x 4 transpose of 32-bit words across the 4 lanes of a quad (lane q = lane % 4): on entry lane q holds w[j] = E(q, j),
+// on exit w[j] = E(j, q). Two butterfly stages (lane ^ 2, then lane ^ 1), each exchanging the two words whose index bit
+// differs from the lane's. Every lane of the warp must take part.
+__device__ __forceinline__ void quad_transpose4(uint32_t (&w)[4], int q) {
+    const bool b1 = q & 2, b0 = q & 1;
+    uint32_t r0 = __shfl_xor_sync(0xffffffffu, b1 ? w[0] : w[2], 2);
+    uint32_t r1 = __shfl_xor_sync(0xffffffffu, b1 ? w[1] : w[3], 2);
+    if (b1) { w[0] = r0; w[1] = r1; } else { w[2] = r0; w[3] = r1; }
+    r0 = __shfl_xor_sync(0xffffffffu, b0 ? w[0] : w[1], 1);
+    r1 = __shfl_xor_sync(0xffffffffu, b0 ? w[2] : w[3], 1);
+    if (b0) { w[0] = r0; w[2] = r1; } else { w[1] = r0; w[3] = r1; }
+}
+
 // LINEAR epilogue of one 64 x 128 row half, the same arithmetic as epi_linear2 in the same order. The output may be the
 // residual itself (in place), so the compiler cannot move a load above an earlier store: written pair by pair, every
 // fragment pair waits for a full memory round trip. Here the loads of PP_EPI_BATCH column groups (both rows) are
@@ -425,12 +439,13 @@ __device__ __forceinline__ void pp_epilogue_linear(const GemmArgs& g, const floa
                 if (e.resid && col_ok && row_ok[h]) res[j][h] = *reinterpret_cast<const float2*>(e.resid + o[h] + c);
             }
         }
+        uint32_t w16[2][PP_EPI_BATCH];  // 16-bit output: the packed pairs, stored below 16 bytes per thread
 #pragma unroll
         for (int j = 0; j < PP_EPI_BATCH; ++j) {
             const int c = n0 + (jb + j) * 8 + q2;
 #pragma unroll
             for (int h = 0; h < 2; ++h) {
-                if (!row_ok[h] || c >= g.N) continue;
+                if (OUT_F32 && (!row_ok[h] || c >= g.N)) continue;
                 float x0 = acc[4 * (jb + j) + 2 * h], x1 = acc[4 * (jb + j) + 2 * h + 1];
                 if (e.bias) { x0 += bias[j].x; x1 += bias[j].y; }
                 if (GELU) gelu_erf2(x0, x1);
@@ -438,7 +453,21 @@ __device__ __forceinline__ void pp_epilogue_linear(const GemmArgs& g, const floa
                 if (e.rowadd) { x0 += add[j][h].x; x1 += add[j][h].y; }
                 if (e.resid) { x0 += res[j][h].x; x1 += res[j][h].y; }
                 if (OUT_F32) *reinterpret_cast<float2*>(reinterpret_cast<float*>(e.out) + o[h] + c) = make_float2(x0, x1);
-                else *reinterpret_cast<uint32_t*>(reinterpret_cast<half16_t<F16>*>(e.out) + o[h] + c) = pack16x2<F16>(x0, x1);
+                else w16[h][j] = pack16x2<F16>(x0, x1);
+            }
+        }
+        if (!OUT_F32) {
+            // lane q of a quad holds columns 8 (jb + j) + 2q, +1 of the batch's column groups j; after the transpose it
+            // holds all 8 columns of column group jb + q: one 16-byte store per row instead of four 4-byte ones (a
+            // warp's store then fills whole 32-byte sectors of its 8 rows instead of half of each)
+            static_assert(PP_EPI_BATCH == 4, "the quad transpose moves 4 column groups");
+            const int q = q2 >> 1, c = n0 + (jb + q) * 8;
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+                quad_transpose4(w16[h], q);
+                if (row_ok[h] && c < g.N)
+                    *reinterpret_cast<uint4*>(reinterpret_cast<half16_t<F16>*>(e.out) + o[h] + c) =
+                        make_uint4(w16[h][0], w16[h][1], w16[h][2], w16[h][3]);
             }
         }
     }

@@ -21,6 +21,7 @@ from typing import Dict, Optional, Sequence, Tuple
 
 import numpy as np
 import torch
+import torch.nn.functional as F
 
 from . import _lib as L
 from . import ops
@@ -29,6 +30,11 @@ from .host import PreparedBatch, prepare_batch
 from .weights import sincos_2d
 
 VIT_HEAD_STRIDE = 80  # 72 padded to a multiple of 16 (the MMA K step); pad rows of Wqkv are zero
+# The ViT MLP width is padded to a multiple of 64 (4304 -> 4352, the tiny config's 1008 -> 1024) with zero rows of fc1_w,
+# zero fc1_b and zero columns of fc2_w: the fc1 output rows and fc2's operand rows then start on 128-byte lines (8608 B
+# rows straddle them), and fc2's last k-block is full. The pad columns of the fc1 output are exactly +0 (0 + 0, GELU(0) =
+# +0), so fc2 adds the same zeros TMA used to fill in past column 4304: the embeddings do not change by a bit.
+VIT_MLP_ALIGN = 64
 
 # CUDA-graph path (small batches): eligibility and cache bounds
 GRAPH_MAX_VIT_TOKENS = 32 * 1024   # up to 32 slices of 448x448: beyond that the kernels are long enough to hide launches
@@ -105,6 +111,8 @@ class VisRAGEngine:
             self._pos_cache: Dict[Tuple[int, int], torch.Tensor] = {}
             self._sincos_cache: Dict[Tuple[int, int], torch.Tensor] = {}
             self.blocks = []
+            mlp = cfg.vit_mlp
+            mlp_pad = -(-mlp // VIT_MLP_ALIGN) * VIT_MLP_ALIGN - mlp
             for i in range(cfg.vit_depth):
                 p = f"vpm.blocks.{i}."
                 wq = sd[p + "attn.qkv.weight"].float().reshape(3, nh, hd, D)
@@ -118,8 +126,9 @@ class VisRAGEngine:
                     qkv_w=_half(wpad.reshape(3 * nh * hs, D), dev, dt), qkv_b=_f32(bpad.reshape(-1), dev),
                     proj_w=_half(sd[p + "attn.proj.weight"], dev, dt), proj_b=_f32(sd[p + "attn.proj.bias"], dev),
                     n2w=_f32(sd[p + "norm2.weight"], dev), n2b=_f32(sd[p + "norm2.bias"], dev),
-                    fc1_w=_half(sd[p + "mlp.fc1.weight"], dev, dt), fc1_b=_f32(sd[p + "mlp.fc1.bias"], dev),
-                    fc2_w=_half(sd[p + "mlp.fc2.weight"], dev, dt), fc2_b=_f32(sd[p + "mlp.fc2.bias"], dev),
+                    fc1_w=_half(F.pad(sd[p + "mlp.fc1.weight"], (0, 0, 0, mlp_pad)), dev, dt),
+                    fc1_b=_f32(F.pad(sd[p + "mlp.fc1.bias"], (0, mlp_pad)), dev),
+                    fc2_w=_half(F.pad(sd[p + "mlp.fc2.weight"], (0, mlp_pad)), dev, dt), fc2_b=_f32(sd[p + "mlp.fc2.bias"], dev),
                 ))
             self.vnorm_w, self.vnorm_b = _f32(sd["vpm.norm.weight"], dev), _f32(sd["vpm.norm.bias"], dev)
             # ---- Resampler
