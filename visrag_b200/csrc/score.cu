@@ -267,7 +267,10 @@ score_filter_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_con
                 }
                 const float tail = sc[h][SC_KT - 1];
                 if (tail > tau[h]) {  // float max through the integer atomics (tail may be negative)
-                    if (tail >= 0.f) atomicMax(reinterpret_cast<int*>(tau_ptr[h]), __float_as_int(tail));
+                    // branch on the sign BIT: -0.0 goes to the unsigned min, where its pattern is the least of all
+                    // negative floats (as a signed int it is INT_MIN, which a signed max never stores over -inf or
+                    // a negative tau)
+                    if (__float_as_int(tail) >= 0) atomicMax(reinterpret_cast<int*>(tau_ptr[h]), __float_as_int(tail));
                     else atomicMin(reinterpret_cast<unsigned int*>(tau_ptr[h]), __float_as_uint(tail));
                 }
             }
