@@ -127,6 +127,11 @@ int vr_resample_u8(const uint8_t* src, int32_t src_pixel_bytes, int32_t n, int32
  * resampler.py:159-163 (64 learned queries x N keys, 18 heads x 128).
  * q/k/v are bf16 (or, with VR_ATTN_F16, fp16) row-major token matrices; head h starts at column *_col0 + h*head_stride
  * (head_stride = head_dim rounded up to a multiple of 16; pad columns must hold zeros).
+ * Causal with fewer query rows than key rows (len_q < len_k, e.g. a sequence whose first len_k - len_q rows come from a
+ * prefix cache): the query rows are the LAST len_q rows of the sequence. Query i of sequence b attends keys
+ * j <= i + (len_k - len_q), and its output row has the same bits as row len_k - len_q + i of the full causal run over the
+ * same keys: key tiles start at the same 128-key offsets from the sequence start, and a tile that lies wholly past a
+ * row's last key adds nothing to that row.
  * ---------------------------------------------------------------------------------- */
 typedef struct {
     const void* q;  int64_t ldq;  int64_t q_rows;   /* q_rows: rows in the q buffer (TMA bound) */
@@ -213,6 +218,17 @@ int vr_build_lm_input_ex(const int32_t* src, int32_t tokens, int32_t dim, const 
  * cluster size, so its output bits do not depend on the batch size or on the other sequences of the batch. */
 int vr_pool_norm(const float* h, int64_t ldh, const float* gamma, float eps, const int32_t* cu, int32_t batch, int32_t dim,
                  int32_t pooling, int32_t normalize, float* reps, void* stream);
+
+/* Prefix-cache row assembly: every sequence b of out becomes [prefix rows ; its own rows]:
+ *   out rows [cu_out[b], cu_out[b] + prefix_len)   = prefix rows 0 .. prefix_len - 1
+ *   out rows [cu_out[b] + prefix_len, cu_out[b+1]) = rows [cu_rows[b], cu_rows[b+1]) of `rows`
+ * so cu_out[b+1] - cu_out[b] = prefix_len + cu_rows[b+1] - cu_rows[b], and out_rows = cu_out[batch]. Each row copies
+ * `cols` elements of elem_size bytes (2: the 16-bit K|V block of a qkv row; 4: the fp32 residual stream) from column 0
+ * of the given pointers; prefix, rows and out must be 16-byte aligned and cols * elem_size and every ld * elem_size
+ * multiples of 16 (refused before any CUDA call otherwise). prefix may be NULL when prefix_len = 0. */
+int vr_prefix_rows(const void* prefix, int64_t ldp, const void* rows, int64_t ldr, void* out, int64_t ldo,
+                   const int32_t* cu_rows, const int32_t* cu_out, int32_t batch, int32_t prefix_len, int32_t out_rows,
+                   int32_t cols, int32_t elem_size, void* stream);
 
 
 /* ------------------------------------------------------------------------------------

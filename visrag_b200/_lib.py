@@ -113,6 +113,8 @@ def _declare(lib: C.CDLL) -> None:
     lib.vr_topk_rows.argtypes = [vp, vp, i32, i64, i32, i64, vp, vp, vp]
     lib.vr_pool_norm.restype = i32
     lib.vr_pool_norm.argtypes = [vp, i64, vp, f32, vp, i32, i32, i32, i32, vp, vp]
+    lib.vr_prefix_rows.restype = i32
+    lib.vr_prefix_rows.argtypes = [vp, i64, vp, i64, vp, i64, vp, vp, i32, i32, i32, i32, i32, vp]
 
 
 def lib() -> C.CDLL:

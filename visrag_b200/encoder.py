@@ -26,7 +26,7 @@ import torch.nn.functional as F
 from . import _lib as L
 from . import ops
 from .config import VisRAGConfig
-from .host import PreparedBatch, prepare_batch
+from .host import PreparedBatch, prepare_batch, select_prefix, suffix_batch
 from .weights import sincos_2d
 
 VIT_HEAD_STRIDE = 80  # 72 padded to a multiple of 16 (the MMA K step); pad rows of Wqkv are zero
@@ -42,9 +42,17 @@ GRAPH_MAX_LM_TOKENS = 4096
 GRAPH_TEXT_BUCKET = 16             # text-only batches: total tokens and longest sequence are padded to multiples of this
 GRAPH_CACHE = 12                   # captured graphs kept (LRU); each owns its activation buffers
 
+PREFIX_CACHE = 4                   # prefix-cache entries kept (LRU); ~378 KB per prefix token at full size
+
 
 class _GraphEntry:
     __slots__ = ("graph", "groups", "src", "pos", "cu", "reps", "launches")
+
+
+class _PrefixEntry:
+    """One cached token prefix: its ids, P = len(ids), the K|V columns of every layer's RoPE'd qkv rows kv [layers, P, 2H]
+    (engine dtype) and the fp32 residual rows before the final norm h [P, H]. `serial` names it in graph signatures."""
+    __slots__ = ("ids", "P", "kv", "h", "serial")
 
 
 def _half(t: torch.Tensor, dev, dtype: torch.dtype) -> torch.Tensor:
@@ -73,7 +81,7 @@ class VisRAGEngine:
 
     def __init__(self, cfg: VisRAGConfig, state_dict: Dict[str, torch.Tensor], device: str = "cuda:0",
                  max_vit_tokens: int = 131072, device_frontend: bool = True, cuda_graphs: Optional[bool] = None,
-                 dtype: torch.dtype = torch.bfloat16):
+                 dtype: torch.dtype = torch.bfloat16, prefix_cache: bool = True):
         cfg.validate()
         if dtype not in ops.HALF_DTYPES:
             raise ValueError(f"VisRAGEngine: dtype must be torch.bfloat16 or torch.float16, got {dtype}")
@@ -91,6 +99,13 @@ class VisRAGEngine:
         self._graphs: "OrderedDict[tuple, _GraphEntry]" = OrderedDict()
         self._graph_seen: Dict[tuple, int] = {}
         self.graph_stats = {"captured": 0, "replayed": 0, "eager": 0}
+        # Text-only batches whose items share a token prefix (every query starts with the same instruction) run only the
+        # suffixes through the LM and read the prefix rows from this cache; the embeddings keep their bits (DESIGN §5).
+        # tokens_skipped counts the LM tokens the full path would have computed and the cached path did not.
+        self.prefix_cache = bool(prefix_cache)
+        self._prefixes: "OrderedDict[tuple, _PrefixEntry]" = OrderedDict()
+        self._prefix_serial = 0
+        self.prefix_stats = {"created": 0, "hits": 0, "tokens_skipped": 0}
         with L.on_device(self.device):
             self._load(cfg, state_dict)
 
@@ -252,8 +267,13 @@ class VisRAGEngine:
     # ------------------------------------------------------------------------------------------ LM
     @_on_own_device
     def lm_hidden(self, token_src: torch.Tensor, positions: torch.Tensor, cu: torch.Tensor, max_len: int,
-                  vision: Optional[torch.Tensor]) -> torch.Tensor:
-        """Packed decoder: returns the fp32 residual stream BEFORE the final RMSNorm, [T, H]."""
+                  vision: Optional[torch.Tensor], prefix: Optional[_PrefixEntry] = None,
+                  cu_full: Optional[torch.Tensor] = None, kv_out: Optional[torch.Tensor] = None) -> torch.Tensor:
+        """Packed decoder: returns the fp32 residual stream BEFORE the final RMSNorm, [T, H].
+        With `prefix`, the rows are the suffixes of sequences that start with the prefix's P tokens (positions stay
+        absolute, cu / max_len count suffix tokens); every layer attends over [prefix K|V ; own K|V] laid out as the full
+        sequences cu_full, and the result is the full sequences' residual stream [T + B*P, H]. `kv_out` [layers, T, 2H]
+        receives every layer's K|V columns (how a prefix entry is built)."""
         cfg, dt = self.cfg, self.dtype
         H, nh = cfg.hidden, cfg.heads
         B = cu.shape[0] - 1
@@ -261,18 +281,31 @@ class VisRAGEngine:
         T = h.shape[0]
         qkv = torch.empty((T, 3 * H), dtype=dt, device=self.device)
         att = torch.empty((T, H), dtype=dt, device=self.device)
+        if prefix is not None:
+            kv = torch.empty((T + B * prefix.P, 2 * H), dtype=dt, device=self.device)
         s = cfg.depth_scale
-        for lyr in self.layers:
+        for i, lyr in enumerate(self.layers):
             a = ops.rmsnorm(h, lyr["in_w"], cfg.rms_eps, dt)
             ops.gemm(a, lyr["qkv_w"], mode=L.VR_EPI_ROPE, positions=positions, rope_cos=self.rope_cos,
                      rope_sin=self.rope_sin, rope_cols=2 * H, out=qkv)
-            ops.attention(qkv, qkv, qkv, q_col0=0, k_col0=H, v_col0=2 * H, head_stride=64, head_dim=64, heads=nh, batch=B,
-                          cu_k=cu, max_k=max_len, cu_q=cu, max_q=max_len, causal=True, scale=cfg.head_dim ** -0.5, out=att)
+            if kv_out is not None:
+                kv_out[i].copy_(qkv[:, H:])
+            if prefix is None:
+                ops.attention(qkv, qkv, qkv, q_col0=0, k_col0=H, v_col0=2 * H, head_stride=64, head_dim=64, heads=nh,
+                              batch=B, cu_k=cu, max_k=max_len, cu_q=cu, max_q=max_len, causal=True,
+                              scale=cfg.head_dim ** -0.5, out=att)
+            else:
+                ops.prefix_rows(prefix.kv[i], qkv[:, H:], kv, cu, cu_full)
+                ops.attention(qkv, kv, kv, q_col0=0, k_col0=0, v_col0=H, head_stride=64, head_dim=64, heads=nh, batch=B,
+                              cu_k=cu_full, max_k=max_len + prefix.P, cu_q=cu, max_q=max_len, causal=True,
+                              scale=cfg.head_dim ** -0.5, out=att)
             ops.gemm(att, lyr["o_w"], resid=h, out=h, scale=s, out_dtype=torch.float32)
             a = ops.rmsnorm(h, lyr["post_w"], cfg.rms_eps, dt)
             a = ops.gemm(a, lyr["gu_w"], mode=L.VR_EPI_SWIGLU)
             ops.gemm(a, lyr["down_w"], resid=h, out=h, scale=s, out_dtype=torch.float32)
-        return h
+        if prefix is None:
+            return h
+        return ops.prefix_rows(prefix.h, h, torch.empty((kv.shape[0], H), dtype=torch.float32, device=self.device), cu, cu_full)
 
     # ------------------------------------------------------------------------------------------ end to end
     def _pinned_buf(self, key, n: int, dtype) -> torch.Tensor:
@@ -361,18 +394,25 @@ class VisRAGEngine:
 
     @_on_own_device
     def encode_device(self, groups, group_row0, n_slices: int, src, pos, cu, max_len: int, pooling: str = "wmean",
-                      normalize: bool = True, return_hidden: bool = False):
-        """Inputs already in HBM -> pooled embeddings [B, hidden] fp32 (the device-resident hot path)."""
+                      normalize: bool = True, return_hidden: bool = False, prefix: Optional[_PrefixEntry] = None):
+        """Inputs already in HBM -> pooled embeddings [B, hidden] fp32 (the device-resident hot path).
+        With `prefix` (text only) src / pos / max_len describe the suffixes, and cu is [cu_suffix ; cu_full], 2 (B+1)
+        offsets (one upload); the hidden rows returned are the full sequences'."""
         vision = self.encode_vision(groups, group_row0, n_slices)
-        h = self.lm_hidden(src, pos, cu, max_len, vision)
-        reps = ops.pool_norm(h, self.final_w, self.cfg.rms_eps, cu, pooling, normalize)
+        cu_full = None
+        if prefix is not None:
+            n = cu.shape[0] // 2
+            cu, cu_full = cu[:n], cu[n:]
+        h = self.lm_hidden(src, pos, cu, max_len, vision, prefix, cu_full)
+        reps = ops.pool_norm(h, self.final_w, self.cfg.rms_eps, cu if prefix is None else cu_full, pooling, normalize)
         return (reps, h) if return_hidden else reps
 
     # ------------------------------------------------------------------------------------------ CUDA graphs
-    def _graph_plan(self, pb: PreparedBatch):
+    def _graph_plan(self, pb: PreparedBatch, prefix_len: int = 0):
         """Decide whether this batch takes the graph path; text-only batches are padded into shape buckets with ONE extra
         dummy sequence (token 0, dropped after pooling) so that different queries share a captured graph.
-        Returns (token_src, positions, cu_seqlens, max_len, n_out) or None."""
+        With prefix_len, pb holds the suffixes of a cached-prefix batch and the dummy is prefix + pad tokens (positions
+        from prefix_len on). Returns (token_src, positions, cu_seqlens, max_len, n_out) or None."""
         if not self.cuda_graphs or pb.n_items == 0:
             return None
         T = int(pb.cu_seqlens[-1])
@@ -386,14 +426,14 @@ class VisRAGEngine:
         Tb = -(-(T + 1) // b) * b          # at least one pad token: the dummy sequence is never empty
         pad = Tb - T
         Lb = min(-(-max(max_len, pad) // b) * b, self.cfg.max_pos)
-        if pad > self.cfg.max_pos:
+        if prefix_len + pad > self.cfg.max_pos:
             return None
         src = np.concatenate([pb.token_src, np.full(pad, -1, dtype=np.int32)])        # -(0 + 1): token id 0
-        pos = np.concatenate([pb.positions, np.arange(pad, dtype=np.int32)])
+        pos = np.concatenate([pb.positions, np.arange(prefix_len, prefix_len + pad, dtype=np.int32)])
         cu = np.concatenate([pb.cu_seqlens, np.asarray([Tb], dtype=np.int32)])
         return src, pos, cu, Lb, pb.n_items
 
-    def _encode_graphed(self, sig, groups, group_row0, n_slices, src, pos, cu, max_len, pooling, normalize):
+    def _encode_graphed(self, sig, groups, group_row0, n_slices, src, pos, cu, max_len, pooling, normalize, prefix=None):
         """Replay (or, on the second sighting of a signature, capture) the device step for this shape. The first sighting
         runs eagerly: it also warms every per-shape table and one-time kernel attribute the capture must not touch."""
         ent = self._graphs.get(sig)
@@ -404,10 +444,10 @@ class VisRAGEngine:
             self._graph_seen[sig] = seen + 1
             if seen == 0:
                 self.graph_stats["eager"] += 1
-                return self.encode_device(groups, group_row0, n_slices, src, pos, cu, max_len, pooling, normalize)
+                return self.encode_device(groups, group_row0, n_slices, src, pos, cu, max_len, pooling, normalize, prefix=prefix)
             if seen < 0:  # an earlier capture of this shape failed: stay on eager launches
                 self.graph_stats["eager"] += 1
-                return self.encode_device(groups, group_row0, n_slices, src, pos, cu, max_len, pooling, normalize)
+                return self.encode_device(groups, group_row0, n_slices, src, pos, cu, max_len, pooling, normalize, prefix=prefix)
             ent = _GraphEntry()
             ent.groups = {k: v.clone() for k, v in groups.items()}
             ent.src, ent.pos, ent.cu = src.clone(), pos.clone(), cu.clone()
@@ -416,14 +456,15 @@ class VisRAGEngine:
             ent.graph = torch.cuda.CUDAGraph()
             try:
                 with torch.cuda.graph(ent.graph):
-                    ent.reps = self.encode_device(ent.groups, group_row0, n_slices, ent.src, ent.pos, ent.cu, max_len, pooling, normalize)
+                    ent.reps = self.encode_device(ent.groups, group_row0, n_slices, ent.src, ent.pos, ent.cu, max_len, pooling, normalize,
+                                                   prefix=prefix)
             except Exception as exc:  # the capture is an optimisation of the launch path only: same kernels, eager launches
                 import warnings
 
                 warnings.warn(f"visrag_b200: CUDA-graph capture failed for this batch shape ({exc!r}); using eager launches")
                 self._graph_seen[sig] = -(1 << 30)
                 self.graph_stats["eager"] += 1
-                return self.encode_device(groups, group_row0, n_slices, src, pos, cu, max_len, pooling, normalize)
+                return self.encode_device(groups, group_row0, n_slices, src, pos, cu, max_len, pooling, normalize, prefix=prefix)
             ent.launches = L.LAUNCHES - launches0
             self._graphs[sig] = ent
             self.graph_stats["captured"] += 1
@@ -448,6 +489,9 @@ class VisRAGEngine:
             return torch.zeros((0, self.cfg.hidden), dtype=torch.float32, device=self.device)
         if int(pb.seq_lens.max()) > self.cfg.max_pos:
             raise ValueError(f"sequence longer than max_pos={self.cfg.max_pos}")
+        ent = self._prefix_for(pb) if self.prefix_cache else None
+        if ent is not None:
+            return self._encode_suffixes(pb, ent, pooling, normalize, return_hidden)
         plan = None if return_hidden or ops.profiling() else self._graph_plan(pb)
         if plan is not None:
             src_h, pos_h, cu_h, max_len, n_out = plan
@@ -460,6 +504,61 @@ class VisRAGEngine:
         groups, src, pos, cu = self.upload(pb)
         return self.encode_device(groups, pb.group_row0, pb.n_slices, src, pos, cu, int(pb.seq_lens.max()), pooling,
                                   normalize, return_hidden)
+
+    # ------------------------------------------------------------------------------------------ prefix cache
+    def _prefix_for(self, pb: PreparedBatch) -> Optional[_PrefixEntry]:
+        """The cache entry this batch runs from (host.select_prefix), created now if the batch calls for a new one;
+        None -> the full path. Runs on the caller's thread: the cache is not shared with prepare()'s workers."""
+        sel = select_prefix(pb, list(self._prefixes))
+        if sel is None:
+            return None
+        ids, new = sel
+        if new:
+            ent = self._make_prefix(ids)
+            self._prefixes[ids] = ent
+            self.prefix_stats["created"] += 1
+            self.prefix_stats["tokens_skipped"] += ent.P * (pb.n_items - 1)  # the prefix itself ran once
+            while len(self._prefixes) > PREFIX_CACHE:
+                _, old = self._prefixes.popitem(last=False)
+                for sig in [s for s in self._graphs if s[-1] == ("prefix", old.serial)]:  # they bake its buffers
+                    del self._graphs[sig]
+        else:
+            ent = self._prefixes[ids]
+            self._prefixes.move_to_end(ids)
+            self.prefix_stats["hits"] += 1
+            self.prefix_stats["tokens_skipped"] += ent.P * pb.n_items
+        return ent
+
+    def _make_prefix(self, ids: Tuple[int, ...]) -> _PrefixEntry:
+        """Run the prefix's tokens as one sequence through the same kernels (eagerly, never captured) and keep every
+        layer's K|V rows and the residual rows before the final norm."""
+        cfg, dev = self.cfg, self.device
+        ent = _PrefixEntry()
+        ent.ids, ent.P = ids, len(ids)
+        self._prefix_serial += 1
+        ent.serial = self._prefix_serial
+        src = torch.tensor([-(i + 1) for i in ids], dtype=torch.int32, device=dev)
+        pos = torch.arange(ent.P, dtype=torch.int32, device=dev)
+        cu = torch.tensor([0, ent.P], dtype=torch.int32, device=dev)
+        ent.kv = torch.empty((cfg.layers, ent.P, 2 * cfg.hidden), dtype=self.dtype, device=dev)
+        ent.h = self.lm_hidden(src, pos, cu, ent.P, None, kv_out=ent.kv)
+        return ent
+
+    def _encode_suffixes(self, pb: PreparedBatch, ent: _PrefixEntry, pooling: str, normalize: bool, return_hidden: bool):
+        """The cached-prefix path: only the suffix tokens run through the LM; the prefix rows come from `ent`. Small
+        batches replay CUDA graphs bucketed on the suffixes as _graph_plan does, one graph per shape and entry."""
+        sb = suffix_batch(pb, ent.P)
+        plan = None if return_hidden or ops.profiling() else self._graph_plan(sb, ent.P)
+        if plan is None:
+            src_h, pos_h, cu_h, max_len, n_out = sb.token_src, sb.positions, sb.cu_seqlens, int(sb.seq_lens.max()), pb.n_items
+        else:
+            src_h, pos_h, cu_h, max_len, n_out = plan
+        cu_full = cu_h + ent.P * np.arange(len(cu_h), dtype=np.int32)
+        _, src, pos, cu = self.upload(PreparedBatch(pb.n_items, sb.seq_lens, np.concatenate([cu_h, cu_full]), pos_h, src_h))
+        if plan is None:
+            return self.encode_device({}, {}, 0, src, pos, cu, max_len, pooling, normalize, return_hidden, prefix=ent)
+        sig = ((), (), 0, int(src.shape[0]), int(cu.shape[0]), max_len, pooling, bool(normalize), ("prefix", ent.serial))
+        return self._encode_graphed(sig, {}, {}, 0, src, pos, cu, max_len, pooling, normalize, prefix=ent)[:n_out]
 
     @_on_own_device
     def encode(self, texts: Sequence[str], images: Sequence, tokenizer, max_inp_length: Optional[int] = 2048,

@@ -220,3 +220,20 @@ def pool_norm(h: torch.Tensor, gamma: torch.Tensor, eps: float, cu: torch.Tensor
     _launch("other", 0.0, L.lib().vr_pool_norm, h.data_ptr(), h.stride(0), gamma.data_ptr(), eps, cu.data_ptr(), B, h.shape[1],
             POOLING[pooling], int(normalize), reps.data_ptr(), L.stream_ptr())
     return reps
+
+
+def prefix_rows(prefix: torch.Tensor, rows: torch.Tensor, out: torch.Tensor, cu_rows: torch.Tensor, cu_out: torch.Tensor) -> torch.Tensor:
+    """Sequence b of `out` (rows cu_out[b]..cu_out[b+1]) = [all rows of `prefix` ; rows cu_rows[b]..cu_rows[b+1] of `rows`].
+    The three are matrices of one dtype (16-bit or fp32) with unit inner stride and the same column count; they may be
+    column blocks of wider rows (include/visrag_b200.h)."""
+    for name, t in (("prefix", prefix), ("rows", rows), ("out", out)):
+        if t.dtype != out.dtype or t.dim() != 2 or t.stride(1) != 1 or t.shape[1] != out.shape[1] or not t.is_cuda:
+            raise ValueError(f"prefix_rows: {name} must be a CUDA {out.dtype} matrix of {out.shape[1]} unit-stride columns, "
+                             f"got {t.dtype} {tuple(t.shape)}")
+        L.check_device(t)
+    if cu_rows.dtype != torch.int32 or cu_out.dtype != torch.int32 or cu_rows.shape != cu_out.shape:
+        raise ValueError("prefix_rows: cu_rows and cu_out must be int32 of the same length")
+    _launch("other", 0.0, L.lib().vr_prefix_rows, prefix.data_ptr(), prefix.stride(0), rows.data_ptr(), rows.stride(0),
+            out.data_ptr(), out.stride(0), cu_rows.data_ptr(), cu_out.data_ptr(), cu_out.shape[0] - 1, prefix.shape[0],
+            out.shape[0], out.shape[1], out.element_size(), L.stream_ptr())
+    return out
