@@ -272,6 +272,25 @@ int vr_topk_rows(const float* scores, const int64_t* ids, int32_t rows, int64_t 
 int vr_topk_rows_chunked(const float* scores, int32_t rows, int64_t cols, int32_t k, int64_t id_offset, int32_t chunks,
                          float* ws_scores, int64_t* ws_ids, float* out_scores, int64_t* out_ids, void* stream);
 
+/* Filtered retrieval: the same operations over a chosen subset of the docs.
+ * doc_mask: ceil(nd / 32) uint32 words in device memory, 4-byte aligned; doc i (local index, before id_offset) is
+ * eligible when bit (i & 31) of word (i >> 5) is set; bits at or past nd are ignored. An ineligible doc is never a
+ * candidate and never a result: the results are those of the plain calls over the eligible docs alone, bit for bit.
+ * When fewer than k docs are eligible, a row holds the eligible ones in order and then (-inf, -1), as for k > nd.
+ * A NULL or misaligned doc_mask, and ids != NULL together with a mask (the mask indexes columns), are refused before
+ * any CUDA call.
+ *   vr_score_filter_masked : vr_score_filter over the eligible docs; the candidate lists hold eligible docs only, so
+ *                            vr_score_rescore takes them unchanged and its proof covers the eligible docs;
+ *   vr_topk_rows_masked    : vr_topk_rows with ids == NULL and columns (docs) filtered by doc_mask;
+ *   vr_topk_rows_chunked_masked : vr_topk_rows_chunked with columns filtered by doc_mask. */
+int vr_score_filter_masked(const void* q_f16, int32_t nq, const void* d_f16, int64_t nd, int32_t dim, int32_t ranges,
+                           float* cand_scores, int32_t* cand_ids, const uint32_t* doc_mask, void* stream);
+int vr_topk_rows_masked(const float* scores, const int64_t* ids, int32_t rows, int64_t cols, int32_t k, int64_t id_offset,
+                        float* out_scores, int64_t* out_ids, const uint32_t* doc_mask, void* stream);
+int vr_topk_rows_chunked_masked(const float* scores, int32_t rows, int64_t cols, int32_t k, int64_t id_offset,
+                                int32_t chunks, float* ws_scores, int64_t* ws_ids, float* out_scores, int64_t* out_ids,
+                                const uint32_t* doc_mask, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

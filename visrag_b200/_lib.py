@@ -111,6 +111,12 @@ def _declare(lib: C.CDLL) -> None:
     lib.vr_topk_rows_chunked.argtypes = [vp, i32, i64, i32, i64, i32, vp, vp, vp, vp, vp]
     lib.vr_topk_rows.restype = i32
     lib.vr_topk_rows.argtypes = [vp, vp, i32, i64, i32, i64, vp, vp, vp]
+    lib.vr_score_filter_masked.restype = i32
+    lib.vr_score_filter_masked.argtypes = [vp, i32, vp, i64, i32, i32, vp, vp, vp, vp]
+    lib.vr_topk_rows_masked.restype = i32
+    lib.vr_topk_rows_masked.argtypes = [vp, vp, i32, i64, i32, i64, vp, vp, vp, vp]
+    lib.vr_topk_rows_chunked_masked.restype = i32
+    lib.vr_topk_rows_chunked_masked.argtypes = [vp, i32, i64, i32, i64, i32, vp, vp, vp, vp, vp, vp]
     lib.vr_pool_norm.restype = i32
     lib.vr_pool_norm.argtypes = [vp, i64, vp, f32, vp, i32, i32, i32, i32, vp, vp]
     lib.vr_prefix_rows.restype = i32

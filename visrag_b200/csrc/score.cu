@@ -17,6 +17,7 @@
 #include "common.h"
 #include "gemm.cuh"
 #include <math.h>
+#include <type_traits>
 
 namespace vr {
 
@@ -44,6 +45,10 @@ struct ScoreArgs {
     int items;         // R * QB
     float* cand_scores;  // [nq, lists*SC_KT]
     int* cand_ids;
+};
+
+struct MaskedScoreArgs : ScoreArgs {
+    const uint32_t* doc_mask;  // ceil(nd / 32) words: doc i is eligible when bit i & 31 of word i >> 5 is set
 };
 
 struct Score2Cfg {
@@ -82,9 +87,16 @@ __device__ __forceinline__ float quad_max(float v) {
 // lives in the 4 lanes of a quad (each lane holds a quarter of the columns), so every lane keeps a sorted top-16 of ITS
 // columns for each of its two rows over all tiles of the item; the four lists of a row are merged by shuffles at the end
 // of the item (top-16 of the union: its tail bounds everything any lane dropped) into one list per (query, doc range).
+// MASKED: doc_mask holds one eligibility bit per doc (bit i & 31 of word i >> 5). An ineligible doc's score becomes -inf
+// before anything looks at it, so it never enters a list, never raises thr and never reaches a published tau: every
+// tail, and so the rescoring kernel's bound, is a tail over eligible docs only.
+// The mask travels in its own argument type, so the unmasked form keeps the parameter list it has without the mask (an
+// unused parameter or ScoreArgs field changes its register allocation and code).
+template <typename Args>
 __global__ void __launch_bounds__(GEMM_THREADS, 1)
 score_filter_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant__ CUtensorMap tmap_d,
-                    const ScoreArgs g) {
+                    const Args g) {
+    constexpr bool MASKED = std::is_same<Args, MaskedScoreArgs>::value;
     using Cfg = Score2Cfg;
     constexpr int STAGES = Cfg::STAGES;
     extern __shared__ uint8_t smem_raw[];
@@ -164,6 +176,14 @@ score_filter_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_con
         }
         const int t1 = item_t1(item);
         for (int u = 2 * item_t0(item); u < 2 * t1; ++u) {
+            // the sub-tile's 4 mask words, loaded before the k-loop so the latency hides under the MMAs (words at or
+            // past the end of the mask read as 0: those columns are >= nd and skipped below anyway)
+            uint32_t mw[4];
+            if constexpr (MASKED) {
+                const long long w0 = static_cast<long long>(u) * (Cfg::SUB_BN / 32), nw = (g.nd + 31) / 32;
+#pragma unroll
+                for (int i = 0; i < 4; ++i) mw[i] = w0 + i < nw ? __ldg(g.doc_mask + w0 + i) : 0u;
+            }
             float acc[Cfg::SUB_BN / 2];
             int prev = -1;
             for (int kb = 0; kb < num_kb; ++kb) {
@@ -187,6 +207,15 @@ score_filter_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_con
             wgmma_touch(acc);
 
             const long long col_base = static_cast<long long>(u) * Cfg::SUB_BN + q4 * 2;
+            // bit 2j + e of elig = eligibility of this lane's column 8j + 2 q4 + e: word j >> 2, bit 8 (j & 3) + 2 q4 + e
+            uint32_t elig = 0;
+            if constexpr (MASKED) {
+#pragma unroll
+                for (int w = 0; w < 4; ++w) {
+                    const uint32_t x = mw[w] >> (2 * q4);
+                    elig |= ((x & 0x3u) | ((x >> 6) & 0xCu) | ((x >> 12) & 0x30u) | ((x >> 18) & 0xC0u)) << (8 * w);
+                }
+            }
 #pragma unroll
             for (int h = 0; h < 2; ++h) {
                 // this lane's 32 scores of the row: v[2j + e] = column 8j + 2 q4 + e of the sub-tile
@@ -195,6 +224,10 @@ score_filter_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_con
                 for (int j = 0; j < 16; ++j) {
                     v[2 * j] = __float_as_uint(acc[4 * j + 2 * h]);
                     v[2 * j + 1] = __float_as_uint(acc[4 * j + 2 * h + 1]);
+                }
+                if constexpr (MASKED) {
+#pragma unroll
+                    for (int j = 0; j < 32; ++j) v[j] = (elig >> j) & 1u ? v[j] : __float_as_uint(-INFINITY);
                 }
                 // fast path: nothing of the 32 scores beats the threshold (the common case after the first tiles)
                 float mx = fmaxf(__uint_as_float(v[0]), __uint_as_float(v[1]));
@@ -518,11 +551,19 @@ exact_scores_kernel(const float* __restrict__ Q, int nq, const float* __restrict
     }
 }
 
+// Column c is eligible when bit c & 31 of mask word c >> 5 is set (the layout of the filter's doc_mask).
+__device__ __forceinline__ bool col_eligible(const uint32_t* __restrict__ mask, long long c) {
+    return (__ldg(mask + (c >> 5)) >> (c & 31)) & 1u;
+}
+
 // top-k of each row of a dense [rows, cols] fp32 matrix (optionally with explicit ids per entry).
+// MASKED (ids == NULL only): ineligible columns are skipped like negative ids - never represented by a -inf score, which
+// would count as a valid entry.
+template <bool MASKED>
 __global__ void __launch_bounds__(256)
 topk_rows_kernel(const float* __restrict__ scores, const long long* __restrict__ ids, long long cols, int k,
                  long long id_offset, long long chunk_cols, float* __restrict__ out_scores,
-                 long long* __restrict__ out_ids) {
+                 long long* __restrict__ out_ids, const uint32_t* __restrict__ mask) {
     // block (row, chunk): top-k of columns [chunk*chunk_cols, ...) of one row, written as list `row*gridDim.y + chunk`
     __shared__ float red_s[8];
     __shared__ long long red_i[8];
@@ -540,6 +581,7 @@ topk_rows_kernel(const float* __restrict__ scores, const long long* __restrict__
         for (long long c = c_lo + threadIdx.x; c < c_hi; c += 256) {
             const long long id = irow ? irow[c] : c;
             if (id < 0) continue;
+            if (MASKED && !col_eligible(mask, c)) continue;
             const float s = srow[c];
             if (!before(last_s, last_i, s, id)) continue;
             if (before(s, id, bs, bi)) { bs = s; bi = id; }
@@ -574,10 +616,11 @@ topk_rows_kernel(const float* __restrict__ scores, const long long* __restrict__
 
 // Short rows (cols <= 32*NPL): one WARP per row, the row lives in registers, k rounds of shuffle arg-max - no block barriers.
 // This is the merge of per-rank / per-shard partial top-k lists ([nq, world*k]) and the second pass of the chunked top-k.
-template <int NPL>
+template <int NPL, bool MASKED>
 __global__ void __launch_bounds__(256)
 topk_rows_warp_kernel(const float* __restrict__ scores, const long long* __restrict__ ids, int rows, int cols, int k,
-                      long long id_offset, float* __restrict__ out_scores, long long* __restrict__ out_ids) {
+                      long long id_offset, float* __restrict__ out_scores, long long* __restrict__ out_ids,
+                      const uint32_t* __restrict__ mask) {
     const int lane = threadIdx.x & 31;
     const int row = blockIdx.x * 8 + (threadIdx.x >> 5);
     if (row >= rows) return;
@@ -588,7 +631,7 @@ topk_rows_warp_kernel(const float* __restrict__ scores, const long long* __restr
 #pragma unroll
     for (int j = 0; j < NPL; ++j) {
         const int c = lane + j * 32;
-        const bool in = c < cols;
+        const bool in = c < cols && (!MASKED || col_eligible(mask, c));
         id[j] = in ? (irow ? irow[c] : static_cast<long long>(c)) : -1;
         s[j] = (in && id[j] >= 0) ? srow[c] : -INFINITY;
     }
@@ -625,14 +668,17 @@ topk_rows_warp_kernel(const float* __restrict__ scores, const long long* __restr
     }
 }
 
+template <bool MASKED>
 static int launch_topk_rows(const float* scores, const long long* ids, int rows, long long cols, int k, long long id_offset,
-                            float* out_scores, long long* out_ids, cudaStream_t s) {
+                            float* out_scores, long long* out_ids, const uint32_t* mask, cudaStream_t s) {
     if (cols <= 128)
-        topk_rows_warp_kernel<4><<<(rows + 7) / 8, 256, 0, s>>>(scores, ids, rows, static_cast<int>(cols), k, id_offset, out_scores, out_ids);
+        topk_rows_warp_kernel<4, MASKED><<<(rows + 7) / 8, 256, 0, s>>>(scores, ids, rows, static_cast<int>(cols), k, id_offset,
+                                                                        out_scores, out_ids, mask);
     else if (cols <= 512)
-        topk_rows_warp_kernel<16><<<(rows + 7) / 8, 256, 0, s>>>(scores, ids, rows, static_cast<int>(cols), k, id_offset, out_scores, out_ids);
+        topk_rows_warp_kernel<16, MASKED><<<(rows + 7) / 8, 256, 0, s>>>(scores, ids, rows, static_cast<int>(cols), k, id_offset,
+                                                                         out_scores, out_ids, mask);
     else
-        topk_rows_kernel<<<rows, 256, 0, s>>>(scores, ids, cols, k, id_offset, cols, out_scores, out_ids);
+        topk_rows_kernel<MASKED><<<rows, 256, 0, s>>>(scores, ids, cols, k, id_offset, cols, out_scores, out_ids, mask);
     return 0;
 }
 
@@ -717,6 +763,58 @@ static ScorePlan score_plan(int nq, long long nd) {
 
 static int score_ranges_for(int nq, long long nd) { return score_plan(nq, nd).lists / 2; }
 
+// A doc mask as the _masked entry points take it: present and 4-byte aligned (one uint32 word per 32 docs).
+static bool mask_ok(const uint32_t* mask) { return mask && (reinterpret_cast<uintptr_t>(mask) & 3) == 0; }
+
+template <bool MASKED>
+static int score_filter(const void* q_f16, int nq, const void* d_f16, long long nd, int dim, int ranges, const uint32_t* doc_mask,
+                        float* cand_scores, int* cand_ids, void* stream) {
+    VR_REQUIRE(q_f16 && d_f16 && cand_scores && cand_ids, "vr_score_filter: null pointer");
+    VR_REQUIRE(nq > 0 && nd > 0 && nd < 2147483647ll && dim % 8 == 0, "vr_score_filter: bad shape nq=%d nd=%lld dim=%d", nq,
+               (long long)nd, dim);
+    VR_REQUIRE(nq < (1 << 30), "vr_score_filter: too many queries");
+    const ScorePlan plan = score_plan(nq, nd);
+    VR_REQUIRE(ranges * 2 == plan.lists, "vr_score_filter: ranges must come from vr_score_ranges()");
+    using Cfg = Score2Cfg;
+    CUtensorMap tq, td;
+    if (int rc = make_tmap_2d(&tq, q_f16, nq, dim, dim, GEMM_BM, GEMM_BK, 128, false)) return rc;
+    if (int rc = make_tmap_2d(&td, d_f16, nd, dim, dim, 128, GEMM_BK, 128, false)) return rc;
+    using Args = typename std::conditional<MASKED, MaskedScoreArgs, ScoreArgs>::type;
+    static unsigned long long attr_set = 0;
+    if (first_use_on_device(&attr_set))
+        VR_CHECK_CUDA(cudaFuncSetAttribute(score_filter_kernel<Args>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES));
+    Args g;
+    g.nq = nq; g.nd = nd; g.dim = dim; g.lists = plan.lists; g.T = plan.T; g.R = plan.R; g.QB = plan.QB; g.items = plan.items;
+    g.cand_scores = cand_scores; g.cand_ids = cand_ids;
+    if constexpr (MASKED) g.doc_mask = doc_mask;
+    cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+    {
+        const long long n = static_cast<long long>(nq) * (plan.lists - plan.R) * SC_KT;
+        long long blocks = (n + 255) / 256;
+        if (blocks > num_sms() * 8) blocks = num_sms() * 8;
+        score_init_lists_kernel<<<static_cast<int>(blocks), 256, 0, st>>>(cand_scores, cand_ids, nq, plan.lists, plan.R);
+        VR_CHECK_CUDA(cudaGetLastError());
+    }
+    score_filter_kernel<Args><<<2 * plan.pairs, GEMM_THREADS, Cfg::SMEM_BYTES, st>>>(tq, td, g);
+    VR_CHECK_CUDA(cudaGetLastError());
+    return 0;
+}
+
+template <bool MASKED>
+static int topk_rows_chunked(const float* scores, int rows, long long cols, int k, long long id_offset, int chunks,
+                             float* ws_scores, long long* ws_ids, float* out_scores, long long* out_ids, const uint32_t* mask,
+                             cudaStream_t s) {
+    const long long chunk_cols = (cols + chunks - 1) / chunks;
+    // pass 1: every (row, chunk) block reduces its column range to a sorted top-k list (ids = column + id_offset)
+    topk_rows_kernel<MASKED><<<dim3(rows, chunks), 256, 0, s>>>(scores, nullptr, cols, k, id_offset, chunk_cols, ws_scores,
+                                                                ws_ids, mask);
+    VR_CHECK_CUDA(cudaGetLastError());
+    // pass 2: merge the `chunks` lists of each row (explicit ids; exhausted lists carry id -1 and are skipped)
+    launch_topk_rows<false>(ws_scores, ws_ids, rows, static_cast<long long>(chunks) * k, k, 0, out_scores, out_ids, nullptr, s);
+    VR_CHECK_CUDA(cudaGetLastError());
+    return 0;
+}
+
 }  // namespace vr
 
 using namespace vr;
@@ -745,33 +843,14 @@ extern "C" int vr_f32_to_f16_rows(const float* src, int64_t rows, int32_t dim, v
 
 extern "C" int vr_score_filter(const void* q_f16, int32_t nq, const void* d_f16, int64_t nd, int32_t dim, int32_t ranges,
                                float* cand_scores, int32_t* cand_ids, void* stream) {
-    VR_REQUIRE(q_f16 && d_f16 && cand_scores && cand_ids, "vr_score_filter: null pointer");
-    VR_REQUIRE(nq > 0 && nd > 0 && nd < 2147483647ll && dim % 8 == 0, "vr_score_filter: bad shape nq=%d nd=%lld dim=%d", nq,
-               (long long)nd, dim);
-    VR_REQUIRE(nq < (1 << 30), "vr_score_filter: too many queries");
-    const ScorePlan plan = score_plan(nq, nd);
-    VR_REQUIRE(ranges * 2 == plan.lists, "vr_score_filter: ranges must come from vr_score_ranges()");
-    using Cfg = Score2Cfg;
-    CUtensorMap tq, td;
-    if (int rc = make_tmap_2d(&tq, q_f16, nq, dim, dim, GEMM_BM, GEMM_BK, 128, false)) return rc;
-    if (int rc = make_tmap_2d(&td, d_f16, nd, dim, dim, 128, GEMM_BK, 128, false)) return rc;
-    static unsigned long long attr_set = 0;
-    if (first_use_on_device(&attr_set))
-        VR_CHECK_CUDA(cudaFuncSetAttribute(score_filter_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES));
-    ScoreArgs g;
-    g.nq = nq; g.nd = nd; g.dim = dim; g.lists = plan.lists; g.T = plan.T; g.R = plan.R; g.QB = plan.QB; g.items = plan.items;
-    g.cand_scores = cand_scores; g.cand_ids = cand_ids;
-    cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-    {
-        const long long n = static_cast<long long>(nq) * (plan.lists - plan.R) * SC_KT;
-        long long blocks = (n + 255) / 256;
-        if (blocks > num_sms() * 8) blocks = num_sms() * 8;
-        score_init_lists_kernel<<<static_cast<int>(blocks), 256, 0, st>>>(cand_scores, cand_ids, nq, plan.lists, plan.R);
-        VR_CHECK_CUDA(cudaGetLastError());
-    }
-    score_filter_kernel<<<2 * plan.pairs, GEMM_THREADS, Cfg::SMEM_BYTES, st>>>(tq, td, g);
-    VR_CHECK_CUDA(cudaGetLastError());
-    return 0;
+    return score_filter<false>(q_f16, nq, d_f16, nd, dim, ranges, nullptr, cand_scores, cand_ids, stream);
+}
+
+extern "C" int vr_score_filter_masked(const void* q_f16, int32_t nq, const void* d_f16, int64_t nd, int32_t dim,
+                                      int32_t ranges, float* cand_scores, int32_t* cand_ids, const uint32_t* doc_mask,
+                                      void* stream) {
+    VR_REQUIRE(mask_ok(doc_mask), "vr_score_filter_masked: doc_mask must be a non-null, 4-byte aligned pointer");
+    return score_filter<true>(q_f16, nq, d_f16, nd, dim, ranges, doc_mask, cand_scores, cand_ids, stream);
 }
 
 extern "C" int vr_score_rescore(const float* q_f32, int32_t nq, const float* d_f32, int64_t nd, int32_t dim, int32_t ranges,
@@ -837,8 +916,21 @@ extern "C" int vr_topk_rows(const float* scores, const int64_t* ids, int32_t row
                             float* out_scores, int64_t* out_ids, void* stream) {
     VR_REQUIRE(scores && out_scores && out_ids, "vr_topk_rows: null pointer");
     VR_REQUIRE(rows > 0 && cols > 0 && k > 0, "vr_topk_rows: bad shape");
-    launch_topk_rows(scores, reinterpret_cast<const long long*>(ids), rows, cols, k, id_offset, out_scores,
-                     reinterpret_cast<long long*>(out_ids), reinterpret_cast<cudaStream_t>(stream));
+    launch_topk_rows<false>(scores, reinterpret_cast<const long long*>(ids), rows, cols, k, id_offset, out_scores,
+                            reinterpret_cast<long long*>(out_ids), nullptr, reinterpret_cast<cudaStream_t>(stream));
+    VR_CHECK_CUDA(cudaGetLastError());
+    return 0;
+}
+
+extern "C" int vr_topk_rows_masked(const float* scores, const int64_t* ids, int32_t rows, int64_t cols, int32_t k,
+                                   int64_t id_offset, float* out_scores, int64_t* out_ids, const uint32_t* doc_mask,
+                                   void* stream) {
+    VR_REQUIRE(mask_ok(doc_mask), "vr_topk_rows_masked: doc_mask must be a non-null, 4-byte aligned pointer");
+    VR_REQUIRE(!ids, "vr_topk_rows_masked: the mask indexes columns, so ids must be NULL");
+    VR_REQUIRE(scores && out_scores && out_ids, "vr_topk_rows_masked: null pointer");
+    VR_REQUIRE(rows > 0 && cols > 0 && k > 0, "vr_topk_rows_masked: bad shape");
+    launch_topk_rows<true>(scores, nullptr, rows, cols, k, id_offset, out_scores, reinterpret_cast<long long*>(out_ids), doc_mask,
+                           reinterpret_cast<cudaStream_t>(stream));
     VR_CHECK_CUDA(cudaGetLastError());
     return 0;
 }
@@ -848,15 +940,18 @@ extern "C" int vr_topk_rows_chunked(const float* scores, int32_t rows, int64_t c
                                     int64_t* out_ids, void* stream) {
     VR_REQUIRE(scores && ws_scores && ws_ids && out_scores && out_ids, "vr_topk_rows_chunked: null pointer");
     VR_REQUIRE(rows > 0 && cols > 0 && k > 0 && chunks > 0 && chunks <= 65535, "vr_topk_rows_chunked: bad shape");
-    cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
-    const long long chunk_cols = (cols + chunks - 1) / chunks;
-    // pass 1: every (row, chunk) block reduces its column range to a sorted top-k list (ids = column + id_offset)
-    topk_rows_kernel<<<dim3(rows, chunks), 256, 0, s>>>(scores, nullptr, cols, k, id_offset, chunk_cols, ws_scores,
-                                                        reinterpret_cast<long long*>(ws_ids));
-    VR_CHECK_CUDA(cudaGetLastError());
-    // pass 2: merge the `chunks` lists of each row (explicit ids; exhausted lists carry id -1 and are skipped)
-    launch_topk_rows(ws_scores, reinterpret_cast<const long long*>(ws_ids), rows, static_cast<long long>(chunks) * k, k, 0,
-                     out_scores, reinterpret_cast<long long*>(out_ids), s);
-    VR_CHECK_CUDA(cudaGetLastError());
-    return 0;
+    return topk_rows_chunked<false>(scores, rows, cols, k, id_offset, chunks, ws_scores, reinterpret_cast<long long*>(ws_ids),
+                                    out_scores, reinterpret_cast<long long*>(out_ids), nullptr,
+                                    reinterpret_cast<cudaStream_t>(stream));
+}
+
+extern "C" int vr_topk_rows_chunked_masked(const float* scores, int32_t rows, int64_t cols, int32_t k, int64_t id_offset,
+                                           int32_t chunks, float* ws_scores, int64_t* ws_ids, float* out_scores,
+                                           int64_t* out_ids, const uint32_t* doc_mask, void* stream) {
+    VR_REQUIRE(mask_ok(doc_mask), "vr_topk_rows_chunked_masked: doc_mask must be a non-null, 4-byte aligned pointer");
+    VR_REQUIRE(scores && ws_scores && ws_ids && out_scores && out_ids, "vr_topk_rows_chunked_masked: null pointer");
+    VR_REQUIRE(rows > 0 && cols > 0 && k > 0 && chunks > 0 && chunks <= 65535, "vr_topk_rows_chunked_masked: bad shape");
+    return topk_rows_chunked<true>(scores, rows, cols, k, id_offset, chunks, ws_scores, reinterpret_cast<long long*>(ws_ids),
+                                   out_scores, reinterpret_cast<long long*>(out_ids), doc_mask,
+                                   reinterpret_cast<cudaStream_t>(stream));
 }

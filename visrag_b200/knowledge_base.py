@@ -8,15 +8,20 @@ Drop-in for the reference's demo pipeline:
 Here the index is loaded once and stays resident in HBM (`KnowledgeBase`); a query is one fp32 scan of the index
 (`vr_score_exact`, HBM bound: n*d*4 bytes) plus a two-level top-k spread over many SMs (`vr_topk_rows_chunked`).
 Scores are the same fp32 dot products; ties are ordered by lower page index (torch.topk leaves tie order unspecified).
+
+Beyond the reference: a search can be restricted to some pages (`within`, e.g. the pages of one PDF), pages can be
+removed (a tombstone bit, so the other pages keep their indices) and added, and `save` writes the live pages back in the
+demo's layout. All of it runs as a doc mask inside the same kernels, with the same exact fp32 results.
 """
 from __future__ import annotations
 
 import os
-from typing import List, Sequence, Tuple
+from typing import Iterable, List, Optional, Sequence, Tuple
 
 import numpy as np
 import torch
 
+from . import _lib as L
 from . import retriever
 
 REPS_FILE = "reps.npy"
@@ -39,7 +44,8 @@ def save_knowledge_base(path: str, reps, filenames: Sequence[str]) -> None:
 
 
 class KnowledgeBase:
-    """A knowledge base resident on one GPU."""
+    """A knowledge base resident on one GPU. Pages keep their index (row) for the life of the object: `remove` only marks
+    a page dead, and `add` appends."""
 
     def __init__(self, path: str, device: str = "cuda"):
         self.path = path
@@ -49,22 +55,92 @@ class KnowledgeBase:
         if reps.ndim != 2 or reps.shape[0] != len(self.filenames):
             raise ValueError(f"{path}: reps.npy has {reps.shape} rows/dims but {len(self.filenames)} filenames")
         self.index = retriever.build_index(np.ascontiguousarray(reps, dtype=np.float32), self.filenames, device)
+        self._row = {name: i for i, name in enumerate(self.filenames)}   # filename -> row, live pages only
+        self._live = torch.ones(len(self.filenames), dtype=torch.bool, device=self.index.emb.device)
+        self._n_live = len(self.filenames)
 
     def __len__(self) -> int:
-        return self.index.nd
+        return self._n_live
 
-    def search(self, query_reps, topk: int) -> Tuple[torch.Tensor, torch.Tensor]:
-        """query_reps [nq, d] (tensor or ndarray, fp32) -> (scores [nq,k] f32, page indices [nq,k] i64) on the device."""
+    def _rows(self, filenames: Iterable[str]) -> List[int]:
+        if isinstance(filenames, str):
+            filenames = [filenames]
+        try:
+            return sorted({self._row[name] for name in filenames})
+        except KeyError as e:
+            raise KeyError(f"no live page named {e.args[0]!r} in the knowledge base") from None
+
+    def search(self, query_reps, topk: int, within: Optional[Iterable[str]] = None) -> Tuple[torch.Tensor, torch.Tensor]:
+        """query_reps [nq, d] (tensor or ndarray, fp32) -> (scores [nq,k] f32, page indices [nq,k] i64) on the device.
+        within: page filenames to search (default: every live page); k = min(topk, pages searched)."""
         q = query_reps if isinstance(query_reps, torch.Tensor) else torch.from_numpy(np.asarray(query_reps, dtype=np.float32))
         q = q.to(self.index.emb.device, torch.float32).reshape(-1, self.index.emb.shape[1]).contiguous()
-        return retriever.score_topk(q, self.index, min(topk, len(self)))  # enters the index's device itself
+        if within is None:
+            n, mask = len(self), None if len(self) == self.index.nd else self._live   # None: the unfiltered kernels
+        else:
+            rows = self._rows(within)
+            n = len(rows)
+            mask = torch.zeros(self.index.nd, dtype=torch.bool, device=q.device)
+            mask[torch.tensor(rows, dtype=torch.int64, device=q.device)] = True
+        k = min(topk, n)
+        if k == 0:
+            return (torch.empty((q.shape[0], 0), dtype=torch.float32, device=q.device),
+                    torch.empty((q.shape[0], 0), dtype=torch.int64, device=q.device))
+        return retriever.score_topk(q, self.index, k, doc_mask=mask)  # enters the index's device itself
 
-    def retrieve(self, query_rep, topk: int) -> List[str]:
+    def retrieve(self, query_rep, topk: int, within: Optional[Iterable[str]] = None) -> List[str]:
         """`answer.py: retrieve` after the query is encoded: paths of the top-k page images, best first."""
-        _, ids = self.search(query_rep, topk)
+        _, ids = self.search(query_rep, topk, within)
         return [os.path.join(self.path, self.filenames[i]) for i in ids[0].tolist()]
 
-    def retrieve_text(self, model, tokenizer, query: str, topk: int) -> List[str]:
+    def retrieve_text(self, model, tokenizer, query: str, topk: int, within: Optional[Iterable[str]] = None) -> List[str]:
         """Full `retrieve(knowledge_base_path, query, topk)`: instruction + query -> embedding (B2 wrapper) -> top-k."""
         out = model(query={"text": [DEMO_QUERY_PREFIX + query], "image": [None]}, tokenizer=tokenizer)
-        return self.retrieve(out.q_reps, topk)
+        return self.retrieve(out.q_reps, topk, within)
+
+    def remove(self, filenames: Iterable[str]) -> None:
+        """Mark pages dead: no search returns them again. The other pages keep their indices, and the index's max row norm
+        (the filter's error bound) stays as it is: an upper bound over a superset of the live pages is still one."""
+        rows = self._rows(filenames)
+        for r in rows:
+            del self._row[self.filenames[r]]
+        self._n_live -= len(rows)
+        if rows:
+            self._live[torch.tensor(rows, dtype=torch.int64, device=self._live.device)] = False
+
+    def add(self, reps, filenames: Sequence[str]) -> None:
+        """Append pages (fp32 [n, d] embeddings, one filename each) after the existing ones. A name may not be a live page
+        already; the name of a removed page may come back, as a new page."""
+        filenames = list(filenames)
+        dev = self.index.emb.device
+        x = reps if isinstance(reps, torch.Tensor) else torch.from_numpy(np.asarray(reps, dtype=np.float32))
+        x = x.to(dev, torch.float32).contiguous()
+        if x.dim() != 2 or x.shape[0] != len(filenames) or x.shape[1] != self.index.emb.shape[1]:
+            raise ValueError(f"reps must be [n, {self.index.emb.shape[1]}] with one filename per row")
+        if any("\n" in f for f in filenames):
+            raise ValueError("filenames must not contain newlines")
+        dup = sorted({f for f in filenames if f in self._row} | {f for f in filenames if filenames.count(f) > 1})
+        if dup:
+            raise ValueError(f"duplicate page filenames: {dup[:5]}")
+        if not filenames:
+            return
+        n0, n, d = self.index.nd, x.shape[0], x.shape[1]
+        f16 = torch.empty((n, d), dtype=torch.float16, device=dev)
+        with L.on_device(dev):
+            # the kernel's atomicMax raises the index's max row norm to cover the new rows
+            L.check(L.lib().vr_f32_to_f16_rows(x.data_ptr(), n, d, f16.data_ptr(), None, self.index.max_norm.data_ptr(),
+                                               L.stream_ptr()))
+        self.index.emb = torch.cat([self.index.emb, x])
+        self.index.emb_f16 = torch.cat([self.index.emb_f16, f16])
+        self._live = torch.cat([self._live, torch.ones(n, dtype=torch.bool, device=dev)])
+        self.filenames.extend(filenames)
+        self._row.update((f, n0 + i) for i, f in enumerate(filenames))
+        self._n_live += n
+
+    def save(self, path: Optional[str] = None) -> None:
+        """Write the live pages, in index order, as the demo's two files (to `path`, default the directory loaded from).
+        A knowledge base loaded from them returns the same pages and score bits for any query."""
+        rows = torch.nonzero(self._live).flatten().tolist()
+        keep = torch.tensor(rows, dtype=torch.int64, device=self.index.emb.device)
+        save_knowledge_base(self.path if path is None else path, self.index.emb.index_select(0, keep),
+                            [self.filenames[r] for r in rows])

@@ -10,7 +10,8 @@ Underneath, `torch.matmul` + `torch.topk` are replaced by the fused wgmma filter
 
 For a corpus that lives in HBM (index build + many query batches) use `CorpusIndex` / `score_topk` directly; the
 multi-GPU form (`sharded_topk`) shards the corpus by page across ranks, takes the local top-k with global ids and
-merges after ONE all-gather of [nq, k] (score, id) pairs.
+merges after ONE all-gather of [nq, k] (score, id) pairs. Both take an optional `doc_mask` (bool [nd], local to the
+shard): only the docs it marks are searched, and the result equals the fp32 scan over those docs alone.
 """
 from __future__ import annotations
 
@@ -73,7 +74,28 @@ def build_index(emb, lookup: Optional[List[str]] = None, device: str = "cuda") -
     return CorpusIndex(emb, f16, mx, lookup)
 
 
-def _exact_topk(q: torch.Tensor, index: CorpusIndex, k: int, id_offset: int):
+def pack_doc_mask(mask: torch.Tensor) -> torch.Tensor:
+    """bool [nd] -> uint32 [ceil(nd / 32)] words on the same device: doc i is bit (i & 31) of word (i >> 5), the layout the
+    _masked kernels read. Bits past nd are 0."""
+    nd = mask.shape[0]
+    bits = torch.zeros(((nd + 31) // 32) * 32, dtype=torch.int64, device=mask.device)
+    bits[:nd] = mask.to(torch.int64)
+    words = (bits.view(-1, 32) << torch.arange(32, device=mask.device)).sum(1)
+    return torch.where(words >= 1 << 31, words - (1 << 32), words).to(torch.int32).view(torch.uint32)
+
+
+def _check_doc_mask(doc_mask: torch.Tensor, index: CorpusIndex) -> torch.Tensor:
+    """Validate a bool [nd] doc mask on the index's device and pack it."""
+    if not isinstance(doc_mask, torch.Tensor) or doc_mask.dtype != torch.bool:
+        raise ValueError("doc_mask must be a torch.bool tensor")
+    if doc_mask.dim() != 1 or doc_mask.shape[0] != index.nd:
+        raise ValueError(f"doc_mask must have shape [{index.nd}] (one entry per doc of the index), got {list(doc_mask.shape)}")
+    if doc_mask.device != index.emb.device:
+        raise ValueError(f"doc_mask lives on {doc_mask.device}, the index on {index.emb.device}")
+    return pack_doc_mask(doc_mask)
+
+
+def _exact_topk(q: torch.Tensor, index: CorpusIndex, k: int, id_offset: int, mask_words: Optional[torch.Tensor] = None):
     nq, d = q.shape
     nd = index.nd
     out_s = torch.empty((nq, k), dtype=torch.float32, device=q.device)
@@ -88,23 +110,34 @@ def _exact_topk(q: torch.Tensor, index: CorpusIndex, k: int, id_offset: int):
         if chunks >= 2:
             ws_s = torch.empty((n, chunks, k), dtype=torch.float32, device=q.device)
             ws_i = torch.empty((n, chunks, k), dtype=torch.int64, device=q.device)
-            L.check(lib.vr_topk_rows_chunked(scratch.data_ptr(), n, nd, k, id_offset, chunks, ws_s.data_ptr(), ws_i.data_ptr(),
-                                             out_s[r0:].data_ptr(), out_i[r0:].data_ptr(), L.stream_ptr()))
-        else:
+            if mask_words is None:
+                L.check(lib.vr_topk_rows_chunked(scratch.data_ptr(), n, nd, k, id_offset, chunks, ws_s.data_ptr(),
+                                                 ws_i.data_ptr(), out_s[r0:].data_ptr(), out_i[r0:].data_ptr(), L.stream_ptr()))
+            else:
+                L.check(lib.vr_topk_rows_chunked_masked(scratch.data_ptr(), n, nd, k, id_offset, chunks, ws_s.data_ptr(),
+                                                        ws_i.data_ptr(), out_s[r0:].data_ptr(), out_i[r0:].data_ptr(),
+                                                        mask_words.data_ptr(), L.stream_ptr()))
+        elif mask_words is None:
             L.check(lib.vr_topk_rows(scratch.data_ptr(), None, n, nd, k, id_offset, out_s[r0:].data_ptr(),
                                      out_i[r0:].data_ptr(), L.stream_ptr()))
+        else:
+            L.check(lib.vr_topk_rows_masked(scratch.data_ptr(), None, n, nd, k, id_offset, out_s[r0:].data_ptr(),
+                                            out_i[r0:].data_ptr(), mask_words.data_ptr(), L.stream_ptr()))
     return out_s, out_i
 
 
 def score_topk(queries: torch.Tensor, index: CorpusIndex, k: int, id_offset: int = 0, force_exact: bool = False,
-               stats: Optional[dict] = None) -> Tuple[torch.Tensor, torch.Tensor]:
+               stats: Optional[dict] = None, doc_mask: Optional[torch.Tensor] = None) -> Tuple[torch.Tensor, torch.Tensor]:
     """Exact fp32 top-k of `queries @ index.emb.T`: (scores [nq,k] f32, ids [nq,k] i64 = local index + id_offset).
-    Rows are sorted by (score desc, id asc); if k > nd the tail is (-inf, -1)."""
+    Rows are sorted by (score desc, id asc); if k > nd the tail is (-inf, -1).
+    doc_mask: optional bool [nd] on the index's device; only docs marked True are searched (the same bits as the fp32 scan
+    over those docs alone). With fewer than k of them the tail is (-inf, -1)."""
     q = _check_f32(queries, "queries")
     if q.device != index.emb.device:
         raise ValueError(f"queries live on {q.device}, the index on {index.emb.device}")
+    mask_words = None if doc_mask is None else _check_doc_mask(doc_mask, index)
     with L.on_device(q.device):
-        return _score_topk(q, index, k, id_offset, force_exact, stats)
+        return _score_topk(q, index, k, id_offset, force_exact, stats, mask_words)
 
 
 class _Stages:
@@ -133,7 +166,8 @@ def resolve_stages(stats: dict) -> dict:
     return stats["stages"]
 
 
-def _score_topk(q: torch.Tensor, index: CorpusIndex, k: int, id_offset: int, force_exact: bool, stats: Optional[dict]):
+def _score_topk(q: torch.Tensor, index: CorpusIndex, k: int, id_offset: int, force_exact: bool, stats: Optional[dict],
+                mask_words: Optional[torch.Tensor] = None):
     nq, d = q.shape
     nd = index.nd
     if nq == 0:
@@ -143,7 +177,7 @@ def _score_topk(q: torch.Tensor, index: CorpusIndex, k: int, id_offset: int, for
     if force_exact or nq * nd <= SMALL_PROBLEM or nd < 256:
         if stats is not None:
             stats.update(path="exact", flagged=0)
-        return _exact_topk(q, index, k, id_offset)
+        return _exact_topk(q, index, k, id_offset, mask_words)
     lib = L.lib()
     ranges = lib.vr_score_ranges(nq, nd)
     lists = ranges * 2 * lib.vr_score_list_len()
@@ -156,8 +190,12 @@ def _score_topk(q: torch.Tensor, index: CorpusIndex, k: int, id_offset: int, for
     sp = L.stream_ptr()
     ev = _Stages(stats)
     ev.mark("q_to_f16")
-    L.check(lib.vr_score_filter(q16.data_ptr(), nq, index.emb_f16.data_ptr(), nd, d, ranges, cand_s.data_ptr(),
-                                cand_i.data_ptr(), sp))
+    if mask_words is None:
+        L.check(lib.vr_score_filter(q16.data_ptr(), nq, index.emb_f16.data_ptr(), nd, d, ranges, cand_s.data_ptr(),
+                                    cand_i.data_ptr(), sp))
+    else:
+        L.check(lib.vr_score_filter_masked(q16.data_ptr(), nq, index.emb_f16.data_ptr(), nd, d, ranges, cand_s.data_ptr(),
+                                           cand_i.data_ptr(), mask_words.data_ptr(), sp))
     ev.mark("filter")
     L.check(lib.vr_score_rescore(q.data_ptr(), nq, index.emb.data_ptr(), nd, d, ranges, cand_s.data_ptr(), cand_i.data_ptr(),
                                  index.max_norm.data_ptr(), k, id_offset, out_s.data_ptr(), out_i.data_ptr(),
@@ -167,7 +205,7 @@ def _score_topk(q: torch.Tensor, index: CorpusIndex, k: int, id_offset: int, for
     if stats is not None:
         stats.update(path="filter+rescore", flagged=int(bad.numel()), ranges=ranges)
     if bad.numel() > 0:
-        s2, i2 = _exact_topk(q.index_select(0, bad), index, k, id_offset)
+        s2, i2 = _exact_topk(q.index_select(0, bad), index, k, id_offset, mask_words)
         out_s.index_copy_(0, bad, s2)
         out_i.index_copy_(0, bad, i2)
     return out_s, out_i
@@ -210,12 +248,14 @@ def gather_partials(scores: torch.Tensor, ids: torch.Tensor, group=None) -> Tupl
     return gs.contiguous(), gi.contiguous()
 
 
-def sharded_topk(queries: torch.Tensor, index: CorpusIndex, k: int, id_offset: int, group=None, stats: Optional[dict] = None):
+def sharded_topk(queries: torch.Tensor, index: CorpusIndex, k: int, id_offset: int, group=None, stats: Optional[dict] = None,
+                 doc_mask: Optional[torch.Tensor] = None):
     """Corpus sharded by page across ranks (every rank holds the same queries): local exact top-k with GLOBAL ids,
-    one all-gather of [nq, k] (score, id) pairs over NCCL/NVLink, k-way merge on every rank (SURVEY.md §8e)."""
+    one all-gather of [nq, k] (score, id) pairs over NCCL/NVLink, k-way merge on every rank (SURVEY.md §8e).
+    doc_mask: this rank's bool [nd] mask of its own shard (see score_topk)."""
     import torch.distributed as dist
 
-    s, i = score_topk(queries, index, k, id_offset, stats=stats)
+    s, i = score_topk(queries, index, k, id_offset, stats=stats, doc_mask=doc_mask)
     if not (dist.is_available() and dist.is_initialized()) or dist.get_world_size(group) == 1:
         return s, i
     ev = _Stages(stats)
