@@ -174,8 +174,9 @@ void vr_attention_force_v1(int32_t variant);
  * 14x14/stride-14 patch conv): modeling_minicpmv.py:84-92 + timm/layers/patch_embed.py:87.
  * pixels: [n_slices, h, w, 3] uint8 (h, w multiples of `patch`); out: [n_slices*(h/patch)*(w/patch), ldo] bf16,
  * column c*patch*patch + ky*patch + kx (the Conv2d weight's flattening); columns [3*patch^2, ldo) are zeroed.
- * bf16(fma(u, 2/255, -1)) - bit-identical to bf16((u/255 - 0.5)/0.5) for all 256 byte values. patch <= 85; a strip of `patch`
- * pixel rows must fit 200 KB of shared memory (w up to ~4800 for patch 14). */
+ * bf16(fma(u, 2/255, -1)) - bit-identical to bf16((u/255 - 0.5)/0.5) for all 256 byte values. patch <= 85, any w: a strip of
+ * `patch` pixel rows that does not fit 200 KB of shared memory (patch 14, ldo 640: w of 4858 and more) is converted in chunks of
+ * patch columns, with the same bits. Returns 2 if ldo is so large that its offset table leaves no room for one patch. */
 int vr_im2col_norm(const uint8_t* pixels, int32_t n_slices, int32_t h, int32_t w, int32_t patch, void* out, int64_t ldo,
                    void* stream);
 /* The same with the output type chosen: out_dtype = VR_BF16 (what vr_im2col_norm writes) or VR_F16, where

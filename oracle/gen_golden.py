@@ -34,7 +34,22 @@ def geometry_cases():
     return sizes
 
 
-def gen_geometry():
+def geometry_v2_cases():
+    """Tall and wide pages: long screenshots, infographics, banners and thin strips, aspect ratios up to about 1:3000 and
+    sides up to 40000 (area at most 6e7 pixels, so that the blank test images stay small)."""
+    sizes = [(1280, 10000), (1280, 40000), (600, 8000), (8000, 600), (3000, 100), (100, 3000), (33964, 287), (287, 33964),
+             (30000, 30), (30, 30000), (3000, 14), (14, 3000), (3000, 1), (1, 3000), (40000, 14), (14, 40000), (40000, 1000),
+             (1000, 40000), (13000, 400), (12288, 500), (12289, 500), (4858, 42), (1, 1), (2, 40000), (40000, 2)]
+    rs = np.random.RandomState(12)
+    while len(sizes) < 200:
+        long_side = int(np.exp(rs.uniform(np.log(100), np.log(40000))))
+        short = max(1, int(round(long_side / np.exp(rs.uniform(0, np.log(3000))))))
+        if long_side * short <= 60_000_000:
+            sizes.append((long_side, short) if rs.randint(2) else (short, long_side))
+    return sizes
+
+
+def gen_geometry(cases=geometry_cases, name="geometry_v1"):
     """Slice geometry from the reference's own slice_image (modeling_minicpmv.py:482-537)."""
     from oracle import reference_shim as RS
 
@@ -42,14 +57,14 @@ def gen_geometry():
     from openmatch.modeling.modeling_minicpmv.modeling_minicpmv import slice_image
 
     rows = []
-    for (w, h) in geometry_cases():
+    for (w, h) in cases():
         src, patches, grid = slice_image(Image.new("RGB", (w, h)), 9, 448, 14)
         g = grid if grid is not None else [0, 0]
         pw, ph = (patches[0][0].size if patches else (0, 0))
         rows.append([w, h, src.size[0], src.size[1], g[0], g[1], pw, ph, sum(len(r) for r in patches)])
-    np.savez(os.path.join(GOLDEN_DIR, "geometry_v1.npz"), cases=np.asarray(rows, dtype=np.int64),
+    np.savez(os.path.join(GOLDEN_DIR, f"{name}.npz"), cases=np.asarray(rows, dtype=np.int64),
              columns=np.asarray(["W", "H", "src_w", "src_h", "grid_x", "grid_y", "patch_w", "patch_h", "n_patches"]))
-    print("geometry:", len(rows), "cases")
+    print(f"{name}:", len(rows), "cases")
 
 
 def gen_model_case(name, cfg, weight_seed, page_sizes, page_seed, n_queries, query_seed, topk):
@@ -221,11 +236,15 @@ def main():
     ap.add_argument("--full", action="store_true", help="also generate the full-size (3.1 B parameter) case")
     ap.add_argument("--full-v2", action="store_true", help="only generate full_v2 (36 pages, 10 queries, top-5; ~15 min of CPU)")
     ap.add_argument("--tiny-v2", action="store_true", help="only generate tiny_v2 (same corpus as full_v2, tiny model)")
+    ap.add_argument("--geometry-v2", action="store_true", help="only generate geometry_v2 (tall and wide pages; ~1 min of CPU)")
     a = ap.parse_args()
     from visrag_b200.config import VisRAGConfig as _C
 
     if a.pins:
         gen_reference_pins()
+        return
+    if a.geometry_v2:
+        gen_geometry(geometry_v2_cases, "geometry_v2")
         return
     if a.full_v2 or a.tiny_v2:
         if not all(os.path.exists(p) for p in REAL_PAGES):
@@ -239,7 +258,8 @@ def main():
     from visrag_b200.config import VisRAGConfig
 
     gen_geometry()
-    sizes = [(224, 224), (448, 448), (224, 224), (700, 900), (760, 141), (1200, 500), (320, 240), (448, 448)]
+    gen_geometry(geometry_v2_cases, "geometry_v2")
+    sizes =[(224, 224), (448, 448), (224, 224), (700, 900), (760, 141), (1200, 500), (320, 240), (448, 448)]
     gen_model_case("tiny_v1", VisRAGConfig.tiny(), 1234, sizes, 7, 4, 5, 5)
     if a.full:
         gen_model_case("full_v1", VisRAGConfig.full(), 4321, [(448, 448), (224, 224), (640, 480)], 17, 3, 15, 3)

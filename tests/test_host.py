@@ -13,15 +13,26 @@ from visrag_b200.tokenizer_stub import StubTokenizer
 CFG = VisRAGConfig.tiny()
 
 
-def test_plan_matches_reference_golden_geometry():
-    z = np.load(f"{GOLDEN}/geometry_v1.npz")
-    for W, H, sw, sh, gx, gy, pw, ph, npatch in z["cases"]:
+def _check_plans(cases):
+    for W, H, sw, sh, gx, gy, pw, ph, npatch in cases:
         plan = host.plan_slices(int(W), int(H), CFG)
         assert plan.source_size == (sw, sh), (W, H)
         if gx == 0:
             assert plan.grid is None and npatch == 0
         else:
             assert plan.grid == (gx, gy) and plan.cell_size == (pw, ph) and plan.n_slices == 1 + npatch, (W, H)
+
+
+def test_plan_matches_reference_golden_geometry():
+    _check_plans(np.load(f"{GOLDEN}/geometry_v1.npz")["cases"])
+
+
+def test_plan_matches_reference_golden_geometry_of_tall_and_wide_pages():
+    """geometry_v2: long screenshots, infographics, banners and thin strips (aspect ratios up to 1:20000, sides up to 40000),
+    whose thumbnails and slices reach 60004 pixels in width and 4525 patches."""
+    cases = np.load(f"{GOLDEN}/geometry_v2.npz")["cases"]
+    assert len(cases) == 200 and cases[:, :2].max() == 40000
+    _check_plans(cases)
 
 
 def test_known_geometries():
@@ -33,7 +44,9 @@ def test_known_geometries():
         assert p.source_size == (448, 448) and p.grid is None
 
 
-@pytest.mark.parametrize("size", [(224, 224), (700, 900), (760, 141), (1200, 500), (449, 449)])
+@pytest.mark.parametrize("size", [(224, 224), (700, 900), (760, 141), (1200, 500), (449, 449),
+                                  # tall and wide pages: slices down to 1 and 3 patches on one side, up to 1000 on the other
+                                  (1280, 40000), (600, 8000), (8000, 600), (3000, 100), (33964, 287), (30000, 30), (3000, 1)])
 def test_render_is_pixel_exact_vs_oracle(size):
     img = synth_pages([size], 3)[0]
     src, patches, grid = O.slice_image(img, 9, 448, 14)

@@ -22,18 +22,23 @@ __device__ __forceinline__ float warp_sum(float v) {
 // FFMA: bf16(fma(u, 2/255, -1)) == bf16((u/255 - 0.5)/0.5) for all 256 byte values (tests/test_gpu_kernels.py checks
 // every value), so the division of the fp32 reference is not needed for a bit-identical bf16 result. The same holds for
 // fp16 (F16): fp16(fma(u, 2/255, -1)) == fp16((u/255 - 0.5)/0.5) for all 256 values (tests/test_fp16_host.py).
+// CHUNKED: for strips wider than the shared-memory buffer (patch 14: 347 patches = 4858 pixels and wider). A CTA then takes
+// one chunk of at most `cg` patch columns of a strip, staged row by row (the chunk's pixel rows are `patch` spans of
+// cg*patch*3 bytes, w*3 bytes apart); every output value is computed by the same FFMA, so the result is the same bits.
 // ---------------------------------------------------------------------------------------------
 constexpr int IM2COL_THREADS = 256;
 
-template <bool F16>
+template <bool F16, bool CHUNKED>
 __global__ void __launch_bounds__(IM2COL_THREADS)
 im2col_norm_kernel(const uint8_t* __restrict__ px, int n_strips, int gw, int patch, half16_t<F16>* __restrict__ out,
-                   long long ldo) {
-    extern __shared__ __align__(16) uint8_t strip[];  // [patch][w*3] + offset table [groups*8] (uint16)
-    const int w3 = gw * patch * 3;
-    const int strip_bytes = patch * w3;
+                   long long ldo, int cg) {
+    extern __shared__ __align__(16) uint8_t strip[];  // [patch][pitch] + offset table [groups*8] (uint16)
+    const int w3 = CHUNKED ? 0 : gw * patch * 3;
+    const int pitch = CHUNKED ? (cg * patch * 3 + 15) & ~15 : w3;  // bytes per staged pixel row (chunks: 16-byte multiple)
+    const int strip_bytes = patch * pitch;
     const int groups = static_cast<int>(ldo / 8);
     const int pp = patch * patch, kvalid = 3 * pp;
+    const int n_chunks = CHUNKED ? (gw + cg - 1) / cg : 1;
     unsigned short* off = reinterpret_cast<unsigned short*>(strip + ((strip_bytes + 15) & ~15));
     // column -> (ky << 8 | kx*3 + c): position inside the strip relative to the patch's first pixel (0xFFFF = pad column)
     for (int col = threadIdx.x; col < groups * 8; col += IM2COL_THREADS) {
@@ -45,23 +50,45 @@ im2col_norm_kernel(const uint8_t* __restrict__ px, int n_strips, int gw, int pat
         }
         off[col] = o;
     }
-    for (int sidx = blockIdx.x; sidx < n_strips; sidx += gridDim.x) {
-        const uint8_t* src = px + static_cast<long long>(sidx) * strip_bytes;
+    for (int unit = blockIdx.x; unit < n_strips * n_chunks; unit += gridDim.x) {
+        const int sidx = CHUNKED ? unit / n_chunks : unit;
+        const int p0 = CHUNKED ? (unit - sidx * n_chunks) * cg : 0;  // first patch column of the chunk
+        const int pc = CHUNKED ? min(cg, gw - p0) : gw;              // patch columns in the chunk
         __syncthreads();  // previous strip fully consumed (and the offset table written, first iteration)
-        if (((reinterpret_cast<uintptr_t>(src) | static_cast<uintptr_t>(strip_bytes)) & 15) == 0) {
-            const uint4* s4 = reinterpret_cast<const uint4*>(src);
-            uint4* d4 = reinterpret_cast<uint4*>(strip);
-            for (int i = threadIdx.x; i < (strip_bytes >> 4); i += IM2COL_THREADS) d4[i] = __ldg(s4 + i);
-        } else if (((reinterpret_cast<uintptr_t>(src) | static_cast<uintptr_t>(strip_bytes)) & 3) == 0) {
-            const uint32_t* s1 = reinterpret_cast<const uint32_t*>(src);
-            uint32_t* d1 = reinterpret_cast<uint32_t*>(strip);
-            for (int i = threadIdx.x; i < (strip_bytes >> 2); i += IM2COL_THREADS) d1[i] = __ldg(s1 + i);
+        if constexpr (CHUNKED) {
+            const long long row_bytes = static_cast<long long>(gw) * patch * 3;
+            const uint8_t* src = px + static_cast<long long>(sidx) * patch * row_bytes + static_cast<long long>(p0) * patch * 3;
+            const int cb = pc * patch * 3;  // bytes of the chunk in each pixel row
+            const uintptr_t al = reinterpret_cast<uintptr_t>(src) | static_cast<uintptr_t>(row_bytes) | static_cast<uintptr_t>(cb);
+            if ((al & 3) == 0) {
+                const int vpr = cb >> 2;
+                for (int i = threadIdx.x; i < patch * vpr; i += IM2COL_THREADS) {
+                    const int r = i / vpr, c = i - r * vpr;
+                    *reinterpret_cast<uint32_t*>(strip + r * pitch + c * 4) = __ldg(reinterpret_cast<const uint32_t*>(src + r * row_bytes) + c);
+                }
+            } else {
+                for (int i = threadIdx.x; i < patch * cb; i += IM2COL_THREADS) {
+                    const int r = i / cb, c = i - r * cb;
+                    strip[r * pitch + c] = __ldg(src + r * row_bytes + c);
+                }
+            }
         } else {
-            for (int i = threadIdx.x; i < strip_bytes; i += IM2COL_THREADS) strip[i] = __ldg(src + i);
+            const uint8_t* src = px + static_cast<long long>(sidx) * strip_bytes;
+            if (((reinterpret_cast<uintptr_t>(src) | static_cast<uintptr_t>(strip_bytes)) & 15) == 0) {
+                const uint4* s4 = reinterpret_cast<const uint4*>(src);
+                uint4* d4 = reinterpret_cast<uint4*>(strip);
+                for (int i = threadIdx.x; i < (strip_bytes >> 4); i += IM2COL_THREADS) d4[i] = __ldg(s4 + i);
+            } else if (((reinterpret_cast<uintptr_t>(src) | static_cast<uintptr_t>(strip_bytes)) & 3) == 0) {
+                const uint32_t* s1 = reinterpret_cast<const uint32_t*>(src);
+                uint32_t* d1 = reinterpret_cast<uint32_t*>(strip);
+                for (int i = threadIdx.x; i < (strip_bytes >> 2); i += IM2COL_THREADS) d1[i] = __ldg(s1 + i);
+            } else {
+                for (int i = threadIdx.x; i < strip_bytes; i += IM2COL_THREADS) strip[i] = __ldg(src + i);
+            }
         }
         __syncthreads();
-        half16_t<F16>* orow0 = out + static_cast<long long>(sidx) * gw * ldo;
-        const int items = gw * groups;
+        half16_t<F16>* orow0 = out + (static_cast<long long>(sidx) * gw + p0) * ldo;
+        const int items = pc * groups;
         for (int it = threadIdx.x; it < items; it += IM2COL_THREADS) {
             const int p = it / groups, g = it - p * groups;
             const uint4 o8 = *reinterpret_cast<const uint4*>(off + g * 8);
@@ -71,7 +98,7 @@ im2col_norm_kernel(const uint8_t* __restrict__ px, int n_strips, int gw, int pat
 #pragma unroll
             for (int j = 0; j < 4; ++j) {
                 const uint32_t oa = ow[j] & 0xFFFFu, ob = ow[j] >> 16;
-                const uint32_t aa = (oa >> 8) * w3 + (oa & 0xFFu), ab = (ob >> 8) * w3 + (ob & 0xFFu);
+                const uint32_t aa = (oa >> 8) * pitch + (oa & 0xFFu), ab = (ob >> 8) * pitch + (ob & 0xFFu);
                 const float va = oa == 0xFFFFu ? 0.f : fmaf(static_cast<float>(base[aa]), 2.0f / 255.0f, -1.0f);
                 const float vb = ob == 0xFFFFu ? 0.f : fmaf(static_cast<float>(base[ab]), 2.0f / 255.0f, -1.0f);
                 pk[j] = pack16x2<F16>(va, vb);
@@ -493,13 +520,34 @@ static int im2col_norm_impl(const uint8_t* pixels, int32_t n_slices, int32_t h, 
         }
     }
     const size_t smem = ((static_cast<size_t>(patch) * w * 3 + 15) & ~static_cast<size_t>(15)) + static_cast<size_t>(ldo) * 2;
-    VR_REQUIRE(smem <= 200 * 1024, "vr_im2col_norm: a %d-pixel-wide slice does not fit the %d-row strip buffer", w, patch);
-    static unsigned long long configured = 0;
-    if (first_use_on_device(&configured))
-        VR_CHECK_CUDA(cudaFuncSetAttribute(im2col_norm_kernel<F16>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
     const long long cap = static_cast<long long>(num_sms()) * 8;
+    static unsigned long long configured = 0;
+    if (first_use_on_device(&configured)) {
+        VR_CHECK_CUDA(cudaFuncSetAttribute(im2col_norm_kernel<F16, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
+        VR_CHECK_CUDA(cudaFuncSetAttribute(im2col_norm_kernel<F16, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
+    }
+    if (smem <= 200 * 1024) {  // the whole strip fits
+        if (blocks > cap) blocks = cap;
+        im2col_norm_kernel<F16, false><<<static_cast<int>(blocks), IM2COL_THREADS, smem, st>>>(pixels, static_cast<int>(n_strips), gw,
+                                                                                               patch, o, ldo, gw);
+        VR_CHECK_CUDA(cudaGetLastError());
+        return 0;
+    }
+    // chunks of at most cg patch columns: the largest count whose pixel rows (each padded to 16 bytes, so that the 4-byte
+    // stores of every row stay aligned) fit next to the offset table, then evened out over the chunks of a strip
+    const long long avail = 200 * 1024 - static_cast<long long>(ldo) * 2;
+    auto rows_bytes = [&](long long c) { return patch * ((c * patch * 3 + 15) & ~15ll); };
+    VR_REQUIRE(rows_bytes(1) <= avail, "vr_im2col_norm: ldo=%lld leaves no shared memory for one %d-pixel patch", (long long)ldo, patch);
+    long long max_cg = avail / (3ll * patch * patch);
+    while (rows_bytes(max_cg) > avail) --max_cg;
+    const long long n_chunks = (gw + max_cg - 1) / max_cg;
+    const int cg = static_cast<int>((gw + n_chunks - 1) / n_chunks);
+    VR_REQUIRE(n_strips * n_chunks < (1ll << 31), "vr_im2col_norm: too many patch rows");
+    const size_t smem_c = static_cast<size_t>(rows_bytes(cg)) + static_cast<size_t>(ldo) * 2;
+    blocks = n_strips * n_chunks;
     if (blocks > cap) blocks = cap;
-    im2col_norm_kernel<F16><<<static_cast<int>(blocks), IM2COL_THREADS, smem, st>>>(pixels, static_cast<int>(n_strips), gw, patch, o, ldo);
+    im2col_norm_kernel<F16, true><<<static_cast<int>(blocks), IM2COL_THREADS, smem_c, st>>>(pixels, static_cast<int>(n_strips), gw,
+                                                                                            patch, o, ldo, cg);
     VR_CHECK_CUDA(cudaGetLastError());
     return 0;
 }
