@@ -23,13 +23,13 @@ static int launch_gemm(const void* A, int64_t lda, const void* B, int64_t ldb, c
     return 0;
 }
 
-template <bool F16, int MODE, bool OUT_F32, bool GELU, int CLUSTER>
+template <bool F16, int MODE, bool OUT_F32, bool GELU, int CLUSTER, bool LEAN>
 static int launch_pingpong(const void* A, int64_t lda, const void* B, int64_t ldb, const GemmArgs& g, bool l2_slices,
                            cudaStream_t stream) {
     CUtensorMap ta, tb;
     if (int rc = make_tmap_2d(&ta, A, g.M, g.K, lda, GEMM_BM, GEMM_BK, 128, !F16)) return rc;
     if (int rc = make_tmap_2d(&tb, B, g.N, g.K, ldb, 64, GEMM_BK, 128, !F16)) return rc;
-    auto kern = gemm_pingpong_kernel<F16, MODE, OUT_F32, GELU, CLUSTER>;
+    auto kern = gemm_pingpong_kernel<F16, MODE, OUT_F32, GELU, CLUSTER, LEAN>;
     cudaLaunchConfig_t cfg = {};
     cudaLaunchAttribute attr[1];
     cfg.blockDim = dim3(GEMM_THREADS);
@@ -100,10 +100,12 @@ static int dispatch_swapped(const void* A, int64_t lda, const void* B, int64_t l
 
 // BN > 0: tile width of the cooperative kernel. BN < 0: the ping-pong kernel (128 x 128 tiles), as the block_n selector
 // -BN names it: PP (L2-sliced tile order), PP_NFAST (plain n-fastest order), PP_MC (CTA pairs with B multicast).
+// LEAN selects the ping-pong kernel's lean epilogue (16-bit LINEAR, bias [+ GELU] only); the cooperative kernel ignores it.
 constexpr int PP = 2, PP_MC = 4, PP_NFAST = 5;
-template <bool F16, int BN, int MODE, bool OUT_F32, bool GELU>
+template <bool F16, int BN, int MODE, bool OUT_F32, bool GELU, bool LEAN = false>
 static int launch_any(const void* A, int64_t lda, const void* B, int64_t ldb, const GemmArgs& g, cudaStream_t s) {
-    if constexpr (BN < 0) return launch_pingpong<F16, MODE, OUT_F32, GELU, -BN == PP_MC ? 2 : 1>(A, lda, B, ldb, g, -BN != PP_NFAST, s);
+    if constexpr (BN < 0)
+        return launch_pingpong<F16, MODE, OUT_F32, GELU, -BN == PP_MC ? 2 : 1, LEAN>(A, lda, B, ldb, g, -BN != PP_NFAST, s);
     else return launch_gemm<F16, BN, MODE, OUT_F32, GELU>(A, lda, B, ldb, g, s);
 }
 
@@ -111,11 +113,17 @@ template <bool F16, int BN>
 static int dispatch_mode(const void* A, int64_t lda, const void* B, int64_t ldb, const GemmArgs& g, cudaStream_t s) {
     const vr_gemm_epilogue& e = g.epi;
     switch (e.mode) {
-        case VR_EPI_LINEAR:
+        case VR_EPI_LINEAR: {
             if (int rc = check_out_dtype<F16>(e)) return rc;
             if (e.out_dtype == VR_F32) return launch_any<F16, BN, VR_EPI_LINEAR, true, false>(A, lda, B, ldb, g, s);
-            if (e.act_gelu) return launch_any<F16, BN, VR_EPI_LINEAR, false, true>(A, lda, B, ldb, g, s);
-            return launch_any<F16, BN, VR_EPI_LINEAR, false, false>(A, lda, B, ldb, g, s);
+            // a NULL bias keeps the generic epilogue: adding a zero bias would turn an accumulator of -0 into +0
+            const bool lean = BN < 0 && e.bias && e.scale == 1.0f && !e.rowadd && !e.resid;
+            if (e.act_gelu)
+                return lean ? launch_any<F16, BN, VR_EPI_LINEAR, false, true, true>(A, lda, B, ldb, g, s)
+                            : launch_any<F16, BN, VR_EPI_LINEAR, false, true>(A, lda, B, ldb, g, s);
+            return lean ? launch_any<F16, BN, VR_EPI_LINEAR, false, false, true>(A, lda, B, ldb, g, s)
+                        : launch_any<F16, BN, VR_EPI_LINEAR, false, false>(A, lda, B, ldb, g, s);
+        }
         case VR_EPI_ROPE:
             VR_REQUIRE(e.positions && e.rope_cos && e.rope_sin, "vr_gemm: ROPE epilogue needs positions/cos/sin");
             VR_REQUIRE(g.N % 64 == 0 && e.rope_cols % 64 == 0, "vr_gemm: ROPE needs N and rope_cols multiples of 64");

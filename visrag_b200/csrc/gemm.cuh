@@ -59,11 +59,6 @@ __device__ __forceinline__ float erf_as(float x) {
 }
 __device__ __forceinline__ float gelu_erf(float x) { return 0.5f * x * (1.0f + erf_as(x * 0.70710678118654752f)); }
 
-// two independent GELUs side by side (instruction-level parallelism for the Horner chains)
-__device__ __forceinline__ void pk_fma(float& d0, float& d1, float a0, float a1, float b0, float b1, float c0, float c1) {
-    d0 = fmaf(a0, b0, c0);
-    d1 = fmaf(a1, b1, c1);
-}
 #ifndef VR_GELU_POLY
 #define VR_GELU_POLY 1
 #endif
@@ -75,28 +70,46 @@ __device__ __forceinline__ void pk_fma(float& d0, float& d1, float a0, float a1,
 // |x| = 100) but stays about 2^-19 relative to the input, far below the bf16 rounding of the result
 // (tests/kernel_bounds.py derives the GEMM's GELU bound from this). The Abramowitz-Stegun form below needs two MUFU ops per
 // element (rcp + ex2): 65536 per 128x256 tile = 4096 SFU cycles on the critical path of the fc1 epilogue. This form is 14 FMA-pipe instructions per element and no MUFU.
-__device__ __forceinline__ void gelu_erf2(float& x0, float& x1) {
+// N GELUs as N interleaved chains: each step is done for all N values before the next, so consecutive FMAs are
+// independent (a single chain stalls on every FMA's latency). Per value the operations are the same for every N.
+template <int N>
+__device__ __forceinline__ void gelu_erf_n(float (&x)[N]) {
     constexpr float R2 = 0.70710678118654752f, ZMAX = 3.2f, A = 2.0f / (ZMAX * ZMAX);
-    const float z0 = fminf(fmaxf(x0 * R2, -ZMAX), ZMAX), z1 = fminf(fmaxf(x1 * R2, -ZMAX), ZMAX);
-    float w0, w1, u0, u1, p0, p1;
-    pk_fma(w0, w1, z0, z1, z0, z1, 0.0f, 0.0f);
-    pk_fma(u0, u1, w0, w1, A, A, -1.0f, -1.0f);
-    pk_fma(p0, p1, u0, u1, 2.982273671e-03f, 2.982273671e-03f, -7.046153472e-03f, -7.046153472e-03f);
-    pk_fma(p0, p1, p0, p1, u0, u1, 7.957076705e-03f, 7.957076705e-03f);
-    pk_fma(p0, p1, p0, p1, u0, u1, -1.521942819e-02f, -1.521942819e-02f);
-    pk_fma(p0, p1, p0, p1, u0, u1, 3.318292224e-02f, 3.318292224e-02f);
-    pk_fma(p0, p1, p0, p1, u0, u1, -5.471928813e-02f, -5.471928813e-02f);
-    pk_fma(p0, p1, p0, p1, u0, u1, 8.062700147e-02f, 8.062700147e-02f);
-    pk_fma(p0, p1, p0, p1, u0, u1, -1.136467381e-01f, -1.136467381e-01f);
-    pk_fma(p0, p1, p0, p1, u0, u1, 1.543549678e-01f, 1.543549678e-01f);
-    pk_fma(p0, p1, p0, p1, u0, u1, -2.173077339e-01f, -2.173077339e-01f);
-    pk_fma(p0, p1, p0, p1, u0, u1, 4.413341836e-01f, 4.413341836e-01f);
-    float r0, r1;
-    pk_fma(r0, r1, p0, p1, z0, z1, 0.0f, 0.0f);  // erf(z)
-    const float h0 = 0.5f * x0, h1 = 0.5f * x1;
-    pk_fma(x0, x1, h0, h1, r0, r1, h0, h1);
+    // P's coefficients, highest degree first
+    constexpr float C[11] = {2.982273671e-03f, -7.046153472e-03f, 7.957076705e-03f, -1.521942819e-02f, 3.318292224e-02f,
+                             -5.471928813e-02f, 8.062700147e-02f, -1.136467381e-01f, 1.543549678e-01f, -2.173077339e-01f,
+                             4.413341836e-01f};
+    float z[N], u[N], p[N];
+#pragma unroll
+    for (int i = 0; i < N; ++i) z[i] = fminf(fmaxf(x[i] * R2, -ZMAX), ZMAX);
+#pragma unroll
+    for (int i = 0; i < N; ++i) u[i] = fmaf(fmaf(z[i], z[i], 0.0f), A, -1.0f);
+#pragma unroll
+    for (int i = 0; i < N; ++i) p[i] = fmaf(u[i], C[0], C[1]);
+#pragma unroll
+    for (int k = 2; k < 11; ++k) {
+#pragma unroll
+        for (int i = 0; i < N; ++i) p[i] = fmaf(p[i], u[i], C[k]);
+    }
+#pragma unroll
+    for (int i = 0; i < N; ++i) {
+        const float r = fmaf(p[i], z[i], 0.0f);  // erf(z)
+        const float h = 0.5f * x[i];
+        x[i] = fmaf(h, r, h);
+    }
+}
+__device__ __forceinline__ void gelu_erf2(float& x0, float& x1) {
+    float x[2] = {x0, x1};
+    gelu_erf_n(x);
+    x0 = x[0];
+    x1 = x[1];
 }
 #else
+// two independent GELUs side by side (instruction-level parallelism for the Horner chains)
+__device__ __forceinline__ void pk_fma(float& d0, float& d1, float a0, float a1, float b0, float b1, float c0, float c1) {
+    d0 = fmaf(a0, b0, c0);
+    d1 = fmaf(a1, b1, c1);
+}
 __device__ __forceinline__ void gelu_erf2(float& x0, float& x1) {
     constexpr float R2 = 0.70710678118654752f;
     const float a0 = fabsf(x0) * R2, a1 = fabsf(x1) * R2;  // |z|, z = x / sqrt(2)
@@ -117,6 +130,11 @@ __device__ __forceinline__ void gelu_erf2(float& x0, float& x1) {
     r1 = copysignf(r1, x1);
     const float h0 = 0.5f * x0, h1 = 0.5f * x1;
     pk_fma(x0, x1, h0, h1, r0, r1, h0, h1);
+}
+template <int N>
+__device__ __forceinline__ void gelu_erf_n(float (&x)[N]) {
+#pragma unroll
+    for (int i = 0; i < N; i += 2) gelu_erf2(x[i], x[i + 1]);
 }
 #endif
 // x * sigmoid(x) with two SFU ops (ex2 + rcp, ~1e-6 relative) instead of an IEEE division
@@ -352,7 +370,11 @@ constexpr int GEMM_PP_A_BYTES = GEMM_BM * GEMM_BK * 2;
 constexpr int GEMM_PP_B_BYTES = GEMM_PP_BN * GEMM_BK * 2;
 constexpr int GEMM_PP_STAGE_BYTES = GEMM_PP_A_BYTES + GEMM_PP_B_BYTES;               // 32 KB
 constexpr int GEMM_PP_STAGES = (192 * 1024) / GEMM_PP_STAGE_BYTES;                    // 6
-constexpr int GEMM_PP_SMEM_BYTES = GEMM_PP_STAGES * GEMM_PP_STAGE_BYTES + 1024 + 256;  // + align slack + barriers
+// + align slack + barriers + the lean epilogue's bias slots (128 fp32 per consumer warpgroup). With the 1 KB the
+// system reserves per block this is 195.25 KB, within the 196 KB shared-memory carveout that the kernel needs
+// without the slots, so the SM's L1 keeps the same size.
+constexpr int GEMM_PP_SMEM_BYTES = GEMM_PP_STAGES * GEMM_PP_STAGE_BYTES + 1024 + 256 + 2 * GEMM_PP_BN * 4;
+constexpr int GEMM_PP_BAR_BIAS = 3;  // named barriers 3 and 4: the lean epilogue's bias slot of warpgroup 1 / 2 is full
 constexpr int GEMM_PP_BAR_TURN = 1;  // named barriers 1 (warpgroup 1's turn) and 2 (warpgroup 2's turn); 0 is __syncthreads
 
 // Tile order. A wave of CTAs reads its weight tiles from L2 only if the weight columns it works on stay resident while
@@ -473,6 +495,54 @@ __device__ __forceinline__ void pp_epilogue_linear(const GemmArgs& g, const floa
     }
 }
 
+// The lean LINEAR epilogue: 16-bit output, a bias, GELU or not, scale 1, no row add, no residual - every 16-bit LINEAR
+// class of the encode step (ViT qkv and fc1, resampler k / v). An epilogue warpgroup has one warp per SM sub-partition,
+// so nothing hides its latencies and its time is its instruction path. This one has no code for the absent terms,
+// reads the bias from a shared-memory slot that was filled while the MMAs ran (pp_stage_bias), runs a batch's 16 GELUs
+// as interleaved chains, and an interior tile (GUARD = false) stores without row or column tests. Per element the
+// arithmetic is pp_epilogue_linear's (acc + bias, then GELU), so the bits are the same.
+// The bias stays out of registers: 128 accumulators plus 32 bias registers leave ptxas too few to interleave the GELUs.
+// Thread t of a consumer warpgroup copies bias column n0 + t of its tile into the warpgroup's slot (none past N: those
+// columns are not stored).
+__device__ __forceinline__ void pp_stage_bias(float* slot, const GemmArgs& g, int n0, int t) {
+    if (n0 + t < g.N) cp_async_4(slot + t, g.epi.bias + n0 + t);
+}
+template <bool F16, bool GELU, bool GUARD>
+__device__ __forceinline__ void pp_epilogue_lean(const GemmArgs& g, const float (&acc)[64], const float* bias, int r0, int n0,
+                                                 int q) {
+    const vr_gemm_epilogue& e = g.epi;
+    // after the quad transpose lane q stores the 8 columns of group jb + q: base column n0 + 8 q
+    half16_t<F16>* out = reinterpret_cast<half16_t<F16>*>(e.out) + static_cast<long long>(r0) * e.ldo + n0 + 8 * q;
+    const long long row8 = 8 * e.ldo;
+    const bool row_ok[2] = {r0 < g.M, r0 + 8 < g.M};
+#pragma unroll
+    for (int jb = 0; jb < GEMM_PP_BN / 8; jb += 4) {
+        float x[16];  // x[4 j + 2 h + k] = acc[4 (jb + j) + 2 h + k]: column group jb + j, row r0 + 8 h, column 2 (lane % 4) + k
+#pragma unroll
+        for (int j = 0; j < 4; ++j) {
+            const float2 b = ld_shared_f2(bias + 8 * (jb + j) + 2 * q);
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+                x[4 * j + 2 * h] = acc[4 * (jb + j) + 2 * h] + b.x;
+                x[4 * j + 2 * h + 1] = acc[4 * (jb + j) + 2 * h + 1] + b.y;
+            }
+        }
+        if (GELU) gelu_erf_n(x);
+        uint32_t w16[2][4];
+#pragma unroll
+        for (int j = 0; j < 4; ++j) {
+#pragma unroll
+            for (int h = 0; h < 2; ++h) w16[h][j] = pack16x2<F16>(x[4 * j + 2 * h], x[4 * j + 2 * h + 1]);
+        }
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+            quad_transpose4(w16[h], q);
+            if (!GUARD || (row_ok[h] && n0 + 8 * (jb + q) < g.N))
+                *reinterpret_cast<uint4*>(out + h * row8 + 8 * jb) = make_uint4(w16[h][0], w16[h][1], w16[h][2], w16[h][3]);
+        }
+    }
+}
+
 // epilogue of one 64 x 128 row half: accumulator rows r0 and r0 + 8, columns n0 + 8 j + q2 (+1), q2 = 2 (lane % 4)
 template <bool F16, int MODE, bool OUT_F32, bool GELU>
 __device__ __forceinline__ void pp_epilogue(const GemmArgs& g, const float (&acc)[64], int r0, int n0, int q2) {
@@ -504,11 +574,13 @@ __device__ __forceinline__ void pp_epilogue(const GemmArgs& g, const float (&acc
 // into it too): every consumer warp arrives on the empty barrier of both CTAs. Both CTAs walk the same unit sequence,
 // so their rings stay in step. With an odd number of M tiles the last pair's second tile lies past M: TMA fills it
 // with zeros (the bytes still count) and the epilogue's row guard drops it.
-template <bool F16, int MODE, bool OUT_F32, bool GELU, int CLUSTER>
+// LEAN: the lean 16-bit LINEAR epilogue (pp_epilogue_lean); the host selects it when the epilogue is exactly bias [+ GELU].
+template <bool F16, int MODE, bool OUT_F32, bool GELU, int CLUSTER, bool LEAN = false>
 __global__ void __launch_bounds__(GEMM_THREADS, 1)
 gemm_pingpong_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b, const GemmArgs g,
                      const PPSched sch) {
     static_assert(CLUSTER == 1 || CLUSTER == 2, "CTA pairs at most");
+    static_assert(!LEAN || (MODE == VR_EPI_LINEAR && !OUT_F32), "the lean epilogue writes 16-bit LINEAR outputs");
     constexpr int STAGES = GEMM_PP_STAGES;
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
@@ -516,6 +588,7 @@ gemm_pingpong_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_co
     uint8_t* smem_b = smem + STAGES * GEMM_PP_A_BYTES;
     uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + STAGES * GEMM_PP_STAGE_BYTES);
     uint64_t* empty_bar = full_bar + STAGES;
+    float* bias_slots = reinterpret_cast<float*>(smem + STAGES * GEMM_PP_STAGE_BYTES + 256);
 
     const int wg = threadIdx.x >> 7;
     const int warp = (threadIdx.x >> 5) & 3;
@@ -573,6 +646,7 @@ gemm_pingpong_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_co
         const uint32_t a_lo0 = smem_u32(smem_a) >> 4, b_lo0 = smem_u32(smem_b) >> 4;
         constexpr uint32_t HALF = (64 * GEMM_BK * 2) >> 4;  // rows 64..127 of the A stage
         const int g8 = lane >> 2, q = lane & 3;
+        float* bias_slot = bias_slots + me * GEMM_PP_BN;  // LEAN only
         // release a stage: one arrival per warp on the empty barrier of every CTA of the cluster
         auto release = [&](int s) {
             if (lane != 0) return;
@@ -588,6 +662,13 @@ gemm_pingpong_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_co
             int stage = pos % STAGES;
             uint32_t phase = (pos / STAGES) & 1;
             if (i > 0) named_bar_sync(GEMM_PP_BAR_TURN + me, 256);  // the previous tile's MMAs are all issued
+            if constexpr (LEAN) {
+                // every warp of this warpgroup has passed the turn barrier, so its reads of the previous tile's bias
+                // are done; the copy completes under the mainloop
+                int um, tn;
+                sch.coords(u, um, tn);
+                pp_stage_bias(bias_slot, g, tn * GEMM_PP_BN, threadIdx.x & 127);
+            }
             float acc0[64], acc1[64];  // rows 0..63 and 64..127 of the tile
             int prev = -1;
             for (int kb = 0; kb < num_kb; ++kb) {
@@ -619,8 +700,20 @@ gemm_pingpong_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_co
             int um, tn;
             sch.coords(u, um, tn);
             const int m0 = (um * CLUSTER + rank) * GEMM_BM, n0 = tn * GEMM_PP_BN;
-            pp_epilogue<F16, MODE, OUT_F32, GELU>(g, acc0, m0 + warp * 16 + g8, n0, q * 2);
-            pp_epilogue<F16, MODE, OUT_F32, GELU>(g, acc1, m0 + 64 + warp * 16 + g8, n0, q * 2);
+            if constexpr (LEAN) {
+                cp_async_wait_all();
+                named_bar_sync(GEMM_PP_BAR_BIAS + me, 128);  // every thread's bias column has landed
+                if (m0 + GEMM_BM <= g.M && n0 + GEMM_PP_BN <= g.N) {
+                    pp_epilogue_lean<F16, GELU, false>(g, acc0, bias_slot, m0 + warp * 16 + g8, n0, q);
+                    pp_epilogue_lean<F16, GELU, false>(g, acc1, bias_slot, m0 + 64 + warp * 16 + g8, n0, q);
+                } else {
+                    pp_epilogue_lean<F16, GELU, true>(g, acc0, bias_slot, m0 + warp * 16 + g8, n0, q);
+                    pp_epilogue_lean<F16, GELU, true>(g, acc1, bias_slot, m0 + 64 + warp * 16 + g8, n0, q);
+                }
+            } else {
+                pp_epilogue<F16, MODE, OUT_F32, GELU>(g, acc0, m0 + warp * 16 + g8, n0, q * 2);
+                pp_epilogue<F16, MODE, OUT_F32, GELU>(g, acc1, m0 + 64 + warp * 16 + g8, n0, q * 2);
+            }
         }
     }
     // The partner may still multicast into this CTA's ring or arrive on its barriers until it has drained its own

@@ -99,6 +99,18 @@ __device__ __forceinline__ void fence_proxy_async_smem() {
 __device__ __forceinline__ void tma_prefetch_desc(const CUtensorMap* m) {
     asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(m)) : "memory");
 }
+// 4-byte asynchronous copy global -> shared (no registers involved); cp_async_wait_all waits for the thread's own copies
+__device__ __forceinline__ void cp_async_4(void* smem_dst, const void* gsrc) {
+    asm volatile("cp.async.ca.shared.global [%0], [%1], 4;" ::"r"(smem_u32(smem_dst)), "l"(gsrc) : "memory");
+}
+__device__ __forceinline__ void cp_async_wait_all() { asm volatile("cp.async.wait_all;" ::: "memory"); }
+// 8-byte shared-memory load (the memory clobber keeps it after the waits and barriers that make the data visible)
+__device__ __forceinline__ float2 ld_shared_f2(const void* p) {
+    float2 v;
+    asm("ld.shared.v2.f32 {%0, %1}, [%2];" : "=f"(v.x), "=f"(v.y) : "r"(smem_u32(p)) : "memory");
+    return v;
+}
+
 // 2-D tiled load: coordinates are (c0 = innermost/contiguous dim, c1 = row).
 __device__ __forceinline__ void tma_load_2d(const CUtensorMap* m, uint64_t* bar, void* smem_dst, int c0, int c1) {
     asm volatile(
