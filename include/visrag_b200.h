@@ -292,6 +292,50 @@ int vr_topk_rows_chunked_masked(const float* scores, int32_t rows, int64_t cols,
                                 int32_t chunks, float* ws_scores, int64_t* ws_ids, float* out_scores, int64_t* out_ids,
                                 const uint32_t* doc_mask, void* stream);
 
+/* Document-level retrieval: the top-k GROUPS (documents) of pages, each scored by its best page.
+ * doc_groups [nd] int32: the group of each doc (page), in [0, G). group_offsets [G+1] / group_pages [nd] int32: the same
+ * mapping as CSR, pages ascending within a group (a stable sort of doc_groups). The score of a group is the maximum exact
+ * fp32 score over its eligible pages (the bits vr_score_exact gives each pair; NaN never selected), its best page the
+ * lowest page with that maximum; groups rank by (score desc, best page asc). Outputs per query: out_scores [k] f32,
+ * out_pages [k] i64 (best page + id_offset), out_groups [k] i64; a group without an eligible page never appears, and
+ * fewer than k groups leave a tail of (-inf, -1, -1). With every page its own group the result equals the page top-k.
+ * doc_mask (optional, NULL: every page eligible) has the layout of the _masked calls. A NULL or misaligned doc_groups or
+ * CSR array, G <= 0, a workspace too small and nd >= 2^31 are refused before any CUDA call.
+ *   vr_score_filter_groups  : vr_score_filter with GROUP-DISTINCT lists: a list holds at most one page per group (a page
+ *                             of a group already listed replaces that entry only when its score is higher). Every page a
+ *                             list dropped is <= that list's tail or <= its own group's entry in that list;
+ *   vr_score_rescore_groups : step 1 as vr_score_rescore; then the distinct groups of the kept candidates, in approximate
+ *                             order, are FULLY rescored (every eligible page, through the CSR) while their pages fit a
+ *                             budget of 4096 per query; the top-k of those groups is certified when
+ *                             max(list tails, pruned heads, approximate entries of kept groups not rescored) + eps is
+ *                             below the k-th group score, else flags[q] = 1 (rerun through vr_score_exact +
+ *                             vr_group_topk_rows). Sound with the lists of any filter (page lists meet the invariant);
+ *   vr_group_topk_rows      : the group top-k of dense score rows [rows, nd] (vr_score_exact output), from doc_groups
+ *                             alone (an order-independent atomicMax of (score, ~page) keys per (row, group), spread over
+ *                             the pages whatever the group sizes); chunks >= 2 spreads each row's groups over `chunks`
+ *                             blocks (few rows x many groups), 0 or 1 does not. Workspace of
+ *                             vr_group_topk_ws_bytes(rows, G, k, chunks) bytes, 16-byte aligned;
+ *   vr_merge_group_topk     : merge of per-rank partial group lists [rows, cols] (score, page, group; page < 0 = empty,
+ *                             cols <= 512, i.e. world * k <= 512; larger is refused): the first k distinct groups in
+ *                             (score desc, page asc) order. A group's best
+ *                             page lies on one rank, whose local top-k holds it whenever the group is in the global
+ *                             top-k, so the merge is exact when documents span ranks. */
+int vr_score_filter_groups(const void* q_f16, int32_t nq, const void* d_f16, int64_t nd, int32_t dim, int32_t ranges,
+                           float* cand_scores, int32_t* cand_ids, const int32_t* doc_groups, const uint32_t* doc_mask,
+                           void* stream);
+int vr_score_rescore_groups(const float* q_f32, int32_t nq, const float* d_f32, int64_t nd, int32_t dim, int32_t ranges,
+                            const float* cand_scores, const int32_t* cand_ids, const int32_t* doc_groups,
+                            const int32_t* group_offsets, const int32_t* group_pages, int32_t G, const uint32_t* doc_mask,
+                            const float* max_doc_norm, int32_t k, int64_t id_offset, float* out_scores, int64_t* out_pages,
+                            int64_t* out_groups, int32_t* flags, void* stream);
+int64_t vr_group_topk_ws_bytes(int32_t rows, int32_t G, int32_t k, int32_t chunks);
+int vr_group_topk_rows(const float* scores, int32_t rows, int64_t nd, const int32_t* doc_groups, int32_t G,
+                       const uint32_t* doc_mask, int32_t k, int64_t id_offset,
+                       int32_t chunks, void* ws, int64_t ws_bytes, float* out_scores, int64_t* out_pages, int64_t* out_groups,
+                       void* stream);
+int vr_merge_group_topk(const float* scores, const int64_t* pages, const int64_t* groups, int32_t rows, int32_t cols, int32_t k,
+                        float* out_scores, int64_t* out_pages, int64_t* out_groups, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

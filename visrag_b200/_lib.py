@@ -117,6 +117,17 @@ def _declare(lib: C.CDLL) -> None:
     lib.vr_topk_rows_masked.argtypes = [vp, vp, i32, i64, i32, i64, vp, vp, vp, vp]
     lib.vr_topk_rows_chunked_masked.restype = i32
     lib.vr_topk_rows_chunked_masked.argtypes = [vp, i32, i64, i32, i64, i32, vp, vp, vp, vp, vp, vp]
+    lib.vr_score_filter_groups.restype = i32
+    lib.vr_score_filter_groups.argtypes = [vp, i32, vp, i64, i32, i32, vp, vp, vp, vp, vp]
+    lib.vr_score_rescore_groups.restype = i32
+    lib.vr_score_rescore_groups.argtypes = [vp, i32, vp, i64, i32, i32, vp, vp, vp, vp, vp, i32, vp, vp, i32, i64, vp, vp, vp,
+                                            vp, vp]
+    lib.vr_group_topk_ws_bytes.restype = i64
+    lib.vr_group_topk_ws_bytes.argtypes = [i32, i32, i32, i32]
+    lib.vr_group_topk_rows.restype = i32
+    lib.vr_group_topk_rows.argtypes = [vp, i32, i64, vp, i32, vp, i32, i64, i32, vp, i64, vp, vp, vp, vp]
+    lib.vr_merge_group_topk.restype = i32
+    lib.vr_merge_group_topk.argtypes = [vp, vp, vp, i32, i32, i32, vp, vp, vp, vp]
     lib.vr_pool_norm.restype = i32
     lib.vr_pool_norm.argtypes = [vp, i64, vp, f32, vp, i32, i32, i32, i32, vp, vp]
     lib.vr_prefix_rows.restype = i32

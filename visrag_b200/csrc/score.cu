@@ -51,6 +51,14 @@ struct MaskedScoreArgs : ScoreArgs {
     const uint32_t* doc_mask;  // ceil(nd / 32) words: doc i is eligible when bit i & 31 of word i >> 5 is set
 };
 
+struct GroupedScoreArgs : ScoreArgs {
+    const int* doc_groups;     // [nd]: the group (document) of each doc (page)
+};
+
+struct MaskedGroupedScoreArgs : MaskedScoreArgs {
+    const int* doc_groups;
+};
+
 struct Score2Cfg {
     static constexpr int STAGES = 6;
     static constexpr int SUB_BN = 128;                      // docs per MMA sub-tile (a 256-doc tile is two of them)
@@ -76,6 +84,37 @@ __device__ __forceinline__ void topk_insert(float (&sc)[SC_KT], int (&id)[SC_KT]
     }
 }
 
+// Group-distinct lists: a list holds at most one doc per group. A doc whose group already has an entry replaces it only
+// when its score is higher, and is dropped otherwise; a doc of a new group goes in as topk_insert puts it (precondition
+// then: v > sc[SC_KT-1]). Every dropped doc is therefore <= the list's final tail or <= its own group's entry. The groups
+// of the entries are looked up, not kept in registers: this runs on the rare insertion path only.
+__device__ __forceinline__ void group_insert(float (&sc)[SC_KT], int (&id)[SC_KT], float v, int i,
+                                             const int* __restrict__ groups) {
+    const int gi = __ldg(groups + i);
+    bool same = false, up = false;
+#pragma unroll
+    for (int j = 0; j < SC_KT; ++j) {
+        if (id[j] >= 0 && __ldg(groups + id[j]) == gi) {
+            same = true;
+            if (v > sc[j]) { sc[j] = v; id[j] = i; up = true; }
+        }
+    }
+    if (!same) {
+        topk_insert(sc, id, v, i);
+    } else if (up) {  // the raised entry moves up to its place (one pass from the bottom carries it)
+#pragma unroll
+        for (int j = SC_KT - 1; j > 0; --j) {
+            const bool sw = sc[j] > sc[j - 1];
+            const float a = sc[j], b = sc[j - 1];
+            const int ia = id[j], ib = id[j - 1];
+            sc[j - 1] = sw ? a : b;
+            sc[j] = sw ? b : a;
+            id[j - 1] = sw ? ia : ib;
+            id[j] = sw ? ib : ia;
+        }
+    }
+}
+
 __device__ __forceinline__ float quad_max(float v) {
     v = fmaxf(v, __shfl_xor_sync(0xffffffffu, v, 1));
     return fmaxf(v, __shfl_xor_sync(0xffffffffu, v, 2));
@@ -92,11 +131,16 @@ __device__ __forceinline__ float quad_max(float v) {
 // tail, and so the rescoring kernel's bound, is a tail over eligible docs only.
 // The mask travels in its own argument type, so the unmasked form keeps the parameter list it has without the mask (an
 // unused parameter or ScoreArgs field changes its register allocation and code).
+// GROUPED ((Masked)GroupedScoreArgs): doc_groups gives each doc its group, and every list is group-distinct (group_insert,
+// in the slow path and in the quad merge); the fast path is that of the page-level form with the same masking. The quad merge keeps the merged tail >= each lane's tail
+// (each lane's 16 groups have an entry at least that high in the union), so thr stays a valid drop threshold, and a
+// published tau is the tail of a group-distinct list.
 template <typename Args>
 __global__ void __launch_bounds__(GEMM_THREADS, 1)
 score_filter_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant__ CUtensorMap tmap_d,
                     const Args g) {
-    constexpr bool MASKED = std::is_same<Args, MaskedScoreArgs>::value;
+    constexpr bool GROUPED = std::is_same<Args, GroupedScoreArgs>::value || std::is_same<Args, MaskedGroupedScoreArgs>::value;
+    constexpr bool MASKED = std::is_same<Args, MaskedScoreArgs>::value || std::is_same<Args, MaskedGroupedScoreArgs>::value;
     using Cfg = Score2Cfg;
     constexpr int STAGES = Cfg::STAGES;
     extern __shared__ uint8_t smem_raw[];
@@ -256,7 +300,8 @@ score_filter_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_con
                         const float sv = __uint_as_float((j & 16) ? s2[1] : s2[0]);
                         const long long col = col_base + (j >> 1) * 8 + (j & 1);
                         if (sv > thr[h] && col < g.nd) {
-                            topk_insert(sc[h], id[h], sv, static_cast<int>(col));
+                            if constexpr (GROUPED) group_insert(sc[h], id[h], sv, static_cast<int>(col), g.doc_groups);
+                            else topk_insert(sc[h], id[h], sv, static_cast<int>(col));
                             thr[h] = fmaxf(thr[h], sc[h][SC_KT - 1]);
                         }
                     }
@@ -285,7 +330,10 @@ score_filter_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_con
 #pragma unroll
                     for (int i = 1; i < SC_KT; ++i)
                         if (i == j) { v2 = os[i]; i2 = oi[i]; }
-                    if (v2 > sc[h][SC_KT - 1]) topk_insert(sc[h], id[h], v2, i2);
+                    if (v2 > sc[h][SC_KT - 1]) {
+                        if constexpr (GROUPED) group_insert(sc[h], id[h], v2, i2, g.doc_groups);
+                        else topk_insert(sc[h], id[h], v2, i2);
+                    }
                 }
             }
             const int row = row0 + 8 * h;
@@ -325,6 +373,66 @@ __device__ __forceinline__ bool before(float sa, long long ia, float sb, long lo
 
 constexpr int RS_THREADS = 128;
 constexpr int RS_MAX_KEEP = 256;
+
+// Step 1 of rescore_groups_kernel (warp 0, every lane returns the bound), the same merge as step 1 of rescore_topk_kernel
+// (which keeps its own inlined copy: compiled through this function its code changes): the `keep` best candidates by
+// approximate score go to sel[] and their scores to sel_s[] (-1 pads when the lists run out); the return value bounds
+// everything else: the list tails and the best pruned head.
+__device__ __forceinline__ float merge_list_heads(const float* __restrict__ cs, const int* __restrict__ ci, int lists,
+                                                  int keep, int lane, int* sel, float* sel_s) {
+    // lane l owns lists l, l+32, ...: head position per owned list (<= 2 lists per lane for lists <= 64; general loop)
+    float tail = -INFINITY;
+    for (int l = lane; l < lists; l += 32) tail = fmaxf(tail, cs[l * SC_KT + SC_KT - 1]);
+    int head[(SC_MAX_RANGES + 31) / 32 + 1];
+#pragma unroll
+    for (int j = 0; j < (SC_MAX_RANGES + 31) / 32 + 1; ++j) head[j] = 0;
+    for (int m = 0; m < keep; ++m) {
+        // best head of this lane
+        float bs = -INFINITY;
+        int bj = -1;
+#pragma unroll
+        for (int j = 0; j < (SC_MAX_RANGES + 31) / 32 + 1; ++j) {
+            const int l = lane + j * 32;
+            if (l < lists && head[j] < SC_KT) {
+                const float v = cs[l * SC_KT + head[j]];
+                if (ci[l * SC_KT + head[j]] >= 0 && (bj < 0 || v > bs)) { bs = v; bj = j; }
+            }
+        }
+        // warp arg-max (ties: lower lane)
+        float ws = bs;
+        int wl = bj >= 0 ? lane : 64;
+#pragma unroll
+        for (int o = 16; o > 0; o >>= 1) {
+            const float os = __shfl_xor_sync(0xffffffffu, ws, o);
+            const int ol = __shfl_xor_sync(0xffffffffu, wl, o);
+            if (ol < 64 && (wl >= 64 || os > ws || (os == ws && ol < wl))) { ws = os; wl = ol; }
+        }
+        if (wl >= 64) {  // every list exhausted
+            for (int r = m + lane; r < keep; r += 32) sel[r] = -1;
+            break;
+        }
+        if (lane == wl) {
+#pragma unroll
+            for (int j = 0; j < (SC_MAX_RANGES + 31) / 32 + 1; ++j)
+                if (j == bj) {
+                    sel[m] = ci[(lane + j * 32) * SC_KT + head[j]];
+                    sel_s[m] = ws;
+                    ++head[j];
+                }
+        }
+    }
+    // what is left in the lists was pruned: bounded by the best remaining head
+    float rem = -INFINITY;
+#pragma unroll
+    for (int j = 0; j < (SC_MAX_RANGES + 31) / 32 + 1; ++j) {
+        const int l = lane + j * 32;
+        if (l < lists && head[j] < SC_KT && ci[l * SC_KT + head[j]] >= 0) rem = fmaxf(rem, cs[l * SC_KT + head[j]]);
+    }
+    float bnd = fmaxf(tail, rem);
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) bnd = fmaxf(bnd, __shfl_xor_sync(0xffffffffu, bnd, o));
+    return bnd;
+}
 
 // One CTA per query. The filter hands over `lists` sorted 16-entry candidate lists (approximate scores). Step 1 (warp 0):
 // multi-way merge of the list heads keeps the `keep` best candidates by approximate score; everything else - docs a list
@@ -486,6 +594,191 @@ rescore_topk_kernel(const float* __restrict__ Q, const float* __restrict__ D, lo
         if (sh_bound > -INFINITY && !(sh_bound + eps < kth)) flag = 1;  // something was dropped that might belong
         // the bound assumes finite fp16 copies of both operands: a row norm >= 65504 (or inf / NaN, for which the
         // comparison is false as well) means some |x| may have overflowed fp16 -> rerun this query through the fp32 scan
+        if (!(sh_qnorm < 65504.f) || !(dn < 65504.f)) flag = 1;
+        flags[q] = flag;
+    }
+}
+
+// ---------------------------------------------------------------------------------------------
+// Document-level (grouped) rescoring. doc_groups [nd] gives every doc (page) its group (document); the CSR group_offsets
+// [G+1] / group_pages lists each group's pages, ascending. The score of a group is the maximum exact score over its
+// eligible pages, its best page the lowest of those with that maximum; groups rank by (score desc, best page asc).
+// Candidate lists may come from either filter: group-distinct lists (every dropped page <= the list's tail or <= its own
+// group's entry in that list) or page lists (every dropped page <= the tail, which satisfies the same invariant).
+constexpr int RG_PAGE_BUDGET = 4096;  // pages one query may fully rescore (36 KB of fp32 rows each at dim 2304)
+
+// One CTA per query. Step 1: the list-head merge and bound of rescore_topk_kernel. Step 2: the distinct groups of the kept
+// candidates, in approximate order; as long as their pages fit RG_PAGE_BUDGET, each is FULLY rescored (every eligible
+// page, exact fp32, the FMA order and warp reduction of the page kernels, so the same bits); the first group that does
+// not fit ends the walk, and it and every later kept group enter the bound with their best approximate entry. Step 3:
+// top-k of the rescored groups and the proof  B + eps < k-th group score, B = max(list tails, pruned heads, approximate
+// entries of kept groups not rescored). A group that was not rescored has every page p either dropped by a list
+// (approx(p) <= that list's tail, or <= its group's entry there, which was kept - so in B - or pruned - so <= a pruned
+// head) or pruned or kept (in B): exact(p) <= B + eps < k-th. Otherwise the query is flagged.
+__global__ void __launch_bounds__(RS_THREADS, 1)  // without the 1, ptxas caps it at 32 registers and spills
+rescore_groups_kernel(const float* __restrict__ Q, const float* __restrict__ D, int dim, int lists, int keep,
+                      const float* __restrict__ cand_scores, const int* __restrict__ cand_ids,
+                      const int* __restrict__ doc_groups, const int* __restrict__ group_offsets,
+                      const int* __restrict__ group_pages, const uint32_t* __restrict__ doc_mask,
+                      const float* __restrict__ max_doc_norm, int k, long long id_offset, float* __restrict__ out_scores,
+                      long long* __restrict__ out_pages, long long* __restrict__ out_groups, int* __restrict__ flags) {
+    extern __shared__ float sm[];
+    float* qs = sm;                                      // [dim]
+    float* ex = qs + dim;                                // [RG_PAGE_BUDGET] exact scores of the rescored pages
+    int* pg = reinterpret_cast<int*>(ex + RG_PAGE_BUDGET);  // [RG_PAGE_BUDGET] their pages (-1: ineligible)
+    float* sel_s = reinterpret_cast<float*>(pg + RG_PAGE_BUDGET);  // [keep] approximate scores of the kept candidates
+    int* sel = reinterpret_cast<int*>(sel_s + keep);     // [keep] their pages
+    int* first = sel + keep;                             // [keep] group of the candidate if it is its group's first, else -1
+    int* gstart = first + keep;                          // [keep + 1] rescored group s owns pg[gstart[s], gstart[s+1])
+    int* gid = gstart + keep + 1;                        // [keep] its group
+    float* gs = reinterpret_cast<float*>(gid + keep);    // [keep] its score
+    int* gp = reinterpret_cast<int*>(gs + keep);         // [keep] its best page (-1: no eligible page)
+    __shared__ float red_s[RS_THREADS / 32];
+    __shared__ long long red_i[RS_THREADS / 32];
+    __shared__ float sh_bound, sh_qnorm;
+    __shared__ int sh_ng;
+    const int q = blockIdx.x;
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const float* qrow = Q + static_cast<long long>(q) * dim;
+    if (warp == 0) {
+        const float bnd = merge_list_heads(cand_scores + static_cast<long long>(q) * lists * SC_KT,
+                                           cand_ids + static_cast<long long>(q) * lists * SC_KT, lists, keep, lane, sel, sel_s);
+        if (lane == 0) sh_bound = bnd;
+    }
+    float qq = 0.f;
+    for (int i = threadIdx.x; i < dim; i += RS_THREADS) {
+        const float v = qrow[i];
+        qs[i] = v;
+        qq += v * v;
+    }
+    qq = warp_sum_f(qq);
+    if (lane == 0) red_s[warp] = qq;
+    __syncthreads();  // qs, sel, sel_s, sh_bound, red_s visible
+    for (int c = threadIdx.x; c < keep; c += RS_THREADS) {
+        const int p = sel[c];
+        int g = p >= 0 ? __ldg(doc_groups + p) : -1;
+        for (int j = 0; j < c && g >= 0; ++j)
+            if (sel[j] >= 0 && __ldg(doc_groups + sel[j]) == g) g = -1;
+        first[c] = g;
+    }
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        float s = 0.f;
+        for (int i = 0; i < RS_THREADS / 32; ++i) s += red_s[i];
+        sh_qnorm = sqrtf(s);
+        float bnd = sh_bound;
+        int ng = 0, total = 0;
+        bool full = false;
+        for (int c = 0; c < keep; ++c) {
+            const int g = first[c];
+            if (g < 0) continue;
+            const int n = __ldg(group_offsets + g + 1) - __ldg(group_offsets + g);
+            if (!full && n <= RG_PAGE_BUDGET - total) {
+                gid[ng] = g;
+                gstart[ng++] = total;
+                total += n;
+            } else {
+                full = true;
+                bnd = fmaxf(bnd, sel_s[c]);  // the group's best kept entry (candidates are in approximate order)
+            }
+        }
+        gstart[ng] = total;
+        sh_ng = ng;
+        sh_bound = bnd;
+    }
+    __syncthreads();
+    const int ng = sh_ng, total = gstart[ng];
+    for (int s = 0; s < ng; ++s) {
+        const int* src = group_pages + __ldg(group_offsets + gid[s]);
+        const int n = gstart[s + 1] - gstart[s];
+        for (int i = threadIdx.x; i < n; i += RS_THREADS) {
+            const int p = __ldg(src + i);
+            pg[gstart[s] + i] = doc_mask && !((__ldg(doc_mask + (p >> 5)) >> (p & 31)) & 1u) ? -1 : p;
+        }
+    }
+    __syncthreads();
+    // exact fp32 rescoring of every eligible page of the rescored groups: one warp per page
+    for (int t = warp; t < total; t += RS_THREADS / 32) {
+        const int id = pg[t];
+        float s = -INFINITY;
+        if (id >= 0) {
+            const float4* drow = reinterpret_cast<const float4*>(D + static_cast<long long>(id) * dim);
+            const float4* q4 = reinterpret_cast<const float4*>(qs);
+            float a = 0.f;
+            for (int i = lane; i < (dim >> 2); i += 32) {
+                const float4 x = drow[i], y = q4[i];
+                a = fmaf(x.x, y.x, a);
+                a = fmaf(x.y, y.y, a);
+                a = fmaf(x.z, y.z, a);
+                a = fmaf(x.w, y.w, a);
+            }
+            s = warp_sum_f(a);
+        }
+        if (lane == 0) ex[t] = s;
+    }
+    __syncthreads();
+    // each group: max over its eligible pages (NaN never selected), lowest page on ties (pages ascend)
+    for (int s = threadIdx.x; s < ng; s += RS_THREADS) {
+        float best = -INFINITY;
+        int bp = -1;
+        for (int t = gstart[s]; t < gstart[s + 1]; ++t) {
+            const float v = ex[t];
+            if (pg[t] >= 0 && !isnan(v) && (bp < 0 || v > best)) { best = v; bp = pg[t]; }
+        }
+        gs[s] = best;
+        gp[s] = bp;
+    }
+    __syncthreads();
+    // k rounds of block arg-max over the rescored groups in (score desc, best page asc) order
+    float last_s = INFINITY;
+    long long last_i = -1;
+    float kth = -INFINITY;
+    for (int round = 0; round < k; ++round) {
+        float bs = -INFINITY;
+        long long bi = 0x7fffffffffffffffll;
+        for (int c = threadIdx.x; c < ng; c += RS_THREADS) {
+            const int id = gp[c];
+            if (id < 0) continue;
+            const float s = gs[c];
+            if (!before(last_s, last_i, s, id)) continue;
+            if (before(s, id, bs, bi)) { bs = s; bi = id; }
+        }
+#pragma unroll
+        for (int o = 16; o > 0; o >>= 1) {
+            const float os = __shfl_xor_sync(0xffffffffu, bs, o);
+            const long long oi = __shfl_xor_sync(0xffffffffu, bi, o);
+            if (before(os, oi, bs, bi)) { bs = os; bi = oi; }
+        }
+        if (lane == 0) { red_s[warp] = bs; red_i[warp] = bi; }
+        __syncthreads();
+        bs = red_s[0]; bi = red_i[0];
+        for (int i = 1; i < RS_THREADS / 32; ++i)
+            if (before(red_s[i], red_i[i], bs, bi)) { bs = red_s[i]; bi = red_i[i]; }
+        __syncthreads();
+        const bool valid = bi != 0x7fffffffffffffffll;
+        const long long o = static_cast<long long>(q) * k;
+        if (threadIdx.x == 0) {
+            out_scores[o + round] = valid ? bs : -INFINITY;
+            out_pages[o + round] = valid ? bi + id_offset : -1;
+            out_groups[o + round] = valid ? __ldg(doc_groups + bi) : -1;
+        }
+        if (!valid) {
+            for (int r2 = round + 1 + threadIdx.x; r2 < k; r2 += RS_THREADS) {
+                out_scores[o + r2] = -INFINITY;
+                out_pages[o + r2] = -1;
+                out_groups[o + r2] = -1;
+            }
+            kth = -INFINITY;
+            break;
+        }
+        last_s = bs; last_i = bi; kth = bs;
+    }
+    if (threadIdx.x == 0) {  // eps and the overflow test of rescore_topk_kernel
+        const float dn = *max_doc_norm;
+        const float eps = (9.765625e-4f + static_cast<float>(dim) * 1.1920929e-7f) * sh_qnorm * dn +
+                          sqrtf(static_cast<float>(dim)) * 5.9604645e-8f * (sh_qnorm + dn) + 1e-6f;
+        int flag = 0;
+        if (sh_bound > -INFINITY && !(sh_bound + eps < kth)) flag = 1;
         if (!(sh_qnorm < 65504.f) || !(dn < 65504.f)) flag = 1;
         flags[q] = flag;
     }
@@ -680,6 +973,129 @@ static int launch_topk_rows(const float* scores, const long long* ids, int rows,
     else
         topk_rows_kernel<MASKED><<<rows, 256, 0, s>>>(scores, ids, cols, k, id_offset, cols, out_scores, out_ids, mask);
     return 0;
+}
+
+// Exact grouped path, after vr_score_exact: every (row, group) of scores [rows, nd] reduces to its maximum over the
+// group's eligible pages (NaN never selected) and the lowest page with it, as one 64-bit key per (row, group):
+// the score's order-preserving bits above ~page, so the largest key is (highest score, lowest page) and atomicMax gives
+// the same answer in any order. -0 counts as +0 (they are equal scores: the lower page wins). Each thread takes a run of
+// GK_RUN consecutive pages of one row and issues one atomic per group run, so any group size - one group of every page
+// included - spreads over the whole grid.
+constexpr int GK_RUN = 8;
+
+__device__ __forceinline__ unsigned long long page_key(float v, int p) {
+    uint32_t b = __float_as_uint(v);
+    if (b == 0x80000000u) b = 0u;
+    const uint32_t o = (b & 0x80000000u) ? ~b : (b | 0x80000000u);  // > 0 for every non-NaN score: key 0 = no page
+    return (static_cast<unsigned long long>(o) << 32) | static_cast<uint32_t>(~p);
+}
+
+__global__ void __launch_bounds__(256)
+group_key_kernel(const float* __restrict__ scores, int rows, long long nd, int G, const int* __restrict__ doc_groups,
+                 const uint32_t* __restrict__ mask, unsigned long long* __restrict__ keys) {
+    const long long runs = (nd + GK_RUN - 1) / GK_RUN, n = static_cast<long long>(rows) * runs;
+    for (long long i = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x; i < n;
+         i += static_cast<long long>(gridDim.x) * blockDim.x) {
+        const long long row = i / runs, p0 = (i - row * runs) * GK_RUN;
+        const float* srow = scores + row * nd;
+        unsigned long long* krow = keys + row * G;
+        int cur = -1;
+        unsigned long long best = 0;
+#pragma unroll
+        for (int j = 0; j < GK_RUN; ++j) {
+            const long long p = p0 + j;
+            if (p >= nd || (mask && !col_eligible(mask, p))) continue;
+            const float v = srow[p];
+            if (isnan(v)) continue;
+            const int g = __ldg(doc_groups + p);
+            if (g != cur) {
+                if (best) atomicMax(krow + cur, best);
+                cur = g;
+                best = 0;
+            }
+            const unsigned long long key = page_key(v, static_cast<int>(p));
+            best = key > best ? key : best;
+        }
+        if (best) atomicMax(krow + cur, best);
+    }
+}
+
+// keys [rows, G] -> best pages (in place; -1: no eligible page) and their scores, read back from the score rows so they
+// keep their bits (a -0 stays -0)
+__global__ void __launch_bounds__(256)
+group_decode_kernel(const float* __restrict__ scores, int rows, long long nd, int G, long long* __restrict__ pages,
+                    float* __restrict__ gscores) {
+    const long long n = static_cast<long long>(rows) * G;
+    for (long long i = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x; i < n;
+         i += static_cast<long long>(gridDim.x) * blockDim.x) {
+        const unsigned long long key = static_cast<unsigned long long>(pages[i]);
+        const int p = key ? static_cast<int>(~static_cast<uint32_t>(key)) : -1;
+        gscores[i] = p >= 0 ? scores[(i / G) * nd + p] : -INFINITY;
+        pages[i] = p;
+    }
+}
+
+// The group of each emitted page (page ids carry id_offset; -1 stays -1).
+__global__ void page_groups_kernel(const long long* __restrict__ pages, long long n, long long id_offset,
+                                   const int* __restrict__ doc_groups, long long* __restrict__ groups) {
+    for (long long i = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x; i < n;
+         i += static_cast<long long>(gridDim.x) * blockDim.x)
+        groups[i] = pages[i] >= 0 ? __ldg(doc_groups + (pages[i] - id_offset)) : -1;
+}
+
+// Merge of per-rank partial group lists [rows, cols] (score, page, group; page < 0 = empty): the first k distinct groups
+// in (score desc, page asc) order, one warp per row, the row in registers. Each round takes the best live entry and then
+// retires every entry of its group: the first entry of a group in that order is its best.
+template <int NPL>
+__global__ void __launch_bounds__(256)
+merge_groups_warp_kernel(const float* __restrict__ scores, const long long* __restrict__ pages,
+                         const long long* __restrict__ groups, int rows, int cols, int k, float* __restrict__ out_scores,
+                         long long* __restrict__ out_pages, long long* __restrict__ out_groups) {
+    const int lane = threadIdx.x & 31;
+    const int row = blockIdx.x * 8 + (threadIdx.x >> 5);
+    if (row >= rows) return;
+    const long long base = static_cast<long long>(row) * cols;
+    float s[NPL];
+    long long id[NPL], gr[NPL];
+#pragma unroll
+    for (int j = 0; j < NPL; ++j) {
+        const int c = lane + j * 32;
+        id[j] = c < cols ? pages[base + c] : -1;
+        gr[j] = id[j] >= 0 ? groups[base + c] : -1;
+        s[j] = id[j] >= 0 ? scores[base + c] : -INFINITY;
+    }
+    for (int round = 0; round < k; ++round) {
+        float bs = -INFINITY;
+        long long bi = 0x7fffffffffffffffll, bg = -1;
+#pragma unroll
+        for (int j = 0; j < NPL; ++j)
+            if (id[j] >= 0 && before(s[j], id[j], bs, bi)) { bs = s[j]; bi = id[j]; bg = gr[j]; }
+#pragma unroll
+        for (int o = 16; o > 0; o >>= 1) {
+            const float os = __shfl_xor_sync(0xffffffffu, bs, o);
+            const long long oi = __shfl_xor_sync(0xffffffffu, bi, o);
+            const long long og = __shfl_xor_sync(0xffffffffu, bg, o);
+            if (before(os, oi, bs, bi)) { bs = os; bi = oi; bg = og; }
+        }
+        const bool valid = bi != 0x7fffffffffffffffll;
+        const long long o = static_cast<long long>(row) * k;
+        if (lane == 0) {
+            out_scores[o + round] = valid ? bs : -INFINITY;
+            out_pages[o + round] = valid ? bi : -1;
+            out_groups[o + round] = valid ? bg : -1;
+        }
+        if (!valid) {
+            for (int r2 = round + 1 + lane; r2 < k; r2 += 32) {
+                out_scores[o + r2] = -INFINITY;
+                out_pages[o + r2] = -1;
+                out_groups[o + r2] = -1;
+            }
+            break;
+        }
+#pragma unroll
+        for (int j = 0; j < NPL; ++j)
+            if (gr[j] == bg) id[j] = -1;
+    }
 }
 
 // fp32 -> fp16 rows, with the row L2 norms and their maximum (norms are >= 0, so the int view orders them).
@@ -954,4 +1370,159 @@ extern "C" int vr_topk_rows_chunked_masked(const float* scores, int32_t rows, in
     return topk_rows_chunked<true>(scores, rows, cols, k, id_offset, chunks, ws_scores, reinterpret_cast<long long*>(ws_ids),
                                    out_scores, reinterpret_cast<long long*>(out_ids), doc_mask,
                                    reinterpret_cast<cudaStream_t>(stream));
+}
+
+// ---------------------------------------------------------------------------------------------- document-level top-k
+// A group table as the _groups entry points take it: 4-byte aligned int32 arrays, G >= 1, nd within the int32 ids.
+static bool i32_ok(const void* p) { return p && (reinterpret_cast<uintptr_t>(p) & 3) == 0; }
+
+template <typename Args>
+static int score_filter_groups(const void* q_f16, int nq, const void* d_f16, long long nd, int dim, const int* doc_groups,
+                               const uint32_t* doc_mask, float* cand_scores, int* cand_ids, cudaStream_t st) {
+    using Cfg = Score2Cfg;
+    CUtensorMap tq, td;
+    if (int rc = make_tmap_2d(&tq, q_f16, nq, dim, dim, GEMM_BM, GEMM_BK, 128, false)) return rc;
+    if (int rc = make_tmap_2d(&td, d_f16, nd, dim, dim, 128, GEMM_BK, 128, false)) return rc;
+    const ScorePlan plan = score_plan(nq, nd);
+    static unsigned long long attr_set = 0;
+    if (first_use_on_device(&attr_set))
+        VR_CHECK_CUDA(cudaFuncSetAttribute(score_filter_kernel<Args>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES));
+    Args g;
+    g.nq = nq; g.nd = nd; g.dim = dim; g.lists = plan.lists; g.T = plan.T; g.R = plan.R; g.QB = plan.QB; g.items = plan.items;
+    g.cand_scores = cand_scores; g.cand_ids = cand_ids; g.doc_groups = doc_groups;
+    if constexpr (std::is_same<Args, MaskedGroupedScoreArgs>::value) g.doc_mask = doc_mask;
+    {
+        const long long n = static_cast<long long>(nq) * (plan.lists - plan.R) * SC_KT;
+        long long blocks = (n + 255) / 256;
+        if (blocks > num_sms() * 8) blocks = num_sms() * 8;
+        score_init_lists_kernel<<<static_cast<int>(blocks), 256, 0, st>>>(cand_scores, cand_ids, nq, plan.lists, plan.R);
+        VR_CHECK_CUDA(cudaGetLastError());
+    }
+    score_filter_kernel<Args><<<2 * plan.pairs, GEMM_THREADS, Cfg::SMEM_BYTES, st>>>(tq, td, g);
+    VR_CHECK_CUDA(cudaGetLastError());
+    return 0;
+}
+
+extern "C" int vr_score_filter_groups(const void* q_f16, int32_t nq, const void* d_f16, int64_t nd, int32_t dim,
+                                      int32_t ranges, float* cand_scores, int32_t* cand_ids, const int32_t* doc_groups,
+                                      const uint32_t* doc_mask, void* stream) {
+    VR_REQUIRE(i32_ok(doc_groups), "vr_score_filter_groups: doc_groups must be a non-null, 4-byte aligned pointer");
+    VR_REQUIRE(!doc_mask || mask_ok(doc_mask), "vr_score_filter_groups: doc_mask must be NULL or 4-byte aligned");
+    VR_REQUIRE(q_f16 && d_f16 && cand_scores && cand_ids, "vr_score_filter_groups: null pointer");
+    VR_REQUIRE(nd > 0 && nd < 2147483647ll, "vr_score_filter_groups: nd=%lld beyond the int32 doc ids", (long long)nd);
+    VR_REQUIRE(nq > 0 && nq < (1 << 30) && dim % 8 == 0, "vr_score_filter_groups: bad shape");
+    VR_REQUIRE(ranges * 2 == score_plan(nq, nd).lists, "vr_score_filter_groups: ranges must come from vr_score_ranges()");
+    cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+    if (doc_mask)
+        return score_filter_groups<MaskedGroupedScoreArgs>(q_f16, nq, d_f16, nd, dim, doc_groups, doc_mask, cand_scores,
+                                                           cand_ids, st);
+    return score_filter_groups<GroupedScoreArgs>(q_f16, nq, d_f16, nd, dim, doc_groups, nullptr, cand_scores, cand_ids, st);
+}
+
+extern "C" int vr_score_rescore_groups(const float* q_f32, int32_t nq, const float* d_f32, int64_t nd, int32_t dim,
+                                       int32_t ranges, const float* cand_scores, const int32_t* cand_ids,
+                                       const int32_t* doc_groups, const int32_t* group_offsets, const int32_t* group_pages,
+                                       int32_t G, const uint32_t* doc_mask, const float* max_doc_norm, int32_t k,
+                                       int64_t id_offset, float* out_scores, int64_t* out_pages, int64_t* out_groups,
+                                       int32_t* flags, void* stream) {
+    VR_REQUIRE(i32_ok(doc_groups) && i32_ok(group_offsets) && i32_ok(group_pages),
+               "vr_score_rescore_groups: doc_groups, group_offsets and group_pages must be non-null, 4-byte aligned pointers");
+    VR_REQUIRE(!doc_mask || mask_ok(doc_mask), "vr_score_rescore_groups: doc_mask must be NULL or 4-byte aligned");
+    VR_REQUIRE(G > 0, "vr_score_rescore_groups: G=%d, needs at least one group", G);
+    VR_REQUIRE(nd > 0 && nd < 2147483647ll, "vr_score_rescore_groups: nd=%lld beyond the int32 doc ids", (long long)nd);
+    VR_REQUIRE(q_f32 && d_f32 && cand_scores && cand_ids && max_doc_norm && out_scores && out_pages && out_groups && flags,
+               "vr_score_rescore_groups: null pointer");
+    VR_REQUIRE(nq > 0 && k > 0 && dim % 4 == 0, "vr_score_rescore_groups: bad shape");
+    const int lists = ranges * 2;
+    VR_REQUIRE(ranges > 0 && lists <= SC_MAX_RANGES + 2, "vr_score_rescore_groups: ranges must come from vr_score_ranges()");
+    int keep = 2 * k > 32 ? 2 * k : 32;  // as vr_score_rescore
+    if (keep > lists * SC_KT) keep = lists * SC_KT;
+    if (keep > RS_MAX_KEEP) keep = RS_MAX_KEEP;
+    const size_t smem = (static_cast<size_t>(dim) + 2 * RG_PAGE_BUDGET + 7 * static_cast<size_t>(keep) + 1) * sizeof(float);
+    VR_REQUIRE(smem <= 200 * 1024, "vr_score_rescore_groups: dim too large for shared memory (%zu bytes)", smem);
+    static unsigned long long attr_set = 0;
+    if (smem > 48 * 1024 && first_use_on_device(&attr_set))
+        VR_CHECK_CUDA(cudaFuncSetAttribute(rescore_groups_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
+    rescore_groups_kernel<<<nq, RS_THREADS, smem, reinterpret_cast<cudaStream_t>(stream)>>>(
+        q_f32, d_f32, dim, lists, keep, cand_scores, cand_ids, doc_groups, group_offsets, group_pages, doc_mask, max_doc_norm,
+        k, id_offset, out_scores, reinterpret_cast<long long*>(out_pages), reinterpret_cast<long long*>(out_groups), flags);
+    VR_CHECK_CUDA(cudaGetLastError());
+    return 0;
+}
+
+// workspace of vr_group_topk_rows: best pages [rows, G] i64, group scores [rows, G] f32, and with chunks >= 2 the first
+// pass's lists [rows, chunks, k] (i64 ids, f32 scores)
+static long long group_topk_ws(int rows, int G, int k, int chunks) {
+    const long long n = static_cast<long long>(rows) * G, w = chunks >= 2 ? static_cast<long long>(rows) * chunks * k : 0;
+    return ((n * 12 + 15) / 16) * 16 + w * 12;
+}
+
+extern "C" int64_t vr_group_topk_ws_bytes(int32_t rows, int32_t G, int32_t k, int32_t chunks) {
+    return rows > 0 && G > 0 && k > 0 ? group_topk_ws(rows, G, k, chunks) : -1;
+}
+
+extern "C" int vr_group_topk_rows(const float* scores, int32_t rows, int64_t nd, const int32_t* doc_groups, int32_t G,
+                                  const uint32_t* doc_mask, int32_t k, int64_t id_offset, int32_t chunks, void* ws,
+                                  int64_t ws_bytes, float* out_scores, int64_t* out_pages, int64_t* out_groups,
+                                  void* stream) {
+    VR_REQUIRE(i32_ok(doc_groups), "vr_group_topk_rows: doc_groups must be a non-null, 4-byte aligned pointer");
+    VR_REQUIRE(!doc_mask || mask_ok(doc_mask), "vr_group_topk_rows: doc_mask must be NULL or 4-byte aligned");
+    VR_REQUIRE(G > 0, "vr_group_topk_rows: G=%d, needs at least one group", G);
+    VR_REQUIRE(nd > 0 && nd < 2147483647ll, "vr_group_topk_rows: nd=%lld beyond the int32 doc ids", (long long)nd);
+    VR_REQUIRE(scores && out_scores && out_pages && out_groups, "vr_group_topk_rows: null pointer");
+    VR_REQUIRE(rows > 0 && k > 0 && chunks >= 0 && chunks <= 65535, "vr_group_topk_rows: bad shape");
+    VR_REQUIRE(ws && (reinterpret_cast<uintptr_t>(ws) & 15) == 0 && ws_bytes >= group_topk_ws(rows, G, k, chunks),
+               "vr_group_topk_rows: workspace too small or misaligned (%lld bytes, need %lld, 16-byte aligned)",
+               (long long)ws_bytes, group_topk_ws(rows, G, k, chunks));
+    cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+    const long long n = static_cast<long long>(rows) * G;
+    long long* gpages = reinterpret_cast<long long*>(ws);
+    float* gscores = reinterpret_cast<float*>(gpages + n);
+    VR_CHECK_CUDA(cudaMemsetAsync(gpages, 0, n * sizeof(long long), st));  // keys: 0 = no page yet
+    const long long runs = static_cast<long long>(rows) * ((nd + GK_RUN - 1) / GK_RUN);
+    long long blocks = (runs + 255) / 256;
+    if (blocks > num_sms() * 16) blocks = num_sms() * 16;
+    group_key_kernel<<<static_cast<int>(blocks), 256, 0, st>>>(scores, rows, nd, G, doc_groups, doc_mask,
+                                                               reinterpret_cast<unsigned long long*>(gpages));
+    VR_CHECK_CUDA(cudaGetLastError());
+    blocks = (n + 255) / 256;
+    if (blocks > num_sms() * 16) blocks = num_sms() * 16;
+    group_decode_kernel<<<static_cast<int>(blocks), 256, 0, st>>>(scores, rows, nd, G, gpages, gscores);
+    VR_CHECK_CUDA(cudaGetLastError());
+    long long* op = reinterpret_cast<long long*>(out_pages);
+    if (chunks >= 2) {  // few rows x many groups: spread each row over `chunks` blocks, then merge their lists
+        long long* ws_i = reinterpret_cast<long long*>(reinterpret_cast<char*>(ws) + ((n * 12 + 15) / 16) * 16);
+        float* ws_s = reinterpret_cast<float*>(ws_i + static_cast<long long>(rows) * chunks * k);
+        topk_rows_kernel<false><<<dim3(rows, chunks), 256, 0, st>>>(gscores, gpages, G, k, id_offset, (G + chunks - 1) / chunks,
+                                                                    ws_s, ws_i, nullptr);
+        VR_CHECK_CUDA(cudaGetLastError());
+        launch_topk_rows<false>(ws_s, ws_i, rows, static_cast<long long>(chunks) * k, k, 0, out_scores, op, nullptr, st);
+    } else {
+        launch_topk_rows<false>(gscores, gpages, rows, G, k, id_offset, out_scores, op, nullptr, st);
+    }
+    VR_CHECK_CUDA(cudaGetLastError());
+    const long long m = static_cast<long long>(rows) * k;
+    page_groups_kernel<<<static_cast<int>((m + 255) / 256 < 4096 ? (m + 255) / 256 : 4096), 256, 0, st>>>(
+        op, m, id_offset, doc_groups, reinterpret_cast<long long*>(out_groups));
+    VR_CHECK_CUDA(cudaGetLastError());
+    return 0;
+}
+
+extern "C" int vr_merge_group_topk(const float* scores, const int64_t* pages, const int64_t* groups, int32_t rows,
+                                   int32_t cols, int32_t k, float* out_scores, int64_t* out_pages, int64_t* out_groups,
+                                   void* stream) {
+    VR_REQUIRE(scores && pages && groups && out_scores && out_pages && out_groups, "vr_merge_group_topk: null pointer");
+    VR_REQUIRE(rows > 0 && cols > 0 && cols <= 512 && k > 0, "vr_merge_group_topk: bad shape (rows=%d, cols=%d <= 512, k=%d)",
+               rows, cols, k);
+    cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+    const long long* p = reinterpret_cast<const long long*>(pages);
+    const long long* g = reinterpret_cast<const long long*>(groups);
+    long long* op = reinterpret_cast<long long*>(out_pages);
+    long long* og = reinterpret_cast<long long*>(out_groups);
+    if (cols <= 128)
+        merge_groups_warp_kernel<4><<<(rows + 7) / 8, 256, 0, st>>>(scores, p, g, rows, cols, k, out_scores, op, og);
+    else
+        merge_groups_warp_kernel<16><<<(rows + 7) / 8, 256, 0, st>>>(scores, p, g, rows, cols, k, out_scores, op, og);
+    VR_CHECK_CUDA(cudaGetLastError());
+    return 0;
 }

@@ -12,10 +12,15 @@ Scores are the same fp32 dot products; ties are ordered by lower page index (tor
 Beyond the reference: a search can be restricted to some pages (`within`, e.g. the pages of one PDF), pages can be
 removed (a tombstone bit, so the other pages keep their indices) and added, and `save` writes the live pages back in the
 demo's layout. All of it runs as a doc mask inside the same kernels, with the same exact fp32 results.
+
+Documents: `build_index.py` stores page i of `report.pdf` as `report.pdf_i.png`, so a page's document is its filename up to
+the last `_` when the rest is `<digits>.png` (any other filename is its own document). `search_documents` returns the
+top-k documents by their best page (`retriever.score_topk_groups`), so one long document cannot fill every slot.
 """
 from __future__ import annotations
 
 import os
+import re
 from typing import Iterable, List, Optional, Sequence, Tuple
 
 import numpy as np
@@ -28,6 +33,16 @@ REPS_FILE = "reps.npy"
 NAMES_FILE = "index2img_filename.txt"
 # the demo's instruction (`answer.py:33`; singular "document", unlike the eval scripts' "documents")
 DEMO_QUERY_PREFIX = "Represent this query for retrieving relevant document: "
+
+
+_PAGE_SUFFIX = re.compile(r"_[0-9]+\.png")
+
+
+def document_of(filename: str) -> str:
+    """The document a page belongs to: `report.pdf_12.png` -> `report.pdf` (`build_index.py`'s naming); any other
+    filename is its own document."""
+    cut = filename.rfind("_")
+    return filename[:cut] if cut >= 0 and _PAGE_SUFFIX.fullmatch(filename[cut:]) else filename
 
 
 def save_knowledge_base(path: str, reps, filenames: Sequence[str]) -> None:
@@ -58,6 +73,22 @@ class KnowledgeBase:
         self._row = {name: i for i, name in enumerate(self.filenames)}   # filename -> row, live pages only
         self._live = torch.ones(len(self.filenames), dtype=torch.bool, device=self.index.emb.device)
         self._n_live = len(self.filenames)
+        self.documents: List[str] = []                # document id -> name; ids are dense and never reused
+        self._doc_id = {}
+        self._doc_groups = torch.empty(0, dtype=torch.int32, device=self.index.emb.device)
+        self._add_documents(self.filenames)
+
+    def _add_documents(self, filenames: Sequence[str]) -> None:
+        """Give every new page its document id: a page of a known document name joins it, a new name takes the next id."""
+        ids = []
+        for f in filenames:
+            doc = document_of(f)
+            if doc not in self._doc_id:
+                self._doc_id[doc] = len(self.documents)
+                self.documents.append(doc)
+            ids.append(self._doc_id[doc])
+        new = torch.tensor(ids, dtype=torch.int32).to(self._doc_groups.device)
+        self._doc_groups = torch.cat([self._doc_groups, new])
 
     def __len__(self) -> int:
         return self._n_live
@@ -87,6 +118,37 @@ class KnowledgeBase:
             return (torch.empty((q.shape[0], 0), dtype=torch.float32, device=q.device),
                     torch.empty((q.shape[0], 0), dtype=torch.int64, device=q.device))
         return retriever.score_topk(q, self.index, k, doc_mask=mask)  # enters the index's device itself
+
+    def search_documents(self, query_reps, topk: int, within: Optional[Iterable[str]] = None
+                         ) -> Tuple[torch.Tensor, torch.Tensor, List[List[str]]]:
+        """The top-k DOCUMENTS, each scored by its best page: (scores [nq,k] f32, best page indices [nq,k] i64 on the
+        device, document names [nq][k]). within: page filenames to search (default: every live page); k = min(topk,
+        documents searched). Ties rank the document with the lower best page index first."""
+        q = query_reps if isinstance(query_reps, torch.Tensor) else torch.from_numpy(np.asarray(query_reps, dtype=np.float32))
+        q = q.to(self.index.emb.device, torch.float32).reshape(-1, self.index.emb.shape[1]).contiguous()
+        if within is None:
+            mask = None if len(self) == self.index.nd else self._live   # None: the unmasked kernels
+        else:
+            mask = torch.zeros(self.index.nd, dtype=torch.bool, device=q.device)
+            mask[torch.tensor(self._rows(within), dtype=torch.int64, device=q.device)] = True
+        searched = self._doc_groups if mask is None else self._doc_groups[mask]
+        k = min(topk, int(torch.unique(searched).numel()))             # documents searched, counted on the device
+        if k == 0:
+            return (torch.empty((q.shape[0], 0), dtype=torch.float32, device=q.device),
+                    torch.empty((q.shape[0], 0), dtype=torch.int64, device=q.device), [[] for _ in range(q.shape[0])])
+        s, p, g = retriever.score_topk_groups(q, self.index, k, self._doc_groups, doc_mask=mask)
+        return s, p, [[self.documents[j] for j in row] for row in g.tolist()]
+
+    def retrieve_documents(self, query_rep, topk: int, within: Optional[Iterable[str]] = None) -> List[Tuple[str, str]]:
+        """[(document name, path of its best page image)] of the top-k documents, best first."""
+        _, pages, names = self.search_documents(query_rep, topk, within)
+        return [(n, os.path.join(self.path, self.filenames[i])) for n, i in zip(names[0], pages[0].tolist())]
+
+    def retrieve_documents_text(self, model, tokenizer, query: str, topk: int,
+                                within: Optional[Iterable[str]] = None) -> List[Tuple[str, str]]:
+        """retrieve_text at the document level: instruction + query -> embedding -> top-k documents."""
+        out = model(query={"text": [DEMO_QUERY_PREFIX + query], "image": [None]}, tokenizer=tokenizer)
+        return self.retrieve_documents(out.q_reps, topk, within)
 
     def retrieve(self, query_rep, topk: int, within: Optional[Iterable[str]] = None) -> List[str]:
         """`answer.py: retrieve` after the query is encoded: paths of the top-k page images, best first."""
@@ -133,6 +195,7 @@ class KnowledgeBase:
         self.index.emb = torch.cat([self.index.emb, x])
         self.index.emb_f16 = torch.cat([self.index.emb_f16, f16])
         self._live = torch.cat([self._live, torch.ones(n, dtype=torch.bool, device=dev)])
+        self._add_documents(filenames)
         self.filenames.extend(filenames)
         self._row.update((f, n0 + i) for i, f in enumerate(filenames))
         self._n_live += n

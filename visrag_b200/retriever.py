@@ -12,12 +12,16 @@ For a corpus that lives in HBM (index build + many query batches) use `CorpusInd
 multi-GPU form (`sharded_topk`) shards the corpus by page across ranks, takes the local top-k with global ids and
 merges after ONE all-gather of [nq, k] (score, id) pairs. Both take an optional `doc_mask` (bool [nd], local to the
 shard): only the docs it marks are searched, and the result equals the fp32 scan over those docs alone.
+
+Document-level retrieval (`score_topk_groups`, `sharded_topk_groups`): `doc_groups` (int [nd]) gives every doc (page) its
+group (document); the top-k groups by their best page's exact fp32 score, ranked by (score desc, best page asc).
 """
 from __future__ import annotations
 
 import glob
 import os
 import pickle
+import weakref
 from dataclasses import dataclass
 from typing import Dict, List, Optional, Tuple
 
@@ -211,6 +215,160 @@ def _score_topk(q: torch.Tensor, index: CorpusIndex, k: int, id_offset: int, for
     return out_s, out_i
 
 
+# ------------------------------------------------------------------------------------------------------
+# Document-level top-k: groups of pages, each scored by its best page
+# ------------------------------------------------------------------------------------------------------
+@dataclass
+class _GroupTable:
+    groups: torch.Tensor    # [nd] int32: the group of each page
+    offsets: torch.Tensor   # [G+1] int32: group g owns pages[offsets[g]:offsets[g+1]]
+    pages: torch.Tensor     # [nd] int32: pages by group, ascending within a group
+    G: int
+
+
+MERGE_GROUPS_MAX = 512  # entries per row vr_merge_group_topk takes: world * k of sharded_topk_groups
+_GROUP_TABLES: Dict[int, Tuple["weakref.ref", int, _GroupTable]] = {}
+
+
+def _group_table(doc_groups: torch.Tensor, index: CorpusIndex) -> _GroupTable:
+    """Validate doc_groups and build its CSR on the device (a stable sort keeps pages ascending within a group). Cached per
+    tensor object until it is freed or modified in place: keep one tensor for repeated searches (a new slice or view per
+    call is a new object and builds the CSR again). The table holds its own copy of the groups, never the key itself,
+    so the entry goes when the caller's tensor does."""
+    if not isinstance(doc_groups, torch.Tensor) or doc_groups.dtype not in (torch.int32, torch.int64):
+        raise ValueError("doc_groups must be an int32 or int64 torch tensor")
+    if doc_groups.dim() != 1 or doc_groups.shape[0] != index.nd:
+        raise ValueError(f"doc_groups must have shape [{index.nd}] (one group per doc of the index), got {list(doc_groups.shape)}")
+    if doc_groups.device != index.emb.device:
+        raise ValueError(f"doc_groups lives on {doc_groups.device}, the index on {index.emb.device}")
+    hit = _GROUP_TABLES.get(id(doc_groups))
+    if hit is not None and hit[0]() is doc_groups and hit[1] == doc_groups._version:
+        return hit[2]
+    lo, hi = (int(v) for v in torch.aminmax(doc_groups))
+    if lo < 0 or hi >= 1 << 31:
+        raise ValueError(f"doc_groups must lie in [0, 2^31), got [{lo}, {hi}]")
+    G = hi + 1
+    order = torch.sort(doc_groups, stable=True).indices
+    counts = torch.bincount(doc_groups, minlength=G)
+    offsets = torch.zeros(G + 1, dtype=torch.int64, device=doc_groups.device)
+    offsets[1:] = torch.cumsum(counts, 0)
+    table = _GroupTable(doc_groups.to(torch.int32, copy=True).contiguous(), offsets.to(torch.int32), order.to(torch.int32), G)
+    key = id(doc_groups)
+    _GROUP_TABLES[key] = (weakref.ref(doc_groups, lambda _r, key=key: _GROUP_TABLES.pop(key, None)), doc_groups._version, table)
+    return table
+
+
+def _exact_topk_groups(q: torch.Tensor, index: CorpusIndex, k: int, id_offset: int, gt: _GroupTable,
+                       mask_words: Optional[torch.Tensor] = None):
+    nq, d = q.shape
+    nd = index.nd
+    out_s = torch.empty((nq, k), dtype=torch.float32, device=q.device)
+    out_p = torch.empty((nq, k), dtype=torch.int64, device=q.device)
+    out_g = torch.empty((nq, k), dtype=torch.int64, device=q.device)
+    # <= 512 MiB of fp32 scores + 1.5 GiB of per-group workspace (G may exceed nd: global group ids on one shard)
+    rows_per = max(1, min(nq, (1 << 27) // max(nd, gt.G, 1)))
+    scratch = torch.empty((rows_per, nd), dtype=torch.float32, device=q.device)
+    lib = L.lib()
+    mw = None if mask_words is None else mask_words.data_ptr()
+    for r0 in range(0, nq, rows_per):
+        n = min(rows_per, nq - r0)
+        L.check(lib.vr_score_exact(q[r0:].data_ptr(), n, index.emb.data_ptr(), nd, d, scratch.data_ptr(), L.stream_ptr()))
+        chunks = min(1024, gt.G // 4096) if n <= 64 else 0  # few queries over many groups: spread each row over many SMs
+        ws_bytes = lib.vr_group_topk_ws_bytes(n, gt.G, k, chunks)
+        ws = torch.empty((ws_bytes + 15) // 16 * 2, dtype=torch.float64, device=q.device)  # 16-byte aligned
+        L.check(lib.vr_group_topk_rows(scratch.data_ptr(), n, nd, gt.groups.data_ptr(), gt.G, mw, k, id_offset, chunks, ws.data_ptr(), ws_bytes,
+                                       out_s[r0:].data_ptr(), out_p[r0:].data_ptr(), out_g[r0:].data_ptr(), L.stream_ptr()))
+    return out_s, out_p, out_g
+
+
+def score_topk_groups(queries: torch.Tensor, index: CorpusIndex, k: int, doc_groups: torch.Tensor, id_offset: int = 0,
+                      force_exact: bool = False, stats: Optional[dict] = None, doc_mask: Optional[torch.Tensor] = None
+                      ) -> Tuple[torch.Tensor, torch.Tensor, torch.Tensor]:
+    """Exact top-k GROUPS (documents) of pages: doc_groups (int32/int64 [nd] on the index's device) gives each page its
+    group in [0, G). A group's score is the maximum exact fp32 page score over its eligible pages, its best page the lowest
+    page with that maximum; groups rank by (score desc, best page asc). Returns (scores [nq,k] f32, best pages [nq,k] i64
+    = local index + id_offset, groups [nq,k] i64); fewer than k groups with an eligible page leave (-inf, -1, -1).
+    With doc_groups = arange(nd) the result equals score_topk's, with groups == pages. doc_mask as in score_topk."""
+    q = _check_f32(queries, "queries")
+    if q.device != index.emb.device:
+        raise ValueError(f"queries live on {q.device}, the index on {index.emb.device}")
+    mask_words = None if doc_mask is None else _check_doc_mask(doc_mask, index)
+    with L.on_device(q.device):
+        gt = _group_table(doc_groups, index)
+        return _score_topk_groups(q, index, k, id_offset, force_exact, stats, gt, mask_words)
+
+
+def _score_topk_groups(q, index, k, id_offset, force_exact, stats, gt: _GroupTable, mask_words, page_lists: bool = False):
+    """page_lists: feed the page filter's lists to the grouped rescoring (tests and measurements of the proof)."""
+    nq, d = q.shape
+    nd = index.nd
+    if nq == 0:
+        e = torch.empty((0, k), dtype=torch.int64, device=q.device)
+        return torch.empty((0, k), dtype=torch.float32, device=q.device), e, e.clone()
+    if d != index.emb.shape[1]:
+        raise ValueError("query / corpus dim mismatch")
+    if force_exact or nq * nd <= SMALL_PROBLEM or nd < 256:
+        if stats is not None:
+            stats.update(path="exact", flagged=0)
+        return _exact_topk_groups(q, index, k, id_offset, gt, mask_words)
+    lib = L.lib()
+    ranges = lib.vr_score_ranges(nq, nd)
+    lists = ranges * 2 * lib.vr_score_list_len()
+    q16 = to_f16_rows(q)
+    cand_s = torch.empty((nq, lists), dtype=torch.float32, device=q.device)
+    cand_i = torch.empty((nq, lists), dtype=torch.int32, device=q.device)
+    out_s = torch.empty((nq, k), dtype=torch.float32, device=q.device)
+    out_p = torch.empty((nq, k), dtype=torch.int64, device=q.device)
+    out_g = torch.empty((nq, k), dtype=torch.int64, device=q.device)
+    flags = torch.empty((nq,), dtype=torch.int32, device=q.device)
+    sp = L.stream_ptr()
+    mw = None if mask_words is None else mask_words.data_ptr()
+    ev = _Stages(stats)
+    ev.mark("q_to_f16")
+    if page_lists and mw is None:
+        L.check(lib.vr_score_filter(q16.data_ptr(), nq, index.emb_f16.data_ptr(), nd, d, ranges, cand_s.data_ptr(),
+                                    cand_i.data_ptr(), sp))
+    elif page_lists:
+        L.check(lib.vr_score_filter_masked(q16.data_ptr(), nq, index.emb_f16.data_ptr(), nd, d, ranges, cand_s.data_ptr(),
+                                           cand_i.data_ptr(), mw, sp))
+    else:
+        L.check(lib.vr_score_filter_groups(q16.data_ptr(), nq, index.emb_f16.data_ptr(), nd, d, ranges, cand_s.data_ptr(),
+                                           cand_i.data_ptr(), gt.groups.data_ptr(), mw, sp))
+    ev.mark("filter")
+    L.check(lib.vr_score_rescore_groups(q.data_ptr(), nq, index.emb.data_ptr(), nd, d, ranges, cand_s.data_ptr(),
+                                        cand_i.data_ptr(), gt.groups.data_ptr(), gt.offsets.data_ptr(), gt.pages.data_ptr(),
+                                        gt.G, mw, index.max_norm.data_ptr(), k, id_offset, out_s.data_ptr(),
+                                        out_p.data_ptr(), out_g.data_ptr(), flags.data_ptr(), sp))
+    ev.mark("rescore")
+    bad = torch.nonzero(flags).flatten()  # host sync: the caller reads the result next anyway
+    if stats is not None:
+        stats.update(path="filter+rescore", flagged=int(bad.numel()), ranges=ranges)
+    if bad.numel() > 0:
+        s2, p2, g2 = _exact_topk_groups(q.index_select(0, bad), index, k, id_offset, gt, mask_words)
+        out_s.index_copy_(0, bad, s2)
+        out_p.index_copy_(0, bad, p2)
+        out_g.index_copy_(0, bad, g2)
+    return out_s, out_p, out_g
+
+
+def merge_topk_groups(scores: torch.Tensor, pages: torch.Tensor, groups: torch.Tensor, k: int):
+    """[nq, m] partial group lists (score, page, group; page < 0 = empty) -> the first k distinct groups in
+    (score desc, page asc) order. m <= MERGE_GROUPS_MAX (the merge keeps a row in one warp's registers)."""
+    if scores.shape[1] > MERGE_GROUPS_MAX:
+        raise ValueError(f"merge_topk_groups merges at most {MERGE_GROUPS_MAX} entries per row (world * k), got {scores.shape[1]}")
+    scores = scores.contiguous().float()
+    pages = pages.contiguous().to(torch.int64)
+    groups = groups.contiguous().to(torch.int64)
+    nq, m = scores.shape
+    out_s = torch.empty((nq, k), dtype=torch.float32, device=scores.device)
+    out_p = torch.empty((nq, k), dtype=torch.int64, device=scores.device)
+    out_g = torch.empty((nq, k), dtype=torch.int64, device=scores.device)
+    with L.on_device(scores.device):
+        L.check(L.lib().vr_merge_group_topk(scores.data_ptr(), pages.data_ptr(), groups.data_ptr(), nq, m, k, out_s.data_ptr(),
+                                            out_p.data_ptr(), out_g.data_ptr(), L.stream_ptr()))
+    return out_s, out_p, out_g
+
+
 def merge_topk(scores: torch.Tensor, ids: torch.Tensor, k: int) -> Tuple[torch.Tensor, torch.Tensor]:
     """[nq, m] candidate (score, id) pairs (id < 0 = empty) -> top-k by (score desc, id asc)."""
     scores = scores.contiguous().float()
@@ -262,6 +420,35 @@ def sharded_topk(queries: torch.Tensor, index: CorpusIndex, k: int, id_offset: i
     gs, gi = gather_partials(s, i, group)
     ev.mark("all_gather_partials")
     out = merge_topk(gs, gi, k)
+    ev.mark("merge")
+    return out
+
+
+def sharded_topk_groups(queries: torch.Tensor, index: CorpusIndex, k: int, doc_groups: torch.Tensor, id_offset: int,
+                        group=None, stats: Optional[dict] = None, doc_mask: Optional[torch.Tensor] = None):
+    """Document-level sharded_topk: doc_groups holds this shard's pages' GLOBAL group ids (a document may span ranks).
+    Local group top-k with global page ids, one all-gather of [nq, k, 3] int64 (score bits, page, group), then the merge
+    keeps the first k distinct groups. A group's best page lies on one rank, and that rank's local top-k holds it whenever
+    the group is in the global top-k, so the result equals score_topk_groups over the whole corpus.
+    world * k must be <= MERGE_GROUPS_MAX (512), checked before any work. Pass the same doc_groups tensor on every call:
+    the CSR is cached per tensor object."""
+    import torch.distributed as dist
+
+    if dist.is_available() and dist.is_initialized() and dist.get_world_size(group) * k > MERGE_GROUPS_MAX:
+        raise ValueError(f"sharded_topk_groups: world * k = {dist.get_world_size(group) * k} > {MERGE_GROUPS_MAX}")
+
+    s, p, g = score_topk_groups(queries, index, k, doc_groups, id_offset, stats=stats, doc_mask=doc_mask)
+    if not (dist.is_available() and dist.is_initialized()) or dist.get_world_size(group) == 1:
+        return s, p, g
+    ev = _Stages(stats)
+    world = dist.get_world_size(group)
+    nq = s.shape[0]
+    packed = torch.stack([s.contiguous().view(torch.int32).to(torch.int64), p, g], dim=-1).contiguous()
+    flat = torch.empty((world * nq, k, 3), dtype=torch.int64, device=packed.device)
+    dist.all_gather_into_tensor(flat, packed, group=group)
+    gathered = flat.view(world, nq, k, 3).permute(1, 0, 2, 3).reshape(nq, world * k, 3)
+    ev.mark("all_gather_partials")
+    out = merge_topk_groups(gathered[..., 0].to(torch.int32).view(torch.float32), gathered[..., 1], gathered[..., 2], k)
     ev.mark("merge")
     return out
 
