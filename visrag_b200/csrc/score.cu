@@ -59,6 +59,11 @@ struct MaskedGroupedScoreArgs : MaskedScoreArgs {
     const int* doc_groups;
 };
 
+template <typename Args>
+constexpr bool kMasked = std::is_base_of<MaskedScoreArgs, Args>::value;
+template <typename Args>
+constexpr bool kGrouped = std::is_same<Args, GroupedScoreArgs>::value || std::is_same<Args, MaskedGroupedScoreArgs>::value;
+
 struct Score2Cfg {
     static constexpr int STAGES = 6;
     static constexpr int SUB_BN = 128;                      // docs per MMA sub-tile (a 256-doc tile is two of them)
@@ -139,8 +144,8 @@ template <typename Args>
 __global__ void __launch_bounds__(GEMM_THREADS, 1)
 score_filter_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant__ CUtensorMap tmap_d,
                     const Args g) {
-    constexpr bool GROUPED = std::is_same<Args, GroupedScoreArgs>::value || std::is_same<Args, MaskedGroupedScoreArgs>::value;
-    constexpr bool MASKED = std::is_same<Args, MaskedScoreArgs>::value || std::is_same<Args, MaskedGroupedScoreArgs>::value;
+    constexpr bool GROUPED = kGrouped<Args>;
+    constexpr bool MASKED = kMasked<Args>;
     using Cfg = Score2Cfg;
     constexpr int STAGES = Cfg::STAGES;
     extern __shared__ uint8_t smem_raw[];
@@ -371,13 +376,67 @@ __device__ __forceinline__ bool before(float sa, long long ia, float sb, long lo
     return sa > sb || (sa == sb && ia < ib);
 }
 
+// Warp arg-max in (score, id) order: every lane ends with the warp's best pair.
+__device__ __forceinline__ void warp_argmax(float& bs, long long& bi) {
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) {
+        const float os = __shfl_xor_sync(0xffffffffu, bs, o);
+        const long long oi = __shfl_xor_sync(0xffffffffu, bi, o);
+        if (before(os, oi, bs, bi)) { bs = os; bi = oi; }
+    }
+}
+
+// Block arg-max over WARPS warps through the per-warp slots red_s / red_i: every thread ends with the block's best pair.
+// The second barrier lets the next call reuse the slots.
+template <int WARPS>
+__device__ __forceinline__ void block_argmax(float& bs, long long& bi, float* red_s, long long* red_i) {
+    warp_argmax(bs, bi);
+    if ((threadIdx.x & 31) == 0) { red_s[threadIdx.x >> 5] = bs; red_i[threadIdx.x >> 5] = bi; }
+    __syncthreads();
+    bs = red_s[0]; bi = red_i[0];
+    for (int i = 1; i < WARPS; ++i)
+        if (before(red_s[i], red_i[i], bs, bi)) { bs = red_s[i]; bi = red_i[i]; }
+    __syncthreads();
+}
+
 constexpr int RS_THREADS = 128;
 constexpr int RS_MAX_KEEP = 256;
 
-// Step 1 of rescore_groups_kernel (warp 0, every lane returns the bound), the same merge as step 1 of rescore_topk_kernel
-// (which keeps its own inlined copy: compiled through this function its code changes): the `keep` best candidates by
-// approximate score go to sel[] and their scores to sel_s[] (-1 pads when the lists run out); the return value bounds
-// everything else: the list tails and the best pruned head.
+// Exact fp32 q . d of one doc row, by one warp (every lane returns it): lane-strided float4 FMAs, then warp_sum_f. This
+// is the order of exact_scores_kernel, so the rescored scores have the bits of vr_score_exact.
+__device__ __forceinline__ float warp_dot_row(const float* qs, const float* __restrict__ d, int dim, int lane) {
+    const float4* drow = reinterpret_cast<const float4*>(d);
+    const float4* q4 = reinterpret_cast<const float4*>(qs);
+    float a = 0.f;
+    for (int i = lane; i < (dim >> 2); i += 32) {
+        const float4 x = drow[i], y = q4[i];
+        a = fmaf(x.x, y.x, a);
+        a = fmaf(x.y, y.y, a);
+        a = fmaf(x.z, y.z, a);
+        a = fmaf(x.w, y.w, a);
+    }
+    return warp_sum_f(a);
+}
+
+// The proof of the rescoring kernels: 1 (rerun the query through the fp32 scan) unless bound + eps < kth, where bound
+// covers every candidate that was not rescored exactly (-inf: none) and kth is the k-th exact score.
+__device__ __forceinline__ int proof_flag(float bound, float kth, float qnorm, float dn, int dim) {
+    // fp16 operand rounding (2^-11 each) + fp32 accumulation slack, times |q| * max|d|, plus an absolute
+    // term for fp16 subnormals (elements below 6.1e-5 carry an absolute error up to 2^-25)
+    const float eps = (9.765625e-4f + static_cast<float>(dim) * 1.1920929e-7f) * qnorm * dn +
+                      sqrtf(static_cast<float>(dim)) * 5.9604645e-8f * (qnorm + dn) + 1e-6f;
+    int flag = 0;
+    if (bound > -INFINITY && !(bound + eps < kth)) flag = 1;  // something was dropped that might belong
+    // the bound assumes finite fp16 copies of both operands: a row norm >= 65504 (or inf / NaN, for which the
+    // comparison is false as well) means some |x| may have overflowed fp16 -> rerun this query through the fp32 scan
+    if (!(qnorm < 65504.f) || !(dn < 65504.f)) flag = 1;
+    return flag;
+}
+
+// Step 1 of the rescoring kernels (warp 0, every lane returns the bound): a multi-way merge of the list heads sends the
+// `keep` best candidates by approximate score to sel[] (-1 pads when the lists run out) and, with SCORES, their scores to
+// sel_s[]; the return value bounds everything else: the list tails and the best pruned head.
+template <bool SCORES>
 __device__ __forceinline__ float merge_list_heads(const float* __restrict__ cs, const int* __restrict__ ci, int lists,
                                                   int keep, int lane, int* sel, float* sel_s) {
     // lane l owns lists l, l+32, ...: head position per owned list (<= 2 lists per lane for lists <= 64; general loop)
@@ -416,7 +475,7 @@ __device__ __forceinline__ float merge_list_heads(const float* __restrict__ cs, 
             for (int j = 0; j < (SC_MAX_RANGES + 31) / 32 + 1; ++j)
                 if (j == bj) {
                     sel[m] = ci[(lane + j * 32) * SC_KT + head[j]];
-                    sel_s[m] = ws;
+                    if constexpr (SCORES) sel_s[m] = ws;
                     ++head[j];
                 }
         }
@@ -457,56 +516,7 @@ rescore_topk_kernel(const float* __restrict__ Q, const float* __restrict__ D, lo
     const float* cs = cand_scores + static_cast<long long>(q) * lists * SC_KT;
     const int* ci = cand_ids + static_cast<long long>(q) * lists * SC_KT;
     if (warp == 0) {
-        // lane l owns lists l, l+32, ...: head position per owned list (<= 2 lists per lane for lists <= 64; general loop)
-        float tail = -INFINITY;
-        for (int l = lane; l < lists; l += 32) tail = fmaxf(tail, cs[l * SC_KT + SC_KT - 1]);
-        int head[(SC_MAX_RANGES + 31) / 32 + 1];
-#pragma unroll
-        for (int j = 0; j < (SC_MAX_RANGES + 31) / 32 + 1; ++j) head[j] = 0;
-        for (int m = 0; m < keep; ++m) {
-            // best head of this lane
-            float bs = -INFINITY;
-            int bj = -1;
-#pragma unroll
-            for (int j = 0; j < (SC_MAX_RANGES + 31) / 32 + 1; ++j) {
-                const int l = lane + j * 32;
-                if (l < lists && head[j] < SC_KT) {
-                    const float v = cs[l * SC_KT + head[j]];
-                    if (ci[l * SC_KT + head[j]] >= 0 && (bj < 0 || v > bs)) { bs = v; bj = j; }
-                }
-            }
-            // warp arg-max (ties: lower lane)
-            float ws = bs;
-            int wl = bj >= 0 ? lane : 64;
-#pragma unroll
-            for (int o = 16; o > 0; o >>= 1) {
-                const float os = __shfl_xor_sync(0xffffffffu, ws, o);
-                const int ol = __shfl_xor_sync(0xffffffffu, wl, o);
-                if (ol < 64 && (wl >= 64 || os > ws || (os == ws && ol < wl))) { ws = os; wl = ol; }
-            }
-            if (wl >= 64) {  // every list exhausted
-                for (int r = m + lane; r < keep; r += 32) sel[r] = -1;
-                break;
-            }
-            if (lane == wl) {
-#pragma unroll
-                for (int j = 0; j < (SC_MAX_RANGES + 31) / 32 + 1; ++j)
-                    if (j == bj) {
-                        sel[m] = ci[(lane + j * 32) * SC_KT + head[j]];
-                        ++head[j];
-                    }
-            }
-        }
-        // what is left in the lists was pruned: bounded by the best remaining head
-        float rem = -INFINITY;
-#pragma unroll
-        for (int j = 0; j < (SC_MAX_RANGES + 31) / 32 + 1; ++j) {
-            const int l = lane + j * 32;
-            if (l < lists && head[j] < SC_KT && ci[l * SC_KT + head[j]] >= 0) rem = fmaxf(rem, cs[l * SC_KT + head[j]]);
-        }
-        float bnd = fmaxf(tail, rem);
-#pragma unroll
-        for (int o = 16; o > 0; o >>= 1) bnd = fmaxf(bnd, __shfl_xor_sync(0xffffffffu, bnd, o));
+        const float bnd = merge_list_heads<false>(cs, ci, lists, keep, lane, sel, nullptr);
         if (lane == 0) sh_bound = bnd;
     }
     float qq = 0.f;
@@ -526,20 +536,7 @@ rescore_topk_kernel(const float* __restrict__ Q, const float* __restrict__ D, lo
     // exact fp32 rescoring: one warp per kept candidate
     for (int c = warp; c < keep; c += RS_THREADS / 32) {
         const int id = sel[c];
-        float s = -INFINITY;
-        if (id >= 0) {
-            const float4* drow = reinterpret_cast<const float4*>(D + static_cast<long long>(id) * dim);
-            const float4* q4 = reinterpret_cast<const float4*>(qs);
-            float a = 0.f;
-            for (int i = lane; i < (dim >> 2); i += 32) {
-                const float4 x = drow[i], y = q4[i];
-                a = fmaf(x.x, y.x, a);
-                a = fmaf(x.y, y.y, a);
-                a = fmaf(x.z, y.z, a);
-                a = fmaf(x.w, y.w, a);
-            }
-            s = warp_sum_f(a);
-        }
+        const float s = id >= 0 ? warp_dot_row(qs, D + static_cast<long long>(id) * dim, dim, lane) : -INFINITY;
         if (lane == 0) ex[c] = s;
     }
     __syncthreads();  // ex[] complete, red_s reusable
@@ -557,18 +554,7 @@ rescore_topk_kernel(const float* __restrict__ Q, const float* __restrict__ D, lo
             if (!before(last_s, last_i, s, id)) continue;  // already emitted (or equal to the previous winner)
             if (before(s, id, bs, bi)) { bs = s; bi = id; }
         }
-#pragma unroll
-        for (int o = 16; o > 0; o >>= 1) {
-            const float os = __shfl_xor_sync(0xffffffffu, bs, o);
-            const long long oi = __shfl_xor_sync(0xffffffffu, bi, o);
-            if (before(os, oi, bs, bi)) { bs = os; bi = oi; }
-        }
-        if (lane == 0) { red_s[warp] = bs; red_i[warp] = bi; }
-        __syncthreads();
-        bs = red_s[0]; bi = red_i[0];
-        for (int i = 1; i < RS_THREADS / 32; ++i)
-            if (before(red_s[i], red_i[i], bs, bi)) { bs = red_s[i]; bi = red_i[i]; }
-        __syncthreads();
+        block_argmax<RS_THREADS / 32>(bs, bi, red_s, red_i);
         const bool valid = bi != 0x7fffffffffffffffll;
         if (threadIdx.x == 0) {
             out_scores[static_cast<long long>(q) * k + round] = valid ? bs : -INFINITY;
@@ -584,19 +570,7 @@ rescore_topk_kernel(const float* __restrict__ Q, const float* __restrict__ D, lo
         }
         last_s = bs; last_i = bi; kth = bs;
     }
-    if (threadIdx.x == 0) {
-        // fp16 operand rounding (2^-11 each) + fp32 accumulation slack, times |q| * max|d|, plus an absolute
-        // term for fp16 subnormals (elements below 6.1e-5 carry an absolute error up to 2^-25)
-        const float dn = *max_doc_norm;
-        const float eps = (9.765625e-4f + static_cast<float>(dim) * 1.1920929e-7f) * sh_qnorm * dn +
-                          sqrtf(static_cast<float>(dim)) * 5.9604645e-8f * (sh_qnorm + dn) + 1e-6f;
-        int flag = 0;
-        if (sh_bound > -INFINITY && !(sh_bound + eps < kth)) flag = 1;  // something was dropped that might belong
-        // the bound assumes finite fp16 copies of both operands: a row norm >= 65504 (or inf / NaN, for which the
-        // comparison is false as well) means some |x| may have overflowed fp16 -> rerun this query through the fp32 scan
-        if (!(sh_qnorm < 65504.f) || !(dn < 65504.f)) flag = 1;
-        flags[q] = flag;
-    }
+    if (threadIdx.x == 0) flags[q] = proof_flag(sh_bound, kth, sh_qnorm, *max_doc_norm, dim);
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -641,7 +615,7 @@ rescore_groups_kernel(const float* __restrict__ Q, const float* __restrict__ D, 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const float* qrow = Q + static_cast<long long>(q) * dim;
     if (warp == 0) {
-        const float bnd = merge_list_heads(cand_scores + static_cast<long long>(q) * lists * SC_KT,
+        const float bnd = merge_list_heads<true>(cand_scores + static_cast<long long>(q) * lists * SC_KT,
                                            cand_ids + static_cast<long long>(q) * lists * SC_KT, lists, keep, lane, sel, sel_s);
         if (lane == 0) sh_bound = bnd;
     }
@@ -700,20 +674,7 @@ rescore_groups_kernel(const float* __restrict__ Q, const float* __restrict__ D, 
     // exact fp32 rescoring of every eligible page of the rescored groups: one warp per page
     for (int t = warp; t < total; t += RS_THREADS / 32) {
         const int id = pg[t];
-        float s = -INFINITY;
-        if (id >= 0) {
-            const float4* drow = reinterpret_cast<const float4*>(D + static_cast<long long>(id) * dim);
-            const float4* q4 = reinterpret_cast<const float4*>(qs);
-            float a = 0.f;
-            for (int i = lane; i < (dim >> 2); i += 32) {
-                const float4 x = drow[i], y = q4[i];
-                a = fmaf(x.x, y.x, a);
-                a = fmaf(x.y, y.y, a);
-                a = fmaf(x.z, y.z, a);
-                a = fmaf(x.w, y.w, a);
-            }
-            s = warp_sum_f(a);
-        }
+        const float s = id >= 0 ? warp_dot_row(qs, D + static_cast<long long>(id) * dim, dim, lane) : -INFINITY;
         if (lane == 0) ex[t] = s;
     }
     __syncthreads();
@@ -743,18 +704,7 @@ rescore_groups_kernel(const float* __restrict__ Q, const float* __restrict__ D, 
             if (!before(last_s, last_i, s, id)) continue;
             if (before(s, id, bs, bi)) { bs = s; bi = id; }
         }
-#pragma unroll
-        for (int o = 16; o > 0; o >>= 1) {
-            const float os = __shfl_xor_sync(0xffffffffu, bs, o);
-            const long long oi = __shfl_xor_sync(0xffffffffu, bi, o);
-            if (before(os, oi, bs, bi)) { bs = os; bi = oi; }
-        }
-        if (lane == 0) { red_s[warp] = bs; red_i[warp] = bi; }
-        __syncthreads();
-        bs = red_s[0]; bi = red_i[0];
-        for (int i = 1; i < RS_THREADS / 32; ++i)
-            if (before(red_s[i], red_i[i], bs, bi)) { bs = red_s[i]; bi = red_i[i]; }
-        __syncthreads();
+        block_argmax<RS_THREADS / 32>(bs, bi, red_s, red_i);
         const bool valid = bi != 0x7fffffffffffffffll;
         const long long o = static_cast<long long>(q) * k;
         if (threadIdx.x == 0) {
@@ -773,15 +723,7 @@ rescore_groups_kernel(const float* __restrict__ Q, const float* __restrict__ D, 
         }
         last_s = bs; last_i = bi; kth = bs;
     }
-    if (threadIdx.x == 0) {  // eps and the overflow test of rescore_topk_kernel
-        const float dn = *max_doc_norm;
-        const float eps = (9.765625e-4f + static_cast<float>(dim) * 1.1920929e-7f) * sh_qnorm * dn +
-                          sqrtf(static_cast<float>(dim)) * 5.9604645e-8f * (sh_qnorm + dn) + 1e-6f;
-        int flag = 0;
-        if (sh_bound > -INFINITY && !(sh_bound + eps < kth)) flag = 1;
-        if (!(sh_qnorm < 65504.f) || !(dn < 65504.f)) flag = 1;
-        flags[q] = flag;
-    }
+    if (threadIdx.x == 0) flags[q] = proof_flag(sh_bound, kth, sh_qnorm, *max_doc_norm, dim);
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -860,7 +802,6 @@ topk_rows_kernel(const float* __restrict__ scores, const long long* __restrict__
     // block (row, chunk): top-k of columns [chunk*chunk_cols, ...) of one row, written as list `row*gridDim.y + chunk`
     __shared__ float red_s[8];
     __shared__ long long red_i[8];
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const long long c_lo = static_cast<long long>(blockIdx.y) * chunk_cols;
     const long long c_hi = min(cols, c_lo + chunk_cols);
     const float* srow = scores + static_cast<long long>(blockIdx.x) * cols;
@@ -879,18 +820,7 @@ topk_rows_kernel(const float* __restrict__ scores, const long long* __restrict__
             if (!before(last_s, last_i, s, id)) continue;
             if (before(s, id, bs, bi)) { bs = s; bi = id; }
         }
-#pragma unroll
-        for (int o = 16; o > 0; o >>= 1) {
-            const float os = __shfl_xor_sync(0xffffffffu, bs, o);
-            const long long oi = __shfl_xor_sync(0xffffffffu, bi, o);
-            if (before(os, oi, bs, bi)) { bs = os; bi = oi; }
-        }
-        if (lane == 0) { red_s[warp] = bs; red_i[warp] = bi; }
-        __syncthreads();
-        bs = red_s[0]; bi = red_i[0];
-        for (int i = 1; i < 8; ++i)
-            if (before(red_s[i], red_i[i], bs, bi)) { bs = red_s[i]; bi = red_i[i]; }
-        __syncthreads();
+        block_argmax<8>(bs, bi, red_s, red_i);
         const bool valid = bi != 0x7fffffffffffffffll;
         if (threadIdx.x == 0) {
             out_scores[row * k + round] = valid ? bs : -INFINITY;
@@ -939,12 +869,7 @@ topk_rows_warp_kernel(const float* __restrict__ scores, const long long* __restr
             if (!before(last_s, last_i, s[j], id[j])) continue;
             if (before(s[j], id[j], bs, bi)) { bs = s[j]; bi = id[j]; }
         }
-#pragma unroll
-        for (int o = 16; o > 0; o >>= 1) {
-            const float os = __shfl_xor_sync(0xffffffffu, bs, o);
-            const long long oi = __shfl_xor_sync(0xffffffffu, bi, o);
-            if (before(os, oi, bs, bi)) { bs = os; bi = oi; }
-        }
+        warp_argmax(bs, bi);
         const bool valid = bi != 0x7fffffffffffffffll;
         if (lane == 0) {
             out_scores[static_cast<long long>(row) * k + round] = valid ? bs : -INFINITY;
@@ -1182,28 +1107,24 @@ static int score_ranges_for(int nq, long long nd) { return score_plan(nq, nd).li
 // A doc mask as the _masked entry points take it: present and 4-byte aligned (one uint32 word per 32 docs).
 static bool mask_ok(const uint32_t* mask) { return mask && (reinterpret_cast<uintptr_t>(mask) & 3) == 0; }
 
-template <bool MASKED>
-static int score_filter(const void* q_f16, int nq, const void* d_f16, long long nd, int dim, int ranges, const uint32_t* doc_mask,
-                        float* cand_scores, int* cand_ids, void* stream) {
-    VR_REQUIRE(q_f16 && d_f16 && cand_scores && cand_ids, "vr_score_filter: null pointer");
-    VR_REQUIRE(nq > 0 && nd > 0 && nd < 2147483647ll && dim % 8 == 0, "vr_score_filter: bad shape nq=%d nd=%lld dim=%d", nq,
-               (long long)nd, dim);
-    VR_REQUIRE(nq < (1 << 30), "vr_score_filter: too many queries");
-    const ScorePlan plan = score_plan(nq, nd);
-    VR_REQUIRE(ranges * 2 == plan.lists, "vr_score_filter: ranges must come from vr_score_ranges()");
+// The list initialisation, then score_filter_kernel<Args> over `plan`, after the caller's argument checks. doc_mask and
+// doc_groups go to the forms whose Args carry them.
+template <typename Args>
+static int launch_score_filter(const ScorePlan& plan, const void* q_f16, int nq, const void* d_f16, long long nd, int dim,
+                               float* cand_scores, int* cand_ids, const uint32_t* doc_mask, const int* doc_groups,
+                               cudaStream_t st) {
     using Cfg = Score2Cfg;
     CUtensorMap tq, td;
     if (int rc = make_tmap_2d(&tq, q_f16, nq, dim, dim, GEMM_BM, GEMM_BK, 128, false)) return rc;
     if (int rc = make_tmap_2d(&td, d_f16, nd, dim, dim, 128, GEMM_BK, 128, false)) return rc;
-    using Args = typename std::conditional<MASKED, MaskedScoreArgs, ScoreArgs>::type;
     static unsigned long long attr_set = 0;
     if (first_use_on_device(&attr_set))
         VR_CHECK_CUDA(cudaFuncSetAttribute(score_filter_kernel<Args>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES));
     Args g;
     g.nq = nq; g.nd = nd; g.dim = dim; g.lists = plan.lists; g.T = plan.T; g.R = plan.R; g.QB = plan.QB; g.items = plan.items;
     g.cand_scores = cand_scores; g.cand_ids = cand_ids;
-    if constexpr (MASKED) g.doc_mask = doc_mask;
-    cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+    if constexpr (kMasked<Args>) g.doc_mask = doc_mask;
+    if constexpr (kGrouped<Args>) g.doc_groups = doc_groups;
     {
         const long long n = static_cast<long long>(nq) * (plan.lists - plan.R) * SC_KT;
         long long blocks = (n + 255) / 256;
@@ -1216,19 +1137,65 @@ static int score_filter(const void* q_f16, int nq, const void* d_f16, long long 
     return 0;
 }
 
-template <bool MASKED>
-static int topk_rows_chunked(const float* scores, int rows, long long cols, int k, long long id_offset, int chunks,
-                             float* ws_scores, long long* ws_ids, float* out_scores, long long* out_ids, const uint32_t* mask,
-                             cudaStream_t s) {
-    const long long chunk_cols = (cols + chunks - 1) / chunks;
-    // pass 1: every (row, chunk) block reduces its column range to a sorted top-k list (ids = column + id_offset)
-    topk_rows_kernel<MASKED><<<dim3(rows, chunks), 256, 0, s>>>(scores, nullptr, cols, k, id_offset, chunk_cols, ws_scores,
-                                                                ws_ids, mask);
-    VR_CHECK_CUDA(cudaGetLastError());
-    // pass 2: merge the `chunks` lists of each row (explicit ids; exhausted lists carry id -1 and are skipped)
-    launch_topk_rows<false>(ws_scores, ws_ids, rows, static_cast<long long>(chunks) * k, k, 0, out_scores, out_ids, nullptr, s);
+// vr_score_filter(_masked): the page lists, masked when doc_mask is not NULL
+static int score_filter(const void* q_f16, int nq, const void* d_f16, long long nd, int dim, int ranges, const uint32_t* doc_mask,
+                        float* cand_scores, int* cand_ids, void* stream) {
+    VR_REQUIRE(q_f16 && d_f16 && cand_scores && cand_ids, "vr_score_filter: null pointer");
+    VR_REQUIRE(nq > 0 && nd > 0 && nd < 2147483647ll && dim % 8 == 0, "vr_score_filter: bad shape nq=%d nd=%lld dim=%d", nq,
+               (long long)nd, dim);
+    VR_REQUIRE(nq < (1 << 30), "vr_score_filter: too many queries");
+    const ScorePlan plan = score_plan(nq, nd);
+    VR_REQUIRE(ranges * 2 == plan.lists, "vr_score_filter: ranges must come from vr_score_ranges()");
+    cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+    if (doc_mask)
+        return launch_score_filter<MaskedScoreArgs>(plan, q_f16, nq, d_f16, nd, dim, cand_scores, cand_ids, doc_mask, nullptr, st);
+    return launch_score_filter<ScoreArgs>(plan, q_f16, nq, d_f16, nd, dim, cand_scores, cand_ids, nullptr, nullptr, st);
+}
+
+// vr_topk_rows(_masked), after the mask checks: the masked form when mask is not NULL (ids is NULL then)
+static int topk_rows(const char* fn, const float* scores, const int64_t* ids, int rows, long long cols, int k,
+                     long long id_offset, float* out_scores, int64_t* out_ids, const uint32_t* mask, void* stream) {
+    VR_REQUIRE(scores && out_scores && out_ids, "%s: null pointer", fn);
+    VR_REQUIRE(rows > 0 && cols > 0 && k > 0, "%s: bad shape", fn);
+    const long long* i = reinterpret_cast<const long long*>(ids);
+    long long* oi = reinterpret_cast<long long*>(out_ids);
+    cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
+    if (mask) launch_topk_rows<true>(scores, i, rows, cols, k, id_offset, out_scores, oi, mask, s);
+    else launch_topk_rows<false>(scores, i, rows, cols, k, id_offset, out_scores, oi, nullptr, s);
     VR_CHECK_CUDA(cudaGetLastError());
     return 0;
+}
+
+// vr_topk_rows_chunked(_masked), after the mask check: the masked form when mask is not NULL
+static int topk_rows_chunked(const char* fn, const float* scores, int rows, long long cols, int k, long long id_offset,
+                             int chunks, float* ws_scores, int64_t* ws_ids, float* out_scores, int64_t* out_ids,
+                             const uint32_t* mask, void* stream) {
+    VR_REQUIRE(scores && ws_scores && ws_ids && out_scores && out_ids, "%s: null pointer", fn);
+    VR_REQUIRE(rows > 0 && cols > 0 && k > 0 && chunks > 0 && chunks <= 65535, "%s: bad shape", fn);
+    long long* wi = reinterpret_cast<long long*>(ws_ids);
+    cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
+    const long long chunk_cols = (cols + chunks - 1) / chunks;
+    // pass 1: every (row, chunk) block reduces its column range to a sorted top-k list (ids = column + id_offset)
+    if (mask)
+        topk_rows_kernel<true><<<dim3(rows, chunks), 256, 0, s>>>(scores, nullptr, cols, k, id_offset, chunk_cols, ws_scores,
+                                                                  wi, mask);
+    else
+        topk_rows_kernel<false><<<dim3(rows, chunks), 256, 0, s>>>(scores, nullptr, cols, k, id_offset, chunk_cols, ws_scores,
+                                                                   wi, nullptr);
+    VR_CHECK_CUDA(cudaGetLastError());
+    // pass 2: merge the `chunks` lists of each row (explicit ids; exhausted lists carry id -1 and are skipped)
+    launch_topk_rows<false>(ws_scores, wi, rows, static_cast<long long>(chunks) * k, k, 0, out_scores,
+                            reinterpret_cast<long long*>(out_ids), nullptr, s);
+    VR_CHECK_CUDA(cudaGetLastError());
+    return 0;
+}
+
+// Candidates rescored per query (the best by approximate score), for vr_score_rescore(_groups)
+static int rescore_keep(int k, int lists) {
+    int keep = 2 * k > 32 ? 2 * k : 32;
+    if (keep > lists * SC_KT) keep = lists * SC_KT;
+    if (keep > RS_MAX_KEEP) keep = RS_MAX_KEEP;
+    return keep;
 }
 
 }  // namespace vr
@@ -1259,14 +1226,14 @@ extern "C" int vr_f32_to_f16_rows(const float* src, int64_t rows, int32_t dim, v
 
 extern "C" int vr_score_filter(const void* q_f16, int32_t nq, const void* d_f16, int64_t nd, int32_t dim, int32_t ranges,
                                float* cand_scores, int32_t* cand_ids, void* stream) {
-    return score_filter<false>(q_f16, nq, d_f16, nd, dim, ranges, nullptr, cand_scores, cand_ids, stream);
+    return score_filter(q_f16, nq, d_f16, nd, dim, ranges, nullptr, cand_scores, cand_ids, stream);
 }
 
 extern "C" int vr_score_filter_masked(const void* q_f16, int32_t nq, const void* d_f16, int64_t nd, int32_t dim,
                                       int32_t ranges, float* cand_scores, int32_t* cand_ids, const uint32_t* doc_mask,
                                       void* stream) {
     VR_REQUIRE(mask_ok(doc_mask), "vr_score_filter_masked: doc_mask must be a non-null, 4-byte aligned pointer");
-    return score_filter<true>(q_f16, nq, d_f16, nd, dim, ranges, doc_mask, cand_scores, cand_ids, stream);
+    return score_filter(q_f16, nq, d_f16, nd, dim, ranges, doc_mask, cand_scores, cand_ids, stream);
 }
 
 extern "C" int vr_score_rescore(const float* q_f32, int32_t nq, const float* d_f32, int64_t nd, int32_t dim, int32_t ranges,
@@ -1277,9 +1244,7 @@ extern "C" int vr_score_rescore(const float* q_f32, int32_t nq, const float* d_f
     VR_REQUIRE(nq > 0 && k > 0 && dim % 4 == 0, "vr_score_rescore: bad shape");
     const int lists = ranges * 2;
     VR_REQUIRE(ranges > 0 && lists <= SC_MAX_RANGES + 2, "vr_score_rescore: ranges must come from vr_score_ranges()");
-    int keep = 2 * k > 32 ? 2 * k : 32;  // candidates rescored per query (the best by approximate score)
-    if (keep > lists * SC_KT) keep = lists * SC_KT;
-    if (keep > RS_MAX_KEEP) keep = RS_MAX_KEEP;
+    const int keep = rescore_keep(k, lists);
     const size_t smem = (static_cast<size_t>(dim) + 2 * static_cast<size_t>(keep)) * sizeof(float);
     VR_REQUIRE(smem <= 200 * 1024, "vr_score_rescore: dim too large for shared memory (%zu bytes)", smem);
     static unsigned long long attr_set = 0;
@@ -1330,12 +1295,7 @@ extern "C" int vr_score_exact(const float* q_f32, int32_t nq, const float* d_f32
 
 extern "C" int vr_topk_rows(const float* scores, const int64_t* ids, int32_t rows, int64_t cols, int32_t k, int64_t id_offset,
                             float* out_scores, int64_t* out_ids, void* stream) {
-    VR_REQUIRE(scores && out_scores && out_ids, "vr_topk_rows: null pointer");
-    VR_REQUIRE(rows > 0 && cols > 0 && k > 0, "vr_topk_rows: bad shape");
-    launch_topk_rows<false>(scores, reinterpret_cast<const long long*>(ids), rows, cols, k, id_offset, out_scores,
-                            reinterpret_cast<long long*>(out_ids), nullptr, reinterpret_cast<cudaStream_t>(stream));
-    VR_CHECK_CUDA(cudaGetLastError());
-    return 0;
+    return topk_rows("vr_topk_rows", scores, ids, rows, cols, k, id_offset, out_scores, out_ids, nullptr, stream);
 }
 
 extern "C" int vr_topk_rows_masked(const float* scores, const int64_t* ids, int32_t rows, int64_t cols, int32_t k,
@@ -1343,65 +1303,27 @@ extern "C" int vr_topk_rows_masked(const float* scores, const int64_t* ids, int3
                                    void* stream) {
     VR_REQUIRE(mask_ok(doc_mask), "vr_topk_rows_masked: doc_mask must be a non-null, 4-byte aligned pointer");
     VR_REQUIRE(!ids, "vr_topk_rows_masked: the mask indexes columns, so ids must be NULL");
-    VR_REQUIRE(scores && out_scores && out_ids, "vr_topk_rows_masked: null pointer");
-    VR_REQUIRE(rows > 0 && cols > 0 && k > 0, "vr_topk_rows_masked: bad shape");
-    launch_topk_rows<true>(scores, nullptr, rows, cols, k, id_offset, out_scores, reinterpret_cast<long long*>(out_ids), doc_mask,
-                           reinterpret_cast<cudaStream_t>(stream));
-    VR_CHECK_CUDA(cudaGetLastError());
-    return 0;
+    return topk_rows("vr_topk_rows_masked", scores, ids, rows, cols, k, id_offset, out_scores, out_ids, doc_mask, stream);
 }
 
 extern "C" int vr_topk_rows_chunked(const float* scores, int32_t rows, int64_t cols, int32_t k, int64_t id_offset,
                                     int32_t chunks, float* ws_scores, int64_t* ws_ids, float* out_scores,
                                     int64_t* out_ids, void* stream) {
-    VR_REQUIRE(scores && ws_scores && ws_ids && out_scores && out_ids, "vr_topk_rows_chunked: null pointer");
-    VR_REQUIRE(rows > 0 && cols > 0 && k > 0 && chunks > 0 && chunks <= 65535, "vr_topk_rows_chunked: bad shape");
-    return topk_rows_chunked<false>(scores, rows, cols, k, id_offset, chunks, ws_scores, reinterpret_cast<long long*>(ws_ids),
-                                    out_scores, reinterpret_cast<long long*>(out_ids), nullptr,
-                                    reinterpret_cast<cudaStream_t>(stream));
+    return topk_rows_chunked("vr_topk_rows_chunked", scores, rows, cols, k, id_offset, chunks, ws_scores, ws_ids, out_scores,
+                             out_ids, nullptr, stream);
 }
 
 extern "C" int vr_topk_rows_chunked_masked(const float* scores, int32_t rows, int64_t cols, int32_t k, int64_t id_offset,
                                            int32_t chunks, float* ws_scores, int64_t* ws_ids, float* out_scores,
                                            int64_t* out_ids, const uint32_t* doc_mask, void* stream) {
     VR_REQUIRE(mask_ok(doc_mask), "vr_topk_rows_chunked_masked: doc_mask must be a non-null, 4-byte aligned pointer");
-    VR_REQUIRE(scores && ws_scores && ws_ids && out_scores && out_ids, "vr_topk_rows_chunked_masked: null pointer");
-    VR_REQUIRE(rows > 0 && cols > 0 && k > 0 && chunks > 0 && chunks <= 65535, "vr_topk_rows_chunked_masked: bad shape");
-    return topk_rows_chunked<true>(scores, rows, cols, k, id_offset, chunks, ws_scores, reinterpret_cast<long long*>(ws_ids),
-                                   out_scores, reinterpret_cast<long long*>(out_ids), doc_mask,
-                                   reinterpret_cast<cudaStream_t>(stream));
+    return topk_rows_chunked("vr_topk_rows_chunked_masked", scores, rows, cols, k, id_offset, chunks, ws_scores, ws_ids,
+                             out_scores, out_ids, doc_mask, stream);
 }
 
 // ---------------------------------------------------------------------------------------------- document-level top-k
 // A group table as the _groups entry points take it: 4-byte aligned int32 arrays, G >= 1, nd within the int32 ids.
 static bool i32_ok(const void* p) { return p && (reinterpret_cast<uintptr_t>(p) & 3) == 0; }
-
-template <typename Args>
-static int score_filter_groups(const void* q_f16, int nq, const void* d_f16, long long nd, int dim, const int* doc_groups,
-                               const uint32_t* doc_mask, float* cand_scores, int* cand_ids, cudaStream_t st) {
-    using Cfg = Score2Cfg;
-    CUtensorMap tq, td;
-    if (int rc = make_tmap_2d(&tq, q_f16, nq, dim, dim, GEMM_BM, GEMM_BK, 128, false)) return rc;
-    if (int rc = make_tmap_2d(&td, d_f16, nd, dim, dim, 128, GEMM_BK, 128, false)) return rc;
-    const ScorePlan plan = score_plan(nq, nd);
-    static unsigned long long attr_set = 0;
-    if (first_use_on_device(&attr_set))
-        VR_CHECK_CUDA(cudaFuncSetAttribute(score_filter_kernel<Args>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES));
-    Args g;
-    g.nq = nq; g.nd = nd; g.dim = dim; g.lists = plan.lists; g.T = plan.T; g.R = plan.R; g.QB = plan.QB; g.items = plan.items;
-    g.cand_scores = cand_scores; g.cand_ids = cand_ids; g.doc_groups = doc_groups;
-    if constexpr (std::is_same<Args, MaskedGroupedScoreArgs>::value) g.doc_mask = doc_mask;
-    {
-        const long long n = static_cast<long long>(nq) * (plan.lists - plan.R) * SC_KT;
-        long long blocks = (n + 255) / 256;
-        if (blocks > num_sms() * 8) blocks = num_sms() * 8;
-        score_init_lists_kernel<<<static_cast<int>(blocks), 256, 0, st>>>(cand_scores, cand_ids, nq, plan.lists, plan.R);
-        VR_CHECK_CUDA(cudaGetLastError());
-    }
-    score_filter_kernel<Args><<<2 * plan.pairs, GEMM_THREADS, Cfg::SMEM_BYTES, st>>>(tq, td, g);
-    VR_CHECK_CUDA(cudaGetLastError());
-    return 0;
-}
 
 extern "C" int vr_score_filter_groups(const void* q_f16, int32_t nq, const void* d_f16, int64_t nd, int32_t dim,
                                       int32_t ranges, float* cand_scores, int32_t* cand_ids, const int32_t* doc_groups,
@@ -1411,12 +1333,13 @@ extern "C" int vr_score_filter_groups(const void* q_f16, int32_t nq, const void*
     VR_REQUIRE(q_f16 && d_f16 && cand_scores && cand_ids, "vr_score_filter_groups: null pointer");
     VR_REQUIRE(nd > 0 && nd < 2147483647ll, "vr_score_filter_groups: nd=%lld beyond the int32 doc ids", (long long)nd);
     VR_REQUIRE(nq > 0 && nq < (1 << 30) && dim % 8 == 0, "vr_score_filter_groups: bad shape");
-    VR_REQUIRE(ranges * 2 == score_plan(nq, nd).lists, "vr_score_filter_groups: ranges must come from vr_score_ranges()");
+    const ScorePlan plan = score_plan(nq, nd);
+    VR_REQUIRE(ranges * 2 == plan.lists, "vr_score_filter_groups: ranges must come from vr_score_ranges()");
     cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
     if (doc_mask)
-        return score_filter_groups<MaskedGroupedScoreArgs>(q_f16, nq, d_f16, nd, dim, doc_groups, doc_mask, cand_scores,
-                                                           cand_ids, st);
-    return score_filter_groups<GroupedScoreArgs>(q_f16, nq, d_f16, nd, dim, doc_groups, nullptr, cand_scores, cand_ids, st);
+        return launch_score_filter<MaskedGroupedScoreArgs>(plan, q_f16, nq, d_f16, nd, dim, cand_scores, cand_ids, doc_mask,
+                                                           doc_groups, st);
+    return launch_score_filter<GroupedScoreArgs>(plan, q_f16, nq, d_f16, nd, dim, cand_scores, cand_ids, nullptr, doc_groups, st);
 }
 
 extern "C" int vr_score_rescore_groups(const float* q_f32, int32_t nq, const float* d_f32, int64_t nd, int32_t dim,
@@ -1435,9 +1358,7 @@ extern "C" int vr_score_rescore_groups(const float* q_f32, int32_t nq, const flo
     VR_REQUIRE(nq > 0 && k > 0 && dim % 4 == 0, "vr_score_rescore_groups: bad shape");
     const int lists = ranges * 2;
     VR_REQUIRE(ranges > 0 && lists <= SC_MAX_RANGES + 2, "vr_score_rescore_groups: ranges must come from vr_score_ranges()");
-    int keep = 2 * k > 32 ? 2 * k : 32;  // as vr_score_rescore
-    if (keep > lists * SC_KT) keep = lists * SC_KT;
-    if (keep > RS_MAX_KEEP) keep = RS_MAX_KEEP;
+    const int keep = rescore_keep(k, lists);
     const size_t smem = (static_cast<size_t>(dim) + 2 * RG_PAGE_BUDGET + 7 * static_cast<size_t>(keep) + 1) * sizeof(float);
     VR_REQUIRE(smem <= 200 * 1024, "vr_score_rescore_groups: dim too large for shared memory (%zu bytes)", smem);
     static unsigned long long attr_set = 0;

@@ -101,18 +101,22 @@ class KnowledgeBase:
         except KeyError as e:
             raise KeyError(f"no live page named {e.args[0]!r} in the knowledge base") from None
 
-    def search(self, query_reps, topk: int, within: Optional[Iterable[str]] = None) -> Tuple[torch.Tensor, torch.Tensor]:
-        """query_reps [nq, d] (tensor or ndarray, fp32) -> (scores [nq,k] f32, page indices [nq,k] i64) on the device.
-        within: page filenames to search (default: every live page); k = min(topk, pages searched)."""
+    def _query_and_mask(self, query_reps, within: Optional[Iterable[str]]):
+        """(queries [nq, d] fp32 on the index's device, bool [nd] mask of the pages searched or None for every page, number
+        of pages searched)."""
         q = query_reps if isinstance(query_reps, torch.Tensor) else torch.from_numpy(np.asarray(query_reps, dtype=np.float32))
         q = q.to(self.index.emb.device, torch.float32).reshape(-1, self.index.emb.shape[1]).contiguous()
         if within is None:
-            n, mask = len(self), None if len(self) == self.index.nd else self._live   # None: the unfiltered kernels
-        else:
-            rows = self._rows(within)
-            n = len(rows)
-            mask = torch.zeros(self.index.nd, dtype=torch.bool, device=q.device)
-            mask[torch.tensor(rows, dtype=torch.int64, device=q.device)] = True
+            return q, None if len(self) == self.index.nd else self._live, len(self)  # None: the unmasked kernels
+        rows = self._rows(within)
+        mask = torch.zeros(self.index.nd, dtype=torch.bool, device=q.device)
+        mask[torch.tensor(rows, dtype=torch.int64, device=q.device)] = True
+        return q, mask, len(rows)
+
+    def search(self, query_reps, topk: int, within: Optional[Iterable[str]] = None) -> Tuple[torch.Tensor, torch.Tensor]:
+        """query_reps [nq, d] (tensor or ndarray, fp32) -> (scores [nq,k] f32, page indices [nq,k] i64) on the device.
+        within: page filenames to search (default: every live page); k = min(topk, pages searched)."""
+        q, mask, n = self._query_and_mask(query_reps, within)
         k = min(topk, n)
         if k == 0:
             return (torch.empty((q.shape[0], 0), dtype=torch.float32, device=q.device),
@@ -124,13 +128,7 @@ class KnowledgeBase:
         """The top-k DOCUMENTS, each scored by its best page: (scores [nq,k] f32, best page indices [nq,k] i64 on the
         device, document names [nq][k]). within: page filenames to search (default: every live page); k = min(topk,
         documents searched). Ties rank the document with the lower best page index first."""
-        q = query_reps if isinstance(query_reps, torch.Tensor) else torch.from_numpy(np.asarray(query_reps, dtype=np.float32))
-        q = q.to(self.index.emb.device, torch.float32).reshape(-1, self.index.emb.shape[1]).contiguous()
-        if within is None:
-            mask = None if len(self) == self.index.nd else self._live   # None: the unmasked kernels
-        else:
-            mask = torch.zeros(self.index.nd, dtype=torch.bool, device=q.device)
-            mask[torch.tensor(self._rows(within), dtype=torch.int64, device=q.device)] = True
+        q, mask, _ = self._query_and_mask(query_reps, within)
         searched = self._doc_groups if mask is None else self._doc_groups[mask]
         k = min(topk, int(torch.unique(searched).numel()))             # documents searched, counted on the device
         if k == 0:

@@ -99,7 +99,8 @@ def _check_doc_mask(doc_mask: torch.Tensor, index: CorpusIndex) -> torch.Tensor:
     return pack_doc_mask(doc_mask)
 
 
-def _exact_topk(q: torch.Tensor, index: CorpusIndex, k: int, id_offset: int, mask_words: Optional[torch.Tensor] = None):
+def _exact_topk(q: torch.Tensor, index: CorpusIndex, k: int, id_offset: int, mask_words: Optional[torch.Tensor]):
+    """The plain fp32 scan: (scores, ids)."""
     nq, d = q.shape
     nd = index.nd
     out_s = torch.empty((nq, k), dtype=torch.float32, device=q.device)
@@ -107,6 +108,7 @@ def _exact_topk(q: torch.Tensor, index: CorpusIndex, k: int, id_offset: int, mas
     rows_per = max(1, min(nq, (1 << 28) // max(nd, 1)))  # <= 1 GiB of fp32 scratch
     scratch = torch.empty((rows_per, nd), dtype=torch.float32, device=q.device)
     lib = L.lib()
+    mw = () if mask_words is None else (mask_words.data_ptr(),)
     for r0 in range(0, nq, rows_per):
         n = min(rows_per, nq - r0)
         L.check(lib.vr_score_exact(q[r0:].data_ptr(), n, index.emb.data_ptr(), nd, d, scratch.data_ptr(), L.stream_ptr()))
@@ -114,19 +116,12 @@ def _exact_topk(q: torch.Tensor, index: CorpusIndex, k: int, id_offset: int, mas
         if chunks >= 2:
             ws_s = torch.empty((n, chunks, k), dtype=torch.float32, device=q.device)
             ws_i = torch.empty((n, chunks, k), dtype=torch.int64, device=q.device)
-            if mask_words is None:
-                L.check(lib.vr_topk_rows_chunked(scratch.data_ptr(), n, nd, k, id_offset, chunks, ws_s.data_ptr(),
-                                                 ws_i.data_ptr(), out_s[r0:].data_ptr(), out_i[r0:].data_ptr(), L.stream_ptr()))
-            else:
-                L.check(lib.vr_topk_rows_chunked_masked(scratch.data_ptr(), n, nd, k, id_offset, chunks, ws_s.data_ptr(),
-                                                        ws_i.data_ptr(), out_s[r0:].data_ptr(), out_i[r0:].data_ptr(),
-                                                        mask_words.data_ptr(), L.stream_ptr()))
-        elif mask_words is None:
-            L.check(lib.vr_topk_rows(scratch.data_ptr(), None, n, nd, k, id_offset, out_s[r0:].data_ptr(),
-                                     out_i[r0:].data_ptr(), L.stream_ptr()))
+            fn = lib.vr_topk_rows_chunked_masked if mw else lib.vr_topk_rows_chunked
+            args = (scratch.data_ptr(), n, nd, k, id_offset, chunks, ws_s.data_ptr(), ws_i.data_ptr())
         else:
-            L.check(lib.vr_topk_rows_masked(scratch.data_ptr(), None, n, nd, k, id_offset, out_s[r0:].data_ptr(),
-                                            out_i[r0:].data_ptr(), mask_words.data_ptr(), L.stream_ptr()))
+            fn = lib.vr_topk_rows_masked if mw else lib.vr_topk_rows
+            args = (scratch.data_ptr(), None, n, nd, k, id_offset)
+        L.check(fn(*args, out_s[r0:].data_ptr(), out_i[r0:].data_ptr(), *mw, L.stream_ptr()))
     return out_s, out_i
 
 
@@ -136,12 +131,17 @@ def score_topk(queries: torch.Tensor, index: CorpusIndex, k: int, id_offset: int
     Rows are sorted by (score desc, id asc); if k > nd the tail is (-inf, -1).
     doc_mask: optional bool [nd] on the index's device; only docs marked True are searched (the same bits as the fp32 scan
     over those docs alone). With fewer than k of them the tail is (-inf, -1)."""
+    q, mask_words = _queries_and_mask(queries, index, doc_mask)
+    with L.on_device(q.device):
+        return _score_topk(q, index, k, id_offset, force_exact, stats, mask_words)
+
+
+def _queries_and_mask(queries: torch.Tensor, index: CorpusIndex, doc_mask: Optional[torch.Tensor]):
+    """The queries as contiguous fp32 on the index's device, and the packed doc mask (None: every doc)."""
     q = _check_f32(queries, "queries")
     if q.device != index.emb.device:
         raise ValueError(f"queries live on {q.device}, the index on {index.emb.device}")
-    mask_words = None if doc_mask is None else _check_doc_mask(doc_mask, index)
-    with L.on_device(q.device):
-        return _score_topk(q, index, k, id_offset, force_exact, stats, mask_words)
+    return q, None if doc_mask is None else _check_doc_mask(doc_mask, index)
 
 
 class _Stages:
@@ -171,48 +171,64 @@ def resolve_stages(stats: dict) -> dict:
 
 
 def _score_topk(q: torch.Tensor, index: CorpusIndex, k: int, id_offset: int, force_exact: bool, stats: Optional[dict],
-                mask_words: Optional[torch.Tensor] = None):
+                mask_words: Optional[torch.Tensor], gt: Optional[_GroupTable] = None, page_lists: bool = False):
+    """The filter + rescoring pipeline. Pages (gt None): (scores, ids); groups (gt, the group table): (scores, best pages,
+    groups). page_lists: feed the page filter's lists to the grouped rescoring (tests and measurements of the proof)."""
     nq, d = q.shape
     nd = index.nd
+
+    def exact(rows: torch.Tensor):
+        if gt is None:
+            return _exact_topk(rows, index, k, id_offset, mask_words)
+        return _exact_topk_groups(rows, index, k, id_offset, mask_words, gt)
+
+    def outputs(n: int):
+        dtypes = (torch.float32, torch.int64) if gt is None else (torch.float32, torch.int64, torch.int64)
+        return tuple([torch.empty((n, k), dtype=t, device=q.device) for t in dtypes])
+
     if nq == 0:
-        return (torch.empty((0, k), dtype=torch.float32, device=q.device), torch.empty((0, k), dtype=torch.int64, device=q.device))
+        return outputs(0)
     if d != index.emb.shape[1]:
         raise ValueError("query / corpus dim mismatch")
     if force_exact or nq * nd <= SMALL_PROBLEM or nd < 256:
         if stats is not None:
             stats.update(path="exact", flagged=0)
-        return _exact_topk(q, index, k, id_offset, mask_words)
+        return exact(q)
     lib = L.lib()
     ranges = lib.vr_score_ranges(nq, nd)
     lists = ranges * 2 * lib.vr_score_list_len()
     q16 = to_f16_rows(q)
     cand_s = torch.empty((nq, lists), dtype=torch.float32, device=q.device)
     cand_i = torch.empty((nq, lists), dtype=torch.int32, device=q.device)
-    out_s = torch.empty((nq, k), dtype=torch.float32, device=q.device)
-    out_i = torch.empty((nq, k), dtype=torch.int64, device=q.device)
+    out = outputs(nq)
     flags = torch.empty((nq,), dtype=torch.int32, device=q.device)
     sp = L.stream_ptr()
+    mw = None if mask_words is None else mask_words.data_ptr()
     ev = _Stages(stats)
     ev.mark("q_to_f16")
-    if mask_words is None:
-        L.check(lib.vr_score_filter(q16.data_ptr(), nq, index.emb_f16.data_ptr(), nd, d, ranges, cand_s.data_ptr(),
-                                    cand_i.data_ptr(), sp))
+    filt = (q16.data_ptr(), nq, index.emb_f16.data_ptr(), nd, d, ranges, cand_s.data_ptr(), cand_i.data_ptr())
+    if gt is not None and not page_lists:
+        L.check(lib.vr_score_filter_groups(*filt, gt.groups.data_ptr(), mw, sp))
+    elif mw is None:
+        L.check(lib.vr_score_filter(*filt, sp))
     else:
-        L.check(lib.vr_score_filter_masked(q16.data_ptr(), nq, index.emb_f16.data_ptr(), nd, d, ranges, cand_s.data_ptr(),
-                                           cand_i.data_ptr(), mask_words.data_ptr(), sp))
+        L.check(lib.vr_score_filter_masked(*filt, mw, sp))
     ev.mark("filter")
-    L.check(lib.vr_score_rescore(q.data_ptr(), nq, index.emb.data_ptr(), nd, d, ranges, cand_s.data_ptr(), cand_i.data_ptr(),
-                                 index.max_norm.data_ptr(), k, id_offset, out_s.data_ptr(), out_i.data_ptr(),
-                                 flags.data_ptr(), sp))
+    cand = (q.data_ptr(), nq, index.emb.data_ptr(), nd, d, ranges, cand_s.data_ptr(), cand_i.data_ptr())
+    tail = (index.max_norm.data_ptr(), k, id_offset, *[t.data_ptr() for t in out], flags.data_ptr(), sp)
+    if gt is None:
+        L.check(lib.vr_score_rescore(*cand, *tail))
+    else:
+        L.check(lib.vr_score_rescore_groups(*cand, gt.groups.data_ptr(), gt.offsets.data_ptr(), gt.pages.data_ptr(), gt.G,
+                                            mw, *tail))
     ev.mark("rescore")
     bad = torch.nonzero(flags).flatten()  # host sync: the caller reads the result next anyway
     if stats is not None:
         stats.update(path="filter+rescore", flagged=int(bad.numel()), ranges=ranges)
     if bad.numel() > 0:
-        s2, i2 = _exact_topk(q.index_select(0, bad), index, k, id_offset, mask_words)
-        out_s.index_copy_(0, bad, s2)
-        out_i.index_copy_(0, bad, i2)
-    return out_s, out_i
+        for t, fix in zip(out, exact(q.index_select(0, bad))):
+            t.index_copy_(0, bad, fix)
+    return out
 
 
 # ------------------------------------------------------------------------------------------------------
@@ -258,8 +274,9 @@ def _group_table(doc_groups: torch.Tensor, index: CorpusIndex) -> _GroupTable:
     return table
 
 
-def _exact_topk_groups(q: torch.Tensor, index: CorpusIndex, k: int, id_offset: int, gt: _GroupTable,
-                       mask_words: Optional[torch.Tensor] = None):
+def _exact_topk_groups(q: torch.Tensor, index: CorpusIndex, k: int, id_offset: int, mask_words: Optional[torch.Tensor],
+                       gt: _GroupTable):
+    """The plain fp32 scan, reduced per group: (scores, best pages, groups)."""
     nq, d = q.shape
     nd = index.nd
     out_s = torch.empty((nq, k), dtype=torch.float32, device=q.device)
@@ -289,66 +306,15 @@ def score_topk_groups(queries: torch.Tensor, index: CorpusIndex, k: int, doc_gro
     page with that maximum; groups rank by (score desc, best page asc). Returns (scores [nq,k] f32, best pages [nq,k] i64
     = local index + id_offset, groups [nq,k] i64); fewer than k groups with an eligible page leave (-inf, -1, -1).
     With doc_groups = arange(nd) the result equals score_topk's, with groups == pages. doc_mask as in score_topk."""
-    q = _check_f32(queries, "queries")
-    if q.device != index.emb.device:
-        raise ValueError(f"queries live on {q.device}, the index on {index.emb.device}")
-    mask_words = None if doc_mask is None else _check_doc_mask(doc_mask, index)
+    q, mask_words = _queries_and_mask(queries, index, doc_mask)
     with L.on_device(q.device):
         gt = _group_table(doc_groups, index)
         return _score_topk_groups(q, index, k, id_offset, force_exact, stats, gt, mask_words)
 
 
 def _score_topk_groups(q, index, k, id_offset, force_exact, stats, gt: _GroupTable, mask_words, page_lists: bool = False):
-    """page_lists: feed the page filter's lists to the grouped rescoring (tests and measurements of the proof)."""
-    nq, d = q.shape
-    nd = index.nd
-    if nq == 0:
-        e = torch.empty((0, k), dtype=torch.int64, device=q.device)
-        return torch.empty((0, k), dtype=torch.float32, device=q.device), e, e.clone()
-    if d != index.emb.shape[1]:
-        raise ValueError("query / corpus dim mismatch")
-    if force_exact or nq * nd <= SMALL_PROBLEM or nd < 256:
-        if stats is not None:
-            stats.update(path="exact", flagged=0)
-        return _exact_topk_groups(q, index, k, id_offset, gt, mask_words)
-    lib = L.lib()
-    ranges = lib.vr_score_ranges(nq, nd)
-    lists = ranges * 2 * lib.vr_score_list_len()
-    q16 = to_f16_rows(q)
-    cand_s = torch.empty((nq, lists), dtype=torch.float32, device=q.device)
-    cand_i = torch.empty((nq, lists), dtype=torch.int32, device=q.device)
-    out_s = torch.empty((nq, k), dtype=torch.float32, device=q.device)
-    out_p = torch.empty((nq, k), dtype=torch.int64, device=q.device)
-    out_g = torch.empty((nq, k), dtype=torch.int64, device=q.device)
-    flags = torch.empty((nq,), dtype=torch.int32, device=q.device)
-    sp = L.stream_ptr()
-    mw = None if mask_words is None else mask_words.data_ptr()
-    ev = _Stages(stats)
-    ev.mark("q_to_f16")
-    if page_lists and mw is None:
-        L.check(lib.vr_score_filter(q16.data_ptr(), nq, index.emb_f16.data_ptr(), nd, d, ranges, cand_s.data_ptr(),
-                                    cand_i.data_ptr(), sp))
-    elif page_lists:
-        L.check(lib.vr_score_filter_masked(q16.data_ptr(), nq, index.emb_f16.data_ptr(), nd, d, ranges, cand_s.data_ptr(),
-                                           cand_i.data_ptr(), mw, sp))
-    else:
-        L.check(lib.vr_score_filter_groups(q16.data_ptr(), nq, index.emb_f16.data_ptr(), nd, d, ranges, cand_s.data_ptr(),
-                                           cand_i.data_ptr(), gt.groups.data_ptr(), mw, sp))
-    ev.mark("filter")
-    L.check(lib.vr_score_rescore_groups(q.data_ptr(), nq, index.emb.data_ptr(), nd, d, ranges, cand_s.data_ptr(),
-                                        cand_i.data_ptr(), gt.groups.data_ptr(), gt.offsets.data_ptr(), gt.pages.data_ptr(),
-                                        gt.G, mw, index.max_norm.data_ptr(), k, id_offset, out_s.data_ptr(),
-                                        out_p.data_ptr(), out_g.data_ptr(), flags.data_ptr(), sp))
-    ev.mark("rescore")
-    bad = torch.nonzero(flags).flatten()  # host sync: the caller reads the result next anyway
-    if stats is not None:
-        stats.update(path="filter+rescore", flagged=int(bad.numel()), ranges=ranges)
-    if bad.numel() > 0:
-        s2, p2, g2 = _exact_topk_groups(q.index_select(0, bad), index, k, id_offset, gt, mask_words)
-        out_s.index_copy_(0, bad, s2)
-        out_p.index_copy_(0, bad, p2)
-        out_g.index_copy_(0, bad, g2)
-    return out_s, out_p, out_g
+    """_score_topk for groups. page_lists=True is the entry of the tests and measurements of the proof on page lists."""
+    return _score_topk(q, index, k, id_offset, force_exact, stats, mask_words, gt, page_lists)
 
 
 def merge_topk_groups(scores: torch.Tensor, pages: torch.Tensor, groups: torch.Tensor, k: int):
@@ -389,21 +355,30 @@ def shard_range(n_items: int, rank: int, world: int) -> Tuple[int, int]:
     return lo, lo + base + (1 if rank < rem else 0)
 
 
-def gather_partials(scores: torch.Tensor, ids: torch.Tensor, group=None) -> Tuple[torch.Tensor, torch.Tensor]:
-    """The ONE collective of the retrieval path: all-gather every rank's [nq, k] (score, global id) pairs.
-    Returns ([nq, world*k] scores, [nq, world*k] ids) on every rank. Score bits travel inside int64 so a single
-    all_gather moves both arrays (12 -> 16 B per entry; the message is latency bound either way)."""
+def _world(group) -> int:
+    """The size of the process group, or 1 outside torch.distributed."""
+    import torch.distributed as dist
+
+    return dist.get_world_size(group) if dist.is_available() and dist.is_initialized() else 1
+
+
+def _all_gather_rows(packed: torch.Tensor, group) -> torch.Tensor:
+    """[nq, k, c] int64 on every rank -> [nq, world*k, c]: rank r's entries of a row at [r*k, (r+1)*k). Callers pack score
+    bits inside int64 so that ONE all_gather moves every array (the message is latency bound either way)."""
     import torch.distributed as dist
 
     world = dist.get_world_size(group)
-    nq, k = scores.shape
-    packed = torch.stack([scores.contiguous().view(torch.int32).to(torch.int64), ids.to(torch.int64)], dim=-1).contiguous()
-    flat = torch.empty((world * nq, k, 2), dtype=torch.int64, device=packed.device)  # rank-major concatenation
-    dist.all_gather_into_tensor(flat, packed, group=group)
-    gathered = flat.view(world, nq, k, 2)
-    gs = gathered[..., 0].to(torch.int32).view(torch.float32).permute(1, 0, 2).reshape(nq, world * k)
-    gi = gathered[..., 1].permute(1, 0, 2).reshape(nq, world * k)
-    return gs.contiguous(), gi.contiguous()
+    nq, k, c = packed.shape
+    flat = torch.empty((world * nq, k, c), dtype=torch.int64, device=packed.device)  # rank-major concatenation
+    dist.all_gather_into_tensor(flat, packed.contiguous(), group=group)
+    return flat.view(world, nq, k, c).permute(1, 0, 2, 3).reshape(nq, world * k, c)
+
+
+def gather_partials(scores: torch.Tensor, ids: torch.Tensor, group=None) -> Tuple[torch.Tensor, torch.Tensor]:
+    """The ONE collective of the retrieval path: all-gather every rank's [nq, k] (score, global id) pairs.
+    Returns ([nq, world*k] scores, [nq, world*k] ids) on every rank."""
+    g = _all_gather_rows(torch.stack([scores.contiguous().view(torch.int32).to(torch.int64), ids.to(torch.int64)], dim=-1), group)
+    return g[..., 0].to(torch.int32).view(torch.float32).contiguous(), g[..., 1].contiguous()
 
 
 def sharded_topk(queries: torch.Tensor, index: CorpusIndex, k: int, id_offset: int, group=None, stats: Optional[dict] = None,
@@ -411,10 +386,8 @@ def sharded_topk(queries: torch.Tensor, index: CorpusIndex, k: int, id_offset: i
     """Corpus sharded by page across ranks (every rank holds the same queries): local exact top-k with GLOBAL ids,
     one all-gather of [nq, k] (score, id) pairs over NCCL/NVLink, k-way merge on every rank (SURVEY.md §8e).
     doc_mask: this rank's bool [nd] mask of its own shard (see score_topk)."""
-    import torch.distributed as dist
-
     s, i = score_topk(queries, index, k, id_offset, stats=stats, doc_mask=doc_mask)
-    if not (dist.is_available() and dist.is_initialized()) or dist.get_world_size(group) == 1:
+    if _world(group) == 1:
         return s, i
     ev = _Stages(stats)
     gs, gi = gather_partials(s, i, group)
@@ -438,15 +411,10 @@ def sharded_topk_groups(queries: torch.Tensor, index: CorpusIndex, k: int, doc_g
         raise ValueError(f"sharded_topk_groups: world * k = {dist.get_world_size(group) * k} > {MERGE_GROUPS_MAX}")
 
     s, p, g = score_topk_groups(queries, index, k, doc_groups, id_offset, stats=stats, doc_mask=doc_mask)
-    if not (dist.is_available() and dist.is_initialized()) or dist.get_world_size(group) == 1:
+    if _world(group) == 1:
         return s, p, g
     ev = _Stages(stats)
-    world = dist.get_world_size(group)
-    nq = s.shape[0]
-    packed = torch.stack([s.contiguous().view(torch.int32).to(torch.int64), p, g], dim=-1).contiguous()
-    flat = torch.empty((world * nq, k, 3), dtype=torch.int64, device=packed.device)
-    dist.all_gather_into_tensor(flat, packed, group=group)
-    gathered = flat.view(world, nq, k, 3).permute(1, 0, 2, 3).reshape(nq, world * k, 3)
+    gathered = _all_gather_rows(torch.stack([s.contiguous().view(torch.int32).to(torch.int64), p, g], dim=-1), group)
     ev.mark("all_gather_partials")
     out = merge_topk_groups(gathered[..., 0].to(torch.int32).view(torch.float32), gathered[..., 1], gathered[..., 2], k)
     ev.mark("merge")
@@ -459,9 +427,9 @@ def gather_queries(local: torch.Tensor, n_total: int, group=None) -> torch.Tenso
     n_total embeddings in query order (10 k x 2304 fp32 = 92 MB: sub-millisecond over NVLink)."""
     import torch.distributed as dist
 
-    if not (dist.is_available() and dist.is_initialized()) or dist.get_world_size(group) == 1:
+    world = _world(group)
+    if world == 1:
         return local
-    world = dist.get_world_size(group)
     per = (n_total + world - 1) // world
     d = local.shape[1]
     block = torch.zeros((per, d), dtype=local.dtype, device=local.device)
