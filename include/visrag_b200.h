@@ -121,6 +121,11 @@ int vr_resample_u8(const uint8_t* src, int32_t src_pixel_bytes, int32_t n, int32
  * O accumulator all live in registers. Sequences longer than 64 queries: two consumer warpgroups (128 queries) per CTA
  * share one K/V stream; up to 64 queries per sequence: one warpgroup per CTA. Both forms (and vr_attention_force_v1)
  * give a sequence the same output bits: it does not depend on max_q, on the other sequences of the batch or on the form.
+ * Non-finite values: a NaN or inf in one sequence's Q, K or V never reaches another sequence's output. (A sequence's last
+ * 128-key tile is read from the packed rows and may hold the next sequence's rows; their scores are masked to -inf and
+ * their V rows are zeroed in shared memory before P V, so no p = 0 multiplies a foreign inf or NaN.) Within one causal
+ * sequence, a non-finite V at key j can reach earlier rows that share j's 128-key tile (their p_j = 0 times inf is NaN),
+ * as a masked softmax followed by a matmul gives; rows whose key tiles all end before j are unaffected.
  * Replaces F.scaled_dot_product_attention in timm/models/vision_transformer.py:92-96 (ViT,
  * 16 heads x 72, no mask), modeling_minicpm.py:895-903 (MiniCPM, causal + right padding ->
  * here: packed var-len sequences, no padding rows at all) and nn.MultiheadAttention in

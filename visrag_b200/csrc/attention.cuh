@@ -50,7 +50,7 @@ struct AttCfg {
     static constexpr int OFF_K = (Q_BYTES + 1023) & ~1023;
     static constexpr int OFF_V = OFF_K + ATT_STAGES * TILE_BYTES;
     static constexpr int OFF_BAR = OFF_V + ATT_STAGES * TILE_BYTES;
-    static constexpr int SMEM_BYTES = OFF_BAR + 128 + 1024;
+    static constexpr int SMEM_BYTES = OFF_BAR + 128 + 1024;  // 10 mbarriers of 8 B in the 128 at OFF_BAR
 };
 
 struct AttArgs {
@@ -163,6 +163,7 @@ attention_wgmma_kernel(const __grid_constant__ AttMaps maps, const AttArgs a) {
     uint64_t* k_empty = k_full + ATT_STAGES;
     uint64_t* v_full = k_empty + ATT_STAGES;
     uint64_t* v_empty = v_full + ATT_STAGES;
+    uint64_t* v_tail = v_empty + ATT_STAGES;       // TMA of a partial last V tile, before its rows past len_k are zeroed
 
     const int wg = threadIdx.x >> 7;
     const int warp = (threadIdx.x >> 5) & 3;
@@ -192,6 +193,7 @@ attention_wgmma_kernel(const __grid_constant__ AttMaps maps, const AttArgs a) {
             mbar_init(&k_empty[i], NWG * 4);  // one arrival per consumer warp
             mbar_init(&v_empty[i], NWG * 4);
         }
+        mbar_init(v_tail, 1);
         fence_mbar_init();
     }
     __syncthreads();
@@ -199,25 +201,50 @@ attention_wgmma_kernel(const __grid_constant__ AttMaps maps, const AttArgs a) {
     if (wg == 0 || wg > NWG) {
         // ---------------------------------------------------------------- TMA producer (warpgroup 0)
         setmaxnreg_dec<40>();
-        if (wg == 0 && warp == 0 && lane == 0) {
-            const int qcol = a.q_col0 + head * HS, kcol = a.k_col0 + head * HS, vcol = a.v_col0 + head * HS;
-            mbar_expect_tx(q_bar, Cfg::Q_BYTES);
+        if (wg == 0 && warp == 0) {
+            // Sequences are packed, so a last tile that ends past len_k holds the next sequence's K and V rows. Its K rows
+            // only give scores that the consumers replace by -inf, but P V would still multiply their p = 0 by those V
+            // rows, and 0 * inf or 0 * NaN is NaN. So the V rows [tail, 128) of that tile are zeroed before the
+            // consumers may read it: its TMA lands on v_tail, this warp clears the rows, and only then arrives on v_full.
+            const int tail = len_k - (nkt - 1) * ATT_BN;  // keys of the last loaded tile inside the sequence
+            const int st_last = (nkt - 1) % ATT_STAGES;
+            if (lane == 0) {
+                const int qcol = a.q_col0 + head * HS, kcol = a.k_col0 + head * HS, vcol = a.v_col0 + head * HS;
+                mbar_expect_tx(q_bar, Cfg::Q_BYTES);
 #pragma unroll
-            for (int c = 0; c < NCH; ++c) tma_load_2d(&maps.q64, q_bar, sQ + c * Cfg::Q_CHUNK, qcol + c * 64, q_begin + q0);
-            if (Cfg::HAS16) tma_load_2d(&maps.q16, q_bar, sQ + NCH * Cfg::Q_CHUNK, qcol + NCH * 64, q_begin + q0);
-            auto load_tile = [&](const CUtensorMap* m64, const CUtensorMap* m16, uint64_t* bar, uint8_t* dst, int col, int row) {
-                mbar_expect_tx(bar, Cfg::TILE_BYTES);
+                for (int c = 0; c < NCH; ++c) tma_load_2d(&maps.q64, q_bar, sQ + c * Cfg::Q_CHUNK, qcol + c * 64, q_begin + q0);
+                if (Cfg::HAS16) tma_load_2d(&maps.q16, q_bar, sQ + NCH * Cfg::Q_CHUNK, qcol + NCH * 64, q_begin + q0);
+                auto load_tile = [&](const CUtensorMap* m64, const CUtensorMap* m16, uint64_t* bar, uint8_t* dst, int col, int row) {
+                    mbar_expect_tx(bar, Cfg::TILE_BYTES);
 #pragma unroll
-                for (int c = 0; c < NCH; ++c) tma_load_2d(m64, bar, dst + c * 16384, col + c * 64, row);
-                if (Cfg::HAS16) tma_load_2d(m16, bar, dst + NCH * 16384, col + NCH * 64, row);
-            };
-            for (int kt = 0; kt < nkt; ++kt) {
-                const int st = kt % ATT_STAGES;
-                const uint32_t ph = (kt / ATT_STAGES) & 1;
-                mbar_wait(&k_empty[st], ph ^ 1);
-                load_tile(&maps.k64, &maps.k16, &k_full[st], sK + st * Cfg::TILE_BYTES, kcol, k_begin + kt * ATT_BN);
-                mbar_wait(&v_empty[st], ph ^ 1);
-                load_tile(&maps.v64, &maps.v16, &v_full[st], sV + st * Cfg::TILE_BYTES, vcol, k_begin + kt * ATT_BN);
+                    for (int c = 0; c < NCH; ++c) tma_load_2d(m64, bar, dst + c * 16384, col + c * 64, row);
+                    if (Cfg::HAS16) tma_load_2d(m16, bar, dst + NCH * 16384, col + NCH * 64, row);
+                };
+                for (int kt = 0; kt < nkt; ++kt) {
+                    const int st = kt % ATT_STAGES;
+                    const uint32_t ph = (kt / ATT_STAGES) & 1;
+                    mbar_wait(&k_empty[st], ph ^ 1);
+                    load_tile(&maps.k64, &maps.k16, &k_full[st], sK + st * Cfg::TILE_BYTES, kcol, k_begin + kt * ATT_BN);
+                    mbar_wait(&v_empty[st], ph ^ 1);
+                    load_tile(&maps.v64, &maps.v16, kt == nkt - 1 && tail < ATT_BN ? v_tail : &v_full[st],
+                              sV + st * Cfg::TILE_BYTES, vcol, k_begin + kt * ATT_BN);
+                }
+            }
+            __syncwarp();
+            if (tail < ATT_BN) {
+                // A key row is contiguous in both layouts (128 B in a 64-wide 128B-swizzled chunk, 32 B in the 16-wide
+                // 32B-swizzled one: the swizzles permute 16-byte units within a row), so rows [tail, 128) are one range.
+                uint8_t* dst = sV + st_last * Cfg::TILE_BYTES;
+                const uint4 zero = make_uint4(0u, 0u, 0u, 0u);
+                mbar_wait(v_tail, 0);
+#pragma unroll
+                for (int c = 0; c < NCH; ++c)
+                    for (int i = tail * 8 + lane; i < ATT_BN * 8; i += 32) reinterpret_cast<uint4*>(dst + c * 16384)[i] = zero;
+                if (Cfg::HAS16)
+                    for (int i = tail * 2 + lane; i < ATT_BN * 2; i += 32) reinterpret_cast<uint4*>(dst + NCH * 16384)[i] = zero;
+                fence_proxy_async_smem();  // the generic-proxy stores, before the consumers' wgmma reads them
+                __syncwarp();
+                if (lane == 0) mbar_arrive(&v_full[st_last]);
             }
         }
         return;
