@@ -14,7 +14,11 @@
  *    synchronisation, so every call is CUDA-graph capturable;
  *  - return value: 0 on success, non-zero on error; vr_last_error() returns a
  *    thread-local message; nothing throws or exits across the ABI;
- *  - row-major matrices; "ld*" = leading dimension in ELEMENTS.
+ *  - row-major matrices; "ld*" = leading dimension in ELEMENTS;
+ *  - "Alignment (bytes) of <entry point>: <pointer> <n>, ..." lines give the base alignment each pointer needs: the
+ *    widest vector access the kernels make to it (with the ld / dim rules of each call, every row is then aligned too).
+ *    A pointer below its alignment is refused (return 2, the message names it) before any CUDA call; NULL optional
+ *    pointers are exempt.
  */
 #ifndef VISRAG_B200_H
 #define VISRAG_B200_H
@@ -47,6 +51,7 @@ int vr_abi_version(void);
  *   GELU writes the operands' 16-bit type only. Any other combination is refused before any CUDA call.
  * An fp16 output rounds to nearest with no clamp: a value beyond 65504 is stored as inf.
  * A LINEAR out must be 16-byte aligned (refused before any CUDA call otherwise); with ldo % 8 == 0 every row then is.
+ * Alignment (bytes) of vr_gemm: A 16, B 16, bias 8, rowadd 8, resid 8, rope_cos 8, rope_sin 8, positions 4, out 16 (LINEAR), out 4 (ROPE, SWIGLU)
  * ---------------------------------------------------------------------------------- */
 typedef enum {
     VR_EPI_LINEAR = 0, /* out = [resid +] scale*(gelu?(acc + bias)) [+ rowadd[row % period]] */
@@ -132,6 +137,7 @@ int vr_resample_u8(const uint8_t* src, int32_t src_pixel_bytes, int32_t n, int32
  * resampler.py:159-163 (64 learned queries x N keys, 18 heads x 128).
  * q/k/v are bf16 (or, with VR_ATTN_F16, fp16) row-major token matrices; head h starts at column *_col0 + h*head_stride
  * (head_stride = head_dim rounded up to a multiple of 16; pad columns must hold zeros).
+ * Alignment (bytes) of vr_attention: q 16, k 16, v 16, cu_q 4, cu_k 4, out 4
  * Causal with fewer query rows than key rows (len_q < len_k, e.g. a sequence whose first len_k - len_q rows come from a
  * prefix cache): the query rows are the LAST len_q rows of the sequence. Query i of sequence b attends keys
  * j <= i + (len_k - len_q), and its output row has the same bits as row len_k - len_q + i of the full causal run over the
@@ -181,7 +187,8 @@ void vr_attention_force_v1(int32_t variant);
  * column c*patch*patch + ky*patch + kx (the Conv2d weight's flattening); columns [3*patch^2, ldo) are zeroed.
  * bf16(fma(u, 2/255, -1)) - bit-identical to bf16((u/255 - 0.5)/0.5) for all 256 byte values. patch <= 85, any w: a strip of
  * `patch` pixel rows that does not fit 200 KB of shared memory (patch 14, ldo 640: w of 4858 and more) is converted in chunks of
- * patch columns, with the same bits. Returns 2 if ldo is so large that its offset table leaves no room for one patch. */
+ * patch columns, with the same bits. Returns 2 if ldo is so large that its offset table leaves no room for one patch.
+ * Alignment (bytes) of vr_im2col_norm: out 16 */
 int vr_im2col_norm(const uint8_t* pixels, int32_t n_slices, int32_t h, int32_t w, int32_t patch, void* out, int64_t ldo,
                    void* stream);
 /* The same with the output type chosen: out_dtype = VR_BF16 (what vr_im2col_norm writes) or VR_F16, where
@@ -190,7 +197,8 @@ int vr_im2col_norm_ex(const uint8_t* pixels, int32_t n_slices, int32_t h, int32_
                       int32_t out_dtype, void* stream);
 
 /* LayerNorm over the last dim (timm vision_transformer.py:142,155,525; resampler.py:155,166): fp32 in -> bf16 out.
- * If out2 != NULL also writes out2 = LN(x) + add[row % add_period] (bf16) — the resampler's K input (kv + pos). */
+ * If out2 != NULL also writes out2 = LN(x) + add[row % add_period] (bf16) — the resampler's K input (kv + pos).
+ * Alignment (bytes) of vr_layernorm: x 16, gamma 16, beta 16, add 16, out 8, out2 8 */
 int vr_layernorm(const float* x, int64_t ldx, const float* gamma, const float* beta, float eps, int32_t rows, int32_t dim,
                  void* out, int64_t ldo, void* out2, const float* add, int32_t add_period, void* stream);
 /* vr_layernorm with out and out2 written as out_dtype = VR_BF16 (vr_layernorm) or VR_F16; mean, variance and the add of
@@ -198,7 +206,8 @@ int vr_layernorm(const float* x, int64_t ldx, const float* gamma, const float* b
 int vr_layernorm_ex(const float* x, int64_t ldx, const float* gamma, const float* beta, float eps, int32_t rows, int32_t dim,
                     void* out, int64_t ldo, void* out2, const float* add, int32_t add_period, int32_t out_dtype, void* stream);
 
-/* RMSNorm (modeling_minicpm.py:119-123): fp32 in -> bf16 out. */
+/* RMSNorm (modeling_minicpm.py:119-123): fp32 in -> bf16 out.
+ * Alignment (bytes) of vr_rmsnorm: x 16, gamma 16, out 8 */
 int vr_rmsnorm(const float* x, int64_t ldx, const float* gamma, float eps, int32_t rows, int32_t dim, void* out, int64_t ldo,
                void* stream);
 /* vr_rmsnorm with out written as out_dtype = VR_BF16 (vr_rmsnorm) or VR_F16; statistics in fp32. */
@@ -208,7 +217,8 @@ int vr_rmsnorm_ex(const float* x, int64_t ldx, const float* gamma, float eps, in
 /* LM input assembly (modeling_minicpmv.py:139-166): for packed token t,
  *   src[t] >= 0 : h[t] = vision[src[t]]            (resampler output row, fp32)
  *   src[t] <  0 : h[t] = embed[-(src[t]+1)] * scale_emb   (bf16 table)
- * h: [tokens, dim] fp32. */
+ * h: [tokens, dim] fp32.
+ * Alignment (bytes) of vr_build_lm_input: src 4, embed 8, vision 16, h 16 */
 int vr_build_lm_input(const int32_t* src, int32_t tokens, int32_t dim, const void* embed_bf16, float scale_emb,
                       const float* vision, int64_t ldv, float* h, int64_t ldh, void* stream);
 /* vr_build_lm_input with the embedding table's type given: embed_dtype = VR_BF16 (vr_build_lm_input) or VR_F16. Either is
@@ -221,7 +231,8 @@ int vr_build_lm_input_ex(const int32_t* src, int32_t tokens, int32_t dim, const 
  * pooling: 0 wmean (w_t = t+1), 1 mean, 2 lasttoken, 3 cls. normalise: x / max(||x||, 1e-12).
  * One thread-block cluster of 8 (or 4) CTAs per sequence, every row read once; h, gamma and reps 16-byte aligned; any
  * sequence length (no per-length shared memory), dim <= 4096. A sequence's sums run in one fixed order whatever the
- * cluster size, so its output bits do not depend on the batch size or on the other sequences of the batch. */
+ * cluster size, so its output bits do not depend on the batch size or on the other sequences of the batch.
+ * Alignment (bytes) of vr_pool_norm: h 16, gamma 16, cu 4, reps 16 */
 int vr_pool_norm(const float* h, int64_t ldh, const float* gamma, float eps, const int32_t* cu, int32_t batch, int32_t dim,
                  int32_t pooling, int32_t normalize, float* reps, void* stream);
 
@@ -231,7 +242,8 @@ int vr_pool_norm(const float* h, int64_t ldh, const float* gamma, float eps, con
  * so cu_out[b+1] - cu_out[b] = prefix_len + cu_rows[b+1] - cu_rows[b], and out_rows = cu_out[batch]. Each row copies
  * `cols` elements of elem_size bytes (2: the 16-bit K|V block of a qkv row; 4: the fp32 residual stream) from column 0
  * of the given pointers; prefix, rows and out must be 16-byte aligned and cols * elem_size and every ld * elem_size
- * multiples of 16 (refused before any CUDA call otherwise). prefix may be NULL when prefix_len = 0. */
+ * multiples of 16 (refused before any CUDA call otherwise). prefix may be NULL when prefix_len = 0.
+ * Alignment (bytes) of vr_prefix_rows: prefix 16, rows 16, out 16, cu_rows 4, cu_out 4 */
 int vr_prefix_rows(const void* prefix, int64_t ldp, const void* rows, int64_t ldr, void* out, int64_t ldo,
                    const int32_t* cu_rows, const int32_t* cu_out, int32_t batch, int32_t prefix_len, int32_t out_rows,
                    int32_t cols, int32_t elem_size, void* stream);
@@ -250,6 +262,10 @@ int vr_prefix_rows(const void* prefix, int64_t ldp, const void* rows, int64_t ld
  *                      the top-k (flags[q] = 1 when the proof fails; the caller then reruns that query through
  *                      vr_score_exact + vr_topk_rows).
  * Results are therefore exactly the fp32 top-k. Doc ids returned are `local index + id_offset`.
+ * Alignment (bytes) of vr_f32_to_f16_rows: src 16, dst_f16 8
+ * Alignment (bytes) of vr_score_filter: q_f16 16, d_f16 16, cand_scores 16, cand_ids 16
+ * Alignment (bytes) of vr_score_rescore: d_f32 16
+ * Alignment (bytes) of vr_score_exact: d_f32 16
  * ---------------------------------------------------------------------------------- */
 int vr_score_ranges(int32_t nq, int64_t nd);   /* sizes the candidate buffers: [nq, ranges*2*16]; host arithmetic only (needs no
                                                 * GPU); pass the value on to vr_score_filter / vr_score_rescore unchanged */
@@ -285,6 +301,7 @@ int vr_topk_rows_chunked(const float* scores, int32_t rows, int64_t cols, int32_
  * When fewer than k docs are eligible, a row holds the eligible ones in order and then (-inf, -1), as for k > nd.
  * A NULL or misaligned doc_mask, and ids != NULL together with a mask (the mask indexes columns), are refused before
  * any CUDA call.
+ * Alignment (bytes) of vr_score_filter_masked: q_f16 16, d_f16 16, cand_scores 16, cand_ids 16, doc_mask 4
  *   vr_score_filter_masked : vr_score_filter over the eligible docs; the candidate lists hold eligible docs only, so
  *                            vr_score_rescore takes them unchanged and its proof covers the eligible docs;
  *   vr_topk_rows_masked    : vr_topk_rows with ids == NULL and columns (docs) filtered by doc_mask;
@@ -306,6 +323,8 @@ int vr_topk_rows_chunked_masked(const float* scores, int32_t rows, int64_t cols,
  * fewer than k groups leave a tail of (-inf, -1, -1). With every page its own group the result equals the page top-k.
  * doc_mask (optional, NULL: every page eligible) has the layout of the _masked calls. A NULL or misaligned doc_groups or
  * CSR array, G <= 0, a workspace too small and nd >= 2^31 are refused before any CUDA call.
+ * Alignment (bytes) of vr_score_filter_groups: q_f16 16, d_f16 16, cand_scores 16, cand_ids 16, doc_groups 4, doc_mask 4
+ * Alignment (bytes) of vr_score_rescore_groups: d_f32 16, doc_groups 4, group_offsets 4, group_pages 4, doc_mask 4
  *   vr_score_filter_groups  : vr_score_filter with GROUP-DISTINCT lists: a list holds at most one page per group (a page
  *                             of a group already listed replaces that entry only when its score is higher). Every page a
  *                             list dropped is <= that list's tail or <= its own group's entry in that list;

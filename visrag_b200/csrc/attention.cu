@@ -64,7 +64,15 @@ extern "C" int vr_attention(const vr_attn_params* p, void* stream) {
                p->head_dim, p->head_stride);
     VR_REQUIRE(p->ldo % 8 == 0, "vr_attention: ldo must be a multiple of 8");
     VR_REQUIRE(!(p->flags & VR_ATTN_V_ONES_COLUMN) || p->head_dim == p->head_stride - 8,
-               "vr_attention: VR_ATTN_V_ONES_COLUMN needs head_dim == head_stride - 8 (got %d / %d)", p->head_dim, p->head_stride);    cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
+               "vr_attention: VR_ATTN_V_ONES_COLUMN needs head_dim == head_stride - 8 (got %d / %d)", p->head_dim, p->head_stride);
+    // q / k / v are TMA sources; the kernels read cu_q / cu_k as int32 and store out as 16-bit pairs
+    VR_REQUIRE_ALIGNED("vr_attention", "q", p->q, 16);
+    VR_REQUIRE_ALIGNED("vr_attention", "k", p->k, 16);
+    VR_REQUIRE_ALIGNED("vr_attention", "v", p->v, 16);
+    VR_REQUIRE_ALIGNED("vr_attention", "cu_q", p->cu_q, 4);
+    VR_REQUIRE_ALIGNED("vr_attention", "cu_k", p->cu_k, 4);
+    VR_REQUIRE_ALIGNED("vr_attention", "out", p->out, 4);
+    cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
     switch (p->head_stride) {
         case 64: return dispatch_attention<64>(*p, s);
         case 80: return dispatch_attention<80>(*p, s);

@@ -39,4 +39,12 @@ int make_tmap_2d(CUtensorMap* out, const void* base, uint64_t rows, uint64_t col
         }                              \
     } while (0)
 
+// Base alignment of a pointer the kernels read or write with `bytes`-wide vector accesses (NULL passes: optional pointers
+// are checked for presence elsewhere). A misaligned base is refused before any CUDA call, naming the argument; launched,
+// it would be a misaligned-address fault that ends the CUDA context.
+inline bool is_aligned(const void* p, unsigned bytes) { return (reinterpret_cast<uintptr_t>(p) & (bytes - 1)) == 0; }
+#define VR_REQUIRE_ALIGNED(fn, name, ptr, bytes)                                                                         \
+    VR_REQUIRE(vr::is_aligned((ptr), (bytes)), "%s: %s must be %d-byte aligned (got %p)", fn, name, (int)(bytes), \
+               (const void*)(ptr))
+
 }  // namespace vr

@@ -580,6 +580,8 @@ extern "C" int vr_im2col_norm_ex(const uint8_t* pixels, int32_t n_slices, int32_
                (long long)ldo, 3 * patch * patch);
     VR_REQUIRE(patch <= 85, "vr_im2col_norm: patch=%d exceeds 85", patch);
     VR_REQUIRE(out_dtype == VR_BF16 || out_dtype == VR_F16, "vr_im2col_norm: out_dtype must be VR_BF16 or VR_F16 (got %d)", out_dtype);
+    // every path stores 8 output columns (16 bytes) at a time; the pixel loads pick their width from the alignment
+    VR_REQUIRE_ALIGNED("vr_im2col_norm", "out", out, 16);
     cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
     return out_dtype == VR_F16 ? im2col_norm_impl<true>(pixels, n_slices, h, w, patch, out, ldo, st)
                                : im2col_norm_impl<false>(pixels, n_slices, h, w, patch, out, ldo, st);
@@ -598,6 +600,13 @@ extern "C" int vr_layernorm_ex(const float* x, int64_t ldx, const float* gamma, 
                rows, dim);
     VR_REQUIRE(!out2 || (add && add_period > 0), "vr_layernorm: out2 needs add/add_period");
     VR_REQUIRE(out_dtype == VR_BF16 || out_dtype == VR_F16, "vr_layernorm: out_dtype must be VR_BF16 or VR_F16 (got %d)", out_dtype);
+    // float4 loads of x, gamma, beta and add; 8-byte stores of out and out2
+    VR_REQUIRE_ALIGNED("vr_layernorm", "x", x, 16);
+    VR_REQUIRE_ALIGNED("vr_layernorm", "gamma", gamma, 16);
+    VR_REQUIRE_ALIGNED("vr_layernorm", "beta", beta, 16);
+    VR_REQUIRE_ALIGNED("vr_layernorm", "add", add, 16);
+    VR_REQUIRE_ALIGNED("vr_layernorm", "out", out, 8);
+    VR_REQUIRE_ALIGNED("vr_layernorm", "out2", out2, 8);
     cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
     return out_dtype == VR_F16 ? norm_impl<false, true>(x, ldx, gamma, beta, eps, rows, dim, out, ldo, out2, add, add_period, s)
                                : norm_impl<false, false>(x, ldx, gamma, beta, eps, rows, dim, out, ldo, out2, add, add_period, s);
@@ -615,6 +624,9 @@ extern "C" int vr_rmsnorm_ex(const float* x, int64_t ldx, const float* gamma, fl
     VR_REQUIRE(rows > 0 && dim > 0 && dim % 4 == 0 && ldx % 4 == 0 && ldo % 4 == 0, "vr_rmsnorm: bad shape rows=%d dim=%d",
                rows, dim);
     VR_REQUIRE(out_dtype == VR_BF16 || out_dtype == VR_F16, "vr_rmsnorm: out_dtype must be VR_BF16 or VR_F16 (got %d)", out_dtype);
+    VR_REQUIRE_ALIGNED("vr_rmsnorm", "x", x, 16);
+    VR_REQUIRE_ALIGNED("vr_rmsnorm", "gamma", gamma, 16);
+    VR_REQUIRE_ALIGNED("vr_rmsnorm", "out", out, 8);
     cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
     return out_dtype == VR_F16 ? norm_impl<true, true>(x, ldx, gamma, nullptr, eps, rows, dim, out, ldo, nullptr, nullptr, 1, s)
                                : norm_impl<true, false>(x, ldx, gamma, nullptr, eps, rows, dim, out, ldo, nullptr, nullptr, 1, s);
@@ -632,6 +644,11 @@ extern "C" int vr_build_lm_input_ex(const int32_t* src, int32_t tokens, int32_t 
                "vr_build_lm_input: bad shape tokens=%d dim=%d", tokens, dim);
     VR_REQUIRE(embed_dtype == VR_BF16 || embed_dtype == VR_F16, "vr_build_lm_input: embed_dtype must be VR_BF16 or VR_F16 (got %d)",
                embed_dtype);
+    // int32 loads of src, 8-byte loads of embed rows (dim % 4 == 0 keeps every row aligned), float4 copies of vision and h
+    VR_REQUIRE_ALIGNED("vr_build_lm_input", "src", src, 4);
+    VR_REQUIRE_ALIGNED("vr_build_lm_input", "embed", embed, 8);
+    VR_REQUIRE_ALIGNED("vr_build_lm_input", "vision", vision, 16);
+    VR_REQUIRE_ALIGNED("vr_build_lm_input", "h", h, 16);
     cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
     if (embed_dtype == VR_F16)
         build_lm_input_kernel<true><<<grid_for(tokens, 8), 256, 0, s>>>(src, tokens, dim, reinterpret_cast<const __half*>(embed),
@@ -657,6 +674,7 @@ extern "C" int vr_pool_norm(const float* h, int64_t ldh, const float* gamma, flo
     VR_REQUIRE((reinterpret_cast<uintptr_t>(h) & 15) == 0 && (reinterpret_cast<uintptr_t>(reps) & 15) == 0 &&
                    (reinterpret_cast<uintptr_t>(gamma) & 15) == 0,
                "vr_pool_norm: h, gamma and reps must be 16-byte aligned");
+    VR_REQUIRE_ALIGNED("vr_pool_norm", "cu", cu, 4);
     cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
     // 8 CTAs per sequence while all clusters fit on the GPU at once (5 CTAs per SM), else 4: one wave of longer CTAs beats
     // a second wave of whole clusters (the kernel is a latency chain: load rows -> CTA sum -> cluster sum -> normalise).

@@ -169,6 +169,17 @@ extern "C" int vr_gemm_tuned(const void* A, int64_t lda, const void* B, int64_t 
     // the ping-pong kernel stores a 16-bit LINEAR output 16 bytes at a time (ldo % 8 == 0 keeps every row aligned)
     VR_REQUIRE(epi->mode != VR_EPI_LINEAR || (reinterpret_cast<uintptr_t>(epi->out) & 15) == 0,
                "vr_gemm: a LINEAR out must be 16-byte aligned (out=%p)", epi->out);
+    // the other bases, at the width of their widest access: A / B are TMA sources; the epilogues read bias, rowadd, resid
+    // and the RoPE tables as float2 and positions as int32, and ROPE / SWIGLU store 16-bit pairs
+    VR_REQUIRE_ALIGNED("vr_gemm", "A", A, 16);
+    VR_REQUIRE_ALIGNED("vr_gemm", "B", B, 16);
+    VR_REQUIRE_ALIGNED("vr_gemm", "bias", epi->bias, 8);
+    VR_REQUIRE_ALIGNED("vr_gemm", "rowadd", epi->rowadd, 8);
+    VR_REQUIRE_ALIGNED("vr_gemm", "resid", epi->resid, 8);
+    VR_REQUIRE_ALIGNED("vr_gemm", "rope_cos", epi->rope_cos, 8);
+    VR_REQUIRE_ALIGNED("vr_gemm", "rope_sin", epi->rope_sin, 8);
+    VR_REQUIRE_ALIGNED("vr_gemm", "positions", epi->positions, 4);
+    VR_REQUIRE_ALIGNED("vr_gemm", "out", epi->out, 4);
     GemmArgs g;
     g.M = M; g.N = N; g.K = K; g.epi = *epi;
     cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);

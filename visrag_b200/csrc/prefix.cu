@@ -60,6 +60,8 @@ extern "C" int vr_prefix_rows(const void* prefix, int64_t ldp, const void* rows,
                "%d-byte elements)", cols, (long long)ldp, (long long)ldr, (long long)ldo, elem_size);
     VR_REQUIRE(((reinterpret_cast<uintptr_t>(prefix) | reinterpret_cast<uintptr_t>(rows) | reinterpret_cast<uintptr_t>(out)) & 15) == 0,
                "vr_prefix_rows: prefix, rows and out must be 16-byte aligned");
+    VR_REQUIRE_ALIGNED("vr_prefix_rows", "cu_rows", cu_rows, 4);
+    VR_REQUIRE_ALIGNED("vr_prefix_rows", "cu_out", cu_out, 4);
     const int per = elem_size == 2 ? 8 : 4;  // elements per 16-byte vector
     const int vecs = static_cast<int>(row_bytes / 16);
     const int chunks = (vecs + PREFIX_CHUNK - 1) / PREFIX_CHUNK;

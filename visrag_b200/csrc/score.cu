@@ -1146,6 +1146,11 @@ static int score_filter(const void* q_f16, int nq, const void* d_f16, long long 
     VR_REQUIRE(nq < (1 << 30), "vr_score_filter: too many queries");
     const ScorePlan plan = score_plan(nq, nd);
     VR_REQUIRE(ranges * 2 == plan.lists, "vr_score_filter: ranges must come from vr_score_ranges()");
+    // q / d are TMA sources; the candidate lists are written 16 bytes at a time
+    VR_REQUIRE_ALIGNED("vr_score_filter", "q_f16", q_f16, 16);
+    VR_REQUIRE_ALIGNED("vr_score_filter", "d_f16", d_f16, 16);
+    VR_REQUIRE_ALIGNED("vr_score_filter", "cand_scores", cand_scores, 16);
+    VR_REQUIRE_ALIGNED("vr_score_filter", "cand_ids", cand_ids, 16);
     cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
     if (doc_mask)
         return launch_score_filter<MaskedScoreArgs>(plan, q_f16, nq, d_f16, nd, dim, cand_scores, cand_ids, doc_mask, nullptr, st);
@@ -1215,6 +1220,8 @@ extern "C" int vr_f32_to_f16_rows(const float* src, int64_t rows, int32_t dim, v
                                   void* stream) {
     VR_REQUIRE(src && dst_f16, "vr_f32_to_f16_rows: null pointer");
     VR_REQUIRE(rows > 0 && dim > 0 && dim % 4 == 0, "vr_f32_to_f16_rows: bad shape rows=%lld dim=%d", (long long)rows, dim);
+    VR_REQUIRE_ALIGNED("vr_f32_to_f16_rows", "src", src, 16);  // float4 loads, 8-byte stores
+    VR_REQUIRE_ALIGNED("vr_f32_to_f16_rows", "dst_f16", dst_f16, 8);
     long long blocks = (rows + 7) / 8;
     const long long cap = static_cast<long long>(num_sms()) * 16;
     if (blocks > cap) blocks = cap;
@@ -1242,6 +1249,7 @@ extern "C" int vr_score_rescore(const float* q_f32, int32_t nq, const float* d_f
     VR_REQUIRE(q_f32 && d_f32 && cand_scores && cand_ids && max_doc_norm && out_scores && out_ids && flags,
                "vr_score_rescore: null pointer");
     VR_REQUIRE(nq > 0 && k > 0 && dim % 4 == 0, "vr_score_rescore: bad shape");
+    VR_REQUIRE_ALIGNED("vr_score_rescore", "d_f32", d_f32, 16);  // float4 rows (dim % 4 == 0 keeps every row aligned)
     const int lists = ranges * 2;
     VR_REQUIRE(ranges > 0 && lists <= SC_MAX_RANGES + 2, "vr_score_rescore: ranges must come from vr_score_ranges()");
     const int keep = rescore_keep(k, lists);
@@ -1261,6 +1269,7 @@ extern "C" int vr_score_exact(const float* q_f32, int32_t nq, const float* d_f32
                               void* stream) {
     VR_REQUIRE(q_f32 && d_f32 && scores, "vr_score_exact: null pointer");
     VR_REQUIRE(nq > 0 && nd > 0 && dim % 4 == 0, "vr_score_exact: bad shape");
+    VR_REQUIRE_ALIGNED("vr_score_exact", "d_f32", d_f32, 16);
     const int NQ = nq >= EX_QB ? EX_QB : (nq >= 4 ? 4 : (nq >= 2 ? 2 : 1));
     const size_t smem = static_cast<size_t>(NQ) * dim * sizeof(float);
     VR_REQUIRE(smem <= 200 * 1024, "vr_score_exact: dim too large");
@@ -1335,6 +1344,10 @@ extern "C" int vr_score_filter_groups(const void* q_f16, int32_t nq, const void*
     VR_REQUIRE(nq > 0 && nq < (1 << 30) && dim % 8 == 0, "vr_score_filter_groups: bad shape");
     const ScorePlan plan = score_plan(nq, nd);
     VR_REQUIRE(ranges * 2 == plan.lists, "vr_score_filter_groups: ranges must come from vr_score_ranges()");
+    VR_REQUIRE_ALIGNED("vr_score_filter_groups", "q_f16", q_f16, 16);
+    VR_REQUIRE_ALIGNED("vr_score_filter_groups", "d_f16", d_f16, 16);
+    VR_REQUIRE_ALIGNED("vr_score_filter_groups", "cand_scores", cand_scores, 16);
+    VR_REQUIRE_ALIGNED("vr_score_filter_groups", "cand_ids", cand_ids, 16);
     cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
     if (doc_mask)
         return launch_score_filter<MaskedGroupedScoreArgs>(plan, q_f16, nq, d_f16, nd, dim, cand_scores, cand_ids, doc_mask,
@@ -1356,6 +1369,7 @@ extern "C" int vr_score_rescore_groups(const float* q_f32, int32_t nq, const flo
     VR_REQUIRE(q_f32 && d_f32 && cand_scores && cand_ids && max_doc_norm && out_scores && out_pages && out_groups && flags,
                "vr_score_rescore_groups: null pointer");
     VR_REQUIRE(nq > 0 && k > 0 && dim % 4 == 0, "vr_score_rescore_groups: bad shape");
+    VR_REQUIRE_ALIGNED("vr_score_rescore_groups", "d_f32", d_f32, 16);
     const int lists = ranges * 2;
     VR_REQUIRE(ranges > 0 && lists <= SC_MAX_RANGES + 2, "vr_score_rescore_groups: ranges must come from vr_score_ranges()");
     const int keep = rescore_keep(k, lists);

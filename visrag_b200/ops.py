@@ -66,6 +66,32 @@ def _half_operands(**named: torch.Tensor) -> torch.dtype:
     return dtype
 
 
+def _operand(fn: str, name: str, t: torch.Tensor, dtypes, shape, align: int, like: torch.Tensor,
+             contiguous: bool = False) -> None:
+    """Refuse, naming the argument, a tensor the kernels cannot read as given: a dtype not in `dtypes`, a shape other than
+    `shape` (None: any size), a non-unit inner stride (or, with `contiguous`, any gap: the kernels index it with its
+    logical width), a base address that is not a multiple of `align` bytes (the widest vector access the kernels make to
+    it), or a device other than `like`'s. Every check runs before anything reaches the library."""
+    if t.dtype not in dtypes:
+        want = " or ".join(str(d).replace("torch.", "") for d in dtypes)
+        raise ValueError(f"{fn}: {name} must be {want}, got {t.dtype}")
+    if t.dim() != len(shape) or any(n is not None and n != m for n, m in zip(shape, t.shape)):
+        want = "[" + ", ".join("*" if n is None else str(n) for n in shape) + "]"
+        raise ValueError(f"{fn}: {name} must have shape {want}, got {tuple(t.shape)}")
+    if contiguous and not t.is_contiguous() or not contiguous and t.dim() and t.shape[-1] > 1 and t.stride(-1) != 1:
+        raise ValueError(f"{fn}: {name} must be {'contiguous' if contiguous else 'unit-stride in its last dimension'}, "
+                         f"got strides {t.stride()}")
+    if not t.is_cuda:
+        raise ValueError(f"{fn}: {name} must be a CUDA tensor, got one on {t.device}")
+    if t.device != like.device:
+        raise ValueError(f"{fn}: {name} is on {t.device} but the operands are on {like.device}")
+    if t.data_ptr() % align:
+        raise ValueError(f"{fn}: {name} must be {align}-byte aligned (its storage offset is {t.storage_offset()} elements)")
+
+
+_F32, _I32 = (torch.float32,), (torch.int32,)
+
+
 def _half_dtype(dtype: torch.dtype, name: str) -> int:
     if dtype not in HALF_DTYPES:
         raise ValueError(f"{name}: the 16-bit output type must be bf16 or fp16, got {dtype}")
@@ -105,15 +131,26 @@ def gemm(
         out_dtype = a.dtype
     if out_dtype not in (a.dtype, torch.float32):
         raise ValueError(f"gemm: {a.dtype} operands write {a.dtype} or float32, not {out_dtype}")
+    # A and W are TMA sources (16-byte bases); the epilogue reads bias, rowadd, resid and the RoPE tables as float2 and
+    # positions as int32; a LINEAR out takes 16-byte stores, ROPE / SWIGLU outputs 4-byte ones (include/visrag_b200.h)
+    _operand("gemm", "a", a, HALF_DTYPES, (M, K), 16, a)
+    _operand("gemm", "w", w, HALF_DTYPES, (N, K), 16, a)
     if out is None:
         out = torch.empty((M, out_cols), dtype=out_dtype, device=a.device)
-    if out.dtype != out_dtype or out.shape != (M, out_cols) or out.stride(1) != 1:
-        raise ValueError("gemm: bad `out`")
-    for t, n in ((bias, "bias"), (resid, "resid"), (rowadd, "rowadd"), (rope_cos, "rope_cos"), (rope_sin, "rope_sin")):
-        if t is not None and (t.dtype != torch.float32 or not t.is_contiguous() and n != "resid"):
-            raise ValueError(f"gemm: {n} must be contiguous fp32")
-    if resid is not None and (resid.shape != out.shape or resid.stride(0) != out.stride(0)):
-        raise ValueError("gemm: resid must match out (shape and row pitch)")
+    _operand("gemm", "out", out, (out_dtype,), (M, out_cols), 16 if mode == L.VR_EPI_LINEAR else 4, a)
+    if bias is not None:
+        _operand("gemm", "bias", bias, _F32, (N,), 8, a, contiguous=True)
+    if rowadd is not None:
+        _operand("gemm", "rowadd", rowadd, _F32, (None, N), 8, a, contiguous=True)
+    if resid is not None:
+        _operand("gemm", "resid", resid, _F32, (M, out_cols), 8, a)
+        if resid.stride(0) != out.stride(0):
+            raise ValueError("gemm: resid must have out's row pitch")
+    if positions is not None:
+        _operand("gemm", "positions", positions, _I32, (M,), 4, a, contiguous=True)
+    for t, n in ((rope_cos, "rope_cos"), (rope_sin, "rope_sin")):
+        if t is not None:
+            _operand("gemm", n, t, _F32, (None, 32), 8, a, contiguous=True)
     e = L.GemmEpilogue()
     e.mode = mode
     e.out_dtype = _VR_DTYPE[out_dtype]
@@ -145,8 +182,12 @@ def attention(
     """softmax(QK^T*scale)V on wgmma; q/k/v/out are bf16 or fp16 token matrices, all of one type (see
     include/visrag_b200.h)."""
     _half_operands(q=q, k=k, v=v, out=out)
-    if cu_k.dtype != torch.int32 or (cu_q is not None and cu_q.dtype != torch.int32):
-        raise ValueError("attention: cu_seqlens must be int32")
+    for name, t in (("q", q), ("k", k), ("v", v)):  # TMA sources
+        _operand("attention", name, t, HALF_DTYPES, (None, None), 16, q)
+    _operand("attention", "out", out, HALF_DTYPES, (None, None), 4, q)
+    _operand("attention", "cu_k", cu_k, _I32, (batch + 1,), 4, q, contiguous=True)
+    if cu_q is not None:
+        _operand("attention", "cu_q", cu_q, _I32, (batch + 1,), 4, q, contiguous=True)
     p = L.AttnParams()
     p.q, p.ldq, p.q_rows = q.data_ptr(), q.stride(0), q.shape[0]
     p.k, p.ldk = k.data_ptr(), k.stride(0)
@@ -179,7 +220,12 @@ def layernorm(x: torch.Tensor, gamma: torch.Tensor, beta: torch.Tensor, eps: flo
               dtype: torch.dtype = torch.bfloat16):
     """fp32 [M,D] -> LN(x) in `dtype` (bf16 or fp16); with ``add`` [P,D] also returns LN(x)+add[row % P] (same dtype)."""
     vr_dtype = _half_dtype(dtype, "layernorm")
+    _operand("layernorm", "x", x, _F32, (None, None), 16, x)
     M, D = x.shape
+    _operand("layernorm", "gamma", gamma, _F32, (D,), 16, x, contiguous=True)
+    _operand("layernorm", "beta", beta, _F32, (D,), 16, x, contiguous=True)
+    if add is not None:
+        _operand("layernorm", "add", add, _F32, (None, D), 16, x, contiguous=True)
     L.check_device(x)
     out = torch.empty((M, D), dtype=dtype, device=x.device)
     out2 = torch.empty_like(out) if add is not None else None
@@ -191,7 +237,9 @@ def layernorm(x: torch.Tensor, gamma: torch.Tensor, beta: torch.Tensor, eps: flo
 def rmsnorm(x: torch.Tensor, gamma: torch.Tensor, eps: float, dtype: torch.dtype = torch.bfloat16) -> torch.Tensor:
     """fp32 [M,D] -> RMSNorm(x) in `dtype` (bf16 or fp16)."""
     vr_dtype = _half_dtype(dtype, "rmsnorm")
+    _operand("rmsnorm", "x", x, _F32, (None, None), 16, x)
     M, D = x.shape
+    _operand("rmsnorm", "gamma", gamma, _F32, (D,), 16, x, contiguous=True)
     L.check_device(x)
     out = torch.empty((M, D), dtype=dtype, device=x.device)
     _launch("norm", 0.0, L.lib().vr_rmsnorm_ex, x.data_ptr(), x.stride(0), gamma.data_ptr(), eps, M, D, out.data_ptr(),
@@ -202,7 +250,11 @@ def rmsnorm(x: torch.Tensor, gamma: torch.Tensor, eps: float, dtype: torch.dtype
 def build_lm_input(src: torch.Tensor, embed: torch.Tensor, scale_emb: float, vision: Optional[torch.Tensor]) -> torch.Tensor:
     """Packed LM input rows (fp32) from the vision rows and a bf16 or fp16 embedding table."""
     vr_dtype = _half_dtype(embed.dtype, "build_lm_input")
+    _operand("build_lm_input", "embed", embed, HALF_DTYPES, (None, None), 8, embed, contiguous=True)
     T, D = src.shape[0], embed.shape[1]
+    _operand("build_lm_input", "src", src, _I32, (T,), 4, embed, contiguous=True)
+    if vision is not None:
+        _operand("build_lm_input", "vision", vision, _F32, (None, D), 16, embed)
     L.check_device(embed)
     h = torch.empty((T, D), dtype=torch.float32, device=embed.device)
     _launch("other", 0.0, L.lib().vr_build_lm_input_ex, src.data_ptr(), T, D, embed.data_ptr(), vr_dtype, scale_emb, L.ptr(vision),
@@ -214,6 +266,12 @@ POOLING = {"wmean": 0, "mean": 1, "lasttoken": 2, "cls": 3}
 
 
 def pool_norm(h: torch.Tensor, gamma: torch.Tensor, eps: float, cu: torch.Tensor, pooling: str, normalize: bool) -> torch.Tensor:
+    """fp32 h [T, D] (any row pitch) -> reps [B, D] fp32: final RMSNorm, pooling over rows cu[b]..cu[b+1], L2 normalise."""
+    _operand("pool_norm", "h", h, _F32, (None, None), 16, h)
+    _operand("pool_norm", "gamma", gamma, _F32, (h.shape[1],), 16, h, contiguous=True)
+    _operand("pool_norm", "cu", cu, _I32, (None,), 4, h, contiguous=True)
+    if pooling not in POOLING:
+        raise ValueError(f"pool_norm: pooling must be one of {sorted(POOLING)}, got {pooling!r}")
     B = cu.shape[0] - 1
     L.check_device(h)
     reps = torch.empty((B, h.shape[1]), dtype=torch.float32, device=h.device)
