@@ -360,6 +360,51 @@ int vr_group_topk_rows(const float* scores, int32_t rows, int64_t nd, const int3
 int vr_merge_group_topk(const float* scores, const int64_t* pages, const int64_t* groups, int32_t rows, int32_t cols, int32_t k,
                         float* out_scores, int64_t* out_pages, int64_t* out_groups, void* stream);
 
+/* Per-query filters: each query of a batch searches its own subset of the docs, in the same one pass over the index.
+ * A mask set holds `count` masks of the _masked layout, row by row: doc i (local index, before id_offset) is eligible for
+ * mask m when bit (i & 31) of words[m * pitch + (i >> 5)] is set; bits at or past nd are ignored. Query row r uses mask
+ * of_query[r], which the caller keeps in [0, count) (the values are in device memory and are not checked); a NULL
+ * of_query means every row uses mask 0, so the single doc_mask of the _masked calls is the mask set
+ * {doc_mask, ceil(nd / 32), NULL, 1}. Each query's result is that of the _masked call of that query alone with its own
+ * mask, bit for bit. words and of_query are device pointers; the struct itself is read on the host during the call.
+ * Alignment (bytes) of the vr_doc_masks arrays: words 4, of_query 4
+ * Every _masks entry point takes the other pointers with the alignment of its _masked or doc_mask counterpart, and
+ * refuses before any CUDA call: masks NULL, words NULL or misaligned, count < 1, pitch < ceil(nd / 32) (nd = cols for
+ * the top-k calls), and count > 1 with a NULL of_query; the message names the field.
+ *   vr_score_filter_masks         : vr_score_filter_masked with a mask per query; the lists of query q hold q's eligible
+ *                                   docs only, so vr_score_rescore takes them unchanged;
+ *   vr_score_filter_groups_masks  : vr_score_filter_groups with a mask per query;
+ *   vr_score_rescore_groups_masks : vr_score_rescore_groups, each query rescoring its own eligible pages;
+ *   vr_topk_rows_masks            : vr_topk_rows_masked, row r of scores filtered by the mask of query r (ids must be NULL);
+ *   vr_topk_rows_chunked_masks    : vr_topk_rows_chunked_masked with a mask per row;
+ *   vr_group_topk_rows_masks      : vr_group_topk_rows with a mask per row.
+ * A call over rows [r0, r0 + n) of a larger batch passes of_query + r0. */
+typedef struct {
+    const uint32_t* words;     /* [count, pitch] mask words */
+    int64_t pitch;             /* words per mask, >= ceil(nd / 32) */
+    const int32_t* of_query;   /* [rows]: the mask of each query row, or NULL: mask 0 for every row */
+    int32_t count;             /* masks in the set, >= 1 */
+} vr_doc_masks;
+
+int vr_score_filter_masks(const void* q_f16, int32_t nq, const void* d_f16, int64_t nd, int32_t dim, int32_t ranges,
+                          float* cand_scores, int32_t* cand_ids, const vr_doc_masks* masks, void* stream);
+int vr_score_filter_groups_masks(const void* q_f16, int32_t nq, const void* d_f16, int64_t nd, int32_t dim, int32_t ranges,
+                                 float* cand_scores, int32_t* cand_ids, const int32_t* doc_groups, const vr_doc_masks* masks,
+                                 void* stream);
+int vr_score_rescore_groups_masks(const float* q_f32, int32_t nq, const float* d_f32, int64_t nd, int32_t dim, int32_t ranges,
+                                  const float* cand_scores, const int32_t* cand_ids, const int32_t* doc_groups,
+                                  const int32_t* group_offsets, const int32_t* group_pages, int32_t G,
+                                  const vr_doc_masks* masks, const float* max_doc_norm, int32_t k, int64_t id_offset,
+                                  float* out_scores, int64_t* out_pages, int64_t* out_groups, int32_t* flags, void* stream);
+int vr_topk_rows_masks(const float* scores, const int64_t* ids, int32_t rows, int64_t cols, int32_t k, int64_t id_offset,
+                       float* out_scores, int64_t* out_ids, const vr_doc_masks* masks, void* stream);
+int vr_topk_rows_chunked_masks(const float* scores, int32_t rows, int64_t cols, int32_t k, int64_t id_offset, int32_t chunks,
+                               float* ws_scores, int64_t* ws_ids, float* out_scores, int64_t* out_ids,
+                               const vr_doc_masks* masks, void* stream);
+int vr_group_topk_rows_masks(const float* scores, int32_t rows, int64_t nd, const int32_t* doc_groups, int32_t G,
+                             const vr_doc_masks* masks, int32_t k, int64_t id_offset, int32_t chunks, void* ws,
+                             int64_t ws_bytes, float* out_scores, int64_t* out_pages, int64_t* out_groups, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

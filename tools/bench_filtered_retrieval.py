@@ -3,7 +3,10 @@ the tensor-core filter path) and one query over 125 k and over 1 M docs (the fp3
 mask, an all-ones mask, and random masks keeping 50 %, 10 % and 1 % of the docs. The arms alternate inside every round, so
 drift of the shared machine falls on all of them alike; each arm reports its median and spread over the rounds, and the
 card's name and power limit are read in the same process. Prints one JSON line per (workload, arm), plus one for the card.
-  python tools/bench_filtered_retrieval.py [--rounds 10] [--out results.jsonl]"""
+Per-query masks (--per-query, on the configs[3] shard): every query with its own mask in one call, against what it costs
+without them: 100 random scopes of 10 % (one shared-mask call per scope), and a run of 8 pages per query (M = nq; a loop
+of single-query calls over the first 1 000 queries, reported as measured), with the unmasked call for reference.
+  python tools/bench_filtered_retrieval.py [--rounds 10] [--out results.jsonl] [--per-query] [--skip-shared]"""
 import argparse
 import json
 import os
@@ -70,6 +73,66 @@ def run(name, Q, index, k, rounds, reps, out):
         out.append(line)
 
 
+def _timed(fn, reps=1):
+    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+    e0.record()
+    for _ in range(reps):
+        fn()
+    e1.record()
+    torch.cuda.synchronize()
+    return e0.elapsed_time(e1) / reps
+
+
+def run_per_query(Q, index, k, rounds, out, loop_queries=1000):
+    """Alternating arms: per-query masks in one call vs the calls they replace, and the unmasked call."""
+    nq, nd = Q.shape[0], index.nd
+    g = torch.Generator(device="cuda").manual_seed(11)
+    scopes = torch.rand((100, nd), device="cuda", generator=g) < 0.1
+    of = torch.randint(0, 100, (nq,), device="cuda", generator=g)
+    members = [torch.nonzero(of == m).flatten() for m in range(100)]
+    start = torch.randint(0, nd - 8, (nq,), device="cuda", generator=g)
+    own = torch.zeros((nq, nd), dtype=torch.bool, device="cuda")
+    own[torch.arange(nq, device="cuda")[:, None], start[:, None] + torch.arange(8, device="cuda")] = True
+
+    def per_scope_calls():
+        for m in range(100):
+            if members[m].numel():
+                R.score_topk(Q[members[m]], index, k, doc_mask=scopes[m])
+
+    def single_calls():
+        for r in range(loop_queries):
+            R.score_topk(Q[r:r + 1], index, k, doc_mask=own[r])
+
+    arms = {"100 scopes of 10%: per-query masks": lambda: R.score_topk(Q, index, k, doc_mask=scopes, mask_of=of),
+            "100 scopes of 10%: one call per scope": per_scope_calls,
+            "8 pages each: per-query masks": lambda: R.score_topk(Q, index, k, doc_mask=own),
+            f"8 pages each: single-query calls, first {loop_queries}": single_calls,
+            "no mask": lambda: R.score_topk(Q, index, k)}
+    stats = {}
+    for a, fn in arms.items():                       # warm-up
+        fn()
+    R.score_topk(Q, index, k, doc_mask=scopes, mask_of=of, stats=stats.setdefault("scopes", {}))
+    R.score_topk(Q, index, k, doc_mask=own, stats=stats.setdefault("own", {}))
+    # the per-query rows equal the calls they replace
+    s, i = R.score_topk(Q, index, k, doc_mask=scopes, mask_of=of)
+    same = all(torch.equal(i[members[m]], R.score_topk(Q[members[m]], index, k, doc_mask=scopes[m])[1]) for m in range(0, 100, 9))
+    s8, i8 = R.score_topk(Q, index, k, doc_mask=own)
+    same &= all(torch.equal(i8[r:r + 1], R.score_topk(Q[r:r + 1], index, k, doc_mask=own[r])[1]) for r in range(0, nq, 997))
+    torch.cuda.synchronize()
+    times = {a: [] for a in arms}
+    for _ in range(rounds):
+        for a, fn in arms.items():
+            times[a].append(_timed(fn))
+    for a in arms:
+        t = sorted(times[a])
+        line = {"workload": "per-query masks", "arm": a, "queries": nq, "docs": nd, "k": k,
+                "ms_median": round(t[len(t) // 2], 3), "ms_min": round(t[0], 3), "ms_max": round(t[-1], 3),
+                "rows_equal_the_calls_they_replace": same,
+                "stats": stats["scopes" if a.startswith("100") else "own"] if a.endswith("per-query masks") else None}
+        print(json.dumps(line), flush=True)
+        out.append(line)
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--corpus", type=int, default=125000)
@@ -79,6 +142,8 @@ def main():
     ap.add_argument("--k", type=int, default=10)
     ap.add_argument("--rounds", type=int, default=10)
     ap.add_argument("--out", default=None, help="also write the JSON lines to this file")
+    ap.add_argument("--per-query", action="store_true", help="also measure per-query masks on the configs[3] shard")
+    ap.add_argument("--skip-shared", action="store_true", help="skip the shared-mask workloads")
     a = ap.parse_args()
     if not torch.cuda.is_available():
         raise SystemExit("bench_filtered_retrieval needs a CUDA device")
@@ -87,13 +152,17 @@ def main():
 
     D = unit(a.corpus, a.dim, 1)
     index = R.build_index(D)
-    run("configs[3] shard: filter path", unit(a.queries, a.dim, 2), index, a.k, a.rounds, 1, out)
-    run("one query", unit(1, a.dim, 4), index, a.k, a.rounds, 20, out)
-    del D, index
-    torch.cuda.empty_cache()
-    D = unit(a.big, a.dim, 3)
-    index = R.build_index(D)
-    run("one query", unit(1, a.dim, 5), index, a.k, a.rounds, 10, out)
+    if not a.skip_shared:
+        run("configs[3] shard: filter path", unit(a.queries, a.dim, 2), index, a.k, a.rounds, 1, out)
+        run("one query", unit(1, a.dim, 4), index, a.k, a.rounds, 20, out)
+    if a.per_query:
+        run_per_query(unit(a.queries, a.dim, 2), index, a.k, a.rounds, out)
+    if not a.skip_shared:
+        del D, index
+        torch.cuda.empty_cache()
+        D = unit(a.big, a.dim, 3)
+        index = R.build_index(D)
+        run("one query", unit(1, a.dim, 5), index, a.k, a.rounds, 10, out)
     if a.out:
         with open(a.out, "w") as f:
             f.write("".join(json.dumps(x) + "\n" for x in out))

@@ -55,6 +55,17 @@ class AttnParams(C.Structure):
     ]
 
 
+class DocMasks(C.Structure):
+    """Mirror of ``vr_doc_masks``: a mask set, query row r searching mask of_query[r] (NULL: mask 0)."""
+
+    _fields_ = [
+        ("words", C.c_void_p),
+        ("pitch", C.c_int64),
+        ("of_query", C.c_void_p),
+        ("count", C.c_int32),
+    ]
+
+
 VR_ATTN_V_ONES_COLUMN = 1
 VR_ATTN_F16 = 2  # q / k / v / out are fp16
 
@@ -128,6 +139,20 @@ def _declare(lib: C.CDLL) -> None:
     lib.vr_group_topk_rows.argtypes = [vp, i32, i64, vp, i32, vp, i32, i64, i32, vp, i64, vp, vp, vp, vp]
     lib.vr_merge_group_topk.restype = i32
     lib.vr_merge_group_topk.argtypes = [vp, vp, vp, i32, i32, i32, vp, vp, vp, vp]
+    dm = C.POINTER(DocMasks)
+    lib.vr_score_filter_masks.restype = i32
+    lib.vr_score_filter_masks.argtypes = [vp, i32, vp, i64, i32, i32, vp, vp, dm, vp]
+    lib.vr_score_filter_groups_masks.restype = i32
+    lib.vr_score_filter_groups_masks.argtypes = [vp, i32, vp, i64, i32, i32, vp, vp, vp, dm, vp]
+    lib.vr_score_rescore_groups_masks.restype = i32
+    lib.vr_score_rescore_groups_masks.argtypes = [vp, i32, vp, i64, i32, i32, vp, vp, vp, vp, vp, i32, dm, vp, i32, i64, vp,
+                                                  vp, vp, vp, vp]
+    lib.vr_topk_rows_masks.restype = i32
+    lib.vr_topk_rows_masks.argtypes = [vp, vp, i32, i64, i32, i64, vp, vp, dm, vp]
+    lib.vr_topk_rows_chunked_masks.restype = i32
+    lib.vr_topk_rows_chunked_masks.argtypes = [vp, i32, i64, i32, i64, i32, vp, vp, vp, vp, dm, vp]
+    lib.vr_group_topk_rows_masks.restype = i32
+    lib.vr_group_topk_rows_masks.argtypes = [vp, i32, i64, vp, i32, dm, i32, i64, i32, vp, i64, vp, vp, vp, vp]
     lib.vr_pool_norm.restype = i32
     lib.vr_pool_norm.argtypes = [vp, i64, vp, f32, vp, i32, i32, i32, i32, vp, vp]
     lib.vr_prefix_rows.restype = i32

@@ -47,8 +47,22 @@ struct ScoreArgs {
     int* cand_ids;
 };
 
+// A mask set (vr_doc_masks on the device): query row r searches mask of_query[r] (of_query NULL: mask 0 for every row),
+// and doc i is eligible for mask m when bit i & 31 of words[m * pitch + (i >> 5)] is set. A single doc mask is the set of
+// one with pitch ceil(nd / 32).
+struct DocMasks {
+    const uint32_t* words;
+    long long pitch;
+    const int* of_query;
+};
+
+// The mask words of query row `row`.
+__device__ __forceinline__ const uint32_t* mask_of_row(const DocMasks& m, long long row) {
+    return m.of_query ? m.words + static_cast<long long>(__ldg(m.of_query + row)) * m.pitch : m.words;
+}
+
 struct MaskedScoreArgs : ScoreArgs {
-    const uint32_t* doc_mask;  // ceil(nd / 32) words: doc i is eligible when bit i & 31 of word i >> 5 is set
+    DocMasks masks;
 };
 
 struct GroupedScoreArgs : ScoreArgs {
@@ -131,9 +145,10 @@ __device__ __forceinline__ float quad_max(float v) {
 // lives in the 4 lanes of a quad (each lane holds a quarter of the columns), so every lane keeps a sorted top-16 of ITS
 // columns for each of its two rows over all tiles of the item; the four lists of a row are merged by shuffles at the end
 // of the item (top-16 of the union: its tail bounds everything any lane dropped) into one list per (query, doc range).
-// MASKED: doc_mask holds one eligibility bit per doc (bit i & 31 of word i >> 5). An ineligible doc's score becomes -inf
-// before anything looks at it, so it never enters a list, never raises thr and never reaches a published tau: every
-// tail, and so the rescoring kernel's bound, is a tail over eligible docs only.
+// MASKED: every query row has its own mask of the set (mask_of_row), one eligibility bit per doc. An ineligible doc's score
+// becomes -inf before anything looks at it, so it never enters that row's lists, never raises the row's thr and never
+// reaches the row's published tau: every tail of a query, and so the rescoring kernel's bound, is a tail over that query's
+// eligible docs only. A thread's two accumulator rows (g8, g8 + 8) are two queries, each with its own mask words.
 // The mask travels in its own argument type, so the unmasked form keeps the parameter list it has without the mask (an
 // unused parameter or ScoreArgs field changes its register allocation and code).
 // GROUPED ((Masked)GroupedScoreArgs): doc_groups gives each doc its group, and every list is group-distinct (group_insert,
@@ -216,22 +231,26 @@ score_filter_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_con
         // rescoring kernel's bound is the maximum over all list tails, and tau is one of them.
         float* tau_ptr[2];
         float tau[2], thr[2];  // thr = max(tau, best tail of the quad's four lists: the merged list's tail is no lower)
+        const uint32_t* mrow[2];  // MASKED: the mask words of each row's query
 #pragma unroll
         for (int h = 0; h < 2; ++h) {
             tau_ptr[h] = g.cand_scores + (static_cast<long long>(min(row0 + 8 * h, g.nq - 1)) * g.lists + g.lists - 1) * SC_KT;
             thr[h] = tau[h] = __ldcg(tau_ptr[h]);
+            if constexpr (MASKED) mrow[h] = mask_of_row(g.masks, min(row0 + 8 * h, g.nq - 1));
 #pragma unroll
             for (int j = 0; j < SC_KT; ++j) { sc[h][j] = -INFINITY; id[h][j] = -1; }
         }
         const int t1 = item_t1(item);
         for (int u = 2 * item_t0(item); u < 2 * t1; ++u) {
-            // the sub-tile's 4 mask words, loaded before the k-loop so the latency hides under the MMAs (words at or
-            // past the end of the mask read as 0: those columns are >= nd and skipped below anyway)
-            uint32_t mw[4];
+            // each row's 4 mask words of the sub-tile, loaded before the k-loop so the latency hides under the MMAs (words
+            // at or past the end of a mask read as 0: those columns are >= nd and skipped below anyway)
+            uint32_t mw[2][4];
             if constexpr (MASKED) {
                 const long long w0 = static_cast<long long>(u) * (Cfg::SUB_BN / 32), nw = (g.nd + 31) / 32;
 #pragma unroll
-                for (int i = 0; i < 4; ++i) mw[i] = w0 + i < nw ? __ldg(g.doc_mask + w0 + i) : 0u;
+                for (int h = 0; h < 2; ++h)
+#pragma unroll
+                    for (int i = 0; i < 4; ++i) mw[h][i] = w0 + i < nw ? __ldg(mrow[h] + w0 + i) : 0u;
             }
             float acc[Cfg::SUB_BN / 2];
             int prev = -1;
@@ -256,15 +275,6 @@ score_filter_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_con
             wgmma_touch(acc);
 
             const long long col_base = static_cast<long long>(u) * Cfg::SUB_BN + q4 * 2;
-            // bit 2j + e of elig = eligibility of this lane's column 8j + 2 q4 + e: word j >> 2, bit 8 (j & 3) + 2 q4 + e
-            uint32_t elig = 0;
-            if constexpr (MASKED) {
-#pragma unroll
-                for (int w = 0; w < 4; ++w) {
-                    const uint32_t x = mw[w] >> (2 * q4);
-                    elig |= ((x & 0x3u) | ((x >> 6) & 0xCu) | ((x >> 12) & 0x30u) | ((x >> 18) & 0xC0u)) << (8 * w);
-                }
-            }
 #pragma unroll
             for (int h = 0; h < 2; ++h) {
                 // this lane's 32 scores of the row: v[2j + e] = column 8j + 2 q4 + e of the sub-tile
@@ -275,6 +285,14 @@ score_filter_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_con
                     v[2 * j + 1] = __float_as_uint(acc[4 * j + 2 * h + 1]);
                 }
                 if constexpr (MASKED) {
+                    // bit 2j + e of elig = eligibility of this lane's column 8j + 2 q4 + e for row h's query: word j >> 2,
+                    // bit 8 (j & 3) + 2 q4 + e
+                    uint32_t elig = 0;
+#pragma unroll
+                    for (int w = 0; w < 4; ++w) {
+                        const uint32_t x = mw[h][w] >> (2 * q4);
+                        elig |= ((x & 0x3u) | ((x >> 6) & 0xCu) | ((x >> 12) & 0x30u) | ((x >> 18) & 0xC0u)) << (8 * w);
+                    }
 #pragma unroll
                     for (int j = 0; j < 32; ++j) v[j] = (elig >> j) & 1u ? v[j] : __float_as_uint(-INFINITY);
                 }
@@ -498,6 +516,8 @@ __device__ __forceinline__ float merge_list_heads(const float* __restrict__ cs, 
 // dropped (<= that list's 16th entry) and candidates pruned here (<= the best remaining head) - is bounded by `bound`.
 // Step 2: exact fp32 rescoring of the kept candidates, one warp per candidate. Step 3: top-k by (score desc, id asc)
 // and the proof  bound + eps < k-th exact score  (else the query is flagged for the fp32 scan).
+// It takes no mask, with a mask set or without: a masked filter's lists of query q hold q's eligible docs only, and every
+// tail of them is a tail over q's eligible docs, so the candidates, the bound and the proof are already q's own.
 __global__ void __launch_bounds__(RS_THREADS)
 rescore_topk_kernel(const float* __restrict__ Q, const float* __restrict__ D, long long nd, int dim, int lists, int keep,
                     const float* __restrict__ cand_scores, const int* __restrict__ cand_ids,
@@ -593,7 +613,7 @@ __global__ void __launch_bounds__(RS_THREADS, 1)  // without the 1, ptxas caps i
 rescore_groups_kernel(const float* __restrict__ Q, const float* __restrict__ D, int dim, int lists, int keep,
                       const float* __restrict__ cand_scores, const int* __restrict__ cand_ids,
                       const int* __restrict__ doc_groups, const int* __restrict__ group_offsets,
-                      const int* __restrict__ group_pages, const uint32_t* __restrict__ doc_mask,
+                      const int* __restrict__ group_pages, const DocMasks masks,
                       const float* __restrict__ max_doc_norm, int k, long long id_offset, float* __restrict__ out_scores,
                       long long* __restrict__ out_pages, long long* __restrict__ out_groups, int* __restrict__ flags) {
     extern __shared__ float sm[];
@@ -614,6 +634,7 @@ rescore_groups_kernel(const float* __restrict__ Q, const float* __restrict__ D, 
     const int q = blockIdx.x;
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const float* qrow = Q + static_cast<long long>(q) * dim;
+    const uint32_t* doc_mask = masks.words ? mask_of_row(masks, q) : nullptr;  // this query's mask (NULL: every page)
     if (warp == 0) {
         const float bnd = merge_list_heads<true>(cand_scores + static_cast<long long>(q) * lists * SC_KT,
                                            cand_ids + static_cast<long long>(q) * lists * SC_KT, lists, keep, lane, sel, sel_s);
@@ -786,19 +807,19 @@ exact_scores_kernel(const float* __restrict__ Q, int nq, const float* __restrict
     }
 }
 
-// Column c is eligible when bit c & 31 of mask word c >> 5 is set (the layout of the filter's doc_mask).
+// Column c is eligible when bit c & 31 of mask word c >> 5 is set (the layout of one mask of a DocMasks set).
 __device__ __forceinline__ bool col_eligible(const uint32_t* __restrict__ mask, long long c) {
     return (__ldg(mask + (c >> 5)) >> (c & 31)) & 1u;
 }
 
 // top-k of each row of a dense [rows, cols] fp32 matrix (optionally with explicit ids per entry).
-// MASKED (ids == NULL only): ineligible columns are skipped like negative ids - never represented by a -inf score, which
-// would count as a valid entry.
+// MASKED (ids == NULL only): row r's ineligible columns (by the mask of row r's query) are skipped like negative ids -
+// never represented by a -inf score, which would count as a valid entry.
 template <bool MASKED>
 __global__ void __launch_bounds__(256)
 topk_rows_kernel(const float* __restrict__ scores, const long long* __restrict__ ids, long long cols, int k,
                  long long id_offset, long long chunk_cols, float* __restrict__ out_scores,
-                 long long* __restrict__ out_ids, const uint32_t* __restrict__ mask) {
+                 long long* __restrict__ out_ids, const DocMasks masks) {
     // block (row, chunk): top-k of columns [chunk*chunk_cols, ...) of one row, written as list `row*gridDim.y + chunk`
     __shared__ float red_s[8];
     __shared__ long long red_i[8];
@@ -807,6 +828,7 @@ topk_rows_kernel(const float* __restrict__ scores, const long long* __restrict__
     const float* srow = scores + static_cast<long long>(blockIdx.x) * cols;
     const long long* irow = ids ? ids + static_cast<long long>(blockIdx.x) * cols : nullptr;
     const long long row = static_cast<long long>(blockIdx.x) * gridDim.y + blockIdx.y;  // output list
+    const uint32_t* mask = MASKED ? mask_of_row(masks, blockIdx.x) : nullptr;
     float last_s = INFINITY;
     long long last_i = -1;
     for (int round = 0; round < k; ++round) {
@@ -843,10 +865,11 @@ template <int NPL, bool MASKED>
 __global__ void __launch_bounds__(256)
 topk_rows_warp_kernel(const float* __restrict__ scores, const long long* __restrict__ ids, int rows, int cols, int k,
                       long long id_offset, float* __restrict__ out_scores, long long* __restrict__ out_ids,
-                      const uint32_t* __restrict__ mask) {
+                      const DocMasks masks) {
     const int lane = threadIdx.x & 31;
     const int row = blockIdx.x * 8 + (threadIdx.x >> 5);
     if (row >= rows) return;
+    const uint32_t* mask = MASKED ? mask_of_row(masks, row) : nullptr;
     const float* srow = scores + static_cast<long long>(row) * cols;
     const long long* irow = ids ? ids + static_cast<long long>(row) * cols : nullptr;
     float s[NPL];
@@ -888,7 +911,7 @@ topk_rows_warp_kernel(const float* __restrict__ scores, const long long* __restr
 
 template <bool MASKED>
 static int launch_topk_rows(const float* scores, const long long* ids, int rows, long long cols, int k, long long id_offset,
-                            float* out_scores, long long* out_ids, const uint32_t* mask, cudaStream_t s) {
+                            float* out_scores, long long* out_ids, const DocMasks& mask, cudaStream_t s) {
     if (cols <= 128)
         topk_rows_warp_kernel<4, MASKED><<<(rows + 7) / 8, 256, 0, s>>>(scores, ids, rows, static_cast<int>(cols), k, id_offset,
                                                                         out_scores, out_ids, mask);
@@ -917,13 +940,14 @@ __device__ __forceinline__ unsigned long long page_key(float v, int p) {
 
 __global__ void __launch_bounds__(256)
 group_key_kernel(const float* __restrict__ scores, int rows, long long nd, int G, const int* __restrict__ doc_groups,
-                 const uint32_t* __restrict__ mask, unsigned long long* __restrict__ keys) {
+                 const DocMasks masks, unsigned long long* __restrict__ keys) {
     const long long runs = (nd + GK_RUN - 1) / GK_RUN, n = static_cast<long long>(rows) * runs;
     for (long long i = blockIdx.x * static_cast<long long>(blockDim.x) + threadIdx.x; i < n;
          i += static_cast<long long>(gridDim.x) * blockDim.x) {
         const long long row = i / runs, p0 = (i - row * runs) * GK_RUN;
         const float* srow = scores + row * nd;
         unsigned long long* krow = keys + row * G;
+        const uint32_t* mask = masks.words ? mask_of_row(masks, row) : nullptr;  // the row's mask (NULL: every page)
         int cur = -1;
         unsigned long long best = 0;
 #pragma unroll
@@ -1107,11 +1131,36 @@ static int score_ranges_for(int nq, long long nd) { return score_plan(nq, nd).li
 // A doc mask as the _masked entry points take it: present and 4-byte aligned (one uint32 word per 32 docs).
 static bool mask_ok(const uint32_t* mask) { return mask && (reinterpret_cast<uintptr_t>(mask) & 3) == 0; }
 
-// The list initialisation, then score_filter_kernel<Args> over `plan`, after the caller's argument checks. doc_mask and
+static const DocMasks kNoMasks = {nullptr, 0, nullptr};
+
+// A single doc mask (the _masked entry points, the doc_mask arguments) is the mask set of one.
+static DocMasks one_mask(const uint32_t* words, long long nd) { return DocMasks{words, (nd + 31) / 32, nullptr}; }
+
+// A mask set as the _masks entry points take it, refused before any CUDA call unless every row it names can be read for
+// nd docs. The values of of_query lie in device memory: the caller keeps them in [0, count).
+static int masks_check(const char* fn, const vr_doc_masks* m, long long nd) {
+    VR_REQUIRE(m, "%s: masks must not be NULL", fn);
+    VR_REQUIRE(m->words, "%s: masks->words must not be NULL", fn);
+    VR_REQUIRE_ALIGNED(fn, "masks->words", m->words, 4);
+    VR_REQUIRE(m->count >= 1, "%s: masks->count=%d, needs at least one mask", fn, m->count);
+    VR_REQUIRE(m->pitch >= (nd + 31) / 32, "%s: masks->pitch=%lld words is below ceil(nd / 32) = %lld", fn,
+               (long long)m->pitch, (long long)((nd + 31) / 32));
+    VR_REQUIRE(m->count == 1 || m->of_query, "%s: masks->of_query is NULL with masks->count=%d masks", fn, m->count);
+    VR_REQUIRE_ALIGNED(fn, "masks->of_query", m->of_query, 4);
+    return 0;
+}
+#define VR_REQUIRE_MASKS(fn, m, nd)                                   \
+    do {                                                              \
+        if (int rc_ = masks_check((fn), (m), (nd))) return rc_;       \
+    } while (0)
+
+static DocMasks device_masks(const vr_doc_masks* m) { return DocMasks{m->words, m->pitch, m->of_query}; }
+
+// The list initialisation, then score_filter_kernel<Args> over `plan`, after the caller's argument checks. masks and
 // doc_groups go to the forms whose Args carry them.
 template <typename Args>
 static int launch_score_filter(const ScorePlan& plan, const void* q_f16, int nq, const void* d_f16, long long nd, int dim,
-                               float* cand_scores, int* cand_ids, const uint32_t* doc_mask, const int* doc_groups,
+                               float* cand_scores, int* cand_ids, const DocMasks& masks, const int* doc_groups,
                                cudaStream_t st) {
     using Cfg = Score2Cfg;
     CUtensorMap tq, td;
@@ -1123,7 +1172,7 @@ static int launch_score_filter(const ScorePlan& plan, const void* q_f16, int nq,
     Args g;
     g.nq = nq; g.nd = nd; g.dim = dim; g.lists = plan.lists; g.T = plan.T; g.R = plan.R; g.QB = plan.QB; g.items = plan.items;
     g.cand_scores = cand_scores; g.cand_ids = cand_ids;
-    if constexpr (kMasked<Args>) g.doc_mask = doc_mask;
+    if constexpr (kMasked<Args>) g.masks = masks;
     if constexpr (kGrouped<Args>) g.doc_groups = doc_groups;
     {
         const long long n = static_cast<long long>(nq) * (plan.lists - plan.R) * SC_KT;
@@ -1137,60 +1186,60 @@ static int launch_score_filter(const ScorePlan& plan, const void* q_f16, int nq,
     return 0;
 }
 
-// vr_score_filter(_masked): the page lists, masked when doc_mask is not NULL
-static int score_filter(const void* q_f16, int nq, const void* d_f16, long long nd, int dim, int ranges, const uint32_t* doc_mask,
-                        float* cand_scores, int* cand_ids, void* stream) {
-    VR_REQUIRE(q_f16 && d_f16 && cand_scores && cand_ids, "vr_score_filter: null pointer");
-    VR_REQUIRE(nq > 0 && nd > 0 && nd < 2147483647ll && dim % 8 == 0, "vr_score_filter: bad shape nq=%d nd=%lld dim=%d", nq,
+// vr_score_filter(_masked, _masks): the page lists, masked when masks is not NULL (after the caller's mask checks)
+static int score_filter(const char* fn, const void* q_f16, int nq, const void* d_f16, long long nd, int dim, int ranges,
+                        const DocMasks* masks, float* cand_scores, int* cand_ids, void* stream) {
+    VR_REQUIRE(q_f16 && d_f16 && cand_scores && cand_ids, "%s: null pointer", fn);
+    VR_REQUIRE(nq > 0 && nd > 0 && nd < 2147483647ll && dim % 8 == 0, "%s: bad shape nq=%d nd=%lld dim=%d", fn, nq,
                (long long)nd, dim);
-    VR_REQUIRE(nq < (1 << 30), "vr_score_filter: too many queries");
+    VR_REQUIRE(nq < (1 << 30), "%s: too many queries", fn);
     const ScorePlan plan = score_plan(nq, nd);
-    VR_REQUIRE(ranges * 2 == plan.lists, "vr_score_filter: ranges must come from vr_score_ranges()");
+    VR_REQUIRE(ranges * 2 == plan.lists, "%s: ranges must come from vr_score_ranges()", fn);
     // q / d are TMA sources; the candidate lists are written 16 bytes at a time
-    VR_REQUIRE_ALIGNED("vr_score_filter", "q_f16", q_f16, 16);
-    VR_REQUIRE_ALIGNED("vr_score_filter", "d_f16", d_f16, 16);
-    VR_REQUIRE_ALIGNED("vr_score_filter", "cand_scores", cand_scores, 16);
-    VR_REQUIRE_ALIGNED("vr_score_filter", "cand_ids", cand_ids, 16);
+    VR_REQUIRE_ALIGNED(fn, "q_f16", q_f16, 16);
+    VR_REQUIRE_ALIGNED(fn, "d_f16", d_f16, 16);
+    VR_REQUIRE_ALIGNED(fn, "cand_scores", cand_scores, 16);
+    VR_REQUIRE_ALIGNED(fn, "cand_ids", cand_ids, 16);
     cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-    if (doc_mask)
-        return launch_score_filter<MaskedScoreArgs>(plan, q_f16, nq, d_f16, nd, dim, cand_scores, cand_ids, doc_mask, nullptr, st);
-    return launch_score_filter<ScoreArgs>(plan, q_f16, nq, d_f16, nd, dim, cand_scores, cand_ids, nullptr, nullptr, st);
+    if (masks)
+        return launch_score_filter<MaskedScoreArgs>(plan, q_f16, nq, d_f16, nd, dim, cand_scores, cand_ids, *masks, nullptr, st);
+    return launch_score_filter<ScoreArgs>(plan, q_f16, nq, d_f16, nd, dim, cand_scores, cand_ids, kNoMasks, nullptr, st);
 }
 
-// vr_topk_rows(_masked), after the mask checks: the masked form when mask is not NULL (ids is NULL then)
+// vr_topk_rows(_masked, _masks), after the mask checks: the masked form when masks is not NULL (ids is NULL then)
 static int topk_rows(const char* fn, const float* scores, const int64_t* ids, int rows, long long cols, int k,
-                     long long id_offset, float* out_scores, int64_t* out_ids, const uint32_t* mask, void* stream) {
+                     long long id_offset, float* out_scores, int64_t* out_ids, const DocMasks* masks, void* stream) {
     VR_REQUIRE(scores && out_scores && out_ids, "%s: null pointer", fn);
     VR_REQUIRE(rows > 0 && cols > 0 && k > 0, "%s: bad shape", fn);
     const long long* i = reinterpret_cast<const long long*>(ids);
     long long* oi = reinterpret_cast<long long*>(out_ids);
     cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
-    if (mask) launch_topk_rows<true>(scores, i, rows, cols, k, id_offset, out_scores, oi, mask, s);
-    else launch_topk_rows<false>(scores, i, rows, cols, k, id_offset, out_scores, oi, nullptr, s);
+    if (masks) launch_topk_rows<true>(scores, i, rows, cols, k, id_offset, out_scores, oi, *masks, s);
+    else launch_topk_rows<false>(scores, i, rows, cols, k, id_offset, out_scores, oi, kNoMasks, s);
     VR_CHECK_CUDA(cudaGetLastError());
     return 0;
 }
 
-// vr_topk_rows_chunked(_masked), after the mask check: the masked form when mask is not NULL
+// vr_topk_rows_chunked(_masked, _masks), after the mask checks: the masked form when masks is not NULL
 static int topk_rows_chunked(const char* fn, const float* scores, int rows, long long cols, int k, long long id_offset,
                              int chunks, float* ws_scores, int64_t* ws_ids, float* out_scores, int64_t* out_ids,
-                             const uint32_t* mask, void* stream) {
+                             const DocMasks* masks, void* stream) {
     VR_REQUIRE(scores && ws_scores && ws_ids && out_scores && out_ids, "%s: null pointer", fn);
     VR_REQUIRE(rows > 0 && cols > 0 && k > 0 && chunks > 0 && chunks <= 65535, "%s: bad shape", fn);
     long long* wi = reinterpret_cast<long long*>(ws_ids);
     cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
     const long long chunk_cols = (cols + chunks - 1) / chunks;
     // pass 1: every (row, chunk) block reduces its column range to a sorted top-k list (ids = column + id_offset)
-    if (mask)
+    if (masks)
         topk_rows_kernel<true><<<dim3(rows, chunks), 256, 0, s>>>(scores, nullptr, cols, k, id_offset, chunk_cols, ws_scores,
-                                                                  wi, mask);
+                                                                  wi, *masks);
     else
         topk_rows_kernel<false><<<dim3(rows, chunks), 256, 0, s>>>(scores, nullptr, cols, k, id_offset, chunk_cols, ws_scores,
-                                                                   wi, nullptr);
+                                                                   wi, kNoMasks);
     VR_CHECK_CUDA(cudaGetLastError());
     // pass 2: merge the `chunks` lists of each row (explicit ids; exhausted lists carry id -1 and are skipped)
     launch_topk_rows<false>(ws_scores, wi, rows, static_cast<long long>(chunks) * k, k, 0, out_scores,
-                            reinterpret_cast<long long*>(out_ids), nullptr, s);
+                            reinterpret_cast<long long*>(out_ids), kNoMasks, s);
     VR_CHECK_CUDA(cudaGetLastError());
     return 0;
 }
@@ -1233,14 +1282,23 @@ extern "C" int vr_f32_to_f16_rows(const float* src, int64_t rows, int32_t dim, v
 
 extern "C" int vr_score_filter(const void* q_f16, int32_t nq, const void* d_f16, int64_t nd, int32_t dim, int32_t ranges,
                                float* cand_scores, int32_t* cand_ids, void* stream) {
-    return score_filter(q_f16, nq, d_f16, nd, dim, ranges, nullptr, cand_scores, cand_ids, stream);
+    return score_filter("vr_score_filter", q_f16, nq, d_f16, nd, dim, ranges, nullptr, cand_scores, cand_ids, stream);
 }
 
 extern "C" int vr_score_filter_masked(const void* q_f16, int32_t nq, const void* d_f16, int64_t nd, int32_t dim,
                                       int32_t ranges, float* cand_scores, int32_t* cand_ids, const uint32_t* doc_mask,
                                       void* stream) {
     VR_REQUIRE(mask_ok(doc_mask), "vr_score_filter_masked: doc_mask must be a non-null, 4-byte aligned pointer");
-    return score_filter(q_f16, nq, d_f16, nd, dim, ranges, doc_mask, cand_scores, cand_ids, stream);
+    const DocMasks m = one_mask(doc_mask, nd);
+    return score_filter("vr_score_filter", q_f16, nq, d_f16, nd, dim, ranges, &m, cand_scores, cand_ids, stream);
+}
+
+extern "C" int vr_score_filter_masks(const void* q_f16, int32_t nq, const void* d_f16, int64_t nd, int32_t dim,
+                                     int32_t ranges, float* cand_scores, int32_t* cand_ids, const vr_doc_masks* masks,
+                                     void* stream) {
+    VR_REQUIRE_MASKS("vr_score_filter_masks", masks, nd);
+    const DocMasks m = device_masks(masks);
+    return score_filter("vr_score_filter_masks", q_f16, nq, d_f16, nd, dim, ranges, &m, cand_scores, cand_ids, stream);
 }
 
 extern "C" int vr_score_rescore(const float* q_f32, int32_t nq, const float* d_f32, int64_t nd, int32_t dim, int32_t ranges,
@@ -1312,7 +1370,17 @@ extern "C" int vr_topk_rows_masked(const float* scores, const int64_t* ids, int3
                                    void* stream) {
     VR_REQUIRE(mask_ok(doc_mask), "vr_topk_rows_masked: doc_mask must be a non-null, 4-byte aligned pointer");
     VR_REQUIRE(!ids, "vr_topk_rows_masked: the mask indexes columns, so ids must be NULL");
-    return topk_rows("vr_topk_rows_masked", scores, ids, rows, cols, k, id_offset, out_scores, out_ids, doc_mask, stream);
+    const DocMasks m = one_mask(doc_mask, cols);
+    return topk_rows("vr_topk_rows_masked", scores, ids, rows, cols, k, id_offset, out_scores, out_ids, &m, stream);
+}
+
+extern "C" int vr_topk_rows_masks(const float* scores, const int64_t* ids, int32_t rows, int64_t cols, int32_t k,
+                                  int64_t id_offset, float* out_scores, int64_t* out_ids, const vr_doc_masks* masks,
+                                  void* stream) {
+    VR_REQUIRE_MASKS("vr_topk_rows_masks", masks, cols);
+    VR_REQUIRE(!ids, "vr_topk_rows_masks: the masks index columns, so ids must be NULL");
+    const DocMasks m = device_masks(masks);
+    return topk_rows("vr_topk_rows_masks", scores, ids, rows, cols, k, id_offset, out_scores, out_ids, &m, stream);
 }
 
 extern "C" int vr_topk_rows_chunked(const float* scores, int32_t rows, int64_t cols, int32_t k, int64_t id_offset,
@@ -1326,33 +1394,108 @@ extern "C" int vr_topk_rows_chunked_masked(const float* scores, int32_t rows, in
                                            int32_t chunks, float* ws_scores, int64_t* ws_ids, float* out_scores,
                                            int64_t* out_ids, const uint32_t* doc_mask, void* stream) {
     VR_REQUIRE(mask_ok(doc_mask), "vr_topk_rows_chunked_masked: doc_mask must be a non-null, 4-byte aligned pointer");
+    const DocMasks m = one_mask(doc_mask, cols);
     return topk_rows_chunked("vr_topk_rows_chunked_masked", scores, rows, cols, k, id_offset, chunks, ws_scores, ws_ids,
-                             out_scores, out_ids, doc_mask, stream);
+                             out_scores, out_ids, &m, stream);
+}
+
+extern "C" int vr_topk_rows_chunked_masks(const float* scores, int32_t rows, int64_t cols, int32_t k, int64_t id_offset,
+                                          int32_t chunks, float* ws_scores, int64_t* ws_ids, float* out_scores,
+                                          int64_t* out_ids, const vr_doc_masks* masks, void* stream) {
+    VR_REQUIRE_MASKS("vr_topk_rows_chunked_masks", masks, cols);
+    const DocMasks m = device_masks(masks);
+    return topk_rows_chunked("vr_topk_rows_chunked_masks", scores, rows, cols, k, id_offset, chunks, ws_scores, ws_ids,
+                             out_scores, out_ids, &m, stream);
 }
 
 // ---------------------------------------------------------------------------------------------- document-level top-k
 // A group table as the _groups entry points take it: 4-byte aligned int32 arrays, G >= 1, nd within the int32 ids.
 static bool i32_ok(const void* p) { return p && (reinterpret_cast<uintptr_t>(p) & 3) == 0; }
 
+// The mask of a _groups call: the set of a _masks entry point (checked here, so that the refusals keep the order of the
+// other arguments' checks), else the optional single doc_mask of the plain entry point.
+static int group_masks(const char* fn, const uint32_t* doc_mask, const vr_doc_masks* set, long long nd, DocMasks* out,
+                       bool* masked) {
+    if (set) {
+        VR_REQUIRE_MASKS(fn, set, nd);
+        *out = device_masks(set);
+    } else {
+        VR_REQUIRE(!doc_mask || mask_ok(doc_mask), "%s: doc_mask must be NULL or 4-byte aligned", fn);
+        *out = doc_mask ? one_mask(doc_mask, nd) : kNoMasks;
+    }
+    *masked = set || doc_mask;
+    return 0;
+}
+
+// vr_score_filter_groups(_masks)
+static int score_filter_groups(const char* fn, const void* q_f16, int nq, const void* d_f16, long long nd, int dim,
+                               int ranges, float* cand_scores, int* cand_ids, const int* doc_groups, const uint32_t* doc_mask,
+                               const vr_doc_masks* set, void* stream) {
+    VR_REQUIRE(i32_ok(doc_groups), "%s: doc_groups must be a non-null, 4-byte aligned pointer", fn);
+    DocMasks masks;
+    bool masked;
+    if (int rc = group_masks(fn, doc_mask, set, nd, &masks, &masked)) return rc;
+    VR_REQUIRE(q_f16 && d_f16 && cand_scores && cand_ids, "%s: null pointer", fn);
+    VR_REQUIRE(nd > 0 && nd < 2147483647ll, "%s: nd=%lld beyond the int32 doc ids", fn, (long long)nd);
+    VR_REQUIRE(nq > 0 && nq < (1 << 30) && dim % 8 == 0, "%s: bad shape", fn);
+    const ScorePlan plan = score_plan(nq, nd);
+    VR_REQUIRE(ranges * 2 == plan.lists, "%s: ranges must come from vr_score_ranges()", fn);
+    VR_REQUIRE_ALIGNED(fn, "q_f16", q_f16, 16);
+    VR_REQUIRE_ALIGNED(fn, "d_f16", d_f16, 16);
+    VR_REQUIRE_ALIGNED(fn, "cand_scores", cand_scores, 16);
+    VR_REQUIRE_ALIGNED(fn, "cand_ids", cand_ids, 16);
+    cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+    if (masked)
+        return launch_score_filter<MaskedGroupedScoreArgs>(plan, q_f16, nq, d_f16, nd, dim, cand_scores, cand_ids, masks,
+                                                           doc_groups, st);
+    return launch_score_filter<GroupedScoreArgs>(plan, q_f16, nq, d_f16, nd, dim, cand_scores, cand_ids, kNoMasks, doc_groups, st);
+}
+
 extern "C" int vr_score_filter_groups(const void* q_f16, int32_t nq, const void* d_f16, int64_t nd, int32_t dim,
                                       int32_t ranges, float* cand_scores, int32_t* cand_ids, const int32_t* doc_groups,
                                       const uint32_t* doc_mask, void* stream) {
-    VR_REQUIRE(i32_ok(doc_groups), "vr_score_filter_groups: doc_groups must be a non-null, 4-byte aligned pointer");
-    VR_REQUIRE(!doc_mask || mask_ok(doc_mask), "vr_score_filter_groups: doc_mask must be NULL or 4-byte aligned");
-    VR_REQUIRE(q_f16 && d_f16 && cand_scores && cand_ids, "vr_score_filter_groups: null pointer");
-    VR_REQUIRE(nd > 0 && nd < 2147483647ll, "vr_score_filter_groups: nd=%lld beyond the int32 doc ids", (long long)nd);
-    VR_REQUIRE(nq > 0 && nq < (1 << 30) && dim % 8 == 0, "vr_score_filter_groups: bad shape");
-    const ScorePlan plan = score_plan(nq, nd);
-    VR_REQUIRE(ranges * 2 == plan.lists, "vr_score_filter_groups: ranges must come from vr_score_ranges()");
-    VR_REQUIRE_ALIGNED("vr_score_filter_groups", "q_f16", q_f16, 16);
-    VR_REQUIRE_ALIGNED("vr_score_filter_groups", "d_f16", d_f16, 16);
-    VR_REQUIRE_ALIGNED("vr_score_filter_groups", "cand_scores", cand_scores, 16);
-    VR_REQUIRE_ALIGNED("vr_score_filter_groups", "cand_ids", cand_ids, 16);
-    cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-    if (doc_mask)
-        return launch_score_filter<MaskedGroupedScoreArgs>(plan, q_f16, nq, d_f16, nd, dim, cand_scores, cand_ids, doc_mask,
-                                                           doc_groups, st);
-    return launch_score_filter<GroupedScoreArgs>(plan, q_f16, nq, d_f16, nd, dim, cand_scores, cand_ids, nullptr, doc_groups, st);
+    return score_filter_groups("vr_score_filter_groups", q_f16, nq, d_f16, nd, dim, ranges, cand_scores, cand_ids, doc_groups,
+                               doc_mask, nullptr, stream);
+}
+
+extern "C" int vr_score_filter_groups_masks(const void* q_f16, int32_t nq, const void* d_f16, int64_t nd, int32_t dim,
+                                            int32_t ranges, float* cand_scores, int32_t* cand_ids, const int32_t* doc_groups,
+                                            const vr_doc_masks* masks, void* stream) {
+    VR_REQUIRE(masks, "vr_score_filter_groups_masks: masks must not be NULL");
+    return score_filter_groups("vr_score_filter_groups_masks", q_f16, nq, d_f16, nd, dim, ranges, cand_scores, cand_ids,
+                               doc_groups, nullptr, masks, stream);
+}
+
+// vr_score_rescore_groups(_masks)
+static int score_rescore_groups(const char* fn, const float* q_f32, int nq, const float* d_f32, long long nd, int dim,
+                                int ranges, const float* cand_scores, const int* cand_ids, const int* doc_groups,
+                                const int* group_offsets, const int* group_pages, int G, const uint32_t* doc_mask,
+                                const vr_doc_masks* set, const float* max_doc_norm, int k, long long id_offset,
+                                float* out_scores, int64_t* out_pages, int64_t* out_groups, int* flags, void* stream) {
+    VR_REQUIRE(i32_ok(doc_groups) && i32_ok(group_offsets) && i32_ok(group_pages),
+               "%s: doc_groups, group_offsets and group_pages must be non-null, 4-byte aligned pointers", fn);
+    DocMasks masks;
+    bool masked;
+    if (int rc = group_masks(fn, doc_mask, set, nd, &masks, &masked)) return rc;
+    VR_REQUIRE(G > 0, "%s: G=%d, needs at least one group", fn, G);
+    VR_REQUIRE(nd > 0 && nd < 2147483647ll, "%s: nd=%lld beyond the int32 doc ids", fn, (long long)nd);
+    VR_REQUIRE(q_f32 && d_f32 && cand_scores && cand_ids && max_doc_norm && out_scores && out_pages && out_groups && flags,
+               "%s: null pointer", fn);
+    VR_REQUIRE(nq > 0 && k > 0 && dim % 4 == 0, "%s: bad shape", fn);
+    VR_REQUIRE_ALIGNED(fn, "d_f32", d_f32, 16);
+    const int lists = ranges * 2;
+    VR_REQUIRE(ranges > 0 && lists <= SC_MAX_RANGES + 2, "%s: ranges must come from vr_score_ranges()", fn);
+    const int keep = rescore_keep(k, lists);
+    const size_t smem = (static_cast<size_t>(dim) + 2 * RG_PAGE_BUDGET + 7 * static_cast<size_t>(keep) + 1) * sizeof(float);
+    VR_REQUIRE(smem <= 200 * 1024, "%s: dim too large for shared memory (%zu bytes)", fn, smem);
+    static unsigned long long attr_set = 0;
+    if (smem > 48 * 1024 && first_use_on_device(&attr_set))
+        VR_CHECK_CUDA(cudaFuncSetAttribute(rescore_groups_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
+    rescore_groups_kernel<<<nq, RS_THREADS, smem, reinterpret_cast<cudaStream_t>(stream)>>>(
+        q_f32, d_f32, dim, lists, keep, cand_scores, cand_ids, doc_groups, group_offsets, group_pages, masks, max_doc_norm,
+        k, id_offset, out_scores, reinterpret_cast<long long*>(out_pages), reinterpret_cast<long long*>(out_groups), flags);
+    VR_CHECK_CUDA(cudaGetLastError());
+    return 0;
 }
 
 extern "C" int vr_score_rescore_groups(const float* q_f32, int32_t nq, const float* d_f32, int64_t nd, int32_t dim,
@@ -1361,28 +1504,21 @@ extern "C" int vr_score_rescore_groups(const float* q_f32, int32_t nq, const flo
                                        int32_t G, const uint32_t* doc_mask, const float* max_doc_norm, int32_t k,
                                        int64_t id_offset, float* out_scores, int64_t* out_pages, int64_t* out_groups,
                                        int32_t* flags, void* stream) {
-    VR_REQUIRE(i32_ok(doc_groups) && i32_ok(group_offsets) && i32_ok(group_pages),
-               "vr_score_rescore_groups: doc_groups, group_offsets and group_pages must be non-null, 4-byte aligned pointers");
-    VR_REQUIRE(!doc_mask || mask_ok(doc_mask), "vr_score_rescore_groups: doc_mask must be NULL or 4-byte aligned");
-    VR_REQUIRE(G > 0, "vr_score_rescore_groups: G=%d, needs at least one group", G);
-    VR_REQUIRE(nd > 0 && nd < 2147483647ll, "vr_score_rescore_groups: nd=%lld beyond the int32 doc ids", (long long)nd);
-    VR_REQUIRE(q_f32 && d_f32 && cand_scores && cand_ids && max_doc_norm && out_scores && out_pages && out_groups && flags,
-               "vr_score_rescore_groups: null pointer");
-    VR_REQUIRE(nq > 0 && k > 0 && dim % 4 == 0, "vr_score_rescore_groups: bad shape");
-    VR_REQUIRE_ALIGNED("vr_score_rescore_groups", "d_f32", d_f32, 16);
-    const int lists = ranges * 2;
-    VR_REQUIRE(ranges > 0 && lists <= SC_MAX_RANGES + 2, "vr_score_rescore_groups: ranges must come from vr_score_ranges()");
-    const int keep = rescore_keep(k, lists);
-    const size_t smem = (static_cast<size_t>(dim) + 2 * RG_PAGE_BUDGET + 7 * static_cast<size_t>(keep) + 1) * sizeof(float);
-    VR_REQUIRE(smem <= 200 * 1024, "vr_score_rescore_groups: dim too large for shared memory (%zu bytes)", smem);
-    static unsigned long long attr_set = 0;
-    if (smem > 48 * 1024 && first_use_on_device(&attr_set))
-        VR_CHECK_CUDA(cudaFuncSetAttribute(rescore_groups_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
-    rescore_groups_kernel<<<nq, RS_THREADS, smem, reinterpret_cast<cudaStream_t>(stream)>>>(
-        q_f32, d_f32, dim, lists, keep, cand_scores, cand_ids, doc_groups, group_offsets, group_pages, doc_mask, max_doc_norm,
-        k, id_offset, out_scores, reinterpret_cast<long long*>(out_pages), reinterpret_cast<long long*>(out_groups), flags);
-    VR_CHECK_CUDA(cudaGetLastError());
-    return 0;
+    return score_rescore_groups("vr_score_rescore_groups", q_f32, nq, d_f32, nd, dim, ranges, cand_scores, cand_ids,
+                                doc_groups, group_offsets, group_pages, G, doc_mask, nullptr, max_doc_norm, k, id_offset,
+                                out_scores, out_pages, out_groups, flags, stream);
+}
+
+extern "C" int vr_score_rescore_groups_masks(const float* q_f32, int32_t nq, const float* d_f32, int64_t nd, int32_t dim,
+                                             int32_t ranges, const float* cand_scores, const int32_t* cand_ids,
+                                             const int32_t* doc_groups, const int32_t* group_offsets,
+                                             const int32_t* group_pages, int32_t G, const vr_doc_masks* masks,
+                                             const float* max_doc_norm, int32_t k, int64_t id_offset, float* out_scores,
+                                             int64_t* out_pages, int64_t* out_groups, int32_t* flags, void* stream) {
+    VR_REQUIRE(masks, "vr_score_rescore_groups_masks: masks must not be NULL");
+    return score_rescore_groups("vr_score_rescore_groups_masks", q_f32, nq, d_f32, nd, dim, ranges, cand_scores, cand_ids,
+                                doc_groups, group_offsets, group_pages, G, nullptr, masks, max_doc_norm, k, id_offset,
+                                out_scores, out_pages, out_groups, flags, stream);
 }
 
 // workspace of vr_group_topk_rows: best pages [rows, G] i64, group scores [rows, G] f32, and with chunks >= 2 the first
@@ -1396,18 +1532,20 @@ extern "C" int64_t vr_group_topk_ws_bytes(int32_t rows, int32_t G, int32_t k, in
     return rows > 0 && G > 0 && k > 0 ? group_topk_ws(rows, G, k, chunks) : -1;
 }
 
-extern "C" int vr_group_topk_rows(const float* scores, int32_t rows, int64_t nd, const int32_t* doc_groups, int32_t G,
-                                  const uint32_t* doc_mask, int32_t k, int64_t id_offset, int32_t chunks, void* ws,
-                                  int64_t ws_bytes, float* out_scores, int64_t* out_pages, int64_t* out_groups,
-                                  void* stream) {
-    VR_REQUIRE(i32_ok(doc_groups), "vr_group_topk_rows: doc_groups must be a non-null, 4-byte aligned pointer");
-    VR_REQUIRE(!doc_mask || mask_ok(doc_mask), "vr_group_topk_rows: doc_mask must be NULL or 4-byte aligned");
-    VR_REQUIRE(G > 0, "vr_group_topk_rows: G=%d, needs at least one group", G);
-    VR_REQUIRE(nd > 0 && nd < 2147483647ll, "vr_group_topk_rows: nd=%lld beyond the int32 doc ids", (long long)nd);
-    VR_REQUIRE(scores && out_scores && out_pages && out_groups, "vr_group_topk_rows: null pointer");
-    VR_REQUIRE(rows > 0 && k > 0 && chunks >= 0 && chunks <= 65535, "vr_group_topk_rows: bad shape");
+// vr_group_topk_rows(_masks)
+static int group_topk_rows(const char* fn, const float* scores, int rows, long long nd, const int* doc_groups, int G,
+                           const uint32_t* doc_mask, const vr_doc_masks* set, int k, long long id_offset, int chunks, void* ws,
+                           long long ws_bytes, float* out_scores, int64_t* out_pages, int64_t* out_groups, void* stream) {
+    VR_REQUIRE(i32_ok(doc_groups), "%s: doc_groups must be a non-null, 4-byte aligned pointer", fn);
+    DocMasks masks;
+    bool masked;
+    if (int rc = group_masks(fn, doc_mask, set, nd, &masks, &masked)) return rc;
+    VR_REQUIRE(G > 0, "%s: G=%d, needs at least one group", fn, G);
+    VR_REQUIRE(nd > 0 && nd < 2147483647ll, "%s: nd=%lld beyond the int32 doc ids", fn, (long long)nd);
+    VR_REQUIRE(scores && out_scores && out_pages && out_groups, "%s: null pointer", fn);
+    VR_REQUIRE(rows > 0 && k > 0 && chunks >= 0 && chunks <= 65535, "%s: bad shape", fn);
     VR_REQUIRE(ws && (reinterpret_cast<uintptr_t>(ws) & 15) == 0 && ws_bytes >= group_topk_ws(rows, G, k, chunks),
-               "vr_group_topk_rows: workspace too small or misaligned (%lld bytes, need %lld, 16-byte aligned)",
+               "%s: workspace too small or misaligned (%lld bytes, need %lld, 16-byte aligned)", fn,
                (long long)ws_bytes, group_topk_ws(rows, G, k, chunks));
     cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
     const long long n = static_cast<long long>(rows) * G;
@@ -1417,7 +1555,7 @@ extern "C" int vr_group_topk_rows(const float* scores, int32_t rows, int64_t nd,
     const long long runs = static_cast<long long>(rows) * ((nd + GK_RUN - 1) / GK_RUN);
     long long blocks = (runs + 255) / 256;
     if (blocks > num_sms() * 16) blocks = num_sms() * 16;
-    group_key_kernel<<<static_cast<int>(blocks), 256, 0, st>>>(scores, rows, nd, G, doc_groups, doc_mask,
+    group_key_kernel<<<static_cast<int>(blocks), 256, 0, st>>>(scores, rows, nd, G, doc_groups, masks,
                                                                reinterpret_cast<unsigned long long*>(gpages));
     VR_CHECK_CUDA(cudaGetLastError());
     blocks = (n + 255) / 256;
@@ -1429,11 +1567,11 @@ extern "C" int vr_group_topk_rows(const float* scores, int32_t rows, int64_t nd,
         long long* ws_i = reinterpret_cast<long long*>(reinterpret_cast<char*>(ws) + ((n * 12 + 15) / 16) * 16);
         float* ws_s = reinterpret_cast<float*>(ws_i + static_cast<long long>(rows) * chunks * k);
         topk_rows_kernel<false><<<dim3(rows, chunks), 256, 0, st>>>(gscores, gpages, G, k, id_offset, (G + chunks - 1) / chunks,
-                                                                    ws_s, ws_i, nullptr);
+                                                                    ws_s, ws_i, kNoMasks);
         VR_CHECK_CUDA(cudaGetLastError());
-        launch_topk_rows<false>(ws_s, ws_i, rows, static_cast<long long>(chunks) * k, k, 0, out_scores, op, nullptr, st);
+        launch_topk_rows<false>(ws_s, ws_i, rows, static_cast<long long>(chunks) * k, k, 0, out_scores, op, kNoMasks, st);
     } else {
-        launch_topk_rows<false>(gscores, gpages, rows, G, k, id_offset, out_scores, op, nullptr, st);
+        launch_topk_rows<false>(gscores, gpages, rows, G, k, id_offset, out_scores, op, kNoMasks, st);
     }
     VR_CHECK_CUDA(cudaGetLastError());
     const long long m = static_cast<long long>(rows) * k;
@@ -1441,6 +1579,24 @@ extern "C" int vr_group_topk_rows(const float* scores, int32_t rows, int64_t nd,
         op, m, id_offset, doc_groups, reinterpret_cast<long long*>(out_groups));
     VR_CHECK_CUDA(cudaGetLastError());
     return 0;
+}
+
+
+extern "C" int vr_group_topk_rows(const float* scores, int32_t rows, int64_t nd, const int32_t* doc_groups, int32_t G,
+                                  const uint32_t* doc_mask, int32_t k, int64_t id_offset, int32_t chunks, void* ws,
+                                  int64_t ws_bytes, float* out_scores, int64_t* out_pages, int64_t* out_groups,
+                                  void* stream) {
+    return group_topk_rows("vr_group_topk_rows", scores, rows, nd, doc_groups, G, doc_mask, nullptr, k, id_offset, chunks, ws,
+                           ws_bytes, out_scores, out_pages, out_groups, stream);
+}
+
+extern "C" int vr_group_topk_rows_masks(const float* scores, int32_t rows, int64_t nd, const int32_t* doc_groups, int32_t G,
+                                        const vr_doc_masks* masks, int32_t k, int64_t id_offset, int32_t chunks, void* ws,
+                                        int64_t ws_bytes, float* out_scores, int64_t* out_pages, int64_t* out_groups,
+                                        void* stream) {
+    VR_REQUIRE(masks, "vr_group_topk_rows_masks: masks must not be NULL");
+    return group_topk_rows("vr_group_topk_rows_masks", scores, rows, nd, doc_groups, G, nullptr, masks, k, id_offset, chunks,
+                           ws, ws_bytes, out_scores, out_pages, out_groups, stream);
 }
 
 extern "C" int vr_merge_group_topk(const float* scores, const int64_t* pages, const int64_t* groups, int32_t rows,

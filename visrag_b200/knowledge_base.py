@@ -11,7 +11,9 @@ Scores are the same fp32 dot products; ties are ordered by lower page index (tor
 
 Beyond the reference: a search can be restricted to some pages (`within`, e.g. the pages of one PDF), pages can be
 removed (a tombstone bit, so the other pages keep their indices) and added, and `save` writes the live pages back in the
-demo's layout. All of it runs as a doc mask inside the same kernels, with the same exact fp32 results.
+demo's layout. All of it runs as a doc mask inside the same kernels, with the same exact fp32 results. A batch of queries
+can give each query its own scope (`within_each`, e.g. each question about its own PDF, or each user's own collections):
+one pass over the index serves them all, and each query's row equals its search alone.
 
 Documents: `build_index.py` stores page i of `report.pdf` as `report.pdf_i.png`, so a page's document is its filename up to
 the last `_` when the rest is `<digits>.png` (any other filename is its own document). `search_documents` returns the
@@ -113,29 +115,73 @@ class KnowledgeBase:
         mask[torch.tensor(rows, dtype=torch.int64, device=q.device)] = True
         return q, mask, len(rows)
 
-    def search(self, query_reps, topk: int, within: Optional[Iterable[str]] = None) -> Tuple[torch.Tensor, torch.Tensor]:
+    def _query_and_scopes(self, query_reps, within, within_each):
+        """Per-query scopes: (queries, bool [M, nd] masks of the M distinct scopes, mask_of [nq] int32, the live page rows
+        of each distinct scope). Identical scopes share one mask row; None is every live page."""
+        if within is not None:
+            raise ValueError("within and within_each cannot be combined: give every query its scope in within_each")
+        q, _, _ = self._query_and_mask(query_reps, None)
+        scopes = list(within_each)
+        if len(scopes) != q.shape[0]:
+            raise ValueError(f"within_each has {len(scopes)} entries for {q.shape[0]} queries (one scope per query)")
+        slot, rows_of, mask_of = {}, [], []
+        for scope in scopes:
+            key = None if scope is None else tuple(self._rows(scope))
+            if key not in slot:
+                slot[key] = len(rows_of)
+                rows_of.append(key)
+            mask_of.append(slot[key])
+        dev = q.device
+        masks = torch.zeros((len(rows_of), self.index.nd), dtype=torch.bool, device=dev)
+        every = [m for m, rows in enumerate(rows_of) if rows is None]
+        pairs = [(m, r) for m, rows in enumerate(rows_of) if rows is not None for r in rows]
+        if every:
+            masks[torch.tensor(every, dtype=torch.int64, device=dev)] = self._live
+        if pairs:
+            idx = torch.tensor(pairs, dtype=torch.int64, device=dev)
+            masks[idx[:, 0], idx[:, 1]] = True
+        live = torch.nonzero(self._live).flatten().tolist() if every else []
+        rows_of = [live if rows is None else list(rows) for rows in rows_of]
+        return q, masks, torch.tensor(mask_of, dtype=torch.int32, device=dev), rows_of
+
+    def search(self, query_reps, topk: int, within: Optional[Iterable[str]] = None,
+               within_each: Optional[Sequence[Optional[Iterable[str]]]] = None) -> Tuple[torch.Tensor, torch.Tensor]:
         """query_reps [nq, d] (tensor or ndarray, fp32) -> (scores [nq,k] f32, page indices [nq,k] i64) on the device.
-        within: page filenames to search (default: every live page); k = min(topk, pages searched)."""
-        q, mask, n = self._query_and_mask(query_reps, within)
-        k = min(topk, n)
+        within: page filenames to search (default: every live page); k = min(topk, pages searched).
+        within_each: one scope per query instead (a list of page filenames, or None for every live page), all searched in
+        one pass; k = min(topk, pages of the largest scope), and a query whose scope is shorter ends in (-inf, -1)."""
+        if within_each is not None:
+            q, masks, mask_of, rows_of = self._query_and_scopes(query_reps, within, within_each)
+            k = min(topk, max(len(rows) for rows in rows_of)) if rows_of else 0
+        else:
+            q, masks, n = self._query_and_mask(query_reps, within)
+            mask_of, k = None, min(topk, n)
         if k == 0:
             return (torch.empty((q.shape[0], 0), dtype=torch.float32, device=q.device),
                     torch.empty((q.shape[0], 0), dtype=torch.int64, device=q.device))
-        return retriever.score_topk(q, self.index, k, doc_mask=mask)  # enters the index's device itself
+        return retriever.score_topk(q, self.index, k, doc_mask=masks, mask_of=mask_of)  # enters the index's device itself
 
-    def search_documents(self, query_reps, topk: int, within: Optional[Iterable[str]] = None
+    def search_documents(self, query_reps, topk: int, within: Optional[Iterable[str]] = None,
+                         within_each: Optional[Sequence[Optional[Iterable[str]]]] = None
                          ) -> Tuple[torch.Tensor, torch.Tensor, List[List[str]]]:
         """The top-k DOCUMENTS, each scored by its best page: (scores [nq,k] f32, best page indices [nq,k] i64 on the
         device, document names [nq][k]). within: page filenames to search (default: every live page); k = min(topk,
-        documents searched). Ties rank the document with the lower best page index first."""
-        q, mask, _ = self._query_and_mask(query_reps, within)
-        searched = self._doc_groups if mask is None else self._doc_groups[mask]
-        k = min(topk, int(torch.unique(searched).numel()))             # documents searched, counted on the device
+        documents searched). Ties rank the document with the lower best page index first.
+        within_each: one scope per query, as in search; k = min(topk, documents of the largest scope), a shorter row ends
+        in (-inf, -1), and each query's names list holds only the documents it found."""
+        if within_each is not None:
+            q, masks, mask_of, rows_of = self._query_and_scopes(query_reps, within, within_each)
+            groups = self._doc_groups.tolist()
+            k = min(topk, max(len({groups[r] for r in rows}) for rows in rows_of)) if rows_of else 0
+        else:
+            q, masks, _ = self._query_and_mask(query_reps, within)
+            searched = self._doc_groups if masks is None else self._doc_groups[masks]
+            mask_of, k = None, min(topk, int(torch.unique(searched).numel()))   # documents searched, counted on the device
         if k == 0:
             return (torch.empty((q.shape[0], 0), dtype=torch.float32, device=q.device),
                     torch.empty((q.shape[0], 0), dtype=torch.int64, device=q.device), [[] for _ in range(q.shape[0])])
-        s, p, g = retriever.score_topk_groups(q, self.index, k, self._doc_groups, doc_mask=mask)
-        return s, p, [[self.documents[j] for j in row] for row in g.tolist()]
+        s, p, g = retriever.score_topk_groups(q, self.index, k, self._doc_groups, doc_mask=masks, mask_of=mask_of)
+        return s, p, [[self.documents[j] for j in row if j >= 0] for row in g.tolist()]
 
     def retrieve_documents(self, query_rep, topk: int, within: Optional[Iterable[str]] = None) -> List[Tuple[str, str]]:
         """[(document name, path of its best page image)] of the top-k documents, best first."""

@@ -11,13 +11,16 @@ Underneath, `torch.matmul` + `torch.topk` are replaced by the fused wgmma filter
 For a corpus that lives in HBM (index build + many query batches) use `CorpusIndex` / `score_topk` directly; the
 multi-GPU form (`sharded_topk`) shards the corpus by page across ranks, takes the local top-k with global ids and
 merges after ONE all-gather of [nq, k] (score, id) pairs. Both take an optional `doc_mask` (bool [nd], local to the
-shard): only the docs it marks are searched, and the result equals the fp32 scan over those docs alone.
+shard): only the docs it marks are searched, and the result equals the fp32 scan over those docs alone. A 2-D doc_mask
+(bool [M, nd]) with `mask_of` (int [nq] in [0, M), default row i for query i) gives every query its own subset, in the
+same one pass over the index: each query's row equals its call alone with its own mask.
 
 Document-level retrieval (`score_topk_groups`, `sharded_topk_groups`): `doc_groups` (int [nd]) gives every doc (page) its
 group (document); the top-k groups by their best page's exact fp32 score, ranked by (score desc, best page asc).
 """
 from __future__ import annotations
 
+import ctypes as C
 import glob
 import os
 import pickle
@@ -80,26 +83,75 @@ def build_index(emb, lookup: Optional[List[str]] = None, device: str = "cuda") -
 
 def pack_doc_mask(mask: torch.Tensor) -> torch.Tensor:
     """bool [nd] -> uint32 [ceil(nd / 32)] words on the same device: doc i is bit (i & 31) of word (i >> 5), the layout the
-    _masked kernels read. Bits past nd are 0."""
-    nd = mask.shape[0]
-    bits = torch.zeros(((nd + 31) // 32) * 32, dtype=torch.int64, device=mask.device)
-    bits[:nd] = mask.to(torch.int64)
-    words = (bits.view(-1, 32) << torch.arange(32, device=mask.device)).sum(1)
-    return torch.where(words >= 1 << 31, words - (1 << 32), words).to(torch.int32).view(torch.uint32)
+    _masked kernels read. Bits past nd are 0. bool [M, nd] -> uint32 [M, ceil(nd / 32)], row by row (a mask set)."""
+    nd = mask.shape[-1]
+    rows = mask.reshape(-1, nd)
+    w = (nd + 31) // 32
+    out = torch.empty((rows.shape[0], w * 4), dtype=torch.uint8, device=mask.device)
+    weights = torch.ones(8, dtype=torch.uint8, device=mask.device) << torch.arange(8, dtype=torch.uint8, device=mask.device)
+    step = max(1, (1 << 26) // (w * 32))  # rows per pass: <= 64 MiB of byte-per-bit scratch
+    for r0 in range(0, rows.shape[0], step):
+        part = rows[r0:r0 + step]
+        bits = torch.zeros((part.shape[0], w * 32), dtype=torch.uint8, device=mask.device)
+        bits[:, :nd] = part
+        out[r0:r0 + step] = (bits.view(part.shape[0], w * 4, 8) * weights).sum(-1, dtype=torch.uint8)
+    # little-endian bytes: byte j of a word holds docs 8j .. 8j + 7 of it
+    return out.view(torch.int32).view(torch.uint32).reshape(*mask.shape[:-1], w)
 
 
-def _check_doc_mask(doc_mask: torch.Tensor, index: CorpusIndex) -> torch.Tensor:
-    """Validate a bool [nd] doc mask on the index's device and pack it."""
+@dataclass
+class _MaskSet:
+    """A packed mask set on the index's device: words uint32 [M, pitch], of_query int32 [nq] (None: mask 0 for every row)."""
+    words: torch.Tensor
+    of_query: Optional[torch.Tensor]
+
+    def rows(self, sel: torch.Tensor) -> "_MaskSet":
+        """The set of the query rows `sel` (an index tensor), each keeping its own mask."""
+        return self if self.of_query is None else _MaskSet(self.words, self.of_query.index_select(0, sel))
+
+    def arg(self, r0: int = 0):
+        """The vr_doc_masks of the query rows from r0 on (a call over rows [r0, r0 + n) of the batch)."""
+        m = L.DocMasks()
+        m.words, m.pitch, m.count = self.words.data_ptr(), self.words.shape[1], self.words.shape[0]
+        m.of_query = None if self.of_query is None else self.of_query[r0:].data_ptr()
+        return C.byref(m)
+
+
+def _check_doc_mask(doc_mask: torch.Tensor, index: CorpusIndex, nq: int, mask_of: Optional[torch.Tensor] = None) -> _MaskSet:
+    """Validate a bool [nd] doc mask, or a bool [M, nd] mask set with its mask_of ([nq] ints in [0, M); None: query i
+    uses row i, so M == nq), on the index's device, and pack it."""
     if not isinstance(doc_mask, torch.Tensor) or doc_mask.dtype != torch.bool:
         raise ValueError("doc_mask must be a torch.bool tensor")
-    if doc_mask.dim() != 1 or doc_mask.shape[0] != index.nd:
-        raise ValueError(f"doc_mask must have shape [{index.nd}] (one entry per doc of the index), got {list(doc_mask.shape)}")
+    if doc_mask.dim() not in (1, 2) or doc_mask.shape[-1] != index.nd:
+        raise ValueError(f"doc_mask must have shape [{index.nd}] or [M, {index.nd}] (one entry per doc of the index), "
+                         f"got {list(doc_mask.shape)}")
     if doc_mask.device != index.emb.device:
         raise ValueError(f"doc_mask lives on {doc_mask.device}, the index on {index.emb.device}")
-    return pack_doc_mask(doc_mask)
+    if doc_mask.dim() == 1:
+        if mask_of is not None:
+            raise ValueError("mask_of picks rows of a 2-D doc_mask [M, nd]; this doc_mask is 1-D")
+        return _MaskSet(pack_doc_mask(doc_mask).view(1, -1), None)
+    M = doc_mask.shape[0]
+    if mask_of is None:
+        if M != nq:
+            raise ValueError(f"doc_mask has {M} rows for {nq} queries: pass mask_of, or one mask row per query")
+        of_query = torch.arange(nq, dtype=torch.int32, device=doc_mask.device)
+    else:
+        if not isinstance(mask_of, torch.Tensor) or mask_of.dtype not in (torch.int32, torch.int64):
+            raise ValueError("mask_of must be an int32 or int64 torch tensor")
+        if mask_of.dim() != 1 or mask_of.shape[0] != nq:
+            raise ValueError(f"mask_of must have shape [{nq}] (one mask row per query), got {list(mask_of.shape)}")
+        if mask_of.device != doc_mask.device:
+            raise ValueError(f"mask_of lives on {mask_of.device}, doc_mask on {doc_mask.device}")
+        if nq > 0:
+            lo, hi = (int(v) for v in torch.aminmax(mask_of))
+            if lo < 0 or hi >= M:
+                raise ValueError(f"mask_of must lie in [0, {M}) (rows of doc_mask), got [{lo}, {hi}]")
+        of_query = mask_of.to(torch.int32).contiguous()
+    return _MaskSet(pack_doc_mask(doc_mask), of_query)
 
 
-def _exact_topk(q: torch.Tensor, index: CorpusIndex, k: int, id_offset: int, mask_words: Optional[torch.Tensor]):
+def _exact_topk(q: torch.Tensor, index: CorpusIndex, k: int, id_offset: int, masks: Optional[_MaskSet]):
     """The plain fp32 scan: (scores, ids)."""
     nq, d = q.shape
     nd = index.nd
@@ -108,40 +160,48 @@ def _exact_topk(q: torch.Tensor, index: CorpusIndex, k: int, id_offset: int, mas
     rows_per = max(1, min(nq, (1 << 28) // max(nd, 1)))  # <= 1 GiB of fp32 scratch
     scratch = torch.empty((rows_per, nd), dtype=torch.float32, device=q.device)
     lib = L.lib()
-    mw = () if mask_words is None else (mask_words.data_ptr(),)
     for r0 in range(0, nq, rows_per):
         n = min(rows_per, nq - r0)
+        mw = () if masks is None else (masks.arg(r0),)  # rows r0.. of the batch keep their own masks
         L.check(lib.vr_score_exact(q[r0:].data_ptr(), n, index.emb.data_ptr(), nd, d, scratch.data_ptr(), L.stream_ptr()))
         chunks = min(1024, nd // 4096) if n <= 64 else 0  # few queries over a long index: spread each row over many SMs
         if chunks >= 2:
             ws_s = torch.empty((n, chunks, k), dtype=torch.float32, device=q.device)
             ws_i = torch.empty((n, chunks, k), dtype=torch.int64, device=q.device)
-            fn = lib.vr_topk_rows_chunked_masked if mw else lib.vr_topk_rows_chunked
+            fn = lib.vr_topk_rows_chunked_masks if mw else lib.vr_topk_rows_chunked
             args = (scratch.data_ptr(), n, nd, k, id_offset, chunks, ws_s.data_ptr(), ws_i.data_ptr())
         else:
-            fn = lib.vr_topk_rows_masked if mw else lib.vr_topk_rows
+            fn = lib.vr_topk_rows_masks if mw else lib.vr_topk_rows
             args = (scratch.data_ptr(), None, n, nd, k, id_offset)
         L.check(fn(*args, out_s[r0:].data_ptr(), out_i[r0:].data_ptr(), *mw, L.stream_ptr()))
     return out_s, out_i
 
 
 def score_topk(queries: torch.Tensor, index: CorpusIndex, k: int, id_offset: int = 0, force_exact: bool = False,
-               stats: Optional[dict] = None, doc_mask: Optional[torch.Tensor] = None) -> Tuple[torch.Tensor, torch.Tensor]:
+               stats: Optional[dict] = None, doc_mask: Optional[torch.Tensor] = None, mask_of: Optional[torch.Tensor] = None
+               ) -> Tuple[torch.Tensor, torch.Tensor]:
     """Exact fp32 top-k of `queries @ index.emb.T`: (scores [nq,k] f32, ids [nq,k] i64 = local index + id_offset).
     Rows are sorted by (score desc, id asc); if k > nd the tail is (-inf, -1).
     doc_mask: optional bool [nd] on the index's device; only docs marked True are searched (the same bits as the fp32 scan
-    over those docs alone). With fewer than k of them the tail is (-inf, -1)."""
-    q, mask_words = _queries_and_mask(queries, index, doc_mask)
+    over those docs alone). With fewer than k of them the tail is (-inf, -1).
+    Per-query masks: doc_mask bool [M, nd] and mask_of int [nq] in [0, M) (default: row i for query i, M == nq); query i
+    searches the docs of row mask_of[i], and its row equals its call alone with that row as a 1-D doc_mask."""
+    q, masks = _queries_and_mask(queries, index, doc_mask, mask_of)
     with L.on_device(q.device):
-        return _score_topk(q, index, k, id_offset, force_exact, stats, mask_words)
+        return _score_topk(q, index, k, id_offset, force_exact, stats, masks)
 
 
-def _queries_and_mask(queries: torch.Tensor, index: CorpusIndex, doc_mask: Optional[torch.Tensor]):
-    """The queries as contiguous fp32 on the index's device, and the packed doc mask (None: every doc)."""
+def _queries_and_mask(queries: torch.Tensor, index: CorpusIndex, doc_mask: Optional[torch.Tensor],
+                      mask_of: Optional[torch.Tensor] = None):
+    """The queries as contiguous fp32 on the index's device, and the packed mask set (None: every doc)."""
     q = _check_f32(queries, "queries")
     if q.device != index.emb.device:
         raise ValueError(f"queries live on {q.device}, the index on {index.emb.device}")
-    return q, None if doc_mask is None else _check_doc_mask(doc_mask, index)
+    if doc_mask is None:
+        if mask_of is not None:
+            raise ValueError("mask_of needs a 2-D doc_mask [M, nd] to pick rows from")
+        return q, None
+    return q, _check_doc_mask(doc_mask, index, q.shape[0], mask_of)
 
 
 class _Stages:
@@ -171,16 +231,17 @@ def resolve_stages(stats: dict) -> dict:
 
 
 def _score_topk(q: torch.Tensor, index: CorpusIndex, k: int, id_offset: int, force_exact: bool, stats: Optional[dict],
-                mask_words: Optional[torch.Tensor], gt: Optional[_GroupTable] = None, page_lists: bool = False):
+                masks: Optional[_MaskSet], gt: Optional[_GroupTable] = None, page_lists: bool = False):
     """The filter + rescoring pipeline. Pages (gt None): (scores, ids); groups (gt, the group table): (scores, best pages,
-    groups). page_lists: feed the page filter's lists to the grouped rescoring (tests and measurements of the proof)."""
+    groups). masks: the packed mask set (None: every doc). page_lists: feed the page filter's lists to the grouped
+    rescoring (tests and measurements of the proof)."""
     nq, d = q.shape
     nd = index.nd
 
-    def exact(rows: torch.Tensor):
+    def exact(rows: torch.Tensor, m: Optional[_MaskSet]):
         if gt is None:
-            return _exact_topk(rows, index, k, id_offset, mask_words)
-        return _exact_topk_groups(rows, index, k, id_offset, mask_words, gt)
+            return _exact_topk(rows, index, k, id_offset, m)
+        return _exact_topk_groups(rows, index, k, id_offset, m, gt)
 
     def outputs(n: int):
         dtypes = (torch.float32, torch.int64) if gt is None else (torch.float32, torch.int64, torch.int64)
@@ -193,7 +254,7 @@ def _score_topk(q: torch.Tensor, index: CorpusIndex, k: int, id_offset: int, for
     if force_exact or nq * nd <= SMALL_PROBLEM or nd < 256:
         if stats is not None:
             stats.update(path="exact", flagged=0)
-        return exact(q)
+        return exact(q, masks)
     lib = L.lib()
     ranges = lib.vr_score_ranges(nq, nd)
     lists = ranges * 2 * lib.vr_score_list_len()
@@ -203,30 +264,36 @@ def _score_topk(q: torch.Tensor, index: CorpusIndex, k: int, id_offset: int, for
     out = outputs(nq)
     flags = torch.empty((nq,), dtype=torch.int32, device=q.device)
     sp = L.stream_ptr()
-    mw = None if mask_words is None else mask_words.data_ptr()
     ev = _Stages(stats)
     ev.mark("q_to_f16")
     filt = (q16.data_ptr(), nq, index.emb_f16.data_ptr(), nd, d, ranges, cand_s.data_ptr(), cand_i.data_ptr())
     if gt is not None and not page_lists:
-        L.check(lib.vr_score_filter_groups(*filt, gt.groups.data_ptr(), mw, sp))
-    elif mw is None:
+        if masks is None:
+            L.check(lib.vr_score_filter_groups(*filt, gt.groups.data_ptr(), None, sp))
+        else:
+            L.check(lib.vr_score_filter_groups_masks(*filt, gt.groups.data_ptr(), masks.arg(), sp))
+    elif masks is None:
         L.check(lib.vr_score_filter(*filt, sp))
     else:
-        L.check(lib.vr_score_filter_masked(*filt, mw, sp))
+        L.check(lib.vr_score_filter_masks(*filt, masks.arg(), sp))
     ev.mark("filter")
     cand = (q.data_ptr(), nq, index.emb.data_ptr(), nd, d, ranges, cand_s.data_ptr(), cand_i.data_ptr())
     tail = (index.max_norm.data_ptr(), k, id_offset, *[t.data_ptr() for t in out], flags.data_ptr(), sp)
     if gt is None:
-        L.check(lib.vr_score_rescore(*cand, *tail))
+        L.check(lib.vr_score_rescore(*cand, *tail))  # a masked filter's lists hold each query's eligible docs only
     else:
-        L.check(lib.vr_score_rescore_groups(*cand, gt.groups.data_ptr(), gt.offsets.data_ptr(), gt.pages.data_ptr(), gt.G,
-                                            mw, *tail))
+        csr = (gt.groups.data_ptr(), gt.offsets.data_ptr(), gt.pages.data_ptr(), gt.G)
+        if masks is None:
+            L.check(lib.vr_score_rescore_groups(*cand, *csr, None, *tail))
+        else:
+            L.check(lib.vr_score_rescore_groups_masks(*cand, *csr, masks.arg(), *tail))
     ev.mark("rescore")
     bad = torch.nonzero(flags).flatten()  # host sync: the caller reads the result next anyway
     if stats is not None:
         stats.update(path="filter+rescore", flagged=int(bad.numel()), ranges=ranges)
     if bad.numel() > 0:
-        for t, fix in zip(out, exact(q.index_select(0, bad))):
+        # each flagged row reruns with its own mask
+        for t, fix in zip(out, exact(q.index_select(0, bad), None if masks is None else masks.rows(bad))):
             t.index_copy_(0, bad, fix)
     return out
 
@@ -274,7 +341,7 @@ def _group_table(doc_groups: torch.Tensor, index: CorpusIndex) -> _GroupTable:
     return table
 
 
-def _exact_topk_groups(q: torch.Tensor, index: CorpusIndex, k: int, id_offset: int, mask_words: Optional[torch.Tensor],
+def _exact_topk_groups(q: torch.Tensor, index: CorpusIndex, k: int, id_offset: int, masks: Optional[_MaskSet],
                        gt: _GroupTable):
     """The plain fp32 scan, reduced per group: (scores, best pages, groups)."""
     nq, d = q.shape
@@ -286,35 +353,36 @@ def _exact_topk_groups(q: torch.Tensor, index: CorpusIndex, k: int, id_offset: i
     rows_per = max(1, min(nq, (1 << 27) // max(nd, gt.G, 1)))
     scratch = torch.empty((rows_per, nd), dtype=torch.float32, device=q.device)
     lib = L.lib()
-    mw = None if mask_words is None else mask_words.data_ptr()
     for r0 in range(0, nq, rows_per):
         n = min(rows_per, nq - r0)
         L.check(lib.vr_score_exact(q[r0:].data_ptr(), n, index.emb.data_ptr(), nd, d, scratch.data_ptr(), L.stream_ptr()))
         chunks = min(1024, gt.G // 4096) if n <= 64 else 0  # few queries over many groups: spread each row over many SMs
         ws_bytes = lib.vr_group_topk_ws_bytes(n, gt.G, k, chunks)
         ws = torch.empty((ws_bytes + 15) // 16 * 2, dtype=torch.float64, device=q.device)  # 16-byte aligned
-        L.check(lib.vr_group_topk_rows(scratch.data_ptr(), n, nd, gt.groups.data_ptr(), gt.G, mw, k, id_offset, chunks, ws.data_ptr(), ws_bytes,
-                                       out_s[r0:].data_ptr(), out_p[r0:].data_ptr(), out_g[r0:].data_ptr(), L.stream_ptr()))
+        fn, mw = (lib.vr_group_topk_rows, None) if masks is None else (lib.vr_group_topk_rows_masks, masks.arg(r0))
+        L.check(fn(scratch.data_ptr(), n, nd, gt.groups.data_ptr(), gt.G, mw, k, id_offset, chunks, ws.data_ptr(), ws_bytes,
+                   out_s[r0:].data_ptr(), out_p[r0:].data_ptr(), out_g[r0:].data_ptr(), L.stream_ptr()))
     return out_s, out_p, out_g
 
 
 def score_topk_groups(queries: torch.Tensor, index: CorpusIndex, k: int, doc_groups: torch.Tensor, id_offset: int = 0,
-                      force_exact: bool = False, stats: Optional[dict] = None, doc_mask: Optional[torch.Tensor] = None
-                      ) -> Tuple[torch.Tensor, torch.Tensor, torch.Tensor]:
+                      force_exact: bool = False, stats: Optional[dict] = None, doc_mask: Optional[torch.Tensor] = None,
+                      mask_of: Optional[torch.Tensor] = None) -> Tuple[torch.Tensor, torch.Tensor, torch.Tensor]:
     """Exact top-k GROUPS (documents) of pages: doc_groups (int32/int64 [nd] on the index's device) gives each page its
     group in [0, G). A group's score is the maximum exact fp32 page score over its eligible pages, its best page the lowest
     page with that maximum; groups rank by (score desc, best page asc). Returns (scores [nq,k] f32, best pages [nq,k] i64
     = local index + id_offset, groups [nq,k] i64); fewer than k groups with an eligible page leave (-inf, -1, -1).
-    With doc_groups = arange(nd) the result equals score_topk's, with groups == pages. doc_mask as in score_topk."""
-    q, mask_words = _queries_and_mask(queries, index, doc_mask)
+    With doc_groups = arange(nd) the result equals score_topk's, with groups == pages. doc_mask and mask_of as in score_topk
+    (per-query masks: each query's documents are scored by its own eligible pages)."""
+    q, masks = _queries_and_mask(queries, index, doc_mask, mask_of)
     with L.on_device(q.device):
         gt = _group_table(doc_groups, index)
-        return _score_topk_groups(q, index, k, id_offset, force_exact, stats, gt, mask_words)
+        return _score_topk_groups(q, index, k, id_offset, force_exact, stats, gt, masks)
 
 
-def _score_topk_groups(q, index, k, id_offset, force_exact, stats, gt: _GroupTable, mask_words, page_lists: bool = False):
+def _score_topk_groups(q, index, k, id_offset, force_exact, stats, gt: _GroupTable, masks, page_lists: bool = False):
     """_score_topk for groups. page_lists=True is the entry of the tests and measurements of the proof on page lists."""
-    return _score_topk(q, index, k, id_offset, force_exact, stats, mask_words, gt, page_lists)
+    return _score_topk(q, index, k, id_offset, force_exact, stats, masks, gt, page_lists)
 
 
 def merge_topk_groups(scores: torch.Tensor, pages: torch.Tensor, groups: torch.Tensor, k: int):
@@ -382,11 +450,12 @@ def gather_partials(scores: torch.Tensor, ids: torch.Tensor, group=None) -> Tupl
 
 
 def sharded_topk(queries: torch.Tensor, index: CorpusIndex, k: int, id_offset: int, group=None, stats: Optional[dict] = None,
-                 doc_mask: Optional[torch.Tensor] = None):
+                 doc_mask: Optional[torch.Tensor] = None, mask_of: Optional[torch.Tensor] = None):
     """Corpus sharded by page across ranks (every rank holds the same queries): local exact top-k with GLOBAL ids,
     one all-gather of [nq, k] (score, id) pairs over NCCL/NVLink, k-way merge on every rank (SURVEY.md §8e).
-    doc_mask: this rank's bool [nd] mask of its own shard (see score_topk)."""
-    s, i = score_topk(queries, index, k, id_offset, stats=stats, doc_mask=doc_mask)
+    doc_mask: this rank's bool [nd] mask of its own shard, or bool [M, nd] (this shard's columns of M masks) with mask_of
+    (see score_topk)."""
+    s, i = score_topk(queries, index, k, id_offset, stats=stats, doc_mask=doc_mask, mask_of=mask_of)
     if _world(group) == 1:
         return s, i
     ev = _Stages(stats)
@@ -398,19 +467,20 @@ def sharded_topk(queries: torch.Tensor, index: CorpusIndex, k: int, id_offset: i
 
 
 def sharded_topk_groups(queries: torch.Tensor, index: CorpusIndex, k: int, doc_groups: torch.Tensor, id_offset: int,
-                        group=None, stats: Optional[dict] = None, doc_mask: Optional[torch.Tensor] = None):
+                        group=None, stats: Optional[dict] = None, doc_mask: Optional[torch.Tensor] = None,
+                        mask_of: Optional[torch.Tensor] = None):
     """Document-level sharded_topk: doc_groups holds this shard's pages' GLOBAL group ids (a document may span ranks).
     Local group top-k with global page ids, one all-gather of [nq, k, 3] int64 (score bits, page, group), then the merge
     keeps the first k distinct groups. A group's best page lies on one rank, and that rank's local top-k holds it whenever
     the group is in the global top-k, so the result equals score_topk_groups over the whole corpus.
     world * k must be <= MERGE_GROUPS_MAX (512), checked before any work. Pass the same doc_groups tensor on every call:
-    the CSR is cached per tensor object."""
+    the CSR is cached per tensor object. doc_mask / mask_of as in sharded_topk."""
     import torch.distributed as dist
 
     if dist.is_available() and dist.is_initialized() and dist.get_world_size(group) * k > MERGE_GROUPS_MAX:
         raise ValueError(f"sharded_topk_groups: world * k = {dist.get_world_size(group) * k} > {MERGE_GROUPS_MAX}")
 
-    s, p, g = score_topk_groups(queries, index, k, doc_groups, id_offset, stats=stats, doc_mask=doc_mask)
+    s, p, g = score_topk_groups(queries, index, k, doc_groups, id_offset, stats=stats, doc_mask=doc_mask, mask_of=mask_of)
     if _world(group) == 1:
         return s, p, g
     ev = _Stages(stats)
