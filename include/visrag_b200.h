@@ -405,6 +405,37 @@ int vr_group_topk_rows_masks(const float* scores, int32_t rows, int64_t nd, cons
                              const vr_doc_masks* masks, int32_t k, int64_t id_offset, int32_t chunks, void* ws,
                              int64_t ws_bytes, float* out_scores, int64_t* out_pages, int64_t* out_groups, void* stream);
 
+/* Candidate lists: each query row scores only the docs of its list, reading those rows and no others.
+ * A list set holds `count` lists of local doc ids (before id_offset) in CSR form: list m is ids[offsets[m], offsets[m+1]).
+ * Query row r uses list of_query[r], which the caller keeps in [0, count); a NULL of_query means every row uses list 0.
+ * A list may be in any order and may repeat an id. offsets, ids and of_query are device pointers; the struct itself is
+ * read on the host during the call. A call over rows [r0, r0 + n) of a larger batch passes of_query + r0.
+ * Alignment (bytes) of the vr_doc_lists arrays: offsets 8, ids 4, of_query 4 */
+typedef struct {
+    const int64_t* offsets;    /* [count + 1], offsets[0] = 0, non-decreasing */
+    const int32_t* ids;        /* [offsets[count]] local doc ids */
+    int32_t count;             /* lists in the set, >= 1 */
+    const int32_t* of_query;   /* [rows]: the list of each query row, or NULL: list 0 for every row */
+} vr_doc_lists;
+
+/* vr_score_lists: the exact fp32 scores of every query row against the docs of its list, as a padded block
+ * [nq, width]: out_scores[r, j] = q_r . d[L(r)[j]] (the bits vr_score_exact gives that pair) and out_ids[r, j] = L(r)[j]
+ * for j < |L(r)|, then (-inf, -1). With doc_groups (the group table of the _groups calls), out_groups[r, j] is the group
+ * of the entry (-1 for padding); doc_groups and out_groups are both given or both NULL. An id outside [0, nd) is never
+ * read and gives (-inf, -1). This is the (scores, ids) input of vr_topk_rows, and with the groups that of
+ * vr_merge_group_topk, so a row's page or document top-k over its list equals the masked calls' with a mask of exactly
+ * the listed docs (a repeated id is emitted once by both selections). Rows that share a list and sit next to each other
+ * (sort the rows by list) read each listed row once per tile of up to 8 queries.
+ * *status (a device int32 the caller zeroes) gets bit 1 when a list is longer than width (its first width entries are
+ * scored) and bit 2 when an of_query value lies outside [0, count) (the row gets padding only).
+ * Refused before any CUDA call, naming the field: lists NULL, offsets or ids NULL or misaligned, count < 1, count > 1
+ * with a NULL of_query, a misaligned of_query, width < 1, dim % 4 != 0, nd >= 2^31, and a misaligned pointer below.
+ * Alignment (bytes) of the vr_score_lists arguments: q_f32 4, d_f32 16, doc_groups 4, out_scores 4, out_ids 8,
+ * out_groups 8, status 4 */
+int vr_score_lists(const float* q_f32, int32_t nq, const float* d_f32, int64_t nd, int32_t dim, const vr_doc_lists* lists,
+                   int32_t width, const int32_t* doc_groups, float* out_scores, int64_t* out_ids, int64_t* out_groups,
+                   int32_t* status, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -66,6 +66,17 @@ class DocMasks(C.Structure):
     ]
 
 
+class DocLists(C.Structure):
+    """Mirror of ``vr_doc_lists``: a list set in CSR form, query row r scoring list of_query[r] (NULL: list 0)."""
+
+    _fields_ = [
+        ("offsets", C.c_void_p),
+        ("ids", C.c_void_p),
+        ("count", C.c_int32),
+        ("of_query", C.c_void_p),
+    ]
+
+
 VR_ATTN_V_ONES_COLUMN = 1
 VR_ATTN_F16 = 2  # q / k / v / out are fp16
 
@@ -153,6 +164,8 @@ def _declare(lib: C.CDLL) -> None:
     lib.vr_topk_rows_chunked_masks.argtypes = [vp, i32, i64, i32, i64, i32, vp, vp, vp, vp, dm, vp]
     lib.vr_group_topk_rows_masks.restype = i32
     lib.vr_group_topk_rows_masks.argtypes = [vp, i32, i64, vp, i32, dm, i32, i64, i32, vp, i64, vp, vp, vp, vp]
+    lib.vr_score_lists.restype = i32
+    lib.vr_score_lists.argtypes = [vp, i32, vp, i64, i32, C.POINTER(DocLists), i32, vp, vp, vp, vp, vp, vp]
     lib.vr_pool_norm.restype = i32
     lib.vr_pool_norm.argtypes = [vp, i64, vp, f32, vp, i32, i32, i32, i32, vp, vp]
     lib.vr_prefix_rows.restype = i32

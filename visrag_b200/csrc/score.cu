@@ -992,6 +992,132 @@ __global__ void page_groups_kernel(const long long* __restrict__ pages, long lon
         groups[i] = pages[i] >= 0 ? __ldg(doc_groups + (pages[i] - id_offset)) : -1;
 }
 
+// ---------------------------------------------------------------------------------------------
+// Candidate lists (vr_doc_lists on the device): query row r scores the docs ids[offsets[m], offsets[m+1]) of list
+// m = of_query[r] (of_query NULL: list 0 for every row).
+struct DocLists {
+    const long long* offsets;
+    const int* ids;
+    int count;
+    const int* of_query;
+};
+
+// Status bits of list_scores_kernel (OR-ed into the caller's word)
+constexpr int LS_TRUNCATED = 1;   // a list is longer than `width`: only its first `width` entries were scored
+constexpr int LS_BAD_LIST = 2;    // an of_query value outside [0, count): the row was given an empty list
+
+// Exact fp32 scores of the listed docs only, into a padded block [nq, width]: position j of row r holds
+// (q_r . D[L(r)[j]], L(r)[j]) for j < |L(r)| and (-inf, -1) after it, and with doc_groups the group of the entry (-1 for
+// padding) in out_groups. Ids outside [0, nd) are skipped: they give (-inf, -1) and are never read. Block (x, y) takes
+// the NQ query rows [x NQ, x NQ + NQ) and list positions [y chunk, (y + 1) chunk). Consecutive rows with the same list
+// (a run: the caller sorts rows by list) are scored together: a warp reads EX_DW listed rows once and applies them to
+// every query of the run from shared memory, as exact_scores_kernel does for the whole index; a row that is alone in
+// its list streams its own rows. A lane's FMA chain and the warp reduction are those of exact_scores_kernel and
+// warp_dot_row (float4s lane, lane + 32, ..., x y z w in turn, then warp_sum_f), so every score has the bits
+// vr_score_exact gives the same (query, doc) pair.
+template <int NQ>
+__global__ void __launch_bounds__(256)
+list_scores_kernel(const float* __restrict__ Q, int nq, const float* __restrict__ D, long long nd, int dim,
+                   const DocLists lists, int width, int chunk, const int* __restrict__ doc_groups,
+                   float* __restrict__ out_scores, long long* __restrict__ out_ids, long long* __restrict__ out_groups,
+                   int* __restrict__ status) {
+    extern __shared__ float qsm[];  // [NQ, dim]: the query rows of the current run
+    __shared__ int row_list[NQ];
+    const int q0 = blockIdx.x * NQ;
+    const int nqb = min(NQ, nq - q0);
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const int nv = dim >> 2;
+    const int p_lo = blockIdx.y * chunk, p_hi = min(width, p_lo + chunk);
+    if (threadIdx.x < nqb) {
+        int m = lists.of_query ? __ldg(lists.of_query + q0 + threadIdx.x) : 0;
+        if (m < 0 || m >= lists.count) {
+            atomicOr(status, LS_BAD_LIST);
+            m = -1;
+        }
+        row_list[threadIdx.x] = m;
+    }
+    __syncthreads();
+    for (int a = 0; a < nqb;) {  // runs [a, b) of rows with one list (block-uniform)
+        const int m = row_list[a];
+        int b = a + 1;
+        while (b < nqb && row_list[b] == m) ++b;
+        const int nr = b - a;
+        long long off = 0, len = 0;
+        if (m >= 0) {
+            off = __ldg(lists.offsets + m);
+            len = __ldg(lists.offsets + m + 1) - off;
+        }
+        if (len > width && blockIdx.y == 0 && threadIdx.x == 0) atomicOr(status, LS_TRUNCATED);
+        const int n = static_cast<int>(max(0ll, min(len, static_cast<long long>(width))));
+        if (p_lo < n)
+            for (int i = threadIdx.x; i < nr * dim; i += blockDim.x) qsm[i] = Q[static_cast<long long>(q0 + a) * dim + i];
+        __syncthreads();
+        for (int pos0 = p_lo + warp * EX_DW; pos0 < p_hi; pos0 += 8 * EX_DW) {
+            if (pos0 >= n) {  // past the list: padding only
+                for (int t = lane; t < nr * EX_DW; t += 32) {
+                    const int pos = pos0 + t % EX_DW;
+                    if (pos < p_hi) {
+                        const long long o = static_cast<long long>(q0 + a + t / EX_DW) * width + pos;
+                        out_scores[o] = -INFINITY;
+                        out_ids[o] = -1;
+                        if (out_groups) out_groups[o] = -1;
+                    }
+                }
+                continue;
+            }
+            int id[EX_DW];
+            const float4* drow[EX_DW];
+#pragma unroll
+            for (int d = 0; d < EX_DW; ++d) {
+                const int v = pos0 + d < n ? __ldg(lists.ids + off + pos0 + d) : -1;
+                id[d] = v >= 0 && v < nd ? v : -1;
+                drow[d] = reinterpret_cast<const float4*>(D + static_cast<long long>(id[d] >= 0 ? id[d] : 0) * dim);
+            }
+            float acc[EX_DW][NQ];
+#pragma unroll
+            for (int d = 0; d < EX_DW; ++d)
+#pragma unroll
+                for (int j = 0; j < NQ; ++j) acc[d][j] = 0.f;
+#pragma unroll(NQ <= 2 ? 3 : 1)
+            for (int i = lane; i < nv; i += 32) {
+                float4 x[EX_DW];
+#pragma unroll
+                for (int d = 0; d < EX_DW; ++d) x[d] = __ldg(drow[d] + i);  // other query tiles may read the row next
+#pragma unroll
+                for (int j = 0; j < NQ; ++j) {
+                    if (j < nr) {
+                        const float4 y = reinterpret_cast<const float4*>(qsm + j * dim)[i];
+#pragma unroll
+                        for (int d = 0; d < EX_DW; ++d) {
+                            acc[d][j] = fmaf(x[d].x, y.x, acc[d][j]);
+                            acc[d][j] = fmaf(x[d].y, y.y, acc[d][j]);
+                            acc[d][j] = fmaf(x[d].z, y.z, acc[d][j]);
+                            acc[d][j] = fmaf(x[d].w, y.w, acc[d][j]);
+                        }
+                    }
+                }
+            }
+#pragma unroll
+            for (int j = 0; j < NQ; ++j) {
+                if (j < nr) {
+#pragma unroll
+                    for (int d = 0; d < EX_DW; ++d) {
+                        const float s = warp_sum_f(acc[d][j]);
+                        if (lane == d && pos0 + d < p_hi) {
+                            const long long o = static_cast<long long>(q0 + a + j) * width + pos0 + d;
+                            out_scores[o] = id[d] >= 0 ? s : -INFINITY;
+                            out_ids[o] = id[d];
+                            if (out_groups) out_groups[o] = id[d] >= 0 ? __ldg(doc_groups + id[d]) : -1;
+                        }
+                    }
+                }
+            }
+        }
+        __syncthreads();  // qsm is reloaded by the next run
+        a = b;
+    }
+}
+
 // Merge of per-rank partial group lists [rows, cols] (score, page, group; page < 0 = empty): the first k distinct groups
 // in (score desc, page asc) order, one warp per row, the row in registers. Each round takes the best live entry and then
 // retires every entry of its group: the first entry of a group in that order is its best.
@@ -1614,6 +1740,73 @@ extern "C" int vr_merge_group_topk(const float* scores, const int64_t* pages, co
         merge_groups_warp_kernel<4><<<(rows + 7) / 8, 256, 0, st>>>(scores, p, g, rows, cols, k, out_scores, op, og);
     else
         merge_groups_warp_kernel<16><<<(rows + 7) / 8, 256, 0, st>>>(scores, p, g, rows, cols, k, out_scores, op, og);
+    VR_CHECK_CUDA(cudaGetLastError());
+    return 0;
+}
+
+// ---------------------------------------------------------------------------------------------------- candidate lists
+// A list set as vr_score_lists takes it, refused before any CUDA call unless its arrays can be read. The offsets, the ids
+// and the values of of_query lie in device memory: the caller keeps them consistent (ids outside [0, nd) are skipped,
+// an of_query value outside [0, count) and a list longer than width are reported in *status).
+static int lists_check(const char* fn, const vr_doc_lists* l) {
+    VR_REQUIRE(l, "%s: lists must not be NULL", fn);
+    VR_REQUIRE(l->offsets, "%s: lists->offsets must not be NULL", fn);
+    VR_REQUIRE(l->ids, "%s: lists->ids must not be NULL", fn);
+    VR_REQUIRE_ALIGNED(fn, "lists->offsets", l->offsets, 8);
+    VR_REQUIRE_ALIGNED(fn, "lists->ids", l->ids, 4);
+    VR_REQUIRE(l->count >= 1, "%s: lists->count=%d, needs at least one list", fn, l->count);
+    VR_REQUIRE(l->count == 1 || l->of_query, "%s: lists->of_query is NULL with lists->count=%d lists", fn, l->count);
+    VR_REQUIRE_ALIGNED(fn, "lists->of_query", l->of_query, 4);
+    return 0;
+}
+
+extern "C" int vr_score_lists(const float* q_f32, int32_t nq, const float* d_f32, int64_t nd, int32_t dim,
+                              const vr_doc_lists* lists, int32_t width, const int32_t* doc_groups, float* out_scores,
+                              int64_t* out_ids, int64_t* out_groups, int32_t* status, void* stream) {
+    const char* fn = "vr_score_lists";
+    if (int rc = lists_check(fn, lists)) return rc;
+    VR_REQUIRE(q_f32 && d_f32 && out_scores && out_ids && status, "%s: null pointer", fn);
+    VR_REQUIRE(!doc_groups == !out_groups, "%s: doc_groups and out_groups go together (both or neither)", fn);
+    VR_REQUIRE(width >= 1, "%s: width=%d, needs at least 1", fn, width);
+    VR_REQUIRE(nq > 0 && dim > 0 && dim % 4 == 0, "%s: bad shape nq=%d dim=%d (dim %% 4 == 0)", fn, nq, dim);
+    VR_REQUIRE(nd > 0 && nd < 2147483647ll, "%s: nd=%lld beyond the int32 doc ids", fn, (long long)nd);
+    VR_REQUIRE_ALIGNED(fn, "q_f32", q_f32, 4);
+    VR_REQUIRE_ALIGNED(fn, "d_f32", d_f32, 16);  // float4 rows (dim % 4 == 0 keeps every row aligned)
+    VR_REQUIRE_ALIGNED(fn, "doc_groups", doc_groups, 4);
+    VR_REQUIRE_ALIGNED(fn, "out_scores", out_scores, 4);
+    VR_REQUIRE_ALIGNED(fn, "out_ids", out_ids, 8);
+    VR_REQUIRE_ALIGNED(fn, "out_groups", out_groups, 8);
+    VR_REQUIRE_ALIGNED(fn, "status", status, 4);
+    // rows per tile: runs of rows sharing a list can only form when some list serves several rows
+    const bool shared = !lists->of_query || lists->count < nq;
+    const int NQ = !shared ? 1 : nq >= EX_QB ? EX_QB : (nq >= 4 ? 4 : (nq >= 2 ? 2 : 1));
+    const size_t smem = static_cast<size_t>(NQ) * dim * sizeof(float);
+    VR_REQUIRE(smem <= 200 * 1024, "%s: dim too large", fn);
+    // list positions per block: about four blocks per SM over the whole block, whole warps of EX_DW, <= 65535 chunks
+    const long long tiles = (nq + NQ - 1) / NQ;
+    long long chunk = static_cast<long long>(width) * tiles / (4ll * num_sms());
+    if (chunk > 2048) chunk = 2048;
+    if (chunk < (width + 65534ll) / 65535) chunk = (width + 65534ll) / 65535;
+    chunk = (chunk + 8 * EX_DW - 1) / (8 * EX_DW) * (8 * EX_DW);
+    if (chunk < 8 * EX_DW) chunk = 8 * EX_DW;
+    const dim3 grid(static_cast<unsigned>(tiles), static_cast<unsigned>((width + chunk - 1) / chunk));
+    const DocLists dl = {reinterpret_cast<const long long*>(lists->offsets), lists->ids, lists->count, lists->of_query};
+    cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+    long long* oi = reinterpret_cast<long long*>(out_ids);
+    long long* og = reinterpret_cast<long long*>(out_groups);
+#define VR_LISTS_LAUNCH(N)                                                                                              \
+    do {                                                                                                                \
+        static unsigned long long attr_set = 0;                                                                         \
+        if (smem > 48 * 1024 && first_use_on_device(&attr_set))                                                         \
+            VR_CHECK_CUDA(cudaFuncSetAttribute(list_scores_kernel<N>, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024)); \
+        list_scores_kernel<N><<<grid, 256, smem, st>>>(q_f32, nq, d_f32, nd, dim, dl, width, static_cast<int>(chunk),      \
+                                                       doc_groups, out_scores, oi, og, status);                         \
+    } while (0)
+    if (NQ == EX_QB) VR_LISTS_LAUNCH(EX_QB);
+    else if (NQ == 4) VR_LISTS_LAUNCH(4);
+    else if (NQ == 2) VR_LISTS_LAUNCH(2);
+    else VR_LISTS_LAUNCH(1);
+#undef VR_LISTS_LAUNCH
     VR_CHECK_CUDA(cudaGetLastError());
     return 0;
 }

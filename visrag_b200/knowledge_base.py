@@ -11,7 +11,8 @@ Scores are the same fp32 dot products; ties are ordered by lower page index (tor
 
 Beyond the reference: a search can be restricted to some pages (`within`, e.g. the pages of one PDF), pages can be
 removed (a tombstone bit, so the other pages keep their indices) and added, and `save` writes the live pages back in the
-demo's layout. All of it runs as a doc mask inside the same kernels, with the same exact fp32 results. A batch of queries
+demo's layout. A scope runs as a doc mask inside the same kernels, or, when it is small, as a candidate list of its pages
+that reads only those pages (`list_path_wins`), with the same exact fp32 results either way. A batch of queries
 can give each query its own scope (`within_each`, e.g. each question about its own PDF, or each user's own collections):
 one pass over the index serves them all, and each query's row equals its search alone.
 
@@ -60,6 +61,24 @@ def save_knowledge_base(path: str, reps, filenames: Sequence[str]) -> None:
         f.write("\n".join(filenames))
 
 
+LIST_TILE = 8              # queries that share a list and read each of its rows once (vr_score_lists' query tile)
+LIST_ROUTE = 1.0           # index rows per 256-query block the masked path costs, per listed row of the list path
+LIST_FIXED_ROWS = 80_000   # the list path's fixed cost (checks, launches, two host reads), in index rows of one query
+
+
+def list_path_wins(list_rows: int, nq: int, nd: int, k: int, documents: bool) -> bool:
+    """The routing rule of scoped searches. list_rows is the listed page rows summed over the distinct scopes, each scope
+    counted once per tile of LIST_TILE queries that search it (a None scope, every live page, counts nd rows): what the
+    list path reads, at 4 * dim bytes a row. The masked path passes over all nd rows once per 256-query block. Lists win
+    when list_rows + LIST_FIXED_ROWS < LIST_ROUTE * nd * ceil(nq / 256). The constants come from the measurements in the
+    README (H100, dim 2304): a listed row and an index row per 256-query block cost about the same (3-6 ns), and the list
+    path's fixed cost is about that of scanning 65-80 k rows for one query. Documents with k above
+    retriever.LIST_GROUPS_MAX_K take the masks."""
+    if documents and k > retriever.LIST_GROUPS_MAX_K:
+        return False
+    return list_rows + LIST_FIXED_ROWS < LIST_ROUTE * nd * -(-nq // 256)
+
+
 class KnowledgeBase:
     """A knowledge base resident on one GPU. Pages keep their index (row) for the life of the object: `remove` only marks
     a page dead, and `add` appends."""
@@ -103,63 +122,94 @@ class KnowledgeBase:
         except KeyError as e:
             raise KeyError(f"no live page named {e.args[0]!r} in the knowledge base") from None
 
+    def _queries(self, query_reps) -> torch.Tensor:
+        """queries [nq, d] fp32 on the index's device."""
+        q = query_reps if isinstance(query_reps, torch.Tensor) else torch.from_numpy(np.asarray(query_reps, dtype=np.float32))
+        return q.to(self.index.emb.device, torch.float32).reshape(-1, self.index.emb.shape[1]).contiguous()
+
     def _query_and_mask(self, query_reps, within: Optional[Iterable[str]]):
         """(queries [nq, d] fp32 on the index's device, bool [nd] mask of the pages searched or None for every page, number
         of pages searched)."""
-        q = query_reps if isinstance(query_reps, torch.Tensor) else torch.from_numpy(np.asarray(query_reps, dtype=np.float32))
-        q = q.to(self.index.emb.device, torch.float32).reshape(-1, self.index.emb.shape[1]).contiguous()
+        q = self._queries(query_reps)
         if within is None:
             return q, None if len(self) == self.index.nd else self._live, len(self)  # None: the unmasked kernels
         rows = self._rows(within)
-        mask = torch.zeros(self.index.nd, dtype=torch.bool, device=q.device)
-        mask[torch.tensor(rows, dtype=torch.int64, device=q.device)] = True
-        return q, mask, len(rows)
+        return q, self._scope_masks([rows]).view(-1), len(rows)
 
-    def _query_and_scopes(self, query_reps, within, within_each):
-        """Per-query scopes: (queries, bool [M, nd] masks of the M distinct scopes, mask_of [nq] int32, the live page rows
-        of each distinct scope). Identical scopes share one mask row; None is every live page."""
-        if within is not None:
-            raise ValueError("within and within_each cannot be combined: give every query its scope in within_each")
-        q, _, _ = self._query_and_mask(query_reps, None)
-        scopes = list(within_each)
-        if len(scopes) != q.shape[0]:
-            raise ValueError(f"within_each has {len(scopes)} entries for {q.shape[0]} queries (one scope per query)")
-        slot, rows_of, mask_of = {}, [], []
-        for scope in scopes:
-            key = None if scope is None else tuple(self._rows(scope))
-            if key not in slot:
-                slot[key] = len(rows_of)
-                rows_of.append(key)
-            mask_of.append(slot[key])
-        dev = q.device
-        masks = torch.zeros((len(rows_of), self.index.nd), dtype=torch.bool, device=dev)
-        every = [m for m, rows in enumerate(rows_of) if rows is None]
-        pairs = [(m, r) for m, rows in enumerate(rows_of) if rows is not None for r in rows]
+    def _scope_masks(self, scopes: Sequence[Optional[Sequence[int]]]) -> torch.Tensor:
+        """bool [M, nd]: row m marks the page rows of scope m (None: every live page)."""
+        dev = self.index.emb.device
+        masks = torch.zeros((len(scopes), self.index.nd), dtype=torch.bool, device=dev)
+        every = [m for m, rows in enumerate(scopes) if rows is None]
+        pairs = [(m, r) for m, rows in enumerate(scopes) if rows is not None for r in rows]
         if every:
             masks[torch.tensor(every, dtype=torch.int64, device=dev)] = self._live
         if pairs:
             idx = torch.tensor(pairs, dtype=torch.int64, device=dev)
             masks[idx[:, 0], idx[:, 1]] = True
-        live = torch.nonzero(self._live).flatten().tolist() if every else []
-        rows_of = [live if rows is None else list(rows) for rows in rows_of]
-        return q, masks, torch.tensor(mask_of, dtype=torch.int32, device=dev), rows_of
+        return masks
+
+    def _query_and_scopes(self, query_reps, within, within_each):
+        """Per-query scopes: (queries, the distinct scopes (sorted page rows, or None for every live page), list_of [nq]
+        int32 (the scope of each query), the live page rows of each distinct scope). Identical scopes are one scope."""
+        if within is not None:
+            raise ValueError("within and within_each cannot be combined: give every query its scope in within_each")
+        q = self._queries(query_reps)
+        scopes = list(within_each)
+        if len(scopes) != q.shape[0]:
+            raise ValueError(f"within_each has {len(scopes)} entries for {q.shape[0]} queries (one scope per query)")
+        slot, keys, scope_of = {}, [], []
+        for scope in scopes:
+            key = None if scope is None else tuple(self._rows(scope))
+            if key not in slot:
+                slot[key] = len(keys)
+                keys.append(key)
+            scope_of.append(slot[key])
+        live = torch.nonzero(self._live).flatten().tolist() if None in slot else []
+        rows_of = [live if rows is None else list(rows) for rows in keys]
+        return q, keys, torch.tensor(scope_of, dtype=torch.int32, device=q.device), rows_of
+
+    def _lists(self, rows_of: Sequence[Sequence[int]]) -> Tuple[torch.Tensor, torch.Tensor]:
+        """The candidate lists (offsets, ids) of the scopes' page rows."""
+        dev = self.index.emb.device
+        offsets = torch.tensor(np.cumsum([0] + [len(r) for r in rows_of]), dtype=torch.int64, device=dev)
+        ids = torch.tensor([r for rows in rows_of for r in rows], dtype=torch.int32, device=dev)
+        return offsets, ids
+
+    def _use_lists(self, keys, rows_of, scope_of: Optional[torch.Tensor], nq: int, k: int, documents: bool) -> bool:
+        """Whether these scopes go through candidate lists (see list_path_wins); a None scope counts as nd pages."""
+        per_scope = torch.bincount(scope_of.long(), minlength=len(keys)).tolist() if scope_of is not None else [nq]
+        rows = sum((self.index.nd if key is None else len(r)) * -(-n // LIST_TILE)
+                   for key, r, n in zip(keys, rows_of, per_scope))
+        return list_path_wins(rows, nq, self.index.nd, k, documents)
 
     def search(self, query_reps, topk: int, within: Optional[Iterable[str]] = None,
                within_each: Optional[Sequence[Optional[Iterable[str]]]] = None) -> Tuple[torch.Tensor, torch.Tensor]:
         """query_reps [nq, d] (tensor or ndarray, fp32) -> (scores [nq,k] f32, page indices [nq,k] i64) on the device.
         within: page filenames to search (default: every live page); k = min(topk, pages searched).
         within_each: one scope per query instead (a list of page filenames, or None for every live page), all searched in
-        one pass; k = min(topk, pages of the largest scope), and a query whose scope is shorter ends in (-inf, -1)."""
+        one pass; k = min(topk, pages of the largest scope), and a query whose scope is shorter ends in (-inf, -1).
+        Small scopes are scored from candidate lists of their pages (list_path_wins), the others through masks of the
+        whole index: the results are the same bits either way."""
         if within_each is not None:
-            q, masks, mask_of, rows_of = self._query_and_scopes(query_reps, within, within_each)
+            q, keys, scope_of, rows_of = self._query_and_scopes(query_reps, within, within_each)
             k = min(topk, max(len(rows) for rows in rows_of)) if rows_of else 0
+        elif within is not None:
+            q, keys, scope_of = self._queries(query_reps), [tuple(self._rows(within))], None
+            rows_of = [list(keys[0])]
+            k = min(topk, len(rows_of[0]))
         else:
-            q, masks, n = self._query_and_mask(query_reps, within)
-            mask_of, k = None, min(topk, n)
+            q, masks, n = self._query_and_mask(query_reps, None)
+            keys, k = None, min(topk, n)
         if k == 0:
             return (torch.empty((q.shape[0], 0), dtype=torch.float32, device=q.device),
                     torch.empty((q.shape[0], 0), dtype=torch.int64, device=q.device))
-        return retriever.score_topk(q, self.index, k, doc_mask=masks, mask_of=mask_of)  # enters the index's device itself
+        if keys is None:
+            return retriever.score_topk(q, self.index, k, doc_mask=masks)  # enters the index's device itself
+        if self._use_lists(keys, rows_of, scope_of, q.shape[0], k, documents=False):
+            return retriever.score_topk(q, self.index, k, doc_lists=self._lists(rows_of), list_of=scope_of)
+        masks = self._scope_masks(keys)
+        return retriever.score_topk(q, self.index, k, doc_mask=masks if scope_of is not None else masks[0], mask_of=scope_of)
 
     def search_documents(self, query_reps, topk: int, within: Optional[Iterable[str]] = None,
                          within_each: Optional[Sequence[Optional[Iterable[str]]]] = None
@@ -168,19 +218,32 @@ class KnowledgeBase:
         device, document names [nq][k]). within: page filenames to search (default: every live page); k = min(topk,
         documents searched). Ties rank the document with the lower best page index first.
         within_each: one scope per query, as in search; k = min(topk, documents of the largest scope), a shorter row ends
-        in (-inf, -1), and each query's names list holds only the documents it found."""
+        in (-inf, -1), and each query's names list holds only the documents it found. Scopes are routed as in search."""
         if within_each is not None:
-            q, masks, mask_of, rows_of = self._query_and_scopes(query_reps, within, within_each)
+            q, keys, scope_of, rows_of = self._query_and_scopes(query_reps, within, within_each)
             groups = self._doc_groups.tolist()
             k = min(topk, max(len({groups[r] for r in rows}) for rows in rows_of)) if rows_of else 0
+        elif within is not None:
+            q, keys, scope_of = self._queries(query_reps), [tuple(self._rows(within))], None
+            rows_of = [list(keys[0])]
+            idx = torch.tensor(rows_of[0], dtype=torch.int64, device=q.device)
+            k = min(topk, int(torch.unique(self._doc_groups[idx]).numel()))   # documents searched, counted on the device
         else:
-            q, masks, _ = self._query_and_mask(query_reps, within)
+            q, masks, _ = self._query_and_mask(query_reps, None)
             searched = self._doc_groups if masks is None else self._doc_groups[masks]
-            mask_of, k = None, min(topk, int(torch.unique(searched).numel()))   # documents searched, counted on the device
+            keys, k = None, min(topk, int(torch.unique(searched).numel()))
         if k == 0:
             return (torch.empty((q.shape[0], 0), dtype=torch.float32, device=q.device),
                     torch.empty((q.shape[0], 0), dtype=torch.int64, device=q.device), [[] for _ in range(q.shape[0])])
-        s, p, g = retriever.score_topk_groups(q, self.index, k, self._doc_groups, doc_mask=masks, mask_of=mask_of)
+        if keys is None:
+            s, p, g = retriever.score_topk_groups(q, self.index, k, self._doc_groups, doc_mask=masks)
+        elif self._use_lists(keys, rows_of, scope_of, q.shape[0], k, documents=True):
+            s, p, g = retriever.score_topk_groups(q, self.index, k, self._doc_groups, doc_lists=self._lists(rows_of),
+                                                  list_of=scope_of)
+        else:
+            masks = self._scope_masks(keys)
+            s, p, g = retriever.score_topk_groups(q, self.index, k, self._doc_groups,
+                                                  doc_mask=masks if scope_of is not None else masks[0], mask_of=scope_of)
         return s, p, [[self.documents[j] for j in row if j >= 0] for row in g.tolist()]
 
     def retrieve_documents(self, query_rep, topk: int, within: Optional[Iterable[str]] = None) -> List[Tuple[str, str]]:

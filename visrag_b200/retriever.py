@@ -14,6 +14,8 @@ merges after ONE all-gather of [nq, k] (score, id) pairs. Both take an optional 
 shard): only the docs it marks are searched, and the result equals the fp32 scan over those docs alone. A 2-D doc_mask
 (bool [M, nd]) with `mask_of` (int [nq] in [0, M), default row i for query i) gives every query its own subset, in the
 same one pass over the index: each query's row equals its call alone with its own mask.
+Candidate lists (`doc_lists=(offsets, ids)`, CSR, with `list_of`): each query scores only the pages of its list and reads
+no others; the result equals the masked call with a mask of exactly the listed pages, bit for bit.
 
 Document-level retrieval (`score_topk_groups`, `sharded_topk_groups`): `doc_groups` (int [nd]) gives every doc (page) its
 group (document); the top-k groups by their best page's exact fp32 score, ranked by (score desc, best page asc).
@@ -178,14 +180,24 @@ def _exact_topk(q: torch.Tensor, index: CorpusIndex, k: int, id_offset: int, mas
 
 
 def score_topk(queries: torch.Tensor, index: CorpusIndex, k: int, id_offset: int = 0, force_exact: bool = False,
-               stats: Optional[dict] = None, doc_mask: Optional[torch.Tensor] = None, mask_of: Optional[torch.Tensor] = None
+               stats: Optional[dict] = None, doc_mask: Optional[torch.Tensor] = None, mask_of: Optional[torch.Tensor] = None,
+               doc_lists: Optional[Tuple[torch.Tensor, torch.Tensor]] = None, list_of: Optional[torch.Tensor] = None
                ) -> Tuple[torch.Tensor, torch.Tensor]:
     """Exact fp32 top-k of `queries @ index.emb.T`: (scores [nq,k] f32, ids [nq,k] i64 = local index + id_offset).
     Rows are sorted by (score desc, id asc); if k > nd the tail is (-inf, -1).
     doc_mask: optional bool [nd] on the index's device; only docs marked True are searched (the same bits as the fp32 scan
     over those docs alone). With fewer than k of them the tail is (-inf, -1).
     Per-query masks: doc_mask bool [M, nd] and mask_of int [nq] in [0, M) (default: row i for query i, M == nq); query i
-    searches the docs of row mask_of[i], and its row equals its call alone with that row as a 1-D doc_mask."""
+    searches the docs of row mask_of[i], and its row equals its call alone with that row as a 1-D doc_mask.
+    Candidate lists: doc_lists = (offsets int [M+1] from 0, non-decreasing; ids int32/int64 local doc ids) holds M lists in
+    CSR form, list m = ids[offsets[m]:offsets[m+1]] (any order, repeats count once), and list_of int [nq] in [0, M) picks
+    each query's list (default: list i for query i when M == nq, or the one list for every query when M == 1). Only the
+    listed docs are read; each row equals this call with a doc_mask of exactly its list's docs. stats["path"] is "lists".
+    doc_lists cannot be combined with doc_mask or mask_of."""
+    if doc_lists is not None or list_of is not None:
+        q, ls = _queries_and_lists(queries, index, doc_mask, mask_of, doc_lists, list_of)
+        with L.on_device(q.device):
+            return _lists_topk(q, index, k, id_offset, ls, None, stats)
     q, masks = _queries_and_mask(queries, index, doc_mask, mask_of)
     with L.on_device(q.device):
         return _score_topk(q, index, k, id_offset, force_exact, stats, masks)
@@ -202,6 +214,178 @@ def _queries_and_mask(queries: torch.Tensor, index: CorpusIndex, doc_mask: Optio
             raise ValueError("mask_of needs a 2-D doc_mask [M, nd] to pick rows from")
         return q, None
     return q, _check_doc_mask(doc_mask, index, q.shape[0], mask_of)
+
+
+@dataclass
+class _ListSet:
+    """A validated list set on the index's device: offsets int64 [M + 1], ids int32, of_query int32 [nq] (None: list 0 for
+    every row), width = the longest list a query uses, sort = the rows must be grouped by list first (list_of given)."""
+    offsets: torch.Tensor
+    ids: torch.Tensor
+    of_query: Optional[torch.Tensor]
+    width: int
+    sort: bool
+
+    def arg(self, of_query: Optional[torch.Tensor], r0: int = 0):
+        """The vr_doc_lists of the query rows from r0 on, of_query being this call's (possibly sorted) list of each row."""
+        ls = L.DocLists()
+        ls.offsets, ls.ids, ls.count = self.offsets.data_ptr(), self.ids.data_ptr(), self.offsets.shape[0] - 1
+        ls.of_query = None if of_query is None else of_query[r0:].data_ptr()
+        return C.byref(ls)
+
+    def masks(self, nd: int) -> Tuple[torch.Tensor, Optional[torch.Tensor]]:
+        """The equivalent (doc_mask, mask_of) of the masked calls: bool [nd] for one shared list, else bool [M, nd]."""
+        M = self.offsets.shape[0] - 1
+        lens = self.offsets[1:] - self.offsets[:-1]
+        m = torch.zeros((M, nd), dtype=torch.bool, device=self.ids.device)
+        m[torch.repeat_interleave(torch.arange(M, device=self.ids.device), lens), self.ids.long()] = True
+        return (m[0], None) if self.of_query is None else (m, self.of_query)
+
+
+def _int_tensor(t, name: str, shape: Optional[int], device) -> None:
+    if not isinstance(t, torch.Tensor) or t.dtype not in (torch.int32, torch.int64):
+        raise ValueError(f"{name} must be an int32 or int64 torch tensor")
+    if t.dim() != 1 or (shape is not None and t.shape[0] != shape):
+        want = f"[{shape}]" if shape is not None else "1-D"
+        raise ValueError(f"{name} must have shape {want}, got {list(t.shape)}")
+    if t.device != device:
+        raise ValueError(f"{name} lives on {t.device}, the index on {device}")
+
+
+def _check_doc_lists(doc_lists, index: CorpusIndex, nq: int, list_of: Optional[torch.Tensor] = None) -> _ListSet:
+    """Validate doc_lists = (offsets, ids) and list_of on the index's device (one host read for all the value checks)."""
+    if not isinstance(doc_lists, (tuple, list)) or len(doc_lists) != 2:
+        raise ValueError("doc_lists must be a pair (offsets, ids) of int tensors")
+    offsets, ids = doc_lists
+    dev = index.emb.device
+    _int_tensor(offsets, "doc_lists offsets", None, dev)
+    _int_tensor(ids, "doc_lists ids", None, dev)
+    M = offsets.shape[0] - 1
+    if M < 1:
+        raise ValueError("doc_lists offsets must have M + 1 >= 2 entries (M lists)")
+    if list_of is None:
+        if M not in (1, nq):
+            raise ValueError(f"doc_lists has {M} lists for {nq} queries: pass list_of, one list per query, or one list")
+        of_query = torch.arange(nq, dtype=torch.int32, device=dev) if M > 1 else None
+    else:
+        _int_tensor(list_of, "list_of", nq, dev)
+        of_query = list_of.to(torch.int32).contiguous()
+    offsets = offsets.to(torch.int64).contiguous()
+    lens = offsets[1:] - offsets[:-1]
+    used = lens if of_query is None else lens.index_select(0, of_query.clamp(0, M - 1).long())
+    z = offsets.new_zeros(())
+    vals = torch.stack([offsets[0], offsets[-1], lens.min(), used.max() if used.numel() else z,
+                        ids.min().long() if ids.numel() else z, ids.max().long() if ids.numel() else z,
+                        of_query.min().long() if nq and of_query is not None else z,
+                        of_query.max().long() if nq and of_query is not None else z]).tolist()
+    first, last, min_len, width, lo, hi, lq, hq = vals
+    if first != 0:
+        raise ValueError(f"doc_lists offsets must start at 0, got {first}")
+    if min_len < 0:
+        raise ValueError("doc_lists offsets must be non-decreasing")
+    if last != ids.shape[0]:
+        raise ValueError(f"doc_lists offsets must end at len(ids) = {ids.shape[0]}, got {last}")
+    if ids.numel() and (lo < 0 or hi >= index.nd):
+        raise ValueError(f"doc_lists ids must lie in [0, {index.nd}) (local docs of the index), got [{lo}, {hi}]")
+    if list_of is not None and nq and (lq < 0 or hq >= M):
+        raise ValueError(f"list_of must lie in [0, {M}) (lists of doc_lists), got [{lq}, {hq}]")
+    ids = ids.to(torch.int32).contiguous() if ids.numel() else torch.zeros(1, dtype=torch.int32, device=dev)  # never read
+    return _ListSet(offsets, ids, of_query, max(1, width), list_of is not None)
+
+
+def _queries_and_lists(queries, index: CorpusIndex, doc_mask, mask_of, doc_lists, list_of):
+    """The queries (as _queries_and_mask) and the validated list set."""
+    if doc_mask is not None or mask_of is not None:
+        raise ValueError("doc_lists cannot be combined with doc_mask or mask_of")
+    if doc_lists is None:
+        raise ValueError("list_of needs doc_lists to pick lists from")
+    q, _ = _queries_and_mask(queries, index, None)
+    return q, _check_doc_lists(doc_lists, index, q.shape[0], list_of)
+
+
+LIST_CHUNK = 4096  # list positions per first-level row of the page selection (the chunked scan's 4096 columns a block)
+
+
+def _lists_topk(q: torch.Tensor, index: CorpusIndex, k: int, id_offset: int, ls: _ListSet, gt: Optional["_GroupTable"],
+                stats: Optional[dict]):
+    """Top-k over candidate lists: vr_score_lists writes each row's listed (score, id[, group]) entries into a padded
+    [n, W] block, and the selection kernels of the masked path pick from it. Pages: vr_topk_rows, in two levels when W
+    > LIST_CHUNK ([n * C, LIST_CHUNK] rows with id_offset 0, then their [n, C * k] lists). Documents (k <= 256):
+    vr_merge_group_topk over [n * C, 512] rows, repeated over the [n, C * k] results until a row fits 512 entries."""
+    nq, d = q.shape
+    grouped = gt is not None
+    dtypes = (torch.float32, torch.int64) if not grouped else (torch.float32, torch.int64, torch.int64)
+    out = tuple(torch.empty((nq, k), dtype=t, device=q.device) for t in dtypes)
+    if stats is not None:
+        stats.update(path="lists", flagged=0)
+    if nq == 0:
+        return out
+    if d != index.emb.shape[1]:
+        raise ValueError("query / corpus dim mismatch")
+    lib, sp = L.lib(), L.stream_ptr()
+    of, order = ls.of_query, None
+    if ls.sort:  # rows of one list next to each other, so that a tile of queries reads each listed row once
+        order = torch.sort(of, stable=True).indices
+        q, of = q.index_select(0, order), of.index_select(0, order)
+    step = MERGE_GROUPS_MAX if grouped else LIST_CHUNK
+    W = ls.width if ls.width <= step else -(-ls.width // step) * step
+    rows_per = max(1, min(nq, (1 << 30) // (W * (20 if grouped else 12))))  # <= 1 GiB of [n, W] entries
+    sc = torch.empty((rows_per, W), dtype=torch.float32, device=q.device)
+    si = torch.empty((rows_per, W), dtype=torch.int64, device=q.device)
+    sg = torch.empty((rows_per, W), dtype=torch.int64, device=q.device) if grouped else None
+    status = torch.zeros(1, dtype=torch.int32, device=q.device)
+    for r0 in range(0, nq, rows_per):
+        n = min(rows_per, nq - r0)
+        L.check(lib.vr_score_lists(q[r0:].data_ptr(), n, index.emb.data_ptr(), index.nd, d, ls.arg(of, r0), W,
+                                   gt.groups.data_ptr() if grouped else None, sc.data_ptr(), si.data_ptr(), L.ptr(sg),
+                                   status.data_ptr(), sp))
+        if grouped:
+            _merge_group_levels(sc[:n], si[:n], sg[:n], k, [t[r0:r0 + n] for t in out])
+        elif W <= LIST_CHUNK:
+            L.check(lib.vr_topk_rows(sc.data_ptr(), si.data_ptr(), n, W, k, id_offset, out[0][r0:].data_ptr(),
+                                     out[1][r0:].data_ptr(), sp))
+        else:
+            c = W // LIST_CHUNK
+            ws_s = torch.empty((n * c, k), dtype=torch.float32, device=q.device)
+            ws_i = torch.empty((n * c, k), dtype=torch.int64, device=q.device)
+            L.check(lib.vr_topk_rows(sc.data_ptr(), si.data_ptr(), n * c, LIST_CHUNK, k, 0, ws_s.data_ptr(), ws_i.data_ptr(), sp))
+            L.check(lib.vr_topk_rows(ws_s.data_ptr(), ws_i.data_ptr(), n, c * k, k, id_offset, out[0][r0:].data_ptr(),
+                                     out[1][r0:].data_ptr(), sp))
+    bad = int(status.item())  # host sync: the caller reads the result next anyway
+    if bad:
+        raise RuntimeError(f"vr_score_lists reported status {bad} (a list longer than its width, or a list index out of range)")
+    if grouped and id_offset:
+        out[1].add_(torch.where(out[1] >= 0, id_offset, 0))
+    if order is None:
+        return out
+    res = tuple(torch.empty_like(t) for t in out)
+    for r, t in zip(res, out):
+        r.index_copy_(0, order, t)
+    return res
+
+
+def _merge_group_levels(s: torch.Tensor, p: torch.Tensor, g: torch.Tensor, k: int, out) -> None:
+    """[n, W] (score, page, group) entries -> the first k distinct groups of each row in (score desc, page asc) order.
+    A group of the row's top-k has fewer than k groups ahead of it in the chunk that holds its best page, so it is among
+    that chunk's first k distinct groups: merging the chunks' lists again is exact, and each level shrinks a row by
+    512 / k (k <= 256)."""
+    lib, sp = L.lib(), L.stream_ptr()
+    n = s.shape[0]
+    while s.shape[1] > MERGE_GROUPS_MAX:
+        c = s.shape[1] // MERGE_GROUPS_MAX  # the width is a multiple of 512 here
+        nxt = (torch.empty((n * c, k), dtype=torch.float32, device=s.device),
+               torch.empty((n * c, k), dtype=torch.int64, device=s.device),
+               torch.empty((n * c, k), dtype=torch.int64, device=s.device))
+        L.check(lib.vr_merge_group_topk(s.data_ptr(), p.data_ptr(), g.data_ptr(), n * c, MERGE_GROUPS_MAX, k,
+                                        *[t.data_ptr() for t in nxt], sp))
+        s, p, g = (t.view(n, c * k) for t in nxt)
+        pad = -s.shape[1] % MERGE_GROUPS_MAX if s.shape[1] > MERGE_GROUPS_MAX else 0
+        if pad:
+            s = torch.nn.functional.pad(s, (0, pad), value=float("-inf"))
+            p, g = (torch.nn.functional.pad(t, (0, pad), value=-1) for t in (p, g))
+    s, p, g = s.contiguous(), p.contiguous(), g.contiguous()
+    L.check(lib.vr_merge_group_topk(s.data_ptr(), p.data_ptr(), g.data_ptr(), n, s.shape[1], k,
+                                    *[t.data_ptr() for t in out], sp))
 
 
 class _Stages:
@@ -310,6 +494,7 @@ class _GroupTable:
 
 
 MERGE_GROUPS_MAX = 512  # entries per row vr_merge_group_topk takes: world * k of sharded_topk_groups
+LIST_GROUPS_MAX_K = MERGE_GROUPS_MAX // 2  # the list path's group merge shrinks a row by 512 / k per level
 _GROUP_TABLES: Dict[int, Tuple["weakref.ref", int, _GroupTable]] = {}
 
 
@@ -367,13 +552,25 @@ def _exact_topk_groups(q: torch.Tensor, index: CorpusIndex, k: int, id_offset: i
 
 def score_topk_groups(queries: torch.Tensor, index: CorpusIndex, k: int, doc_groups: torch.Tensor, id_offset: int = 0,
                       force_exact: bool = False, stats: Optional[dict] = None, doc_mask: Optional[torch.Tensor] = None,
-                      mask_of: Optional[torch.Tensor] = None) -> Tuple[torch.Tensor, torch.Tensor, torch.Tensor]:
+                      mask_of: Optional[torch.Tensor] = None, doc_lists: Optional[Tuple[torch.Tensor, torch.Tensor]] = None,
+                      list_of: Optional[torch.Tensor] = None) -> Tuple[torch.Tensor, torch.Tensor, torch.Tensor]:
     """Exact top-k GROUPS (documents) of pages: doc_groups (int32/int64 [nd] on the index's device) gives each page its
     group in [0, G). A group's score is the maximum exact fp32 page score over its eligible pages, its best page the lowest
     page with that maximum; groups rank by (score desc, best page asc). Returns (scores [nq,k] f32, best pages [nq,k] i64
     = local index + id_offset, groups [nq,k] i64); fewer than k groups with an eligible page leave (-inf, -1, -1).
     With doc_groups = arange(nd) the result equals score_topk's, with groups == pages. doc_mask and mask_of as in score_topk
-    (per-query masks: each query's documents are scored by its own eligible pages)."""
+    (per-query masks: each query's documents are scored by its own eligible pages). doc_lists and list_of as in
+    score_topk: each query's documents are scored by the pages of its list; k > 256 takes the masked path with the
+    equivalent masks (the same result)."""
+    if doc_lists is not None or list_of is not None:
+        q, ls = _queries_and_lists(queries, index, doc_mask, mask_of, doc_lists, list_of)
+        with L.on_device(q.device):
+            gt = _group_table(doc_groups, index)
+            if k <= LIST_GROUPS_MAX_K:
+                return _lists_topk(q, index, k, id_offset, ls, gt, stats)
+            doc_mask, mask_of = ls.masks(index.nd)
+            return _score_topk_groups(q, index, k, id_offset, force_exact, stats, gt,
+                                      _check_doc_mask(doc_mask, index, q.shape[0], mask_of))
     q, masks = _queries_and_mask(queries, index, doc_mask, mask_of)
     with L.on_device(q.device):
         gt = _group_table(doc_groups, index)
@@ -450,12 +647,14 @@ def gather_partials(scores: torch.Tensor, ids: torch.Tensor, group=None) -> Tupl
 
 
 def sharded_topk(queries: torch.Tensor, index: CorpusIndex, k: int, id_offset: int, group=None, stats: Optional[dict] = None,
-                 doc_mask: Optional[torch.Tensor] = None, mask_of: Optional[torch.Tensor] = None):
+                 doc_mask: Optional[torch.Tensor] = None, mask_of: Optional[torch.Tensor] = None,
+                 doc_lists: Optional[Tuple[torch.Tensor, torch.Tensor]] = None, list_of: Optional[torch.Tensor] = None):
     """Corpus sharded by page across ranks (every rank holds the same queries): local exact top-k with GLOBAL ids,
     one all-gather of [nq, k] (score, id) pairs over NCCL/NVLink, k-way merge on every rank (SURVEY.md §8e).
     doc_mask: this rank's bool [nd] mask of its own shard, or bool [M, nd] (this shard's columns of M masks) with mask_of
-    (see score_topk)."""
-    s, i = score_topk(queries, index, k, id_offset, stats=stats, doc_mask=doc_mask, mask_of=mask_of)
+    (see score_topk). doc_lists / list_of: this rank's lists of its own shard, in local ids (see score_topk)."""
+    s, i = score_topk(queries, index, k, id_offset, stats=stats, doc_mask=doc_mask, mask_of=mask_of, doc_lists=doc_lists,
+                      list_of=list_of)
     if _world(group) == 1:
         return s, i
     ev = _Stages(stats)
@@ -468,19 +667,21 @@ def sharded_topk(queries: torch.Tensor, index: CorpusIndex, k: int, id_offset: i
 
 def sharded_topk_groups(queries: torch.Tensor, index: CorpusIndex, k: int, doc_groups: torch.Tensor, id_offset: int,
                         group=None, stats: Optional[dict] = None, doc_mask: Optional[torch.Tensor] = None,
-                        mask_of: Optional[torch.Tensor] = None):
+                        mask_of: Optional[torch.Tensor] = None, doc_lists: Optional[Tuple[torch.Tensor, torch.Tensor]] = None,
+                        list_of: Optional[torch.Tensor] = None):
     """Document-level sharded_topk: doc_groups holds this shard's pages' GLOBAL group ids (a document may span ranks).
     Local group top-k with global page ids, one all-gather of [nq, k, 3] int64 (score bits, page, group), then the merge
     keeps the first k distinct groups. A group's best page lies on one rank, and that rank's local top-k holds it whenever
     the group is in the global top-k, so the result equals score_topk_groups over the whole corpus.
     world * k must be <= MERGE_GROUPS_MAX (512), checked before any work. Pass the same doc_groups tensor on every call:
-    the CSR is cached per tensor object. doc_mask / mask_of as in sharded_topk."""
+    the CSR is cached per tensor object. doc_mask / mask_of and doc_lists / list_of as in sharded_topk."""
     import torch.distributed as dist
 
     if dist.is_available() and dist.is_initialized() and dist.get_world_size(group) * k > MERGE_GROUPS_MAX:
         raise ValueError(f"sharded_topk_groups: world * k = {dist.get_world_size(group) * k} > {MERGE_GROUPS_MAX}")
 
-    s, p, g = score_topk_groups(queries, index, k, doc_groups, id_offset, stats=stats, doc_mask=doc_mask, mask_of=mask_of)
+    s, p, g = score_topk_groups(queries, index, k, doc_groups, id_offset, stats=stats, doc_mask=doc_mask, mask_of=mask_of,
+                                doc_lists=doc_lists, list_of=list_of)
     if _world(group) == 1:
         return s, p, g
     ev = _Stages(stats)
