@@ -436,6 +436,51 @@ int vr_score_lists(const float* q_f32, int32_t nq, const float* d_f32, int64_t n
                    int32_t width, const int32_t* doc_groups, float* out_scores, int64_t* out_ids, int64_t* out_groups,
                    int32_t* status, void* stream);
 
+/* Range search: for query row r with threshold t_r (thresholds [nq] f32, never NaN), every eligible doc j with exact
+ * score s_rj >= t_r (the bits vr_score_exact gives that pair; NaN scores never qualify), ordered by (score desc, id asc).
+ * masks (optional, NULL: every doc) is a mask set as in the _masks calls. Three producers and one ordering step:
+ *   vr_score_filter_range  : the wgmma fp16 filter of vr_score_filter with a fixed drop threshold per row,
+ *                            thr = t_r - eps(|q_r|, max|d|, dim) rounded toward -inf (eps: the bound of the top-k proof),
+ *                            appends every doc with approximate score >= thr to cand_ids [nq, cap] (row r's first
+ *                            min(counts[r], cap) entries, in no order). counts [nq] is set by the call; counts[r] > cap
+ *                            means the row overflowed (only its first cap slots were written), and a row whose |q|
+ *                            (q_norms, e.g. the norms output of vr_f32_to_f16_rows) or *max_doc_norm is not < 65504
+ *                            has no bound and is marked overflowed too. Every doc with s >= t is a candidate of a row
+ *                            that did not overflow;
+ *   vr_score_rescore_range : exact fp32 scores of each row's candidates; those with s >= t_r go to out_scores / out_ids
+ *                            [nq, cap] (row r's first kept[r] entries, in no order). Overflowed rows get kept[r] = 0:
+ *                            rerun them through vr_score_exact + vr_range_rows;
+ *   vr_range_rows          : rows of vr_score_exact output [rows, nd] (row r with threshold thresholds[r] and, with
+ *                            masks, the mask of row r): the eligible columns with s >= t, as (score, column) into
+ *                            out_scores / out_ids [rows, pitch] (first counts[r] entries, in no order; pitch >= nd);
+ *   vr_range_sort          : orders such a region (scores / ids [*, pitch], counts[*]) into CSR rows: call row i sorts
+ *                            region row r = row_of[i] (row_of NULL: r = i) by (score desc, id asc) and writes it at
+ *                            out_scores / out_ids [out_offsets[r], out_offsets[r] + counts[r]), ids + id_offset. The
+ *                            caller keeps every counts[r] <= max_count <= pitch. Up to 4096 entries a row sort in shared
+ *                            memory; longer rows need a workspace of vr_range_sort_ws_bytes(rows, max_count) bytes.
+ * Every entry refuses, before any CUDA call and naming the argument: a NULL or misaligned pointer, nq, rows or nd out of
+ * range (rows <= 65535 for vr_range_rows and vr_range_sort), dim not a positive multiple of 8 (4 for the fp32 calls),
+ * cap < 1, pitch < nd, max_count outside [0, pitch], a workspace too small, and a bad mask set.
+ * Alignment (bytes) of the vr_score_filter_range arguments: q_f16 16, d_f16 16, thresholds 4, q_norms 4, max_doc_norm 4,
+ * counts 4, cand_ids 4
+ * Alignment (bytes) of the vr_score_rescore_range arguments: q_f32 4, d_f32 16, thresholds 4, counts 4, cand_ids 4,
+ * out_scores 4, out_ids 4, kept 4
+ * Alignment (bytes) of the vr_range_rows arguments: scores 4, thresholds 4, out_scores 4, out_ids 4, counts 4
+ * Alignment (bytes) of the vr_range_sort arguments: scores 4, ids 4, counts 4, row_of 4, out_offsets 8, out_scores 4,
+ * out_ids 8, ws 8 */
+int vr_score_filter_range(const void* q_f16, int32_t nq, const void* d_f16, int64_t nd, int32_t dim, const float* thresholds,
+                          const float* q_norms, const float* max_doc_norm, const vr_doc_masks* masks, int32_t cap,
+                          int32_t* counts, int32_t* cand_ids, void* stream);
+int vr_score_rescore_range(const float* q_f32, int32_t nq, const float* d_f32, int64_t nd, int32_t dim,
+                           const float* thresholds, int32_t cap, const int32_t* counts, const int32_t* cand_ids,
+                           float* out_scores, int32_t* out_ids, int32_t* kept, void* stream);
+int vr_range_rows(const float* scores, int32_t rows, int64_t nd, const float* thresholds, const vr_doc_masks* masks,
+                  int64_t pitch, float* out_scores, int32_t* out_ids, int32_t* counts, void* stream);
+int64_t vr_range_sort_ws_bytes(int32_t rows, int32_t max_count);
+int vr_range_sort(const float* scores, const int32_t* ids, int64_t pitch, const int32_t* counts, int32_t rows,
+                  const int32_t* row_of, const int64_t* out_offsets, int32_t max_count, int64_t id_offset, void* ws,
+                  int64_t ws_bytes, float* out_scores, int64_t* out_ids, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -166,6 +166,16 @@ def _declare(lib: C.CDLL) -> None:
     lib.vr_group_topk_rows_masks.argtypes = [vp, i32, i64, vp, i32, dm, i32, i64, i32, vp, i64, vp, vp, vp, vp]
     lib.vr_score_lists.restype = i32
     lib.vr_score_lists.argtypes = [vp, i32, vp, i64, i32, C.POINTER(DocLists), i32, vp, vp, vp, vp, vp, vp]
+    lib.vr_score_filter_range.restype = i32
+    lib.vr_score_filter_range.argtypes = [vp, i32, vp, i64, i32, vp, vp, vp, dm, i32, vp, vp, vp]
+    lib.vr_score_rescore_range.restype = i32
+    lib.vr_score_rescore_range.argtypes = [vp, i32, vp, i64, i32, vp, i32, vp, vp, vp, vp, vp, vp]
+    lib.vr_range_rows.restype = i32
+    lib.vr_range_rows.argtypes = [vp, i32, i64, vp, dm, i64, vp, vp, vp, vp]
+    lib.vr_range_sort_ws_bytes.restype = i64
+    lib.vr_range_sort_ws_bytes.argtypes = [i32, i32]
+    lib.vr_range_sort.restype = i32
+    lib.vr_range_sort.argtypes = [vp, vp, i64, vp, i32, vp, vp, i32, i64, vp, i64, vp, vp, vp]
     lib.vr_pool_norm.restype = i32
     lib.vr_pool_norm.argtypes = [vp, i64, vp, f32, vp, i32, i32, i32, i32, vp, vp]
     lib.vr_prefix_rows.restype = i32

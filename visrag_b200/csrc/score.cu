@@ -73,10 +73,54 @@ struct MaskedGroupedScoreArgs : MaskedScoreArgs {
     const int* doc_groups;
 };
 
+// Range search ((Masked)RangeScoreArgs): instead of lists, every doc whose approximate score is >= the row's drop
+// threshold t - eps is appended to the row's candidate region (see the epilogue).
+struct RangeFields {
+    const float* thresholds;    // [nq] t of each query row
+    const float* qnorms;        // [nq] fp32 L2 norm of each query row
+    const float* max_doc_norm;  // [1] max L2 norm of the doc rows
+    int cap;                    // candidate slots per query row
+    int* counts;                // [nq] candidates found (zeroed by the host); > cap: the row overflowed
+    int* cand;                  // [nq, cap] their doc ids, in no particular order
+};
+
+struct RangeScoreArgs : ScoreArgs {
+    RangeFields range;
+};
+
+struct MaskedRangeScoreArgs : MaskedScoreArgs {
+    RangeFields range;
+};
+
 template <typename Args>
 constexpr bool kMasked = std::is_base_of<MaskedScoreArgs, Args>::value;
 template <typename Args>
 constexpr bool kGrouped = std::is_same<Args, GroupedScoreArgs>::value || std::is_same<Args, MaskedGroupedScoreArgs>::value;
+template <typename Args>
+constexpr bool kRange = std::is_same<Args, RangeScoreArgs>::value || std::is_same<Args, MaskedRangeScoreArgs>::value;
+
+// The bound of the filter: |approximate score - exact fp32 score| <= score_eps(|q|, max|d|, dim) for finite fp16 copies of
+// both operands. fp16 operand rounding (2^-11 each) + fp32 accumulation slack, times |q| * max|d|, plus an absolute term
+// for fp16 subnormals (elements below 6.1e-5 carry an absolute error up to 2^-25). The one statement of eps: the top-k
+// proof (proof_flag) and the range filter's drop threshold both call it.
+__device__ __forceinline__ float score_eps(float qnorm, float dn, int dim) {
+    return (9.765625e-4f + static_cast<float>(dim) * 1.1920929e-7f) * qnorm * dn +
+           sqrtf(static_cast<float>(dim)) * 5.9604645e-8f * (qnorm + dn) + 1e-6f;
+}
+
+// The range filter's drop threshold of query row `row`: t - eps rounded toward -inf, so that every doc with exact
+// score >= t has approximate score >= it. NaN (no comparison passes, nothing is appended) for rows past nq and for rows
+// without a bound: a query or max doc norm that is not < 65504 (inf / NaN included) means some fp16 operand may have
+// overflowed, and lane `mark` records such a row as overflowed so that the host reruns it through the fp32 scan.
+__device__ __forceinline__ float range_drop_threshold(const RangeFields& f, int row, int nq, int dim, bool mark) {
+    if (row >= nq) return __int_as_float(0x7fffffff);
+    const float qn = __ldg(f.qnorms + row), dn = __ldg(f.max_doc_norm);
+    if (!(qn < 65504.f) || !(dn < 65504.f)) {
+        if (mark) atomicMax(f.counts + row, f.cap + 1);
+        return __int_as_float(0x7fffffff);
+    }
+    return __fsub_rd(__ldg(f.thresholds + row), score_eps(qn, dn, dim));
+}
 
 struct Score2Cfg {
     static constexpr int STAGES = 6;
@@ -155,12 +199,18 @@ __device__ __forceinline__ float quad_max(float v) {
 // in the slow path and in the quad merge); the fast path is that of the page-level form with the same masking. The quad merge keeps the merged tail >= each lane's tail
 // (each lane's 16 groups have an entry at least that high in the union), so thr stays a valid drop threshold, and a
 // published tau is the tail of a group-distinct list.
+// RANGE ((Masked)RangeScoreArgs): no lists, no quad merge, no tau. Each accumulator row has one fixed drop threshold
+// thr = t - eps (range_drop_threshold); the fast path is max >= thr over the lane's 32 scores, and the slow path appends
+// every column with score >= thr to the row's candidate region: the quad's four lanes take their slots with ONE atomicAdd
+// on the row's counter, and write only while slot < cap (the counter keeps counting, so counts > cap marks an overflow).
+// Masked-out columns become NaN, which no comparison passes (-inf would pass a threshold of -inf).
 template <typename Args>
 __global__ void __launch_bounds__(GEMM_THREADS, 1)
 score_filter_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant__ CUtensorMap tmap_d,
                     const Args g) {
     constexpr bool GROUPED = kGrouped<Args>;
     constexpr bool MASKED = kMasked<Args>;
+    constexpr bool RANGE = kRange<Args>;
     using Cfg = Score2Cfg;
     constexpr int STAGES = Cfg::STAGES;
     extern __shared__ uint8_t smem_raw[];
@@ -234,11 +284,17 @@ score_filter_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_con
         const uint32_t* mrow[2];  // MASKED: the mask words of each row's query
 #pragma unroll
         for (int h = 0; h < 2; ++h) {
-            tau_ptr[h] = g.cand_scores + (static_cast<long long>(min(row0 + 8 * h, g.nq - 1)) * g.lists + g.lists - 1) * SC_KT;
-            thr[h] = tau[h] = __ldcg(tau_ptr[h]);
+            if constexpr (RANGE) {
+                thr[h] = range_drop_threshold(g.range, row0 + 8 * h, g.nq, g.dim, q4 == 0);
+            } else {
+                tau_ptr[h] = g.cand_scores + (static_cast<long long>(min(row0 + 8 * h, g.nq - 1)) * g.lists + g.lists - 1) * SC_KT;
+                thr[h] = tau[h] = __ldcg(tau_ptr[h]);
+            }
             if constexpr (MASKED) mrow[h] = mask_of_row(g.masks, min(row0 + 8 * h, g.nq - 1));
+            if constexpr (!RANGE) {
 #pragma unroll
-            for (int j = 0; j < SC_KT; ++j) { sc[h][j] = -INFINITY; id[h][j] = -1; }
+                for (int j = 0; j < SC_KT; ++j) { sc[h][j] = -INFINITY; id[h][j] = -1; }
+            }
         }
         const int t1 = item_t1(item);
         for (int u = 2 * item_t0(item); u < 2 * t1; ++u) {
@@ -293,13 +349,50 @@ score_filter_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_con
                         const uint32_t x = mw[h][w] >> (2 * q4);
                         elig |= ((x & 0x3u) | ((x >> 6) & 0xCu) | ((x >> 12) & 0x30u) | ((x >> 18) & 0xC0u)) << (8 * w);
                     }
+                    if constexpr (RANGE) {
 #pragma unroll
-                    for (int j = 0; j < 32; ++j) v[j] = (elig >> j) & 1u ? v[j] : __float_as_uint(-INFINITY);
+                        for (int j = 0; j < 32; ++j) v[j] = (elig >> j) & 1u ? v[j] : 0x7fffffffu;
+                    } else {
+#pragma unroll
+                        for (int j = 0; j < 32; ++j) v[j] = (elig >> j) & 1u ? v[j] : __float_as_uint(-INFINITY);
+                    }
                 }
                 // fast path: nothing of the 32 scores beats the threshold (the common case after the first tiles)
                 float mx = fmaxf(__uint_as_float(v[0]), __uint_as_float(v[1]));
 #pragma unroll
                 for (int j = 2; j < 32; j += 2) mx = fmaxf(mx, fmaxf(__uint_as_float(v[j]), __uint_as_float(v[j + 1])));
+                if constexpr (RANGE) {
+                    const bool hit = mx >= thr[h];
+                    if (__any_sync(0xffffffffu, hit)) {  // warp-uniform: the quad exchange below needs every lane
+                        uint32_t m = 0;
+                        if (hit) {
+#pragma unroll
+                            for (int j = 0; j < 32; ++j)
+                                m |= (__uint_as_float(v[j]) >= thr[h] && col_base + (j >> 1) * 8 + (j & 1) < g.nd ? 1u : 0u) << j;
+                        }
+                        // slots of the quad's lanes: an exclusive prefix of their counts, one atomicAdd for the row
+                        const int n = __popc(m);
+                        int pre = n;
+                        int o = __shfl_up_sync(0xffffffffu, pre, 1, 4);
+                        if (q4 >= 1) pre += o;
+                        o = __shfl_up_sync(0xffffffffu, pre, 2, 4);
+                        if (q4 >= 2) pre += o;
+                        const int total = __shfl_sync(0xffffffffu, pre, 3, 4);
+                        const int row = row0 + 8 * h;
+                        int base = 0;
+                        if (q4 == 0 && total > 0) base = atomicAdd(g.range.counts + row, total);
+                        int slot = __shfl_sync(0xffffffffu, base, 0, 4) + pre - n;
+                        int* dst = g.range.cand + static_cast<long long>(row) * g.range.cap;
+#pragma unroll 1
+                        while (m) {
+                            const int j = __ffs(m) - 1;
+                            m &= m - 1;
+                            if (slot < g.range.cap) dst[slot] = static_cast<int>(col_base + (j >> 1) * 8 + (j & 1));
+                            ++slot;
+                        }
+                    }
+                    continue;
+                }
                 if (mx > thr[h]) {
                     // slow path, ONE compact instance of the insertion code per row (a fully unrolled form - 32 inlined
                     // insertions - would thrash the instruction cache)
@@ -332,6 +425,7 @@ score_filter_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_con
                 thr[h] = fmaxf(thr[h], quad_max(sc[h][SC_KT - 1]));
             }
         }
+        if constexpr (RANGE) continue;  // the candidates are already in their regions
         // one candidate list per (query row, doc range): merge the quad's four column subsets (after the two exchange
         // steps every lane of the quad holds the top-16 of the union), write it, publish its tail as the query's new tau
 #pragma unroll
@@ -439,10 +533,7 @@ __device__ __forceinline__ float warp_dot_row(const float* qs, const float* __re
 // The proof of the rescoring kernels: 1 (rerun the query through the fp32 scan) unless bound + eps < kth, where bound
 // covers every candidate that was not rescored exactly (-inf: none) and kth is the k-th exact score.
 __device__ __forceinline__ int proof_flag(float bound, float kth, float qnorm, float dn, int dim) {
-    // fp16 operand rounding (2^-11 each) + fp32 accumulation slack, times |q| * max|d|, plus an absolute
-    // term for fp16 subnormals (elements below 6.1e-5 carry an absolute error up to 2^-25)
-    const float eps = (9.765625e-4f + static_cast<float>(dim) * 1.1920929e-7f) * qnorm * dn +
-                      sqrtf(static_cast<float>(dim)) * 5.9604645e-8f * (qnorm + dn) + 1e-6f;
+    const float eps = score_eps(qnorm, dn, dim);
     int flag = 0;
     if (bound > -INFINITY && !(bound + eps < kth)) flag = 1;  // something was dropped that might belong
     // the bound assumes finite fp16 copies of both operands: a row norm >= 65504 (or inf / NaN, for which the
@@ -1282,12 +1373,12 @@ static int masks_check(const char* fn, const vr_doc_masks* m, long long nd) {
 
 static DocMasks device_masks(const vr_doc_masks* m) { return DocMasks{m->words, m->pitch, m->of_query}; }
 
-// The list initialisation, then score_filter_kernel<Args> over `plan`, after the caller's argument checks. masks and
-// doc_groups go to the forms whose Args carry them.
+// The list initialisation (range forms: the zeroing of the candidate counters), then score_filter_kernel<Args> over
+// `plan`, after the caller's argument checks. masks, doc_groups and range go to the forms whose Args carry them.
 template <typename Args>
 static int launch_score_filter(const ScorePlan& plan, const void* q_f16, int nq, const void* d_f16, long long nd, int dim,
                                float* cand_scores, int* cand_ids, const DocMasks& masks, const int* doc_groups,
-                               cudaStream_t st) {
+                               cudaStream_t st, const RangeFields* range = nullptr) {
     using Cfg = Score2Cfg;
     CUtensorMap tq, td;
     if (int rc = make_tmap_2d(&tq, q_f16, nq, dim, dim, GEMM_BM, GEMM_BK, 128, false)) return rc;
@@ -1300,7 +1391,10 @@ static int launch_score_filter(const ScorePlan& plan, const void* q_f16, int nq,
     g.cand_scores = cand_scores; g.cand_ids = cand_ids;
     if constexpr (kMasked<Args>) g.masks = masks;
     if constexpr (kGrouped<Args>) g.doc_groups = doc_groups;
-    {
+    if constexpr (kRange<Args>) {
+        g.range = *range;
+        VR_CHECK_CUDA(cudaMemsetAsync(range->counts, 0, static_cast<size_t>(nq) * sizeof(int), st));
+    } else {
         const long long n = static_cast<long long>(nq) * (plan.lists - plan.R) * SC_KT;
         long long blocks = (n + 255) / 256;
         if (blocks > num_sms() * 8) blocks = num_sms() * 8;
@@ -1376,6 +1470,212 @@ static int rescore_keep(int k, int lists) {
     if (keep > lists * SC_KT) keep = lists * SC_KT;
     if (keep > RS_MAX_KEEP) keep = RS_MAX_KEEP;
     return keep;
+}
+
+// ---------------------------------------------------------------------------------------------------- range search
+// Every eligible doc with exact score s >= t of its query row, ordered by (score desc, id asc). Two producers fill a
+// per-row REGION (scores, ids, a row pitch, a count per row) in no particular order: the candidate rescoring after the
+// range filter, and the selection over rows of the fp32 scan. One ordering step (vr_range_sort) turns any region into
+// CSR rows.
+
+// Exact fp32 rescoring of the filter's candidates: block (x, y) takes candidates y, y + gridDim.y * 8, ... of query row
+// x, one warp per candidate through warp_dot_row (the bits of vr_score_exact), and appends those with s >= t to the
+// row's region [cap] (kept[row] counts them; zeroed by the host). A row whose counter says it overflowed (count > cap)
+// is skipped: the host reruns it through the fp32 scan.
+constexpr int RR_THREADS = 256;
+
+__global__ void __launch_bounds__(RR_THREADS)
+range_rescore_kernel(const float* __restrict__ Q, const float* __restrict__ D, int dim, const float* __restrict__ thresholds,
+                     int cap, const int* __restrict__ counts, const int* __restrict__ cand, float* __restrict__ out_scores,
+                     int* __restrict__ out_ids, int* __restrict__ kept) {
+    extern __shared__ float qs[];  // [dim]
+    const int q = blockIdx.x;
+    const int n = __ldg(counts + q);
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const int c0 = blockIdx.y * (RR_THREADS / 32) + warp, stride = gridDim.y * (RR_THREADS / 32);
+    if (n > cap || blockIdx.y * (RR_THREADS / 32) >= n) return;  // block-uniform
+    const float* qrow = Q + static_cast<long long>(q) * dim;
+    for (int i = threadIdx.x; i < dim; i += RR_THREADS) qs[i] = qrow[i];
+    __syncthreads();
+    const float t = __ldg(thresholds + q);
+    const long long base = static_cast<long long>(q) * cap;
+    for (int c = c0; c < n; c += stride) {
+        const int id = __ldg(cand + base + c);
+        const float s = warp_dot_row(qs, D + static_cast<long long>(id) * dim, dim, lane);
+        if (lane == 0 && s >= t) {
+            const int o = atomicAdd(kept + q, 1);
+            out_scores[base + o] = s;
+            out_ids[base + o] = id;
+        }
+    }
+}
+
+// Selection over rows of vr_score_exact output [rows, nd]: the eligible columns (by the mask of each row, masks.words
+// NULL: every column) with s >= t_row, appended to the row's region [pitch] with one atomicAdd per warp (counts zeroed by
+// the host). NaN scores never pass. Block (x, y): row y, column strides of 256 from 256 x.
+__global__ void __launch_bounds__(256)
+range_select_kernel(const float* __restrict__ scores, long long nd, const float* __restrict__ thresholds, const DocMasks masks,
+                    long long pitch, float* __restrict__ out_scores, int* __restrict__ out_ids, int* __restrict__ counts) {
+    const int row = blockIdx.y, lane = threadIdx.x & 31;
+    const float t = __ldg(thresholds + row);
+    const uint32_t* mask = masks.words ? mask_of_row(masks, row) : nullptr;
+    const float* srow = scores + static_cast<long long>(row) * nd;
+    const long long o_row = static_cast<long long>(row) * pitch;
+    for (long long c0 = static_cast<long long>(blockIdx.x) * 256; c0 < nd; c0 += static_cast<long long>(gridDim.x) * 256) {
+        const long long c = c0 + threadIdx.x;
+        float s = 0.f;
+        bool keep = false;
+        if (c < nd) {
+            s = srow[c];
+            keep = s >= t && (!mask || col_eligible(mask, c));
+        }
+        const uint32_t b = __ballot_sync(0xffffffffu, keep);
+        if (b) {
+            int base = 0;
+            if (lane == 0) base = atomicAdd(counts + row, __popc(b));
+            base = __shfl_sync(0xffffffffu, base, 0);
+            if (keep) {
+                const int o = base + __popc(b & ((1u << lane) - 1u));
+                out_scores[o_row + o] = s;
+                out_ids[o_row + o] = static_cast<int>(c);
+            }
+        }
+    }
+}
+
+// Sort key of an entry: ascending keys = (score desc, id asc), the before() order. High word: the order-preserving bits
+// of the score, inverted; -0 is canonicalised to +0 (they tie under before(), so the id decides). Low word: id << 1, and
+// bit 0 remembers a -0 so that the output keeps the score's own bits (it never decides an order: ids are distinct).
+// The all-ones key is the padding: it would need a NaN score, which no producer emits.
+__device__ __forceinline__ unsigned long long range_key(float s, int id) {
+    uint32_t b = __float_as_uint(s);
+    const uint32_t negzero = b == 0x80000000u ? 1u : 0u;
+    if (negzero) b = 0u;
+    const uint32_t o = (b & 0x80000000u) ? ~b : (b | 0x80000000u);
+    return (static_cast<unsigned long long>(~o) << 32) | (static_cast<uint32_t>(id) << 1) | negzero;
+}
+
+__device__ __forceinline__ void range_unkey(unsigned long long key, float& s, long long& id) {
+    const uint32_t o = ~static_cast<uint32_t>(key >> 32), lo = static_cast<uint32_t>(key);
+    const uint32_t b = (lo & 1u) ? 0x80000000u : (o & 0x80000000u) ? (o & 0x7fffffffu) : ~o;
+    s = __uint_as_float(b);
+    id = static_cast<long long>(lo >> 1);
+}
+
+constexpr int RSORT_TILE = 4096;   // entries a block orders in shared memory (32 KB of keys)
+constexpr int RSORT_THREADS = 512;
+
+// One bitonic compare-exchange stage (k, j) over keys[0, n) of shared memory; idx0 is the global index of keys[0], which
+// sets the direction of each pair (ascending when (index & k) == 0).
+__device__ __forceinline__ void bitonic_stage(unsigned long long* keys, int n, long long idx0, long long k, int j) {
+    for (int t = threadIdx.x; t < n / 2; t += blockDim.x) {
+        const int i = ((t & ~(j - 1)) << 1) | (t & (j - 1));
+        const unsigned long long a = keys[i], b = keys[i + j];
+        const bool up = ((idx0 + i) & k) == 0;
+        if ((a > b) == up) { keys[i] = b; keys[i + j] = a; }
+    }
+    __syncthreads();
+}
+
+__device__ __forceinline__ long long region_row(const int* row_of, int i) {
+    return row_of ? static_cast<long long>(__ldg(row_of + i)) : i;
+}
+
+// Rows of at most RSORT_TILE entries: block i loads region row r = row_of[i] as keys (padded to a power of two), sorts
+// them in shared memory and writes the CSR row at out_offsets[r].
+__global__ void __launch_bounds__(RSORT_THREADS)
+range_sort_smem_kernel(const float* __restrict__ scores, const int* __restrict__ ids, long long pitch,
+                       const int* __restrict__ counts, const int* __restrict__ row_of, const long long* __restrict__ out_offsets,
+                       long long id_offset, float* __restrict__ out_scores, long long* __restrict__ out_ids) {
+    __shared__ unsigned long long keys[RSORT_TILE];
+    const long long r = region_row(row_of, blockIdx.x);
+    const int n = __ldg(counts + r);
+    if (n <= 0) return;
+    int P = 1;
+    while (P < n) P <<= 1;
+    for (int j = threadIdx.x; j < P; j += RSORT_THREADS)
+        keys[j] = j < n ? range_key(scores[r * pitch + j], ids[r * pitch + j]) : ~0ull;
+    __syncthreads();
+    for (int k = 2; k <= P; k <<= 1)
+        for (int j = k >> 1; j > 0; j >>= 1) bitonic_stage(keys, P, 0, k, j);
+    const long long o = __ldg(out_offsets + r);
+    for (int j = threadIdx.x; j < n; j += RSORT_THREADS) {
+        float s;
+        long long id;
+        range_unkey(keys[j], s, id);
+        out_scores[o + j] = s;
+        out_ids[o + j] = id + id_offset;
+    }
+}
+
+// Longer rows: a bitonic sort of P = 2^m >= RSORT_TILE keys per row in the workspace [rows, P]. Stages with j >= TILE
+// run over global memory (range_bitonic_global_kernel, one launch per stage); all stages with j < TILE of one k run in
+// shared memory, tile by tile (range_bitonic_tile_kernel).
+__global__ void __launch_bounds__(256)
+range_keys_kernel(const float* __restrict__ scores, const int* __restrict__ ids, long long pitch, const int* __restrict__ counts,
+                  const int* __restrict__ row_of, long long P, unsigned long long* __restrict__ ws) {
+    const long long r = region_row(row_of, blockIdx.y);
+    const int n = __ldg(counts + r);
+    unsigned long long* w = ws + static_cast<long long>(blockIdx.y) * P;
+    for (long long j = blockIdx.x * 256ll + threadIdx.x; j < P; j += static_cast<long long>(gridDim.x) * 256)
+        w[j] = j < n ? range_key(scores[r * pitch + j], ids[r * pitch + j]) : ~0ull;
+}
+
+// k_lo == 2: every stage of k = 2 .. TILE (each tile sorted in the direction its global index gives); else the stages
+// j = TILE/2 .. 1 of k = k_lo.
+__global__ void __launch_bounds__(RSORT_THREADS)
+range_bitonic_tile_kernel(unsigned long long* __restrict__ ws, long long P, long long k_lo) {
+    __shared__ unsigned long long keys[RSORT_TILE];
+    const long long idx0 = static_cast<long long>(blockIdx.x) * RSORT_TILE;
+    unsigned long long* w = ws + static_cast<long long>(blockIdx.y) * P + idx0;
+    for (int j = threadIdx.x; j < RSORT_TILE; j += RSORT_THREADS) keys[j] = w[j];
+    __syncthreads();
+    if (k_lo == 2) {
+        for (int k = 2; k <= RSORT_TILE; k <<= 1)
+            for (int j = k >> 1; j > 0; j >>= 1) bitonic_stage(keys, RSORT_TILE, idx0, k, j);
+    } else {
+        for (int j = RSORT_TILE / 2; j > 0; j >>= 1) bitonic_stage(keys, RSORT_TILE, idx0, k_lo, j);
+    }
+    for (int j = threadIdx.x; j < RSORT_TILE; j += RSORT_THREADS) w[j] = keys[j];
+}
+
+__global__ void __launch_bounds__(256)
+range_bitonic_global_kernel(unsigned long long* __restrict__ ws, long long P, long long k, long long j) {
+    unsigned long long* w = ws + static_cast<long long>(blockIdx.y) * P;
+    for (long long t = blockIdx.x * 256ll + threadIdx.x; t < P / 2; t += static_cast<long long>(gridDim.x) * 256) {
+        const long long i = ((t & ~(j - 1)) << 1) | (t & (j - 1));
+        const unsigned long long a = w[i], b = w[i + j];
+        const bool up = (i & k) == 0;
+        if ((a > b) == up) { w[i] = b; w[i + j] = a; }
+    }
+}
+
+__global__ void __launch_bounds__(256)
+range_emit_kernel(const unsigned long long* __restrict__ ws, long long P, const int* __restrict__ counts,
+                  const int* __restrict__ row_of, const long long* __restrict__ out_offsets, long long id_offset,
+                  float* __restrict__ out_scores, long long* __restrict__ out_ids) {
+    const long long r = region_row(row_of, blockIdx.y);
+    const int n = __ldg(counts + r);
+    const long long o = __ldg(out_offsets + r);
+    const unsigned long long* w = ws + static_cast<long long>(blockIdx.y) * P;
+    for (long long j = blockIdx.x * 256ll + threadIdx.x; j < n; j += static_cast<long long>(gridDim.x) * 256) {
+        float s;
+        long long id;
+        range_unkey(w[j], s, id);
+        out_scores[o + j] = s;
+        out_ids[o + j] = id + id_offset;
+    }
+}
+
+// The workspace of vr_range_sort: none up to RSORT_TILE entries a row, else rows x P keys.
+static long long range_sort_P(int max_count) {
+    long long P = RSORT_TILE;
+    while (P < max_count) P <<= 1;
+    return P;
+}
+
+static long long range_sort_ws(int rows, int max_count) {
+    return max_count <= RSORT_TILE ? 0 : static_cast<long long>(rows) * range_sort_P(max_count) * 8;
 }
 
 }  // namespace vr
@@ -1807,6 +2107,145 @@ extern "C" int vr_score_lists(const float* q_f32, int32_t nq, const float* d_f32
     else if (NQ == 2) VR_LISTS_LAUNCH(2);
     else VR_LISTS_LAUNCH(1);
 #undef VR_LISTS_LAUNCH
+    VR_CHECK_CUDA(cudaGetLastError());
+    return 0;
+}
+
+// ---------------------------------------------------------------------------------------------------- range search
+#define VR_REQUIRE_PTR(fn, name, ptr, bytes)                             \
+    do {                                                                 \
+        VR_REQUIRE((ptr), "%s: %s must not be NULL", fn, name);          \
+        VR_REQUIRE_ALIGNED(fn, name, ptr, bytes);                        \
+    } while (0)
+
+extern "C" int vr_score_filter_range(const void* q_f16, int32_t nq, const void* d_f16, int64_t nd, int32_t dim,
+                                     const float* thresholds, const float* q_norms, const float* max_doc_norm,
+                                     const vr_doc_masks* masks, int32_t cap, int32_t* counts, int32_t* cand_ids,
+                                     void* stream) {
+    const char* fn = "vr_score_filter_range";
+    if (masks) VR_REQUIRE_MASKS(fn, masks, nd);
+    VR_REQUIRE_PTR(fn, "q_f16", q_f16, 16);  // TMA sources
+    VR_REQUIRE_PTR(fn, "d_f16", d_f16, 16);
+    VR_REQUIRE_PTR(fn, "thresholds", thresholds, 4);
+    VR_REQUIRE_PTR(fn, "q_norms", q_norms, 4);
+    VR_REQUIRE_PTR(fn, "max_doc_norm", max_doc_norm, 4);
+    VR_REQUIRE_PTR(fn, "counts", counts, 4);
+    VR_REQUIRE_PTR(fn, "cand_ids", cand_ids, 4);
+    VR_REQUIRE(nq > 0 && nq < (1 << 30), "%s: nq=%d, needs 0 < nq < 2^30", fn, nq);
+    VR_REQUIRE(nd > 0 && nd < 2147483647ll, "%s: nd=%lld beyond the int32 doc ids", fn, (long long)nd);
+    VR_REQUIRE(dim > 0 && dim % 8 == 0, "%s: dim=%d, needs a positive multiple of 8", fn, dim);
+    VR_REQUIRE(cap >= 1, "%s: cap=%d, needs at least 1", fn, cap);
+    const ScorePlan plan = score_plan(nq, nd);
+    const RangeFields rf = {thresholds, q_norms, max_doc_norm, cap, counts, cand_ids};
+    cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+    if (masks)
+        return launch_score_filter<MaskedRangeScoreArgs>(plan, q_f16, nq, d_f16, nd, dim, nullptr, nullptr,
+                                                         device_masks(masks), nullptr, st, &rf);
+    return launch_score_filter<RangeScoreArgs>(plan, q_f16, nq, d_f16, nd, dim, nullptr, nullptr, kNoMasks, nullptr, st, &rf);
+}
+
+extern "C" int vr_score_rescore_range(const float* q_f32, int32_t nq, const float* d_f32, int64_t nd, int32_t dim,
+                                      const float* thresholds, int32_t cap, const int32_t* counts, const int32_t* cand_ids,
+                                      float* out_scores, int32_t* out_ids, int32_t* kept, void* stream) {
+    const char* fn = "vr_score_rescore_range";
+    VR_REQUIRE_PTR(fn, "q_f32", q_f32, 4);
+    VR_REQUIRE_PTR(fn, "d_f32", d_f32, 16);  // float4 rows (dim % 4 == 0 keeps every row aligned)
+    VR_REQUIRE_PTR(fn, "thresholds", thresholds, 4);
+    VR_REQUIRE_PTR(fn, "counts", counts, 4);
+    VR_REQUIRE_PTR(fn, "cand_ids", cand_ids, 4);
+    VR_REQUIRE_PTR(fn, "out_scores", out_scores, 4);
+    VR_REQUIRE_PTR(fn, "out_ids", out_ids, 4);
+    VR_REQUIRE_PTR(fn, "kept", kept, 4);
+    VR_REQUIRE(nq > 0, "%s: nq=%d, needs at least 1", fn, nq);
+    VR_REQUIRE(nd > 0 && nd < 2147483647ll, "%s: nd=%lld beyond the int32 doc ids", fn, (long long)nd);
+    VR_REQUIRE(dim > 0 && dim % 4 == 0, "%s: dim=%d, needs a positive multiple of 4", fn, dim);
+    VR_REQUIRE(cap >= 1, "%s: cap=%d, needs at least 1", fn, cap);
+    const size_t smem = static_cast<size_t>(dim) * sizeof(float);
+    VR_REQUIRE(smem <= 200 * 1024, "%s: dim=%d too large for shared memory", fn, dim);
+    cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+    VR_CHECK_CUDA(cudaMemsetAsync(kept, 0, static_cast<size_t>(nq) * sizeof(int), st));
+    static unsigned long long attr_set = 0;
+    if (smem > 48 * 1024 && first_use_on_device(&attr_set))
+        VR_CHECK_CUDA(cudaFuncSetAttribute(range_rescore_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
+    // candidate blocks per row: about four blocks per SM over the whole call, no more than a row's slots need
+    long long gy = (4ll * num_sms() + nq - 1) / nq;
+    const long long most = (cap + RR_THREADS / 32 - 1) / (RR_THREADS / 32);
+    if (gy > most) gy = most;
+    if (gy > 65535) gy = 65535;
+    range_rescore_kernel<<<dim3(nq, static_cast<unsigned>(gy)), RR_THREADS, smem, st>>>(q_f32, d_f32, dim, thresholds, cap,
+                                                                                      counts, cand_ids, out_scores, out_ids, kept);
+    VR_CHECK_CUDA(cudaGetLastError());
+    return 0;
+}
+
+extern "C" int vr_range_rows(const float* scores, int32_t rows, int64_t nd, const float* thresholds, const vr_doc_masks* masks,
+                             int64_t pitch, float* out_scores, int32_t* out_ids, int32_t* counts, void* stream) {
+    const char* fn = "vr_range_rows";
+    if (masks) VR_REQUIRE_MASKS(fn, masks, nd);
+    VR_REQUIRE_PTR(fn, "scores", scores, 4);
+    VR_REQUIRE_PTR(fn, "thresholds", thresholds, 4);
+    VR_REQUIRE_PTR(fn, "out_scores", out_scores, 4);
+    VR_REQUIRE_PTR(fn, "out_ids", out_ids, 4);
+    VR_REQUIRE_PTR(fn, "counts", counts, 4);
+    VR_REQUIRE(rows > 0 && rows <= 65535, "%s: rows=%d, needs 0 < rows <= 65535", fn, rows);
+    VR_REQUIRE(nd > 0 && nd < 2147483647ll, "%s: nd=%lld beyond the int32 doc ids", fn, (long long)nd);
+    VR_REQUIRE(pitch >= nd, "%s: pitch=%lld is below nd=%lld", fn, (long long)pitch, (long long)nd);
+    cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+    VR_CHECK_CUDA(cudaMemsetAsync(counts, 0, static_cast<size_t>(rows) * sizeof(int), st));
+    long long gx = (nd + 255) / 256;
+    const long long want = (8ll * num_sms() + rows - 1) / rows;
+    if (gx > want) gx = want;
+    const DocMasks m = masks ? device_masks(masks) : kNoMasks;
+    range_select_kernel<<<dim3(static_cast<unsigned>(gx), rows), 256, 0, st>>>(scores, nd, thresholds, m, pitch, out_scores,
+                                                                             out_ids, counts);
+    VR_CHECK_CUDA(cudaGetLastError());
+    return 0;
+}
+
+extern "C" int64_t vr_range_sort_ws_bytes(int32_t rows, int32_t max_count) {
+    return rows > 0 && max_count >= 0 ? range_sort_ws(rows, max_count) : -1;
+}
+
+extern "C" int vr_range_sort(const float* scores, const int32_t* ids, int64_t pitch, const int32_t* counts, int32_t rows,
+                             const int32_t* row_of, const int64_t* out_offsets, int32_t max_count, int64_t id_offset, void* ws,
+                             int64_t ws_bytes, float* out_scores, int64_t* out_ids, void* stream) {
+    const char* fn = "vr_range_sort";
+    VR_REQUIRE_PTR(fn, "scores", scores, 4);
+    VR_REQUIRE_PTR(fn, "ids", ids, 4);
+    VR_REQUIRE_PTR(fn, "counts", counts, 4);
+    VR_REQUIRE_ALIGNED(fn, "row_of", row_of, 4);  // optional
+    VR_REQUIRE_PTR(fn, "out_offsets", out_offsets, 8);
+    VR_REQUIRE_PTR(fn, "out_scores", out_scores, 4);
+    VR_REQUIRE_PTR(fn, "out_ids", out_ids, 8);
+    VR_REQUIRE(rows > 0 && rows <= 65535, "%s: rows=%d, needs 0 < rows <= 65535", fn, rows);
+    VR_REQUIRE(max_count >= 0 && max_count <= pitch, "%s: max_count=%d, needs 0 <= max_count <= pitch=%lld", fn, max_count,
+               (long long)pitch);
+    const long long need = range_sort_ws(rows, max_count);
+    VR_REQUIRE(need == 0 || (ws && ws_bytes >= need), "%s: ws of %lld bytes, needs %lld (vr_range_sort_ws_bytes)", fn,
+               (long long)ws_bytes, need);
+    VR_REQUIRE_ALIGNED(fn, "ws", ws, 8);
+    cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+    long long* oi = reinterpret_cast<long long*>(out_ids);
+    const long long* oo = reinterpret_cast<const long long*>(out_offsets);
+    if (max_count == 0) return 0;
+    if (need == 0) {
+        range_sort_smem_kernel<<<rows, RSORT_THREADS, 0, st>>>(scores, ids, pitch, counts, row_of, oo, id_offset, out_scores, oi);
+        VR_CHECK_CUDA(cudaGetLastError());
+        return 0;
+    }
+    const long long P = range_sort_P(max_count);
+    unsigned long long* w = reinterpret_cast<unsigned long long*>(ws);
+    long long gx = P / 256;
+    const long long cap = (8ll * num_sms() + rows - 1) / rows;
+    if (gx > cap) gx = cap;
+    const dim3 grid(static_cast<unsigned>(gx), rows), tiles(static_cast<unsigned>(P / RSORT_TILE), rows);
+    range_keys_kernel<<<grid, 256, 0, st>>>(scores, ids, pitch, counts, row_of, P, w);
+    range_bitonic_tile_kernel<<<tiles, RSORT_THREADS, 0, st>>>(w, P, 2);
+    for (long long k = 2 * RSORT_TILE; k <= P; k <<= 1) {
+        for (long long j = k >> 1; j >= RSORT_TILE; j >>= 1) range_bitonic_global_kernel<<<grid, 256, 0, st>>>(w, P, k, j);
+        range_bitonic_tile_kernel<<<tiles, RSORT_THREADS, 0, st>>>(w, P, k);
+    }
+    range_emit_kernel<<<grid, 256, 0, st>>>(w, P, counts, row_of, oo, id_offset, out_scores, oi);
     VR_CHECK_CUDA(cudaGetLastError());
     return 0;
 }

@@ -246,6 +246,51 @@ class KnowledgeBase:
                                                   doc_mask=masks if scope_of is not None else masks[0], mask_of=scope_of)
         return s, p, [[self.documents[j] for j in row if j >= 0] for row in g.tolist()]
 
+    def search_above(self, query_reps, min_score, within: Optional[Iterable[str]] = None,
+                     within_each: Optional[Sequence[Optional[Iterable[str]]]] = None
+                     ) -> Tuple[torch.Tensor, torch.Tensor, torch.Tensor]:
+        """Every page scoring at least min_score (a float, or an f32 tensor [nq] on the device: one threshold per query),
+        as CSR on the device: (offsets int64 [nq + 1], scores f32 [R], page indices int64 [R]); query i's pages are
+        [offsets[i], offsets[i + 1]), by (score desc, page asc), with the exact fp32 scores (retriever.score_range).
+        within / within_each: the pages searched, as in search (default: every live page); removed pages never appear."""
+        if within_each is not None:
+            q, keys, scope_of, _ = self._query_and_scopes(query_reps, within, within_each)
+            if q.shape[0] == 0:
+                return retriever.score_range(q, self.index, min_score)
+            return retriever.score_range(q, self.index, min_score, doc_mask=self._scope_masks(keys), mask_of=scope_of)
+        q, mask, _ = self._query_and_mask(query_reps, within)
+        return retriever.score_range(q, self.index, min_score, doc_mask=mask)
+
+    NEAR_DUPLICATE_ROWS = 8192  # pages scored as queries per pass of near_duplicates
+
+    def near_duplicates(self, min_score: float, within: Optional[Iterable[str]] = None
+                        ) -> Tuple[torch.Tensor, torch.Tensor, torch.Tensor]:
+        """Every pair of live pages (of `within`, default every live page) with a < b and exact fp32 score
+        reps[a] . reps[b] >= min_score: (a int64 [P], b int64 [P], scores f32 [P]) on the device, by a ascending, then
+        (score desc, b asc). Each page's row of score_range over the same pages, without the entries b <= a: the score
+        of (a, b) has the same bits as that of (b, a) (the fp32 FMA chain multiplies the same pairs in the same order),
+        so each pair is reported once, from its lower page. Pages are scored as queries in chunks."""
+        dev = self.index.emb.device
+        if within is None:
+            rows = torch.nonzero(self._live).flatten()
+            mask = None if len(self) == self.index.nd else self._live
+        else:
+            rows = torch.tensor(self._rows(within), dtype=torch.int64, device=dev)
+            mask = self._scope_masks([rows.tolist()]).view(-1)
+        a_parts, b_parts, s_parts = [], [], []
+        for r0 in range(0, rows.numel(), self.NEAR_DUPLICATE_ROWS):
+            sel = rows[r0:r0 + self.NEAR_DUPLICATE_ROWS]
+            off, s, b = retriever.score_range(self.index.emb.index_select(0, sel), self.index, min_score, doc_mask=mask)
+            a = torch.repeat_interleave(sel, off[1:] - off[:-1])
+            keep = b > a
+            a_parts.append(a[keep])
+            b_parts.append(b[keep])
+            s_parts.append(s[keep])
+        if not a_parts:
+            e = torch.empty(0, dtype=torch.int64, device=dev)
+            return e, e.clone(), torch.empty(0, dtype=torch.float32, device=dev)
+        return torch.cat(a_parts), torch.cat(b_parts), torch.cat(s_parts)
+
     def retrieve_documents(self, query_rep, topk: int, within: Optional[Iterable[str]] = None) -> List[Tuple[str, str]]:
         """[(document name, path of its best page image)] of the top-k documents, best first."""
         _, pages, names = self.search_documents(query_rep, topk, within)

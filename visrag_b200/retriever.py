@@ -613,6 +613,205 @@ def merge_topk(scores: torch.Tensor, ids: torch.Tensor, k: int) -> Tuple[torch.T
     return out_s, out_i
 
 
+# ------------------------------------------------------------------------------------------------------
+# Range search: every page scoring at least a threshold
+# ------------------------------------------------------------------------------------------------------
+RANGE_CAP = 16384          # candidate slots per query row of the filter path; a row with more reruns through the scan
+RANGE_SORT_SMEM = 4096     # rows of up to this many entries are ordered in shared memory (vr_range_sort)
+RANGE_BUDGET = 1 << 26     # entries of scratch per pass: query rows are processed in chunks of this many (row x slot)
+
+
+def _check_min_score(min_score, nq: int, device) -> torch.Tensor:
+    """min_score as an f32 [nq] tensor on the index's device: a float for every query, or an f32 tensor [nq]."""
+    if isinstance(min_score, torch.Tensor):
+        if min_score.dtype != torch.float32:
+            raise ValueError(f"min_score must be a float or a torch.float32 tensor, got {min_score.dtype}")
+        if min_score.dim() != 1 or min_score.shape[0] != nq:
+            raise ValueError(f"min_score must have shape [{nq}] (one threshold per query), got {list(min_score.shape)}")
+        if min_score.device != device:
+            raise ValueError(f"min_score lives on {min_score.device}, the index on {device}")
+        t = min_score.contiguous()
+        if nq and bool(torch.isnan(t).any()):
+            raise ValueError("min_score must not be NaN")
+        return t
+    if isinstance(min_score, bool) or not isinstance(min_score, (int, float, np.floating, np.integer)):
+        raise ValueError(f"min_score must be a float or a torch.float32 tensor, got {type(min_score).__name__}")
+    if np.isnan(min_score):
+        raise ValueError("min_score must not be NaN")
+    return torch.full((nq,), float(min_score), dtype=torch.float32, device=device)
+
+
+def _check_cap(cap: Optional[int]) -> int:
+    if cap is None:
+        return RANGE_CAP
+    if isinstance(cap, bool) or not isinstance(cap, (int, np.integer)) or cap < 1 or cap >= 1 << 31:
+        raise ValueError(f"cap must be an int in [1, 2^31), got {cap!r}")
+    return int(cap)
+
+
+def score_range(queries: torch.Tensor, index: CorpusIndex, min_score, id_offset: int = 0,
+                doc_mask: Optional[torch.Tensor] = None, mask_of: Optional[torch.Tensor] = None, force_exact: bool = False,
+                stats: Optional[dict] = None, cap: Optional[int] = None
+                ) -> Tuple[torch.Tensor, torch.Tensor, torch.Tensor]:
+    """Range search: for query i, every eligible doc j with exact fp32 score s_ij >= t_i, where t = min_score (a float
+    for every query, or an f32 tensor [nq] on the index's device; NaN is refused). Returns CSR on the index's device:
+    (offsets int64 [nq + 1], scores f32 [R], ids int64 [R] = local index + id_offset); row i is
+    [offsets[i], offsets[i + 1]), ordered by (score desc, id asc). Scores have the bits of the fp32 scan; NaN scores never
+    qualify, t = -inf returns every eligible doc and t = +inf only +inf scores. doc_mask / mask_of as in score_topk.
+    The tensor-core filter keeps every doc whose approximate score is >= t - eps (eps: the filter's error bound, DESIGN
+    §4), so its candidates hold every result; they are rescored exactly. A query with more than `cap` candidates
+    (default RANGE_CAP), or whose norms allow no bound, reruns through the fp32 scan, as do small problems and
+    force_exact. stats: path ("exact" or "filter+rescore"), candidates (rescored: the filter's candidates of the rows
+    that did not overflow), fallback (rows rerun through the scan), cap."""
+    q, masks = _queries_and_mask(queries, index, doc_mask, mask_of)
+    t = _check_min_score(min_score, q.shape[0], index.emb.device)
+    cap = _check_cap(cap)
+    with L.on_device(q.device):
+        return _score_range(q, index, t, id_offset, masks, force_exact, stats, cap)
+
+
+def _score_range(q: torch.Tensor, index: CorpusIndex, t: torch.Tensor, id_offset: int, masks: Optional[_MaskSet],
+                 force_exact: bool, stats: Optional[dict], cap: int):
+    nq, d = q.shape
+    nd = index.nd
+    if d != index.emb.shape[1]:
+        raise ValueError("query / corpus dim mismatch")
+    rows = torch.arange(nq, dtype=torch.int64)
+    info = dict(path="exact", candidates=0, fallback=0, cap=cap)
+    if nq == 0:
+        pieces = []
+    elif force_exact or nq * nd <= SMALL_PROBLEM or nd < 256:
+        pieces = _range_scan(q, index, t, masks, rows, id_offset)
+    else:
+        info["path"] = "filter+rescore"
+        pieces = []
+        step = max(1, min(nq, RANGE_BUDGET // cap))
+        for r0 in range(0, nq, step):
+            n = min(step, nq - r0)
+            pieces += _range_filter(q[r0:r0 + n], index, t[r0:r0 + n], masks, r0, rows[r0:r0 + n], cap, id_offset, info)
+    if stats is not None:
+        stats.update(info)
+    return _range_assemble(nq, pieces, q.device)
+
+
+def _range_filter(q: torch.Tensor, index: CorpusIndex, t: torch.Tensor, masks: Optional[_MaskSet], r0: int,
+                  rows: torch.Tensor, cap: int, id_offset: int, info: dict):
+    """Query rows r0 .. r0 + n of the batch through the range filter and the candidate rescoring; rows that overflowed
+    (or have no bound) rerun through the scan. Returns the CSR pieces of these rows."""
+    n, d = q.shape
+    nd, dev = index.nd, q.device
+    lib, sp = L.lib(), L.stream_ptr()
+    q16 = torch.empty((n, d), dtype=torch.float16, device=dev)
+    qn = torch.empty(n, dtype=torch.float32, device=dev)
+    L.check(lib.vr_f32_to_f16_rows(q.data_ptr(), n, d, q16.data_ptr(), qn.data_ptr(), None, sp))
+    counts = torch.empty(n, dtype=torch.int32, device=dev)
+    cand = torch.empty((n, cap), dtype=torch.int32, device=dev)
+    L.check(lib.vr_score_filter_range(q16.data_ptr(), n, index.emb_f16.data_ptr(), nd, d, t.data_ptr(), qn.data_ptr(),
+                                      index.max_norm.data_ptr(), None if masks is None else masks.arg(r0), cap,
+                                      counts.data_ptr(), cand.data_ptr(), sp))
+    del q16
+    rs = torch.empty((n, cap), dtype=torch.float32, device=dev)
+    ri = torch.empty((n, cap), dtype=torch.int32, device=dev)
+    kept = torch.empty(n, dtype=torch.int32, device=dev)
+    L.check(lib.vr_score_rescore_range(q.data_ptr(), n, index.emb.data_ptr(), nd, d, t.data_ptr(), cap, counts.data_ptr(),
+                                       cand.data_ptr(), rs.data_ptr(), ri.data_ptr(), kept.data_ptr(), sp))
+    del cand
+    host = torch.stack([counts, kept]).cpu()  # host sync: the CSR sizes are needed to allocate the output
+    over = host[0] > cap
+    info["candidates"] += int(host[0][~over].sum())
+    ok = torch.nonzero(~over).flatten()
+    pieces = []
+    if ok.numel():
+        pieces.append(_range_sort(rs, ri, cap, kept, host[1], ok, rows, id_offset))
+    bad = torch.nonzero(over).flatten()
+    if bad.numel():
+        info["fallback"] += int(bad.numel())
+        sel = bad.to(dev)
+        m = None if masks is None else _MaskSet(masks.words, None if masks.of_query is None else masks.of_query[r0:r0 + n]).rows(sel)
+        pieces += _range_scan(q.index_select(0, sel), index, t.index_select(0, sel), m, rows[bad], id_offset)
+    return pieces
+
+
+def _range_scan(q: torch.Tensor, index: CorpusIndex, t: torch.Tensor, masks: Optional[_MaskSet], rows: torch.Tensor,
+                id_offset: int):
+    """The fp32 scan path over query rows q (global row ids `rows`): vr_score_exact, then vr_range_rows keeps the eligible
+    columns with s >= t, in chunks of rows that bound the [rows, nd] scratch. Returns the CSR pieces."""
+    n, d = q.shape
+    nd, dev = index.nd, q.device
+    lib, sp = L.lib(), L.stream_ptr()
+    step = max(1, min(n, RANGE_BUDGET // nd, 65535))
+    scratch = torch.empty((step, nd), dtype=torch.float32, device=dev)
+    rs = torch.empty((step, nd), dtype=torch.float32, device=dev)
+    ri = torch.empty((step, nd), dtype=torch.int32, device=dev)
+    counts = torch.empty(step, dtype=torch.int32, device=dev)
+    pieces = []
+    for r0 in range(0, n, step):
+        m = min(step, n - r0)
+        L.check(lib.vr_score_exact(q[r0:].data_ptr(), m, index.emb.data_ptr(), nd, d, scratch.data_ptr(), sp))
+        L.check(lib.vr_range_rows(scratch.data_ptr(), m, nd, t[r0:].data_ptr(), None if masks is None else masks.arg(r0), nd,
+                                  rs.data_ptr(), ri.data_ptr(), counts.data_ptr(), sp))
+        pieces.append(_range_sort(rs, ri, nd, counts, counts[:m].cpu(), torch.arange(m), rows[r0:r0 + m], id_offset))
+    return pieces
+
+
+def _range_sort(rs: torch.Tensor, ri: torch.Tensor, pitch: int, counts: torch.Tensor, counts_host: torch.Tensor,
+                sel: torch.Tensor, rows: torch.Tensor, id_offset: int):
+    """Order the region rows `sel` (host int64) of (rs, ri, pitch, counts) into one CSR piece: (global rows, counts,
+    scores, ids), the entries of rows[sel] one after the other in that order."""
+    dev = rs.device
+    lib, sp = L.lib(), L.stream_ptr()
+    c = counts_host.to(torch.int64)
+    off = torch.zeros(c.shape[0], dtype=torch.int64)
+    cs = c[sel]
+    off[sel] = torch.cumsum(cs, 0) - cs           # each selected region row's place in the piece
+    total = int(cs.sum())
+    out_s = torch.empty(total, dtype=torch.float32, device=dev)
+    out_i = torch.empty(total, dtype=torch.int64, device=dev)
+    if total:
+        off_d = off.to(dev)
+        short, long_ = sel[(cs > 0) & (cs <= RANGE_SORT_SMEM)], sel[cs > RANGE_SORT_SMEM]
+        for r0 in range(0, short.numel(), 65535):
+            part = short[r0:r0 + 65535]
+            L.check(lib.vr_range_sort(rs.data_ptr(), ri.data_ptr(), pitch, counts.data_ptr(), part.numel(),
+                                      part.to(torch.int32).to(dev).data_ptr(), off_d.data_ptr(), int(c[part].max()), id_offset,
+                                      None, 0, out_s.data_ptr(), out_i.data_ptr(), sp))
+        if long_.numel():
+            most = int(c[long_].max())
+            per = max(1, min(65535, RANGE_BUDGET // (lib.vr_range_sort_ws_bytes(1, most) // 8)))
+            ws = torch.empty(lib.vr_range_sort_ws_bytes(min(per, long_.numel()), most) // 8, dtype=torch.int64, device=dev)
+            for r0 in range(0, long_.numel(), per):
+                part = long_[r0:r0 + per]
+                L.check(lib.vr_range_sort(rs.data_ptr(), ri.data_ptr(), pitch, counts.data_ptr(), part.numel(),
+                                          part.to(torch.int32).to(dev).data_ptr(), off_d.data_ptr(), most, id_offset,
+                                          ws.data_ptr(), ws.numel() * 8, out_s.data_ptr(), out_i.data_ptr(), sp))
+    return rows[sel], cs, out_s, out_i
+
+
+def _range_assemble(nq: int, pieces, device) -> Tuple[torch.Tensor, torch.Tensor, torch.Tensor]:
+    """CSR (offsets, scores, ids) of all rows from pieces (rows, counts, scores, ids) that cover each row once."""
+    counts = torch.zeros(nq, dtype=torch.int64)
+    for rows, c, _, _ in pieces:
+        counts[rows] = c
+    offsets = torch.zeros(nq + 1, dtype=torch.int64)
+    offsets[1:] = torch.cumsum(counts, 0)
+    if pieces and torch.equal(torch.cat([p[0] for p in pieces]), torch.arange(nq)):  # the pieces are in row order
+        if len(pieces) == 1:
+            return offsets.to(device), pieces[0][2], pieces[0][3]
+        return offsets.to(device), torch.cat([p[2] for p in pieces]), torch.cat([p[3] for p in pieces])
+    total = int(offsets[-1])
+    out_s = torch.empty(total, dtype=torch.float32, device=device)
+    out_i = torch.empty(total, dtype=torch.int64, device=device)
+    for rows, c, s, i in pieces:
+        if s.numel() == 0:
+            continue
+        # entry e of the piece's row k goes to offsets[rows[k]] + (e - the piece's start of row k)
+        shift = offsets[rows] - (torch.cumsum(c, 0) - c)
+        dst = torch.arange(s.numel(), device=device) + torch.repeat_interleave(shift.to(device), c.to(device))
+        out_s[dst] = s
+        out_i[dst] = i
+    return offsets.to(device), out_s, out_i
+
+
 def shard_range(n_items: int, rank: int, world: int) -> Tuple[int, int]:
     """Contiguous page range [lo, hi) owned by `rank` (SURVEY.md §8e: corpus sharded by page)."""
     base, rem = divmod(n_items, world)
