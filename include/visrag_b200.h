@@ -481,6 +481,29 @@ int vr_range_sort(const float* scores, const int32_t* ids, int64_t pitch, const 
                   const int32_t* row_of, const int64_t* out_offsets, int32_t max_count, int64_t id_offset, void* ws,
                   int64_t ws_bytes, float* out_scores, int64_t* out_ids, void* stream);
 
+/* vr_mmr_select: maximal marginal relevance (DESIGN §4) over given candidates. Query row r has the candidates
+ * cand_ids [nq, fetch] (local doc ids, row-major) with relevance scores cand_scores [nq, fetch], in (score desc, id asc)
+ * order as vr_topk_rows returns them; the first id outside [0, nd) ends the row's candidates (F' of them) and is never
+ * read. lambda [nq] f32 is each row's lambda (1: relevance only, 0: diversity only). sim(a, b) is the fp32 dot product of
+ * emb rows a and b with the bits vr_score_exact gives that pair. Pick 1 is candidate 0; pick t >= 2 is the unpicked
+ * candidate j with the largest v_j = fl(fl(lambda * s_j) - fl(mu * r_j)), mu = fl(1 - lambda), r_j = the maxNum of
+ * sim(c_j, e) over the picked e (NaN ignored); NaN ranks below every number and equal values (+0 = -0) go to the lower
+ * position. out_scores / out_ids [nq, k] hold the min(k, F') picks in pick order, (s_j, id + id_offset), then (-inf, -1).
+ * One thread-block cluster per row holds the row's candidate rows in shared memory (each read from HBM once): the
+ * smallest of 1, 2, 4, 8 CTAs whose ceil(fetch / C) rows take at most 144 KiB each, chosen from fetch and dim alone (the
+ * bits do not depend on it); each CTA also keeps a copy of the latest pick's row. No allocation and no synchronisation:
+ * the call can be captured in a CUDA graph.
+ * Refused before any CUDA call, naming the argument: a NULL or misaligned pointer, nq outside (0, 2^28), nd < 1, dim not
+ * a positive multiple of 4, fetch outside [1, 128], fetch * dim > 128 * 2304, no cluster size whose share fits 144 KiB,
+ * or a share that does not fit 200 KiB with the pick's row (dims of 2304 and less always fit; see
+ * visrag_b200.retriever.mmr_fetch_max), and k outside [1, fetch]. lambda's values are the caller's to check (visrag_b200.retriever.mmr_select refuses NaN and
+ * values outside [0, 1]).
+ * Alignment (bytes) of the vr_mmr_select arguments: emb 16, cand_scores 4, cand_ids 8, lambda 4, out_scores 4,
+ * out_ids 8 */
+int vr_mmr_select(const float* emb, int64_t nd, int32_t dim, const float* cand_scores, const int64_t* cand_ids, int32_t nq,
+                  int32_t fetch, const float* lambda, int32_t k, int64_t id_offset, float* out_scores, int64_t* out_ids,
+                  void* stream);
+
 #ifdef __cplusplus
 }
 #endif

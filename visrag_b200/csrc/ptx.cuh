@@ -89,6 +89,17 @@ __device__ __forceinline__ float4 ld_shared_cluster_f4(uint32_t cluster_addr) {
     asm volatile("ld.shared::cluster.v4.f32 {%0, %1, %2, %3}, [%4];" : "=f"(v.x), "=f"(v.y), "=f"(v.z), "=f"(v.w) : "r"(cluster_addr) : "memory");
     return v;
 }
+__device__ __forceinline__ void st_shared_cluster_u64(uint32_t cluster_addr, unsigned long long v) {
+    asm volatile("st.shared::cluster.u64 [%0], %1;" ::"r"(cluster_addr), "l"(v) : "memory");
+}
+// generic address of the same smem location in CTA `rank` of the cluster: ordinary loads through it read that CTA's
+// shared memory (DSMEM)
+template <typename T>
+__device__ __forceinline__ T* map_cluster_ptr(T* p, uint32_t rank) {
+    uint64_t r;
+    asm volatile("mapa.u64 %0, %1, %2;" : "=l"(r) : "l"(p), "r"(rank));
+    return reinterpret_cast<T*>(r);
+}
 
 // ---------------------------------------------------------------- fences
 __device__ __forceinline__ void fence_proxy_async_smem() {

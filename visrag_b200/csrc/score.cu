@@ -1678,6 +1678,140 @@ static long long range_sort_ws(int rows, int max_count) {
     return max_count <= RSORT_TILE ? 0 : static_cast<long long>(rows) * range_sort_P(max_count) * 8;
 }
 
+// ---------------------------------------------------------------------------------------------------- MMR selection
+// Maximal marginal relevance over each query row's candidates (DESIGN §4). One thread-block cluster of C CTAs per query
+// row: CTA c holds candidate rows [c * R, c * R + R) (R = ceil(fetch / C)) in shared memory, read from HBM once by 1-D
+// bulk copies. Pick 1 is candidate 0. Each later pick is one round: every CTA reads the previous pick's row from its
+// owner over DSMEM and folds sim(c_j, pick) into r_j of its own unpicked rows (one warp per row, warp_dot_row: the bits
+// of vr_score_exact), takes its best key of v_j = fl(fl(lambda * s_j) - fl(mu * r_j)), and stores it into slot
+// [round & 1][rank] of every CTA. After one cluster barrier every CTA reduces the same C slots and so agrees on the pick.
+// The other parity lets a CTA write round t + 1's key while a slower one still reads round t's; round t + 2 needs the
+// barrier of round t + 1, which the slower CTA passes only after reading.
+constexpr int MMR_THREADS = 256;
+constexpr int MMR_WARPS = MMR_THREADS / 32;
+constexpr int MMR_MAX_FETCH = 128;
+constexpr long long MMR_MAX_ELEMS = 128ll * 2304;   // fetch * dim
+constexpr int MMR_CTA_BYTES = 144 * 1024;           // candidate rows held by one CTA
+constexpr int MMR_MAX_CLUSTER = 8;
+
+// (v, position j) as one key, larger = picked first: v's order bits (any NaN = 1, below -inf; -0 = +0) above ~j, so
+// equal values go to the lower position. 0 is no candidate.
+__device__ __forceinline__ unsigned long long mmr_key(float v, int j) {
+    unsigned o = 1u;
+    if (!isnan(v)) {
+        const unsigned b = v == 0.f ? 0u : __float_as_uint(v);
+        o = (b & 0x80000000u) ? ~b : (b | 0x80000000u);
+    }
+    return (static_cast<unsigned long long>(o) << 32) | (0xffffffffu - static_cast<unsigned>(j));
+}
+
+__global__ void __launch_bounds__(MMR_THREADS, 1)
+mmr_select_kernel(const float* __restrict__ emb, long long nd, int dim, const float* __restrict__ cand_scores,
+                  const long long* __restrict__ cand_ids, int fetch, const float* __restrict__ lambda, int k, int R,
+                  long long id_offset, float* __restrict__ out_scores, long long* __restrict__ out_ids) {
+    extern __shared__ __align__(16) float mmr_rows[];   // [R][dim]: this CTA's candidate rows, then [dim]: the pick's row
+    __shared__ long long cid[MMR_MAX_FETCH];            // the row's candidate ids
+    __shared__ float rel[MMR_MAX_FETCH], red[MMR_MAX_FETCH];  // s_j and r_j of this CTA's rows
+    __shared__ int taken[MMR_MAX_FETCH], picks[MMR_MAX_FETCH];
+    __shared__ unsigned long long slots[2][MMR_MAX_CLUSTER];
+    __shared__ __align__(8) uint64_t bar;
+    __shared__ int sh_n;
+    const unsigned C = cluster_nctarank(), rank = cluster_ctarank();
+    const int q = blockIdx.x / C;
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const float* cs = cand_scores + static_cast<long long>(q) * fetch;
+    if (threadIdx.x == 0) {
+        sh_n = fetch;
+        mbar_init(&bar, 1);
+        fence_mbar_init();
+    }
+    __syncthreads();
+    // the first id outside [0, nd) ends the row's candidates
+    for (int j = threadIdx.x; j < fetch; j += MMR_THREADS) {
+        const long long id = cand_ids[static_cast<long long>(q) * fetch + j];
+        cid[j] = id;
+        if (id < 0 || id >= nd) atomicMin(&sh_n, j);
+    }
+    __syncthreads();
+    const int n = sh_n;
+    const int base = static_cast<int>(rank) * R;
+    const int own = max(0, min(R, n - base));
+    const uint32_t row_bytes = static_cast<uint32_t>(dim) * 4;
+    if (threadIdx.x == 0) {
+        mbar_expect_tx(&bar, row_bytes * own);
+        for (int j = 0; j < own; ++j)
+            bulk_load_1d(mmr_rows + static_cast<long long>(j) * dim, emb + cid[base + j] * dim, row_bytes, &bar);
+    }
+    for (int j = threadIdx.x; j < own; j += MMR_THREADS) {
+        rel[j] = cs[base + j];
+        red[j] = -INFINITY;
+        taken[j] = 0;
+    }
+    const float lam = lambda[q];
+    const float mu = __fsub_rn(1.f, lam);
+    const int npick = min(k, n);
+    mbar_wait(&bar, 0);
+    cluster_sync_all();  // every CTA of the cluster runs and holds its rows
+    int p = 0;           // the latest pick
+    float* prow = mmr_rows + static_cast<long long>(R) * dim;
+    for (int t = 1; t < npick; ++t) {
+        // one copy of the pick's row per CTA: every warp reading it over DSMEM for each of its rows would make the
+        // owner's SM serve C * R rows a round
+        const int owner = p / R;
+        const float4* src = reinterpret_cast<const float4*>(
+            map_cluster_ptr(mmr_rows + static_cast<long long>(p - owner * R) * dim, owner));
+        for (int i = threadIdx.x; i < (dim >> 2); i += MMR_THREADS) reinterpret_cast<float4*>(prow)[i] = src[i];
+        __syncthreads();
+        for (int j = warp; j < own; j += MMR_WARPS) {
+            if (taken[j] || base + j == p) continue;
+            const float s = warp_dot_row(prow, mmr_rows + static_cast<long long>(j) * dim, dim, lane);
+            if (lane == 0) red[j] = fmaxf(red[j], s);  // maxNum: a NaN similarity leaves r_j as it is
+        }
+        __syncthreads();
+        if (warp == 0) {
+            if (lane == 0 && p >= base && p < base + own) taken[p - base] = 1;
+            __syncwarp();
+            unsigned long long best = 0;
+            for (int j = lane; j < own; j += 32) {
+                if (taken[j]) continue;
+                const float v = __fsub_rn(__fmul_rn(lam, rel[j]), __fmul_rn(mu, red[j]));
+                const unsigned long long key = mmr_key(v, base + j);
+                best = key > best ? key : best;
+            }
+#pragma unroll
+            for (int o = 16; o > 0; o >>= 1) {
+                const unsigned long long other = __shfl_xor_sync(0xffffffffu, best, o);
+                best = other > best ? other : best;
+            }
+            if (lane < static_cast<int>(C)) st_shared_cluster_u64(mapa_u32(smem_u32(&slots[t & 1][rank]), lane), best);
+        }
+        cluster_sync_all();  // also the last DSMEM access of the round: no CTA exits while another reads its rows
+        unsigned long long best = slots[t & 1][0];
+        for (unsigned c = 1; c < C; ++c) best = slots[t & 1][c] > best ? slots[t & 1][c] : best;
+        p = static_cast<int>(0xffffffffu - static_cast<unsigned>(best & 0xffffffffu));
+        if (threadIdx.x == 0) picks[t] = p;
+    }
+    if (rank != 0) return;
+    if (threadIdx.x == 0) picks[0] = 0;
+    __syncthreads();
+    for (int t = threadIdx.x; t < k; t += MMR_THREADS) {
+        const long long o = static_cast<long long>(q) * k + t;
+        out_scores[o] = t < npick ? cs[picks[t]] : -INFINITY;
+        out_ids[o] = t < npick ? cid[picks[t]] + id_offset : -1;
+    }
+}
+
+// Cluster size of a call: the smallest of 1, 2, 4, 8 CTAs whose share of the fetch rows fits MMR_CTA_BYTES, provided
+// that share and the pick's row fit MMR_SMEM_BYTES (0: none).
+constexpr int MMR_SMEM_BYTES = 200 * 1024;
+static int mmr_cluster(int fetch, int dim) {
+    for (int c = 1; c <= MMR_MAX_CLUSTER; c *= 2) {
+        const long long rows = (fetch + c - 1) / c;
+        if (rows * dim * 4 <= MMR_CTA_BYTES) return (rows + 1) * dim * 4 <= MMR_SMEM_BYTES ? c : 0;
+    }
+    return 0;
+}
+
 }  // namespace vr
 
 using namespace vr;
@@ -2246,6 +2380,49 @@ extern "C" int vr_range_sort(const float* scores, const int32_t* ids, int64_t pi
         range_bitonic_tile_kernel<<<tiles, RSORT_THREADS, 0, st>>>(w, P, k);
     }
     range_emit_kernel<<<grid, 256, 0, st>>>(w, P, counts, row_of, oo, id_offset, out_scores, oi);
+    VR_CHECK_CUDA(cudaGetLastError());
+    return 0;
+}
+
+// ---------------------------------------------------------------------------------------------------- MMR selection
+extern "C" int vr_mmr_select(const float* emb, int64_t nd, int32_t dim, const float* cand_scores, const int64_t* cand_ids,
+                             int32_t nq, int32_t fetch, const float* lambda, int32_t k, int64_t id_offset, float* out_scores,
+                             int64_t* out_ids, void* stream) {
+    const char* fn = "vr_mmr_select";
+    VR_REQUIRE_PTR(fn, "emb", emb, 16);  // bulk-copy sources
+    VR_REQUIRE_PTR(fn, "cand_scores", cand_scores, 4);
+    VR_REQUIRE_PTR(fn, "cand_ids", cand_ids, 8);
+    VR_REQUIRE_PTR(fn, "lambda", lambda, 4);
+    VR_REQUIRE_PTR(fn, "out_scores", out_scores, 4);
+    VR_REQUIRE_PTR(fn, "out_ids", out_ids, 8);
+    VR_REQUIRE(nq > 0 && nq < (1 << 28), "%s: nq=%d, needs 0 < nq < 2^28", fn, nq);
+    VR_REQUIRE(nd > 0, "%s: nd=%lld, needs at least 1", fn, (long long)nd);
+    VR_REQUIRE(dim > 0 && dim % 4 == 0, "%s: dim=%d, needs a positive multiple of 4", fn, dim);
+    VR_REQUIRE(fetch >= 1 && fetch <= MMR_MAX_FETCH, "%s: fetch=%d, needs 1 <= fetch <= %d", fn, fetch, MMR_MAX_FETCH);
+    VR_REQUIRE(static_cast<long long>(fetch) * dim <= MMR_MAX_ELEMS, "%s: fetch=%d x dim=%d exceeds %lld floats of rows", fn,
+               fetch, dim, MMR_MAX_ELEMS);
+    const int C = mmr_cluster(fetch, dim);
+    VR_REQUIRE(C > 0, "%s: fetch=%d rows of dim=%d do not fit %d CTAs of %d bytes (%d with the pick's row)", fn, fetch,
+               dim, MMR_MAX_CLUSTER, MMR_CTA_BYTES, MMR_SMEM_BYTES);
+    VR_REQUIRE(k >= 1 && k <= fetch, "%s: k=%d, needs 1 <= k <= fetch=%d", fn, k, fetch);
+    const int R = (fetch + C - 1) / C;
+    static unsigned long long attr_set = 0;
+    if (first_use_on_device(&attr_set))
+        VR_CHECK_CUDA(cudaFuncSetAttribute(mmr_select_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, MMR_SMEM_BYTES));
+    cudaLaunchConfig_t cfg = {};
+    cfg.gridDim = dim3(static_cast<unsigned>(nq) * C);
+    cfg.blockDim = dim3(MMR_THREADS);
+    cfg.dynamicSmemBytes = static_cast<size_t>(R + 1) * dim * sizeof(float);
+    cfg.stream = reinterpret_cast<cudaStream_t>(stream);
+    cudaLaunchAttribute attr;
+    attr.id = cudaLaunchAttributeClusterDimension;
+    attr.val.clusterDim.x = C; attr.val.clusterDim.y = 1; attr.val.clusterDim.z = 1;
+    cfg.attrs = &attr;
+    cfg.numAttrs = 1;
+    VR_CHECK_CUDA(cudaLaunchKernelEx(&cfg, mmr_select_kernel, emb, static_cast<long long>(nd), static_cast<int>(dim),
+                                     cand_scores, reinterpret_cast<const long long*>(cand_ids), static_cast<int>(fetch),
+                                     lambda, static_cast<int>(k), R, static_cast<long long>(id_offset), out_scores,
+                                     reinterpret_cast<long long*>(out_ids)));
     VR_CHECK_CUDA(cudaGetLastError());
     return 0;
 }

@@ -19,6 +19,8 @@ one pass over the index serves them all, and each query's row equals its search 
 Documents: `build_index.py` stores page i of `report.pdf` as `report.pdf_i.png`, so a page's document is its filename up to
 the last `_` when the rest is `<digits>.png` (any other filename is its own document). `search_documents` returns the
 top-k documents by their best page (`retriever.score_topk_groups`), so one long document cannot fill every slot.
+`search_diverse` / `retrieve_diverse` pick pages by maximal marginal relevance (`retriever.mmr_select`), so near-copies
+of one page, in one document or several, do not fill every slot either.
 """
 from __future__ import annotations
 
@@ -290,6 +292,36 @@ class KnowledgeBase:
             e = torch.empty(0, dtype=torch.int64, device=dev)
             return e, e.clone(), torch.empty(0, dtype=torch.float32, device=dev)
         return torch.cat(a_parts), torch.cat(b_parts), torch.cat(s_parts)
+
+    def search_diverse(self, query_reps, topk: int, lambda_mult=0.5, fetch_k: Optional[int] = None,
+                       within: Optional[Iterable[str]] = None,
+                       within_each: Optional[Sequence[Optional[Iterable[str]]]] = None) -> Tuple[torch.Tensor, torch.Tensor]:
+        """Diverse top-k pages by maximal marginal relevance: (relevance scores [nq,k] f32, page indices [nq,k] i64) on the
+        device, in pick order. The candidates are search(query_reps, fetch_k, within, within_each), so scopes and removed
+        pages behave exactly as there, and retriever.mmr_select picks k = min(topk, candidates) of them. lambda_mult: a
+        float in [0, 1] or an f32 tensor [nq] on the device (1: the order of search; lower values trade relevance for
+        pages unlike those already picked). fetch_k None: the largest allowed value <= max(20, 4 topk)."""
+        _, fetch = retriever._check_fetch(topk, fetch_k, self.index.emb.shape[1])
+        q = self._queries(query_reps)
+        lam = retriever._check_lambda(lambda_mult, q.shape[0], self.index.emb.device)
+        s, ids = self.search(q, fetch, within, within_each)
+        k = min(topk, s.shape[1])
+        if k == 0 or s.shape[0] == 0:
+            return s[:, :k], ids[:, :k]
+        with L.on_device(s.device):
+            return retriever._mmr_select(self.index, s, ids, k, lam, 0)
+
+    def retrieve_diverse(self, query_rep, topk: int, lambda_mult=0.5, fetch_k: Optional[int] = None,
+                         within: Optional[Iterable[str]] = None) -> List[str]:
+        """Paths of k diverse page images (search_diverse), in pick order: for a generator with a small image budget."""
+        _, ids = self.search_diverse(query_rep, topk, lambda_mult, fetch_k, within)
+        return [os.path.join(self.path, self.filenames[i]) for i in ids[0].tolist() if i >= 0]
+
+    def retrieve_diverse_text(self, model, tokenizer, query: str, topk: int, lambda_mult=0.5,
+                              fetch_k: Optional[int] = None, within: Optional[Iterable[str]] = None) -> List[str]:
+        """retrieve_text with diverse pages: instruction + query -> embedding -> retrieve_diverse."""
+        out = model(query={"text": [DEMO_QUERY_PREFIX + query], "image": [None]}, tokenizer=tokenizer)
+        return self.retrieve_diverse(out.q_reps, topk, lambda_mult, fetch_k, within)
 
     def retrieve_documents(self, query_rep, topk: int, within: Optional[Iterable[str]] = None) -> List[Tuple[str, str]]:
         """[(document name, path of its best page image)] of the top-k documents, best first."""

@@ -19,6 +19,9 @@ no others; the result equals the masked call with a mask of exactly the listed p
 
 Document-level retrieval (`score_topk_groups`, `sharded_topk_groups`): `doc_groups` (int [nd]) gives every doc (page) its
 group (document); the top-k groups by their best page's exact fp32 score, ranked by (score desc, best page asc).
+
+Diverse retrieval (`score_mmr`, `mmr_select`): maximal marginal relevance over each query's top fetch_k pages, picked
+on the GPU (vr_mmr_select) with the bits fixed by the definition in DESIGN §4.
 """
 from __future__ import annotations
 
@@ -810,6 +813,138 @@ def _range_assemble(nq: int, pieces, device) -> Tuple[torch.Tensor, torch.Tensor
         out_s[dst] = s
         out_i[dst] = i
     return offsets.to(device), out_s, out_i
+
+
+# ------------------------------------------------------------------------------------------------------
+# Diverse retrieval: maximal marginal relevance over the top candidates
+# ------------------------------------------------------------------------------------------------------
+MMR_MAX_FETCH = 128               # candidates per query row (vr_mmr_select)
+MMR_MAX_ELEMS = 128 * 2304        # fetch * dim: the candidate rows one cluster holds
+MMR_CTA_FLOATS = 144 * 1024 // 4  # ceil(fetch / C) rows of dim: one CTA's share in a cluster of C <= 8
+MMR_SMEM_FLOATS = 200 * 1024 // 4  # that share and a copy of the pick's row
+
+
+def _mmr_fits(fetch: int, dim: int) -> bool:
+    """vr_mmr_select's caps (mmr_cluster in score.cu): the smallest cluster whose share fits also fits the pick's row."""
+    if fetch > MMR_MAX_FETCH or fetch * dim > MMR_MAX_ELEMS:
+        return False
+    for c in (1, 2, 4, 8):
+        rows = -(-fetch // c)
+        if rows * dim <= MMR_CTA_FLOATS:
+            return (rows + 1) * dim <= MMR_SMEM_FLOATS
+    return False
+
+
+def mmr_fetch_max(dim: int) -> int:
+    """The largest fetch_k vr_mmr_select takes at this embedding dim (0: none)."""
+    return next((f for f in range(MMR_MAX_FETCH, 0, -1) if _mmr_fits(f, dim)), 0)
+
+
+def _check_count(v, name: str) -> int:
+    if isinstance(v, bool) or not isinstance(v, (int, np.integer)):
+        raise ValueError(f"{name} must be an int, got {v!r}")
+    return int(v)
+
+
+def _check_fetch(k, fetch_k, dim: int) -> Tuple[int, int]:
+    """(k, fetch): 1 <= k <= fetch <= mmr_fetch_max(dim); fetch_k None: the largest allowed value <= max(20, 4 k)."""
+    k = _check_count(k, "k")
+    top = mmr_fetch_max(dim)
+    if top == 0:
+        raise ValueError(f"dim={dim} is too large for the selection: two candidate rows must fit {MMR_SMEM_FLOATS} floats")
+    fetch =min(max(20, 4 * k), top) if fetch_k is None else _check_count(fetch_k, "fetch_k")
+    if fetch < 1 or not _mmr_fits(fetch, dim):
+        raise ValueError(f"fetch_k={fetch} must lie in [1, {top}] at dim {dim} (at most {MMR_MAX_FETCH} candidates and "
+                         f"{MMR_MAX_ELEMS} floats of candidate rows)")
+    if k < 1 or k > fetch:
+        raise ValueError(f"k={k} must lie in [1, fetch_k={fetch}]")
+    return k, fetch
+
+
+def _check_lambda(lambda_mult, nq: int, device) -> torch.Tensor:
+    """lambda_mult as an f32 [nq] tensor on the index's device: a float for every query, or an f32 tensor [nq]; every
+    value in [0, 1]."""
+    if isinstance(lambda_mult, torch.Tensor):
+        if lambda_mult.dtype != torch.float32:
+            raise ValueError(f"lambda_mult must be a float or a torch.float32 tensor, got {lambda_mult.dtype}")
+        if lambda_mult.dim() != 1 or lambda_mult.shape[0] != nq:
+            raise ValueError(f"lambda_mult must have shape [{nq}] (one lambda per query), got {list(lambda_mult.shape)}")
+        if lambda_mult.device != device:
+            raise ValueError(f"lambda_mult lives on {lambda_mult.device}, the index on {device}")
+        t = lambda_mult.contiguous()
+        if nq:
+            nan, lo, hi = torch.stack([t.isnan().any().float(), t.min(), t.max()]).tolist()
+            if nan or lo < 0 or hi > 1:
+                raise ValueError(f"lambda_mult must lie in [0, 1] and not be NaN, got values in [{lo}, {hi}]")
+        return t
+    if isinstance(lambda_mult, bool) or not isinstance(lambda_mult, (int, float, np.floating, np.integer)):
+        raise ValueError(f"lambda_mult must be a float or a torch.float32 tensor, got {type(lambda_mult).__name__}")
+    if not 0 <= lambda_mult <= 1:  # NaN fails too
+        raise ValueError(f"lambda_mult must lie in [0, 1] and not be NaN, got {lambda_mult}")
+    return torch.full((nq,), float(lambda_mult), dtype=torch.float32, device=device)
+
+
+def mmr_select(index: CorpusIndex, scores: torch.Tensor, ids: torch.Tensor, k: int, lambda_mult=0.5, id_offset: int = 0
+               ) -> Tuple[torch.Tensor, torch.Tensor]:
+    """Maximal marginal relevance over given candidates (DESIGN §4). scores f32 / ids int [nq, F] on the index's device are
+    each query's candidates in (score desc, id asc) order with a (-inf, -1) tail, as score_topk returns them (local ids:
+    id_offset 0). Pick 1 is the first candidate; each later pick is the unpicked candidate j with the largest
+    fl(fl(lambda s_j) - fl((1 - lambda) r_j)), r_j = the largest exact fp32 similarity emb[c_j] . emb[e] over the picks e
+    so far (NaN ignored); NaN values rank last and ties go to the earlier candidate. lambda_mult: a float in [0, 1]
+    (1: relevance only, as score_topk; 0: diversity only), or an f32 tensor [nq] of them on the index's device.
+    Returns (scores [nq, k] f32, ids [nq, k] i64 = local id + id_offset) in pick order, each pick with its relevance
+    score; a row with fewer than k candidates ends in (-inf, -1). Caps: 1 <= k <= F <= mmr_fetch_max(dim)."""
+    dev = index.emb.device
+    if not isinstance(scores, torch.Tensor) or scores.dtype != torch.float32 or scores.dim() != 2:
+        raise ValueError("scores must be a torch.float32 tensor [nq, F]")
+    if not isinstance(ids, torch.Tensor) or ids.dtype not in (torch.int32, torch.int64) or ids.shape != scores.shape:
+        raise ValueError(f"ids must be an int32 or int64 torch tensor of the shape of scores {list(scores.shape)}")
+    if scores.device != dev or ids.device != dev:
+        raise ValueError(f"scores live on {scores.device} and ids on {ids.device}, the index on {dev}")
+    nq, F = scores.shape
+    k, _ = _check_fetch(k, F, index.emb.shape[1])
+    lam = _check_lambda(lambda_mult, nq, dev)
+    ids = ids.to(torch.int64).contiguous()
+    if ids.numel():
+        lo, hi = torch.aminmax(ids)
+        lo, hi = int(lo), int(hi)
+        if lo < -1 or hi >= index.nd:
+            raise ValueError(f"ids must lie in [0, {index.nd}) (local docs of the index; -1 ends a row), got [{lo}, {hi}]")
+    with L.on_device(dev):
+        return _mmr_select(index, scores.contiguous(), ids, k, lam, id_offset)
+
+
+def _mmr_select(index: CorpusIndex, scores: torch.Tensor, ids: torch.Tensor, k: int, lam: torch.Tensor, id_offset: int):
+    nq, F = scores.shape
+    out_s = torch.empty((nq, k), dtype=torch.float32, device=scores.device)
+    out_i = torch.empty((nq, k), dtype=torch.int64, device=scores.device)
+    if nq:
+        L.check(L.lib().vr_mmr_select(index.emb.data_ptr(), index.nd, index.emb.shape[1], scores.data_ptr(), ids.data_ptr(),
+                                      nq, F, lam.data_ptr(), k, id_offset, out_s.data_ptr(), out_i.data_ptr(),
+                                      L.stream_ptr()))
+    return out_s, out_i
+
+
+def score_mmr(queries: torch.Tensor, index: CorpusIndex, k: int, lambda_mult=0.5, fetch_k: Optional[int] = None,
+              id_offset: int = 0, doc_mask: Optional[torch.Tensor] = None, mask_of: Optional[torch.Tensor] = None,
+              doc_lists: Optional[Tuple[torch.Tensor, torch.Tensor]] = None, list_of: Optional[torch.Tensor] = None,
+              stats: Optional[dict] = None) -> Tuple[torch.Tensor, torch.Tensor]:
+    """Diverse top-k: score_topk(queries, index, fetch_k, doc_mask=..., mask_of=..., doc_lists=..., list_of=...) gives each
+    query's fetch_k best pages, and mmr_select picks k of them (see there). fetch_k None: the largest allowed value <=
+    max(20, 4 k). stats: score_topk's (path, ...), fetch_k, and with stats={"stages": {}} the CUDA-event times of the
+    stages "candidates" and "select" (ms, after a synchronize and resolve_stages)."""
+    k, fetch = _check_fetch(k, fetch_k, index.emb.shape[1])
+    nq = queries.shape[0] if isinstance(queries, torch.Tensor) else 0
+    lam = _check_lambda(lambda_mult, nq, index.emb.device)
+    with L.on_device(index.emb.device):
+        ev = _Stages(stats)
+        s, i = score_topk(queries, index, fetch, 0, False, stats, doc_mask, mask_of, doc_lists, list_of)
+        ev.mark("candidates")
+        out = _mmr_select(index, s, i, k, lam, id_offset)
+        ev.mark("select")
+    if stats is not None:
+        stats["fetch_k"] = fetch
+    return out
 
 
 def shard_range(n_items: int, rank: int, world: int) -> Tuple[int, int]:
