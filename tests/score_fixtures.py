@@ -286,3 +286,245 @@ def closeness(fx: Fixture):
     ap = approx_scores(q, fx.D[[fx.true_doc]])[0, 0]
     eps = eps_of(row_norms(q)[0], row_norms(fx.D).max(), fx.Q.shape[1])
     return float((ex - ap) / eps), float(eps)
+
+
+# ---------------------------------------------------------------------------------------------------- masked filters
+
+
+def masked_filter_lists(approx, mask, p, tau_from_unmasked=False):
+    """filter_lists with the kernel's masking: ineligible scores are -inf before the threshold test and the insertion,
+    so lists and tau see eligible docs only. tau_from_unmasked: the mutant that publishes tau from the unmasked lists."""
+    nq, nd = approx.shape
+    masked = np.where(mask[None, :], approx, -np.inf).astype(np.float32)
+    cs = np.full((nq, p["lists"], KT), -np.inf, np.float32)
+    ci = np.full((nq, p["lists"], KT), -1, np.int64)
+    tau = np.full(nq, -np.inf, np.float32)
+    for b in range(p["QB"]):
+        rows = slice(256 * b, min(nq, 256 * b + 256))
+        by_wave = {}
+        for r in range(p["R"]):
+            by_wave.setdefault(wave(p, r, b), []).append(r)
+        for w in sorted(by_wave):
+            start = tau[rows].copy()
+            for r in by_wave[w]:
+                lo, hi = range_docs(p, nd, r)
+                tails = []
+                for src in (masked, approx) if tau_from_unmasked else (masked,):
+                    s = np.where(src[rows, lo:hi] > start[:, None], src[rows, lo:hi], -np.inf).astype(np.float32)
+                    o = np.argsort(-s, axis=1, kind="stable")[:, :KT]
+                    v = np.take_along_axis(s, o, 1)
+                    if src is masked:
+                        cs[rows, r, :v.shape[1]] = v
+                        ci[rows, r, :v.shape[1]] = np.where(np.isinf(v), -1, o + lo)
+                    tails.append(v[:, KT - 1] if v.shape[1] == KT else np.full(v.shape[0], -np.inf, np.float32))
+                tau[rows] = np.maximum(tau[rows], tails[-1])
+    cs[:, -1, 0] = tau
+    return cs, ci
+
+
+def filter_lists_per_query(approx, elig, p, leak=False):
+    """filter_lists with a mask per query row (elig [nq, nd]): ineligible scores are -inf before the threshold test and
+    the insertion. leak: the mutant that publishes the tail of the thread's other accumulator row (row ^ 8 of the block)
+    as this row's tau."""
+    nq, nd = approx.shape
+    masked = np.where(elig, approx, -np.inf).astype(np.float32)
+    cs = np.full((nq, p["lists"], KT), -np.inf, np.float32)
+    ci = np.full((nq, p["lists"], KT), -1, np.int64)
+    tau = np.full(nq, -np.inf, np.float32)
+    for b in range(p["QB"]):
+        rows = slice(256 * b, min(nq, 256 * b + 256))
+        n = rows.stop - rows.start
+        by_wave = {}
+        for r in range(p["R"]):
+            by_wave.setdefault(wave(p, r, b), []).append(r)
+        for w in sorted(by_wave):
+            start = tau[rows].copy()
+            for r in by_wave[w]:
+                lo, hi = range_docs(p, nd, r)
+                s = np.where(masked[rows, lo:hi] > start[:, None], masked[rows, lo:hi], -np.inf).astype(np.float32)
+                o = np.argsort(-s, axis=1, kind="stable")[:, :KT]
+                v = np.take_along_axis(s, o, 1)
+                cs[rows, r, :v.shape[1]] = v
+                ci[rows, r, :v.shape[1]] = np.where(np.isinf(v), -1, o + lo)
+                tail = v[:, KT - 1] if v.shape[1] == KT else np.full(n, -np.inf, np.float32)
+                if leak:
+                    tail = tail[np.minimum(np.arange(n) ^ 8, n - 1)]
+                tau[rows] = np.maximum(tau[rows], tail)
+    cs[:, -1, 0] = tau
+    return cs, ci
+
+
+def reference_per_query(exact, elig, k):
+    """Each query's fp32 scan over its own eligible docs: (score desc, id asc), then (-inf, -1)."""
+    s = np.where(elig, exact, -np.inf).astype(np.float32)
+    order = np.lexsort((np.broadcast_to(np.arange(s.shape[1]), s.shape), -s), axis=1)[:, :k]
+    out_s = np.take_along_axis(s, order, 1)
+    out_i = np.where(np.isinf(out_s) & (out_s < 0), -1, order)
+    return out_s, out_i.astype(np.int64)
+
+
+# ---------------------------------------------------------------------------------------------------- documents
+
+
+BUDGET = 4096  # RG_PAGE_BUDGET of csrc/score.cu
+
+
+def grouped_reference(exact, groups, k, mask=None):
+    """The contract: walk the eligible pages in (score desc, page asc) order, keep the first page of each group."""
+    nq, nd = exact.shape
+    cols = np.arange(nd) if mask is None else np.nonzero(mask)[0]
+    out_s = np.full((nq, k), -np.inf, np.float32)
+    out_p = np.full((nq, k), -1, np.int64)
+    out_g = np.full((nq, k), -1, np.int64)
+    for r in range(nq):
+        order = cols[np.lexsort((cols, -exact[r, cols]))]
+        _, first = np.unique(groups[order], return_index=True)
+        pick = order[np.sort(first)][:k]
+        out_s[r, :len(pick)], out_p[r, :len(pick)], out_g[r, :len(pick)] = exact[r, pick], pick, groups[pick]
+    return out_s, out_p, out_g
+
+
+def grouped_filter_lists(approx, groups, p, elig=None):
+    """filter_lists with group-distinct lists: each (query, doc range) list holds the 16 best groups of the range by
+    their best approximate page above the starting threshold, one entry (that page) per group. elig [nq, nd] (optional):
+    only the eligible pages of each query enter its lists."""
+    nq, nd = approx.shape
+    L_ = p["lists"]
+    cs = np.full((nq, L_, KT), -np.inf, np.float32)
+    ci = np.full((nq, L_, KT), -1, np.int64)
+    tau = np.full(nq, -np.inf, np.float32)
+    for b in range(p["QB"]):
+        rows = range(256 * b, min(nq, 256 * b + 256))
+        by_wave = {}
+        for r in range(p["R"]):
+            by_wave.setdefault(wave(p, r, b), []).append(r)
+        for w in sorted(by_wave):
+            start = tau.copy()
+            for r in by_wave[w]:
+                lo, hi = range_docs(p, nd, r)
+                for q in rows:
+                    s = approx[q, lo:hi]
+                    above = s > start[q]
+                    if elig is not None:
+                        above &= elig[q, lo:hi]
+                    cand = np.nonzero(above)[0]
+                    order = cand[np.lexsort((cand, -s[cand]))]
+                    _, first = np.unique(groups[lo + order], return_index=True)
+                    pick = order[np.sort(first)][:KT]
+                    cs[q, r, :len(pick)] = s[pick]
+                    ci[q, r, :len(pick)] = pick + lo
+                    tau[q] = max(tau[q], cs[q, r, KT - 1])
+    cs[:, L_ - 1, 0] = tau
+    return cs, ci
+
+
+def grouped_rescore(cs, ci, exact, groups, qn, dn, k, dim, budget=BUDGET, mut=None, elig=None):
+    """rescore_groups_kernel: (scores, pages, groups, flags). mut: 'entry score' takes a group's score from its kept
+    entries without full rescoring; 'B without unrescored groups' leaves their approximate entries out of the bound.
+    elig [nq, nd] (optional): a rescored group's ineligible pages are not scored (they still count against the budget),
+    and a group without an eligible page is no result."""
+    nq, L_, _ = cs.shape
+    keep = min(max(2 * k, 32), L_ * KT, 256)
+    lane, j = np.arange(L_) % 32, np.arange(L_) // 32
+    sizes = np.bincount(groups)
+    out_s = np.full((nq, k), -np.inf, np.float32)
+    out_p = np.full((nq, k), -1, np.int64)
+    out_g = np.full((nq, k), -1, np.int64)
+    flags = np.zeros(nq, np.int32)
+    for q in range(nq):
+        l, pos = np.nonzero(ci[q] >= 0)
+        sc = cs[q][l, pos]
+        order = np.lexsort((pos, j[l], lane[l], -sc))
+        kept, kept_s = ci[q][l, pos][order[:keep]], sc[order[:keep]]
+        rem = sc[order[keep:]].max() if len(order) > keep else -np.inf
+        bound = max(cs[q, :, KT - 1].max(), rem)
+        done, seen, total, full = [], set(), 0, False
+        for c in range(len(kept)):                    # distinct groups of the kept candidates, in approximate order
+            g = groups[kept[c]]
+            if g in seen:
+                continue
+            seen.add(g)
+            if not full and sizes[g] <= budget - total:
+                done.append(g)
+                total += sizes[g]
+            else:                                     # the first group that does not fit ends the walk
+                full = True
+                if mut != "B without unrescored groups":
+                    bound = max(bound, kept_s[c])
+        res = []
+        for g in done:
+            pages = kept[groups[kept] == g] if mut == "entry score" else np.nonzero(groups == g)[0]
+            if elig is not None:
+                pages = pages[elig[q, pages]]
+                if len(pages) == 0:
+                    continue
+            s = exact[q, pages]
+            b = pages[np.lexsort((pages, -s))][0]
+            res.append((exact[q, b], b, g))
+        res.sort(key=lambda x: (-x[0], x[1]))
+        res = res[:k]
+        for i, (s, b, g) in enumerate(res):
+            out_s[q, i], out_p[q, i], out_g[q, i] = s, b, g
+        kth = out_s[q, k - 1]
+        e = eps_of(qn[q], dn, dim)
+        flags[q] = (bound > -np.inf and not (bound + e < kth)) or not (qn[q] < 65504) or not (dn < 65504)
+    return out_s, out_p, out_g, flags
+
+
+def emulate_grouped(Q, D, groups, k, pairs=PAIRS, page_lists=False, budget=BUDGET, mut=None):
+    nq, dim = Q.shape
+    p = plan(nq, D.shape[0], pairs)
+    exact, approx = exact_scores(Q, D), approx_scores(Q, D)
+    cs, ci = filter_lists(approx, p) if page_lists else grouped_filter_lists(approx, groups, p)
+    s, pg, g, flags = grouped_rescore(cs, ci, exact, groups, row_norms(Q), row_norms(D).max(), k, dim, budget, mut)
+    ref = grouped_reference(exact, groups, k)
+    bad = flags.astype(bool)
+    s[bad], pg[bad], g[bad] = ref[0][bad], ref[1][bad], ref[2][bad]
+    return (s, pg, g), flags, dict(plan=p, cs=cs, ci=ci, ref=ref)
+
+
+def _true_with_decoys(fx):
+    """The true document and the 20 decoys next to it form one group; every other page is its own group."""
+    groups = np.arange(fx.D.shape[0])
+    groups[fx.true_doc:fx.true_doc + 21] = fx.true_doc
+    _, groups = np.unique(groups, return_inverse=True)
+    return groups
+
+
+def _budget_fixture():
+    """One query over 8192 pages at dim 2304 with correlated fp16 rounding (as correlated): the true page T
+    has the highest exact score, but a decoy Y of exactly representable components beats it in approximate score by
+    less than eps. Y is a group of its own; T shares its group with 4097 low pages, more than the page budget. The walk
+    rescores Y's group and stops at T's: only T's approximate entry in the bound keeps the proof from certifying Y."""
+    rs = np.random.RandomState(31)
+    nd, dim = 8192, 2304
+    c = 2.0 ** -6 + 0.49 * 2.0 ** -16
+    t16 = float(to_f16(np.float32(c)))
+    D = t16 * np.where(rs.rand(nd, dim) < 0.5, -1.0, 1.0)
+    T, Y = 7 * SC_BN + 5, 20 * SC_BN + 11
+    D[T] = c
+    D[Y] = _rep(t16, 2, dim, rs)
+    groups = np.arange(nd) + 1
+    groups[T] = 0
+    groups[np.setdiff1d(np.arange(nd), [T, Y])[:BUDGET + 1]] = 0
+    _, groups = np.unique(groups, return_inverse=True)
+    return np.full((1, dim), c, np.float32), D.astype(np.float32), groups, T, Y
+
+
+# ---------------------------------------------------------------------------------------------------- range
+
+
+def fsub_rd(a, b):
+    """a - b in fp32, rounded toward -inf (__fsub_rd)."""
+    a, b = np.float32(a), np.float32(b)
+    exact = float(a) - float(b)                    # exact in float64 for these magnitudes
+    r = np.float32(exact)
+    return np.nextafter(r, np.float32(-np.inf)) if float(r) > exact else r
+
+
+def range_model(approx, exact, t, eps, sub=fsub_rd):
+    """The threshold filter and the rescoring on one query row: candidates are the docs with approximate score >= the
+    drop threshold, results the candidates with exact score >= t."""
+    thr = sub(t, eps)
+    cand = np.nonzero(approx >= thr)[0]
+    return set(cand[exact[cand] >= t].tolist())

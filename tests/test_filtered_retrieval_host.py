@@ -54,37 +54,6 @@ def test_masked_entry_points_refuse_a_bad_mask_before_any_cuda_call(lib):
 # ------------------------------------------------------------------------------------------------------ emulation
 
 
-def masked_filter_lists(approx, mask, p, tau_from_unmasked=False):
-    """SF.filter_lists with the kernel's masking: ineligible scores are -inf before the threshold test and the insertion,
-    so lists and tau see eligible docs only. tau_from_unmasked: the mutant that publishes tau from the unmasked lists."""
-    nq, nd = approx.shape
-    masked = np.where(mask[None, :], approx, -np.inf).astype(np.float32)
-    cs = np.full((nq, p["lists"], SF.KT), -np.inf, np.float32)
-    ci = np.full((nq, p["lists"], SF.KT), -1, np.int64)
-    tau = np.full(nq, -np.inf, np.float32)
-    for b in range(p["QB"]):
-        rows = slice(256 * b, min(nq, 256 * b + 256))
-        by_wave = {}
-        for r in range(p["R"]):
-            by_wave.setdefault(SF.wave(p, r, b), []).append(r)
-        for w in sorted(by_wave):
-            start = tau[rows].copy()
-            for r in by_wave[w]:
-                lo, hi = SF.range_docs(p, nd, r)
-                tails = []
-                for src in (masked, approx) if tau_from_unmasked else (masked,):
-                    s = np.where(src[rows, lo:hi] > start[:, None], src[rows, lo:hi], -np.inf).astype(np.float32)
-                    o = np.argsort(-s, axis=1, kind="stable")[:, :SF.KT]
-                    v = np.take_along_axis(s, o, 1)
-                    if src is masked:
-                        cs[rows, r, :v.shape[1]] = v
-                        ci[rows, r, :v.shape[1]] = np.where(np.isinf(v), -1, o + lo)
-                    tails.append(v[:, SF.KT - 1] if v.shape[1] == SF.KT else np.full(v.shape[0], -np.inf, np.float32))
-                tau[rows] = np.maximum(tau[rows], tails[-1])
-    cs[:, -1, 0] = tau
-    return cs, ci
-
-
 def masked_reference(exact, mask, k):
     """The fp32 scan over the eligible docs: (score desc, id asc), then (-inf, -1)."""
     s = np.where(mask[None, :], exact, -np.inf).astype(np.float32)
@@ -98,7 +67,7 @@ def emulate_masked(Q, D, k, mask, pairs=SF.PAIRS, tau_from_unmasked=False):
     nq, dim = Q.shape
     p = SF.plan(nq, D.shape[0], pairs)
     exact, approx = SF.exact_scores(Q, D), SF.approx_scores(Q, D)
-    cs, ci = masked_filter_lists(approx, mask, p, tau_from_unmasked)
+    cs, ci = SF.masked_filter_lists(approx, mask, p, tau_from_unmasked)
     # the index's max row norm covers every doc, eligible or not: still an upper bound over the eligible ones
     s, i, flags, _, _ = SF.rescore(cs, ci, exact, SF.row_norms(Q), SF.row_norms(D).max(), k, dim, p)
     ref_s, ref_i = masked_reference(exact, mask, k)

@@ -16,9 +16,6 @@ from tests import score_fixtures as SF
 from visrag_b200 import _lib as L
 from visrag_b200.knowledge_base import document_of
 
-BUDGET = 4096  # RG_PAGE_BUDGET of csrc/score.cu
-
-
 @pytest.fixture(scope="module")
 def lib():
     if not os.path.exists(L.LIB_PATH):
@@ -107,110 +104,6 @@ def test_filename_to_document_rule():
 # ------------------------------------------------------------------------------------------------------ emulation
 
 
-def grouped_reference(exact, groups, k, mask=None):
-    """The contract: walk the eligible pages in (score desc, page asc) order, keep the first page of each group."""
-    nq, nd = exact.shape
-    cols = np.arange(nd) if mask is None else np.nonzero(mask)[0]
-    out_s = np.full((nq, k), -np.inf, np.float32)
-    out_p = np.full((nq, k), -1, np.int64)
-    out_g = np.full((nq, k), -1, np.int64)
-    for r in range(nq):
-        order = cols[np.lexsort((cols, -exact[r, cols]))]
-        _, first = np.unique(groups[order], return_index=True)
-        pick = order[np.sort(first)][:k]
-        out_s[r, :len(pick)], out_p[r, :len(pick)], out_g[r, :len(pick)] = exact[r, pick], pick, groups[pick]
-    return out_s, out_p, out_g
-
-
-def grouped_filter_lists(approx, groups, p):
-    """SF.filter_lists with group-distinct lists: each (query, doc range) list holds the 16 best groups of the range by
-    their best approximate page above the starting threshold, one entry (that page) per group."""
-    nq, nd = approx.shape
-    L_ = p["lists"]
-    cs = np.full((nq, L_, SF.KT), -np.inf, np.float32)
-    ci = np.full((nq, L_, SF.KT), -1, np.int64)
-    tau = np.full(nq, -np.inf, np.float32)
-    for b in range(p["QB"]):
-        rows = range(256 * b, min(nq, 256 * b + 256))
-        by_wave = {}
-        for r in range(p["R"]):
-            by_wave.setdefault(SF.wave(p, r, b), []).append(r)
-        for w in sorted(by_wave):
-            start = tau.copy()
-            for r in by_wave[w]:
-                lo, hi = SF.range_docs(p, nd, r)
-                for q in rows:
-                    s = approx[q, lo:hi]
-                    cand = np.nonzero(s > start[q])[0]
-                    order = cand[np.lexsort((cand, -s[cand]))]
-                    _, first = np.unique(groups[lo + order], return_index=True)
-                    pick = order[np.sort(first)][:SF.KT]
-                    cs[q, r, :len(pick)] = s[pick]
-                    ci[q, r, :len(pick)] = pick + lo
-                    tau[q] = max(tau[q], cs[q, r, SF.KT - 1])
-    cs[:, L_ - 1, 0] = tau
-    return cs, ci
-
-
-def grouped_rescore(cs, ci, exact, groups, qn, dn, k, dim, budget=BUDGET, mut=None):
-    """rescore_groups_kernel: (scores, pages, groups, flags). mut: 'entry score' takes a group's score from its kept
-    entries without full rescoring; 'B without unrescored groups' leaves their approximate entries out of the bound."""
-    nq, L_, _ = cs.shape
-    keep = min(max(2 * k, 32), L_ * SF.KT, 256)
-    lane, j = np.arange(L_) % 32, np.arange(L_) // 32
-    sizes = np.bincount(groups)
-    out_s = np.full((nq, k), -np.inf, np.float32)
-    out_p = np.full((nq, k), -1, np.int64)
-    out_g = np.full((nq, k), -1, np.int64)
-    flags = np.zeros(nq, np.int32)
-    for q in range(nq):
-        l, pos = np.nonzero(ci[q] >= 0)
-        sc = cs[q][l, pos]
-        order = np.lexsort((pos, j[l], lane[l], -sc))
-        kept, kept_s = ci[q][l, pos][order[:keep]], sc[order[:keep]]
-        rem = sc[order[keep:]].max() if len(order) > keep else -np.inf
-        bound = max(cs[q, :, SF.KT - 1].max(), rem)
-        done, seen, total, full = [], set(), 0, False
-        for c in range(len(kept)):                    # distinct groups of the kept candidates, in approximate order
-            g = groups[kept[c]]
-            if g in seen:
-                continue
-            seen.add(g)
-            if not full and sizes[g] <= budget - total:
-                done.append(g)
-                total += sizes[g]
-            else:                                     # the first group that does not fit ends the walk
-                full = True
-                if mut != "B without unrescored groups":
-                    bound = max(bound, kept_s[c])
-        res = []
-        for g in done:
-            pages = kept[groups[kept] == g] if mut == "entry score" else np.nonzero(groups == g)[0]
-            s = exact[q, pages]
-            b = pages[np.lexsort((pages, -s))][0]
-            res.append((exact[q, b], b, g))
-        res.sort(key=lambda x: (-x[0], x[1]))
-        res = res[:k]
-        for i, (s, b, g) in enumerate(res):
-            out_s[q, i], out_p[q, i], out_g[q, i] = s, b, g
-        kth = out_s[q, k - 1]
-        e = SF.eps_of(qn[q], dn, dim)
-        flags[q] = (bound > -np.inf and not (bound + e < kth)) or not (qn[q] < 65504) or not (dn < 65504)
-    return out_s, out_p, out_g, flags
-
-
-def emulate_grouped(Q, D, groups, k, pairs=SF.PAIRS, page_lists=False, budget=BUDGET, mut=None):
-    nq, dim = Q.shape
-    p = SF.plan(nq, D.shape[0], pairs)
-    exact, approx = SF.exact_scores(Q, D), SF.approx_scores(Q, D)
-    cs, ci = SF.filter_lists(approx, p) if page_lists else grouped_filter_lists(approx, groups, p)
-    s, pg, g, flags = grouped_rescore(cs, ci, exact, groups, SF.row_norms(Q), SF.row_norms(D).max(), k, dim, budget, mut)
-    ref = grouped_reference(exact, groups, k)
-    bad = flags.astype(bool)
-    s[bad], pg[bad], g[bad] = ref[0][bad], ref[1][bad], ref[2][bad]
-    return (s, pg, g), flags, dict(plan=p, cs=cs, ci=ci, ref=ref)
-
-
 def _same(a, b):
     return all(np.array_equal(x, y) for x, y in zip(a, b))
 
@@ -228,24 +121,16 @@ def test_grouped_emulation_returns_the_grouped_fp32_answer_on_the_proof_fixtures
     p = SF.plan(fx.Q.shape[0], nd)
     exact, approx = SF.exact_scores(Q, fx.D), SF.approx_scores(Q, fx.D)
     for what, groups in {"one page each": np.arange(nd), "contiguous 8": np.arange(nd) // 8,
-                         "true doc with its decoys": _true_with_decoys(fx)}.items():
-        cs, ci = grouped_filter_lists(approx, groups, p)
+                         "true doc with its decoys": SF._true_with_decoys(fx)}.items():
+        cs, ci = SF.grouped_filter_lists(approx, groups, p)
         for r in range(p["lists"] - 1):
             g = groups[ci[0, r][ci[0, r] >= 0]]
             assert len(g) == len(set(g.tolist())), (what, r)
-        out = grouped_rescore(cs, ci, exact, groups, SF.row_norms(Q), SF.row_norms(fx.D).max(), fx.k, Q.shape[1])
-        ref = grouped_reference(exact, groups, fx.k)
+        out = SF.grouped_rescore(cs, ci, exact, groups, SF.row_norms(Q), SF.row_norms(fx.D).max(), fx.k, Q.shape[1])
+        ref = SF.grouped_reference(exact, groups, fx.k)
         if out[3][0]:
             out = ref
         assert _same(out[:3], ref), what
-
-
-def _true_with_decoys(fx):
-    """The true document and the 20 decoys next to it form one group; every other page is its own group."""
-    groups = np.arange(fx.D.shape[0])
-    groups[fx.true_doc:fx.true_doc + 21] = fx.true_doc
-    _, groups = np.unique(groups, return_inverse=True)
-    return groups
 
 
 def test_group_score_from_the_kept_entry_returns_a_wrong_answer():
@@ -254,48 +139,28 @@ def test_group_score_from_the_kept_entry_returns_a_wrong_answer():
     group finds it; taking the group's score from its kept entry does not."""
     fx = {f.name: f for f in _fixtures()}["fp16 rounds down 0.49 ulp"]
     Q, D = fx.Q[:1], fx.D
-    groups = _true_with_decoys(fx)
+    groups = SF._true_with_decoys(fx)
     p = SF.plan(fx.Q.shape[0], D.shape[0])
     exact, approx = SF.exact_scores(Q, D), SF.approx_scores(Q, D)
-    cs, ci = grouped_filter_lists(approx, groups, p)
+    cs, ci = SF.grouped_filter_lists(approx, groups, p)
     assert fx.true_doc not in ci[0]                                   # dropped: <= its group's entry
-    ref = grouped_reference(exact, groups, 1)
+    ref = SF.grouped_reference(exact, groups, 1)
     assert ref[1][0, 0] == fx.true_doc
     args = (cs, ci, exact, groups, SF.row_norms(Q), SF.row_norms(D).max(), 1, Q.shape[1])
-    good = grouped_rescore(*args)
+    good = SF.grouped_rescore(*args)
     assert not good[3][0] and _same(good[:3], ref)
-    bad = grouped_rescore(*args, mut="entry score")
+    bad = SF.grouped_rescore(*args, mut="entry score")
     assert not bad[3][0] and bad[1][0, 0] != fx.true_doc and bad[0][0, 0] < ref[0][0, 0]
 
 
-def _budget_fixture():
-    """One query over 8192 pages at dim 2304 with correlated fp16 rounding (as score_fixtures.correlated): the true page T
-    has the highest exact score, but a decoy Y of exactly representable components beats it in approximate score by
-    less than eps. Y is a group of its own; T shares its group with 4097 low pages, more than the page budget. The walk
-    rescores Y's group and stops at T's: only T's approximate entry in the bound keeps the proof from certifying Y."""
-    rs = np.random.RandomState(31)
-    nd, dim = 8192, 2304
-    c = 2.0 ** -6 + 0.49 * 2.0 ** -16
-    t16 = float(SF.to_f16(np.float32(c)))
-    D = t16 * np.where(rs.rand(nd, dim) < 0.5, -1.0, 1.0)
-    T, Y = 7 * SF.SC_BN + 5, 20 * SF.SC_BN + 11
-    D[T] = c
-    D[Y] = SF._rep(t16, 2, dim, rs)
-    groups = np.arange(nd) + 1
-    groups[T] = 0
-    groups[np.setdiff1d(np.arange(nd), [T, Y])[:BUDGET + 1]] = 0
-    _, groups = np.unique(groups, return_inverse=True)
-    return np.full((1, dim), c, np.float32), D.astype(np.float32), groups, T, Y
-
-
 def test_bound_without_the_unrescored_groups_returns_a_wrong_answer():
-    Q, D, groups, T, Y = _budget_fixture()
+    Q, D, groups, T, Y = SF._budget_fixture()
     exact, approx = SF.exact_scores(Q, D)[0], SF.approx_scores(Q, D)[0]
     assert exact[T] > exact[Y] and approx[Y] > approx[T] and np.argsort(-approx)[:2].tolist() == [Y, T]
-    assert (groups == groups[T]).sum() > BUDGET
-    got, flags, info = emulate_grouped(Q, D, groups, 1)
+    assert (groups == groups[T]).sum() > SF.BUDGET
+    got, flags, info = SF.emulate_grouped(Q, D, groups, 1)
     assert flags.all() and _same(got, info["ref"]) and got[1][0, 0] == T     # T's group is not rescored: flagged
-    bad, flags, info = emulate_grouped(Q, D, groups, 1, mut="B without unrescored groups")
+    bad, flags, info = SF.emulate_grouped(Q, D, groups, 1, mut="B without unrescored groups")
     assert not flags.any() and bad[1][0, 0] == Y and not _same(bad, info["ref"])
 
 
@@ -316,9 +181,9 @@ def test_grouped_emulation_on_a_clustered_multi_wave_fixture():
     p = SF.plan(Q.shape[0], D.shape[0], pairs)
     assert p["items"] > p["pairs"] and p["R"] > 1, p
     for k in (1, 10):
-        got, flags_g, info = emulate_grouped(Q, D, groups, k, pairs)
+        got, flags_g, info = SF.emulate_grouped(Q, D, groups, k, pairs)
         assert _same(got, info["ref"]), k
-        got, flags_p, info = emulate_grouped(Q, D, groups, k, pairs, page_lists=True)
+        got, flags_p, info = SF.emulate_grouped(Q, D, groups, k, pairs, page_lists=True)
         assert _same(got, info["ref"]), k
         if k == 10:   # page lists hold a few documents each: their tails sit above the 10th document
             assert flags_g.sum() == 0 and flags_p.sum() > len(Q) // 2, (flags_g.sum(), flags_p.sum())
@@ -357,6 +222,6 @@ def test_per_rank_group_lists_merge_to_the_global_answer():
         parts = []
         for rank in range(world):
             lo, hi = rank * nd // world, (rank + 1) * nd // world
-            s, p, g = grouped_reference(exact[:, lo:hi], groups[lo:hi], k)
+            s, p, g = SF.grouped_reference(exact[:, lo:hi], groups[lo:hi], k)
             parts.append((s, np.where(p >= 0, p + lo, -1), g))
-        assert _same(merge_groups(parts, k), grouped_reference(exact, groups, k)), k
+        assert _same(merge_groups(parts, k), SF.grouped_reference(exact, groups, k)), k

@@ -15,7 +15,6 @@ import torch
 
 import __graft_entry__ as G
 from tests import score_fixtures as SF
-from tests import test_filtered_retrieval_host as FR
 from visrag_b200 import _lib as L
 from visrag_b200.retriever import CorpusIndex, _check_doc_mask, pack_doc_mask
 
@@ -164,55 +163,14 @@ def test_masks_entry_points_keep_the_other_pointer_checks(lib):
 
 
 # ------------------------------------------------------------------------------------------------ emulation
-def filter_lists_per_query(approx, elig, p, leak=False):
-    """SF.filter_lists with a mask per query row (elig [nq, nd]): ineligible scores are -inf before the threshold test and
-    the insertion. leak: the mutant that publishes the tail of the thread's other accumulator row (row ^ 8 of the block)
-    as this row's tau."""
-    nq, nd = approx.shape
-    masked = np.where(elig, approx, -np.inf).astype(np.float32)
-    cs = np.full((nq, p["lists"], SF.KT), -np.inf, np.float32)
-    ci = np.full((nq, p["lists"], SF.KT), -1, np.int64)
-    tau = np.full(nq, -np.inf, np.float32)
-    for b in range(p["QB"]):
-        rows = slice(256 * b, min(nq, 256 * b + 256))
-        n = rows.stop - rows.start
-        by_wave = {}
-        for r in range(p["R"]):
-            by_wave.setdefault(SF.wave(p, r, b), []).append(r)
-        for w in sorted(by_wave):
-            start = tau[rows].copy()
-            for r in by_wave[w]:
-                lo, hi = SF.range_docs(p, nd, r)
-                s = np.where(masked[rows, lo:hi] > start[:, None], masked[rows, lo:hi], -np.inf).astype(np.float32)
-                o = np.argsort(-s, axis=1, kind="stable")[:, :SF.KT]
-                v = np.take_along_axis(s, o, 1)
-                cs[rows, r, :v.shape[1]] = v
-                ci[rows, r, :v.shape[1]] = np.where(np.isinf(v), -1, o + lo)
-                tail = v[:, SF.KT - 1] if v.shape[1] == SF.KT else np.full(n, -np.inf, np.float32)
-                if leak:
-                    tail = tail[np.minimum(np.arange(n) ^ 8, n - 1)]
-                tau[rows] = np.maximum(tau[rows], tail)
-    cs[:, -1, 0] = tau
-    return cs, ci
-
-
-def reference_per_query(exact, elig, k):
-    """Each query's fp32 scan over its own eligible docs: (score desc, id asc), then (-inf, -1)."""
-    s = np.where(elig, exact, -np.inf).astype(np.float32)
-    order = np.lexsort((np.broadcast_to(np.arange(s.shape[1]), s.shape), -s), axis=1)[:, :k]
-    out_s = np.take_along_axis(s, order, 1)
-    out_i = np.where(np.isinf(out_s) & (out_s < 0), -1, order)
-    return out_s, out_i.astype(np.int64)
-
-
 def emulate_per_query(Q, D, k, masks, of_query, pairs=SF.PAIRS, leak=False):
     nq, dim = Q.shape
     p = SF.plan(nq, D.shape[0], pairs)
     elig = masks[of_query]
     exact, approx = SF.exact_scores(Q, D), SF.approx_scores(Q, D)
-    cs, ci = filter_lists_per_query(approx, elig, p, leak)
+    cs, ci = SF.filter_lists_per_query(approx, elig, p, leak)
     s, i, flags, _, _ = SF.rescore(cs, ci, exact, SF.row_norms(Q), SF.row_norms(D).max(), k, dim, p)
-    ref_s, ref_i = reference_per_query(exact, elig, k)
+    ref_s, ref_i = SF.reference_per_query(exact, elig, k)
     bad = flags.astype(bool)
     s[bad], i[bad] = ref_s[bad], ref_i[bad]          # flagged: each query's own masked fp32 scan answers
     return s, i, flags, dict(plan=p, ci=ci, elig=elig, ref=(ref_s, ref_i))
@@ -242,7 +200,7 @@ def test_per_query_emulation_returns_each_querys_masked_fp32_topk_on_the_proof_f
     assert info["elig"][rows, info["ci"][listed]].all()  # every list holds its own query's eligible docs only
     # a mask set of one with of_query all zeros gives the lists of the single-mask emulation
     _, _, _, one = emulate_per_query(fx.Q, fx.D, fx.k, masks[1:2], np.zeros(nq, np.int64))
-    _, ci = FR.masked_filter_lists(SF.approx_scores(fx.Q, fx.D), masks[1], one["plan"])
+    _, ci = SF.masked_filter_lists(SF.approx_scores(fx.Q, fx.D), masks[1], one["plan"])
     assert np.array_equal(one["ci"], ci)
 
 

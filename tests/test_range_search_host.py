@@ -20,24 +20,8 @@ HEADER = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))
 
 
 # ------------------------------------------------------------------------------------------------ the margin
-def fsub_rd(a, b):
-    """a - b in fp32, rounded toward -inf (__fsub_rd)."""
-    a, b = np.float32(a), np.float32(b)
-    exact = float(a) - float(b)                    # exact in float64 for these magnitudes
-    r = np.float32(exact)
-    return np.nextafter(r, np.float32(-np.inf)) if float(r) > exact else r
-
-
 def fsub_rn(a, b):
     return np.float32(np.float32(a) - np.float32(b))
-
-
-def range_model(approx, exact, t, eps, sub=fsub_rd):
-    """The threshold filter and the rescoring on one query row: candidates are the docs with approximate score >= the
-    drop threshold, results the candidates with exact score >= t."""
-    thr = sub(t, eps)
-    cand = np.nonzero(approx >= thr)[0]
-    return set(cand[exact[cand] >= t].tolist())
 
 
 def _fixture_scores(fx):
@@ -56,7 +40,7 @@ def test_threshold_filter_returns_the_scan_set_on_every_fixture(name):
     ex, ap, eps = _fixture_scores(fx)
     s = ex[fx.true_doc]
     for t in (s, np.nextafter(s, np.float32(-1)), np.nextafter(s, np.float32(2)), np.float32(s - eps), np.float32(0.0)):
-        assert range_model(ap, ex, t, eps) == set(np.nonzero(ex >= t)[0].tolist())
+        assert F.range_model(ap, ex, t, eps) == set(np.nonzero(ex >= t)[0].tolist())
 
 
 def test_the_fixture_puts_the_true_page_most_of_eps_low():
@@ -70,15 +54,15 @@ def test_threshold_without_margin_loses_the_page():
     fx = next(F.fixtures())
     ex, ap, eps = _fixture_scores(fx)
     t = ex[fx.true_doc]
-    assert fx.true_doc not in range_model(ap, ex, t, np.float32(0.0))
+    assert fx.true_doc not in F.range_model(ap, ex, t, np.float32(0.0))
 
 
 def test_eps_halved_loses_the_page():
     fx = next(F.fixtures())
     ex, ap, eps = _fixture_scores(fx)
     t = ex[fx.true_doc]
-    assert fx.true_doc in range_model(ap, ex, t, eps)
-    assert fx.true_doc not in range_model(ap, ex, t, np.float32(eps * 0.5))
+    assert fx.true_doc in F.range_model(ap, ex, t, eps)
+    assert fx.true_doc not in F.range_model(ap, ex, t, np.float32(eps * 0.5))
 
 
 def test_rounding_t_minus_eps_to_nearest_loses_the_page_where_it_rounds_up():
@@ -91,8 +75,8 @@ def test_rounding_t_minus_eps_to_nearest_loses_the_page_where_it_rounds_up():
     ulp = float(np.nextafter(a, np.float32(1))) - float(a)
     short = np.float32(float(t) - float(a) - 0.75 * ulp)  # t - short lies 3/4 ulp above a
     assert float(t) - float(short) > float(a) + 0.5 * ulp
-    assert fx.true_doc in range_model(ap, ex, t, short, fsub_rd)
-    assert fx.true_doc not in range_model(ap, ex, t, short, fsub_rn)
+    assert fx.true_doc in F.range_model(ap, ex, t, short, F.fsub_rd)
+    assert fx.true_doc not in F.range_model(ap, ex, t, short, fsub_rn)
 
 
 # ------------------------------------------------------------------------------------------------ the sort key
