@@ -504,6 +504,28 @@ int vr_mmr_select(const float* emb, int64_t nd, int32_t dim, const float* cand_s
                   int32_t fetch, const float* lambda, int32_t k, int64_t id_offset, float* out_scores, int64_t* out_ids,
                   void* stream);
 
+/* vr_group_pages_topm: the m best eligible pages of given groups (documents), the stage of the capped top-k and the
+ * inner hits (DESIGN §4). For query row r and slot j < kg, with g = groups[r, j] (int64 [nq, kg], e.g. the out_groups of
+ * the _groups calls), the pages of g come from the group CSR of the _groups calls (group_offsets [G+1], group_pages);
+ * those eligible under masks (optional, NULL: every page; a mask set as in the _masks calls, row r using the mask of
+ * query row r) are scored exactly (the bits vr_score_exact gives each pair; NaN never selected) and the first m by
+ * (score desc, page asc) go to out_scores / out_pages [nq, kg, pieces, m] as (score, page + id_offset), then (-inf, -1).
+ * A group longer than `piece` pages is split: piece y of (r, j) covers its pages [y piece, (y + 1) piece), and the
+ * caller keeps pieces * piece >= the largest group (pages beyond are not read). With pieces > 1, vr_topk_rows over rows
+ * nq * kg and cols pieces * m reduces the pieces of each (r, j) to the group's m best. A g < 0 or >= G is empty:
+ * padding only, no page is read (a sharded rank passes global groups it does not hold). One block per (r, j, piece), a
+ * warp per page, the query row in shared memory. No allocation and no synchronisation: the call can be captured in a
+ * CUDA graph.
+ * Refused before any CUDA call, naming the argument: a NULL or misaligned pointer, nq < 1, nd outside [1, 2^31), dim not
+ * a positive multiple of 4, kg < 1, nq * kg >= 2^31, G < 1, m outside [1, 256], piece outside [1, 4096], pieces outside
+ * [1, 65535], dim * 4 + piece * 8 bytes beyond 200 KiB of shared memory, and a bad mask set.
+ * Alignment (bytes) of the vr_group_pages_topm arguments: q_f32 4, d_f32 16, groups 8, group_offsets 4, group_pages 4,
+ * out_scores 4, out_pages 8 */
+int vr_group_pages_topm(const float* q_f32, int32_t nq, const float* d_f32, int64_t nd, int32_t dim, const int64_t* groups,
+                        int32_t kg, const int32_t* group_offsets, const int32_t* group_pages, int32_t G,
+                        const vr_doc_masks* masks, int32_t m, int32_t piece, int32_t pieces, int64_t id_offset,
+                        float* out_scores, int64_t* out_pages, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

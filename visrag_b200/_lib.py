@@ -178,6 +178,8 @@ def _declare(lib: C.CDLL) -> None:
     lib.vr_range_sort.argtypes = [vp, vp, i64, vp, i32, vp, vp, i32, i64, vp, i64, vp, vp, vp]
     lib.vr_mmr_select.restype = i32
     lib.vr_mmr_select.argtypes = [vp, i64, i32, vp, vp, i32, i32, vp, i32, i64, vp, vp, vp]
+    lib.vr_group_pages_topm.restype = i32
+    lib.vr_group_pages_topm.argtypes = [vp, i32, vp, i64, i32, vp, i32, vp, vp, i32, dm, i32, i32, i32, i64, vp, vp, vp]
     lib.vr_pool_norm.restype = i32
     lib.vr_pool_norm.argtypes = [vp, i64, vp, f32, vp, i32, i32, i32, i32, vp, vp]
     lib.vr_prefix_rows.restype = i32

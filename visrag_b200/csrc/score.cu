@@ -1812,6 +1812,75 @@ static int mmr_cluster(int fetch, int dim) {
     return 0;
 }
 
+// ---------------------------------------------------------------------------------------------
+// Per-document top-m: the m best eligible pages of given groups (DESIGN §4, capped top-k and inner hits).
+// ---------------------------------------------------------------------------------------------
+constexpr int GROUP_PAGES_MAX = 256;   // m: pages kept per (row, slot, piece)
+constexpr int GROUP_PIECE_MAX = 4096;  // pages of one group a block scores
+
+// Block (row * kg + slot, piece) scores pages [piece * y, piece * (y + 1)) of group g = groups[row, slot] through the
+// CSR, one warp per page (warp_dot_row: the lane loop of exact_scores_kernel, so every score has the bits
+// vr_score_exact gives that pair), with the query row in shared memory. An ineligible page is never read and counts as
+// NaN, which is never selected. Page keys are distinct, so each entry's rank in (score desc, page asc) order is the
+// number of entries before it: the entries of rank < m go straight to their slot, and the rest of the m slots get
+// (-inf, -1). A group outside [0, G) is empty: padding, and nothing is read.
+__global__ void __launch_bounds__(256)
+group_pages_topm_kernel(const float* __restrict__ Q, const float* __restrict__ D, int dim, const long long* __restrict__ groups,
+                        int kg, const int* __restrict__ offsets, const int* __restrict__ pages, int G, const DocMasks masks,
+                        int m, int piece, long long id_offset, float* __restrict__ out_scores,
+                        long long* __restrict__ out_pages) {
+    extern __shared__ float gsm[];  // [dim] query row, then [piece] scores and [piece] pages
+    float* qs = gsm;
+    float* ps = gsm + dim;
+    int* pp = reinterpret_cast<int*>(ps + piece);
+    const long long rs = blockIdx.x;
+    const long long row = rs / kg;
+    const long long o = (rs * gridDim.y + blockIdx.y) * m;
+    const long long g = groups[rs];
+    int n = 0, lo = 0;
+    if (g >= 0 && g < G) {
+        lo = __ldg(offsets + g) + static_cast<int>(blockIdx.y) * piece;
+        n = min(__ldg(offsets + g + 1) - lo, piece);
+    }
+    if (n <= 0) {  // block-uniform
+        for (int t = threadIdx.x; t < m; t += blockDim.x) {
+            out_scores[o + t] = -INFINITY;
+            out_pages[o + t] = -1;
+        }
+        return;
+    }
+    for (int i = threadIdx.x; i < dim; i += blockDim.x) qs[i] = Q[row * dim + i];
+    __syncthreads();
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, warps = blockDim.x >> 5;
+    const uint32_t* mask = masks.words ? mask_of_row(masks, row) : nullptr;
+    for (int j = warp; j < n; j += warps) {
+        const int p = __ldg(pages + lo + j);
+        const float s = !mask || col_eligible(mask, p) ? warp_dot_row(qs, D + static_cast<long long>(p) * dim, dim, lane) : NAN;
+        if (lane == 0) { ps[j] = s; pp[j] = p; }
+    }
+    __syncthreads();
+    int valid = 0;
+    for (int t0 = 0; t0 < n; t0 += blockDim.x) {  // uniform trip count: __syncthreads_count in every iteration
+        const int t = t0 + threadIdx.x;
+        const bool live = t < n && !isnan(ps[t]);
+        if (live) {
+            const float s = ps[t];
+            const int p = pp[t];
+            int rank = 0;
+            for (int j = 0; j < n && rank < m; ++j) rank += !isnan(ps[j]) && before(ps[j], pp[j], s, p);
+            if (rank < m) {
+                out_scores[o + rank] = s;
+                out_pages[o + rank] = p + id_offset;
+            }
+        }
+        valid += __syncthreads_count(live);
+    }
+    for (int t = min(valid, m) + threadIdx.x; t < m; t += blockDim.x) {
+        out_scores[o + t] = -INFINITY;
+        out_pages[o + t] = -1;
+    }
+}
+
 }  // namespace vr
 
 using namespace vr;
@@ -2423,6 +2492,44 @@ extern "C" int vr_mmr_select(const float* emb, int64_t nd, int32_t dim, const fl
                                      cand_scores, reinterpret_cast<const long long*>(cand_ids), static_cast<int>(fetch),
                                      lambda, static_cast<int>(k), R, static_cast<long long>(id_offset), out_scores,
                                      reinterpret_cast<long long*>(out_ids)));
+    VR_CHECK_CUDA(cudaGetLastError());
+    return 0;
+}
+
+// ---------------------------------------------------------------------------------------------------- per-document top-m
+extern "C" int vr_group_pages_topm(const float* q_f32, int32_t nq, const float* d_f32, int64_t nd, int32_t dim,
+                                   const int64_t* groups, int32_t kg, const int32_t* group_offsets, const int32_t* group_pages,
+                                   int32_t G, const vr_doc_masks* masks, int32_t m, int32_t piece, int32_t pieces,
+                                   int64_t id_offset, float* out_scores, int64_t* out_pages, void* stream) {
+    const char* fn = "vr_group_pages_topm";
+    if (masks) VR_REQUIRE_MASKS(fn, masks, nd);
+    VR_REQUIRE_PTR(fn, "q_f32", q_f32, 4);
+    VR_REQUIRE_PTR(fn, "d_f32", d_f32, 16);  // float4 rows (dim % 4 == 0 keeps every row aligned)
+    VR_REQUIRE_PTR(fn, "groups", groups, 8);
+    VR_REQUIRE_PTR(fn, "group_offsets", group_offsets, 4);
+    VR_REQUIRE_PTR(fn, "group_pages", group_pages, 4);
+    VR_REQUIRE_PTR(fn, "out_scores", out_scores, 4);
+    VR_REQUIRE_PTR(fn, "out_pages", out_pages, 8);
+    VR_REQUIRE(nq > 0, "%s: nq=%d, needs at least 1", fn, nq);
+    VR_REQUIRE(nd > 0 && nd < 2147483647ll, "%s: nd=%lld beyond the int32 doc ids", fn, (long long)nd);
+    VR_REQUIRE(dim > 0 && dim % 4 == 0, "%s: dim=%d, needs a positive multiple of 4", fn, dim);
+    VR_REQUIRE(kg >= 1, "%s: kg=%d, needs at least 1", fn, kg);
+    VR_REQUIRE(static_cast<long long>(nq) * kg < 2147483647ll, "%s: nq=%d x kg=%d rows, needs fewer than 2^31", fn, nq, kg);
+    VR_REQUIRE(G >= 1, "%s: G=%d, needs at least 1", fn, G);
+    VR_REQUIRE(m >= 1 && m <= GROUP_PAGES_MAX, "%s: m=%d, needs 1 <= m <= %d", fn, m, GROUP_PAGES_MAX);
+    VR_REQUIRE(piece >= 1 && piece <= GROUP_PIECE_MAX, "%s: piece=%d, needs 1 <= piece <= %d", fn, piece, GROUP_PIECE_MAX);
+    VR_REQUIRE(pieces >= 1 && pieces <= 65535, "%s: pieces=%d, needs 1 <= pieces <= 65535", fn, pieces);
+    const size_t smem = static_cast<size_t>(dim) * sizeof(float) + static_cast<size_t>(piece) * 8;
+    VR_REQUIRE(smem <= 200 * 1024, "%s: dim=%d with piece=%d too large for shared memory", fn, dim, piece);
+    static unsigned long long attr_set = 0;
+    if (smem > 48 * 1024 && first_use_on_device(&attr_set))
+        VR_CHECK_CUDA(cudaFuncSetAttribute(group_pages_topm_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
+    const int threads = 32 * (piece < 8 ? piece : 8);  // a warp per page: no idle warps for short documents
+    const DocMasks dm = masks ? device_masks(masks) : kNoMasks;
+    group_pages_topm_kernel<<<dim3(static_cast<unsigned>(nq * kg), static_cast<unsigned>(pieces)), threads, smem,
+                              reinterpret_cast<cudaStream_t>(stream)>>>(
+        q_f32, d_f32, dim, reinterpret_cast<const long long*>(groups), kg, group_offsets, group_pages, G, dm, m, piece,
+        static_cast<long long>(id_offset), out_scores, reinterpret_cast<long long*>(out_pages));
     VR_CHECK_CUDA(cudaGetLastError());
     return 0;
 }

@@ -19,7 +19,8 @@ one pass over the index serves them all, and each query's row equals its search 
 Documents: `build_index.py` stores page i of `report.pdf` as `report.pdf_i.png`, so a page's document is its filename up to
 the last `_` when the rest is `<digits>.png` (any other filename is its own document). `search_documents` returns the
 top-k documents by their best page (`retriever.score_topk_groups`), so one long document cannot fill every slot.
-`search_diverse` / `retrieve_diverse` pick pages by maximal marginal relevance (`retriever.mmr_select`), so near-copies
+`search(…, per_document=m)` caps the pages of any one document at m, and `search_document_pages` returns the top-k
+documents each with its m best pages. `search_diverse` / `retrieve_diverse` pick pages by maximal marginal relevance (`retriever.mmr_select`), so near-copies
 of one page, in one document or several, do not fill every slot either.
 """
 from __future__ import annotations
@@ -185,33 +186,64 @@ class KnowledgeBase:
                    for key, r, n in zip(keys, rows_of, per_scope))
         return list_path_wins(rows, nq, self.index.nd, k, documents)
 
+    def _scopes(self, query_reps, within, within_each):
+        """(queries, the distinct scopes (sorted page rows; keys None: every live page, in one scope), list_of [nq] int32
+        (the scope of each query, None: one scope for every query), the live page rows of each distinct scope)."""
+        if within_each is not None:
+            return self._query_and_scopes(query_reps, within, within_each)
+        if within is not None:
+            key = tuple(self._rows(within))
+            return self._queries(query_reps), [key], None, [list(key)]
+        return self._queries(query_reps), None, None, None
+
+    def _scope_args(self, q, keys, rows_of, scope_of, k: int, documents: bool) -> dict:
+        """The scope arguments of a retriever call: every live page through the mask of the live pages (none when no page
+        was removed), else candidate lists of the scopes' pages when they win (list_path_wins), else their masks."""
+        if keys is None:
+            return dict(doc_mask=None if len(self) == self.index.nd else self._live)
+        if self._use_lists(keys, rows_of, scope_of, q.shape[0], k, documents):
+            return dict(doc_lists=self._lists(rows_of), list_of=scope_of)
+        masks = self._scope_masks(keys)
+        return dict(doc_mask=masks if scope_of is not None else masks[0], mask_of=scope_of)
+
+    def _n_documents(self, q, keys, rows_of) -> int:
+        """The documents of the largest scope."""
+        if keys is None:
+            searched = self._doc_groups if len(self) == self.index.nd else self._doc_groups[self._live]
+            return int(torch.unique(searched).numel())
+        if len(keys) == 1:
+            idx = torch.tensor(rows_of[0], dtype=torch.int64, device=q.device)
+            return int(torch.unique(self._doc_groups[idx]).numel())   # documents searched, counted on the device
+        groups = self._doc_groups.tolist()
+        return max(len({groups[r] for r in rows}) for rows in rows_of)
+
     def search(self, query_reps, topk: int, within: Optional[Iterable[str]] = None,
-               within_each: Optional[Sequence[Optional[Iterable[str]]]] = None) -> Tuple[torch.Tensor, torch.Tensor]:
+               within_each: Optional[Sequence[Optional[Iterable[str]]]] = None,
+               per_document: Optional[int] = None) -> Tuple[torch.Tensor, torch.Tensor]:
         """query_reps [nq, d] (tensor or ndarray, fp32) -> (scores [nq,k] f32, page indices [nq,k] i64) on the device.
         within: page filenames to search (default: every live page); k = min(topk, pages searched).
         within_each: one scope per query instead (a list of page filenames, or None for every live page), all searched in
         one pass; k = min(topk, pages of the largest scope), and a query whose scope is shorter ends in (-inf, -1).
         Small scopes are scored from candidate lists of their pages (list_path_wins), the others through masks of the
-        whole index: the results are the same bits either way."""
-        if within_each is not None:
-            q, keys, scope_of, rows_of = self._query_and_scopes(query_reps, within, within_each)
-            k = min(topk, max(len(rows) for rows in rows_of)) if rows_of else 0
-        elif within is not None:
-            q, keys, scope_of = self._queries(query_reps), [tuple(self._rows(within))], None
-            rows_of = [list(keys[0])]
-            k = min(topk, len(rows_of[0]))
+        whole index: the results are the same bits either way.
+        per_document: at most this many pages of any one document (retriever.score_topk_capped): the pages are walked
+        best first and a page is skipped once its document has per_document pages. When the caps leave fewer than k
+        pages, the row ends in (-inf, -1)."""
+        if per_document is not None:
+            retriever._check_per_group(per_document, "per_document")
+        q, keys, scope_of, rows_of = self._scopes(query_reps, within, within_each)
+        if keys is None:
+            k = min(topk, len(self))
         else:
-            q, masks, n = self._query_and_mask(query_reps, None)
-            keys, k = None, min(topk, n)
+            k = min(topk, max(len(rows) for rows in rows_of)) if rows_of else 0
         if k == 0:
             return (torch.empty((q.shape[0], 0), dtype=torch.float32, device=q.device),
                     torch.empty((q.shape[0], 0), dtype=torch.int64, device=q.device))
-        if keys is None:
-            return retriever.score_topk(q, self.index, k, doc_mask=masks)  # enters the index's device itself
-        if self._use_lists(keys, rows_of, scope_of, q.shape[0], k, documents=False):
-            return retriever.score_topk(q, self.index, k, doc_lists=self._lists(rows_of), list_of=scope_of)
-        masks = self._scope_masks(keys)
-        return retriever.score_topk(q, self.index, k, doc_mask=masks if scope_of is not None else masks[0], mask_of=scope_of)
+        if per_document is None:
+            return retriever.score_topk(q, self.index, k, **self._scope_args(q, keys, rows_of, scope_of, k, False))
+        s, p, _ = retriever.score_topk_capped(q, self.index, k, self._doc_groups, per_document,
+                                              **self._scope_args(q, keys, rows_of, scope_of, k, True))
+        return s, p
 
     def search_documents(self, query_reps, topk: int, within: Optional[Iterable[str]] = None,
                          within_each: Optional[Sequence[Optional[Iterable[str]]]] = None
@@ -221,32 +253,35 @@ class KnowledgeBase:
         documents searched). Ties rank the document with the lower best page index first.
         within_each: one scope per query, as in search; k = min(topk, documents of the largest scope), a shorter row ends
         in (-inf, -1), and each query's names list holds only the documents it found. Scopes are routed as in search."""
-        if within_each is not None:
-            q, keys, scope_of, rows_of = self._query_and_scopes(query_reps, within, within_each)
-            groups = self._doc_groups.tolist()
-            k = min(topk, max(len({groups[r] for r in rows}) for rows in rows_of)) if rows_of else 0
-        elif within is not None:
-            q, keys, scope_of = self._queries(query_reps), [tuple(self._rows(within))], None
-            rows_of = [list(keys[0])]
-            idx = torch.tensor(rows_of[0], dtype=torch.int64, device=q.device)
-            k = min(topk, int(torch.unique(self._doc_groups[idx]).numel()))   # documents searched, counted on the device
-        else:
-            q, masks, _ = self._query_and_mask(query_reps, None)
-            searched = self._doc_groups if masks is None else self._doc_groups[masks]
-            keys, k = None, min(topk, int(torch.unique(searched).numel()))
+        q, keys, scope_of, rows_of = self._scopes(query_reps, within, within_each)
+        k = min(topk, self._n_documents(q, keys, rows_of)) if rows_of != [] else 0
         if k == 0:
             return (torch.empty((q.shape[0], 0), dtype=torch.float32, device=q.device),
                     torch.empty((q.shape[0], 0), dtype=torch.int64, device=q.device), [[] for _ in range(q.shape[0])])
-        if keys is None:
-            s, p, g = retriever.score_topk_groups(q, self.index, k, self._doc_groups, doc_mask=masks)
-        elif self._use_lists(keys, rows_of, scope_of, q.shape[0], k, documents=True):
-            s, p, g = retriever.score_topk_groups(q, self.index, k, self._doc_groups, doc_lists=self._lists(rows_of),
-                                                  list_of=scope_of)
-        else:
-            masks = self._scope_masks(keys)
-            s, p, g = retriever.score_topk_groups(q, self.index, k, self._doc_groups,
-                                                  doc_mask=masks if scope_of is not None else masks[0], mask_of=scope_of)
-        return s, p, [[self.documents[j] for j in row if j >= 0] for row in g.tolist()]
+        s, p, g = retriever.score_topk_groups(q, self.index, k, self._doc_groups,
+                                              **self._scope_args(q, keys, rows_of, scope_of, k, True))
+        return s, p, self._names(g)
+
+    def _names(self, groups: torch.Tensor) -> List[List[str]]:
+        return [[self.documents[j] for j in row if j >= 0] for row in groups.tolist()]
+
+    def search_document_pages(self, query_reps, topk: int, pages: int, within: Optional[Iterable[str]] = None,
+                              within_each: Optional[Sequence[Optional[Iterable[str]]]] = None
+                              ) -> Tuple[torch.Tensor, torch.Tensor, torch.Tensor, List[List[str]]]:
+        """The top-k documents of search_documents, each with its `pages` best pages (inner hits,
+        retriever.score_topk_groups_pages): (document scores [nq,k] f32, page scores [nq,k,pages] f32, page indices
+        [nq,k,pages] i64 on the device, document names [nq][k]). A document's pages are in (score desc, page asc) order,
+        column 0 its best page; fewer pages end in (-inf, -1). within / within_each and k as in search_documents."""
+        pages = retriever._check_pages(pages)
+        q, keys, scope_of, rows_of = self._scopes(query_reps, within, within_each)
+        k = min(topk, self._n_documents(q, keys, rows_of)) if rows_of != [] else 0
+        if k == 0:
+            return (torch.empty((q.shape[0], 0), dtype=torch.float32, device=q.device),
+                    torch.empty((q.shape[0], 0, pages), dtype=torch.float32, device=q.device),
+                    torch.empty((q.shape[0], 0, pages), dtype=torch.int64, device=q.device), [[] for _ in range(q.shape[0])])
+        s, _, g, ps, pp = retriever.score_topk_groups_pages(q, self.index, k, self._doc_groups, pages,
+                                                            **self._scope_args(q, keys, rows_of, scope_of, k, True))
+        return s, ps, pp, self._names(g)
 
     def search_above(self, query_reps, min_score, within: Optional[Iterable[str]] = None,
                      within_each: Optional[Sequence[Optional[Iterable[str]]]] = None
@@ -323,6 +358,14 @@ class KnowledgeBase:
         out = model(query={"text": [DEMO_QUERY_PREFIX + query], "image": [None]}, tokenizer=tokenizer)
         return self.retrieve_diverse(out.q_reps, topk, lambda_mult, fetch_k, within)
 
+    def retrieve_document_pages(self, query_rep, topk: int, pages: int,
+                                within: Optional[Iterable[str]] = None) -> List[Tuple[str, List[str]]]:
+        """[(document name, paths of its best page images, best first)] of the top-k documents, best first: for a list
+        of documents with page thumbnails."""
+        _, _, idx, names = self.search_document_pages(query_rep, topk, pages, within)
+        return [(n, [os.path.join(self.path, self.filenames[i]) for i in row if i >= 0])
+                for n, row in zip(names[0], idx[0].tolist())]
+
     def retrieve_documents(self, query_rep, topk: int, within: Optional[Iterable[str]] = None) -> List[Tuple[str, str]]:
         """[(document name, path of its best page image)] of the top-k documents, best first."""
         _, pages, names = self.search_documents(query_rep, topk, within)
@@ -334,15 +377,18 @@ class KnowledgeBase:
         out = model(query={"text": [DEMO_QUERY_PREFIX + query], "image": [None]}, tokenizer=tokenizer)
         return self.retrieve_documents(out.q_reps, topk, within)
 
-    def retrieve(self, query_rep, topk: int, within: Optional[Iterable[str]] = None) -> List[str]:
-        """`answer.py: retrieve` after the query is encoded: paths of the top-k page images, best first."""
-        _, ids = self.search(query_rep, topk, within)
-        return [os.path.join(self.path, self.filenames[i]) for i in ids[0].tolist()]
+    def retrieve(self, query_rep, topk: int, within: Optional[Iterable[str]] = None,
+                 per_document: Optional[int] = None) -> List[str]:
+        """`answer.py: retrieve` after the query is encoded: paths of the top-k page images, best first. per_document: at
+        most this many pages of any one document (see search); the list is shorter when the caps leave fewer pages."""
+        _, ids = self.search(query_rep, topk, within, per_document=per_document)
+        return [os.path.join(self.path, self.filenames[i]) for i in ids[0].tolist() if i >= 0]
 
-    def retrieve_text(self, model, tokenizer, query: str, topk: int, within: Optional[Iterable[str]] = None) -> List[str]:
+    def retrieve_text(self, model, tokenizer, query: str, topk: int, within: Optional[Iterable[str]] = None,
+                      per_document: Optional[int] = None) -> List[str]:
         """Full `retrieve(knowledge_base_path, query, topk)`: instruction + query -> embedding (B2 wrapper) -> top-k."""
         out = model(query={"text": [DEMO_QUERY_PREFIX + query], "image": [None]}, tokenizer=tokenizer)
-        return self.retrieve(out.q_reps, topk, within)
+        return self.retrieve(out.q_reps, topk, within, per_document)
 
     def remove(self, filenames: Iterable[str]) -> None:
         """Mark pages dead: no search returns them again. The other pages keep their indices, and the index's max row norm

@@ -20,6 +20,9 @@ no others; the result equals the masked call with a mask of exactly the listed p
 Document-level retrieval (`score_topk_groups`, `sharded_topk_groups`): `doc_groups` (int [nd]) gives every doc (page) its
 group (document); the top-k groups by their best page's exact fp32 score, ranked by (score desc, best page asc).
 
+Per-document caps (`score_topk_capped`, `score_topk_groups_pages`, `group_pages_topm` and the sharded forms): k pages with
+at most m from any document, or the top-k documents each with its m best pages, with the bits of the fp32 scan (DESIGN §4).
+
 Diverse retrieval (`score_mmr`, `mmr_select`): maximal marginal relevance over each query's top fetch_k pages, picked
 on the GPU (vr_mmr_select) with the bits fixed by the definition in DESIGN §4.
 """
@@ -494,6 +497,7 @@ class _GroupTable:
     offsets: torch.Tensor   # [G+1] int32: group g owns pages[offsets[g]:offsets[g+1]]
     pages: torch.Tensor     # [nd] int32: pages by group, ascending within a group
     G: int
+    max_pages: int          # pages of the largest group (the pieces of vr_group_pages_topm)
 
 
 MERGE_GROUPS_MAX = 512  # entries per row vr_merge_group_topk takes: world * k of sharded_topk_groups
@@ -523,7 +527,8 @@ def _group_table(doc_groups: torch.Tensor, index: CorpusIndex) -> _GroupTable:
     counts = torch.bincount(doc_groups, minlength=G)
     offsets = torch.zeros(G + 1, dtype=torch.int64, device=doc_groups.device)
     offsets[1:] = torch.cumsum(counts, 0)
-    table = _GroupTable(doc_groups.to(torch.int32, copy=True).contiguous(), offsets.to(torch.int32), order.to(torch.int32), G)
+    table = _GroupTable(doc_groups.to(torch.int32, copy=True).contiguous(), offsets.to(torch.int32), order.to(torch.int32), G,
+                        int(counts.max()))
     key = id(doc_groups)
     _GROUP_TABLES[key] = (weakref.ref(doc_groups, lambda _r, key=key: _GROUP_TABLES.pop(key, None)), doc_groups._version, table)
     return table
@@ -614,6 +619,155 @@ def merge_topk(scores: torch.Tensor, ids: torch.Tensor, k: int) -> Tuple[torch.T
         L.check(L.lib().vr_topk_rows(scores.data_ptr(), ids.data_ptr(), nq, m, k, 0, out_s.data_ptr(), out_i.data_ptr(),
                                      L.stream_ptr()))
     return out_s, out_i
+
+
+# ------------------------------------------------------------------------------------------------------
+# Per-document caps: capped page top-k and inner hits (DESIGN §4)
+# ------------------------------------------------------------------------------------------------------
+GROUP_PAGES_MAX = 256   # m (pages per document) vr_group_pages_topm keeps
+GROUP_PIECE = 256       # pages of one document a block of vr_group_pages_topm scores
+GROUP_STAGE_BUDGET = 1 << 26  # [rows, kg, pieces, m] entries of the stage per pass: query rows go in chunks
+
+
+def _check_per_group(v, name: str) -> int:
+    v = _check_count(v, name)
+    if v < 1:
+        raise ValueError(f"{name}={v} must be at least 1")
+    return v
+
+
+def _check_pages(m) -> int:
+    m = _check_per_group(m, "pages")
+    if m > GROUP_PAGES_MAX:
+        raise ValueError(f"pages={m} must lie in [1, {GROUP_PAGES_MAX}]")
+    return m
+
+
+def _group_pages_topm(q: torch.Tensor, index: CorpusIndex, groups: torch.Tensor, gt: _GroupTable, m: int, id_offset: int,
+                      masks: Optional[_MaskSet]) -> Tuple[torch.Tensor, torch.Tensor]:
+    """vr_group_pages_topm over every (row, slot) of groups [nq, kg] (int64), with the pieces of long documents reduced
+    to each document's m best by vr_topk_rows: (scores [nq, kg, m], pages [nq, kg, m] = page + id_offset)."""
+    nq, kg = groups.shape
+    dev = q.device
+    out_s = torch.empty((nq, kg, m), dtype=torch.float32, device=dev)
+    out_p = torch.empty((nq, kg, m), dtype=torch.int64, device=dev)
+    if nq == 0:
+        return out_s, out_p
+    if q.shape[1] != index.emb.shape[1]:
+        raise ValueError("query / corpus dim mismatch")
+    piece = max(1, min(GROUP_PIECE, gt.max_pages))
+    pieces = max(1, -(-gt.max_pages // piece))
+    lib, sp = L.lib(), L.stream_ptr()
+    rows_per = max(1, min(nq, GROUP_STAGE_BUDGET // (kg * pieces * m)))
+    ws_s = torch.empty((rows_per, kg, pieces, m), dtype=torch.float32, device=dev) if pieces > 1 else None
+    ws_p = torch.empty((rows_per, kg, pieces, m), dtype=torch.int64, device=dev) if pieces > 1 else None
+    for r0 in range(0, nq, rows_per):
+        n = min(rows_per, nq - r0)
+        s, p = (out_s[r0:], out_p[r0:]) if pieces == 1 else (ws_s, ws_p)
+        L.check(lib.vr_group_pages_topm(q[r0:].data_ptr(), n, index.emb.data_ptr(), index.nd, q.shape[1],
+                                        groups[r0:].data_ptr(), kg, gt.offsets.data_ptr(), gt.pages.data_ptr(), gt.G,
+                                        None if masks is None else masks.arg(r0), m, piece, pieces, id_offset, s.data_ptr(),
+                                        p.data_ptr(), sp))
+        if pieces > 1:
+            L.check(lib.vr_topk_rows(ws_s.data_ptr(), ws_p.data_ptr(), n * kg, pieces * m, m, 0, out_s[r0:].data_ptr(),
+                                     out_p[r0:].data_ptr(), sp))
+    return out_s, out_p
+
+
+def group_pages_topm(queries: torch.Tensor, index: CorpusIndex, groups: torch.Tensor, doc_groups: torch.Tensor, m: int,
+                     id_offset: int = 0, doc_mask: Optional[torch.Tensor] = None, mask_of: Optional[torch.Tensor] = None
+                     ) -> Tuple[torch.Tensor, torch.Tensor]:
+    """The m best eligible pages of given documents: groups int [nq, kg] on the index's device (e.g. the groups of
+    score_topk_groups; a value outside [0, G) is an empty document) -> (scores [nq, kg, m] f32, pages [nq, kg, m] i64 =
+    local page + id_offset), each (row, slot) the document's pages in (exact fp32 score desc, page asc) order, ending in
+    (-inf, -1). Scores have the bits of the fp32 scan; NaN is never selected. doc_mask / mask_of as in score_topk."""
+    m = _check_pages(m)
+    q, masks = _queries_and_mask(queries, index, doc_mask, mask_of)
+    if not isinstance(groups, torch.Tensor) or groups.dtype not in (torch.int32, torch.int64) or groups.dim() != 2:
+        raise ValueError("groups must be an int32 or int64 torch tensor [nq, kg]")
+    if groups.shape[0] != q.shape[0] or groups.shape[1] < 1:
+        raise ValueError(f"groups must have shape [{q.shape[0]}, kg >= 1] (one row per query), got {list(groups.shape)}")
+    if groups.device != index.emb.device:
+        raise ValueError(f"groups live on {groups.device}, the index on {index.emb.device}")
+    with L.on_device(q.device):
+        gt = _group_table(doc_groups, index)
+        return _group_pages_topm(q, index, groups.to(torch.int64).contiguous(), gt, m, id_offset, masks)
+
+
+def _stage_masks(q: torch.Tensor, index: CorpusIndex, doc_mask, mask_of, doc_lists, list_of) -> Optional[_MaskSet]:
+    """The mask set of the stage for a search's scope: the masks themselves, or the masks equivalent to doc_lists."""
+    if doc_lists is not None or list_of is not None:
+        _, ls = _queries_and_lists(q, index, doc_mask, mask_of, doc_lists, list_of)
+        doc_mask, mask_of = ls.masks(index.nd)
+    return _queries_and_mask(q, index, doc_mask, mask_of)[1]
+
+
+def score_topk_groups_pages(queries: torch.Tensor, index: CorpusIndex, k: int, doc_groups: torch.Tensor, pages: int,
+                            id_offset: int = 0, force_exact: bool = False, stats: Optional[dict] = None,
+                            doc_mask: Optional[torch.Tensor] = None, mask_of: Optional[torch.Tensor] = None,
+                            doc_lists: Optional[Tuple[torch.Tensor, torch.Tensor]] = None,
+                            list_of: Optional[torch.Tensor] = None):
+    """Inner hits: the top-k documents of score_topk_groups (same arguments, same result), each with its `pages` best
+    eligible pages. Returns (scores [nq,k] f32, best pages [nq,k] i64, groups [nq,k] i64, page scores [nq,k,pages] f32,
+    pages [nq,k,pages] i64 = local page + id_offset); column 0 is the best page and its score, a document with fewer
+    pages and a missing document end in (-inf, -1). stats: score_topk_groups', and with stats={"stages": {}} the
+    CUDA-event times of "documents" and "pages"."""
+    m = _check_pages(pages)
+    q = _check_f32(queries, "queries")
+    ev = _Stages(stats)
+    s, p, g = score_topk_groups(q, index, k, doc_groups, id_offset, force_exact, stats, doc_mask, mask_of, doc_lists, list_of)
+    ev.mark("documents")
+    with L.on_device(q.device):
+        masks = _stage_masks(q, index, doc_mask, mask_of, doc_lists, list_of)
+        ps, pp = _group_pages_topm(q, index, g, _group_table(doc_groups, index), m, id_offset, masks)
+    ev.mark("pages")
+    return s, p, g, ps, pp
+
+
+def _capped_merge(scores: torch.Tensor, pages: torch.Tensor, groups: torch.Tensor, k: int):
+    """[nq, n] distinct candidate pages (score, page, group; page < 0 = empty) -> the top-k pages by (score desc,
+    page asc) with their groups: (scores, pages, groups) [nq, k]."""
+    nq = scores.shape[0]
+    if nq == 0 or scores.shape[1] == 0:
+        e = torch.full((nq, k), -1, dtype=torch.int64, device=scores.device)
+        return torch.full((nq, k), float("-inf"), device=scores.device), e, e.clone()
+    s, p = merge_topk(scores, pages, k)
+    key, order = torch.sort(pages.to(torch.int64), dim=1)  # each page appears once: find each pick's candidate
+    at = torch.searchsorted(key, p).clamp(max=key.shape[1] - 1)
+    g = torch.gather(groups.to(torch.int64), 1, torch.gather(order, 1, at))
+    return s, p, torch.where(p >= 0, g, -1)
+
+
+def score_topk_capped(queries: torch.Tensor, index: CorpusIndex, k: int, doc_groups: torch.Tensor, per_group: int,
+                      id_offset: int = 0, force_exact: bool = False, stats: Optional[dict] = None,
+                      doc_mask: Optional[torch.Tensor] = None, mask_of: Optional[torch.Tensor] = None,
+                      doc_lists: Optional[Tuple[torch.Tensor, torch.Tensor]] = None, list_of: Optional[torch.Tensor] = None
+                      ) -> Tuple[torch.Tensor, torch.Tensor, torch.Tensor]:
+    """Capped page top-k: walk the eligible pages in (exact fp32 score desc, page asc) order and pick each page whose
+    document has fewer than per_group picks, until k picks. Returns (scores [nq,k] f32, pages [nq,k] i64 = local page +
+    id_offset, groups [nq,k] i64) in pick order, ending in (-inf, -1, -1) when the caps leave fewer than k pages. Scope
+    arguments as in score_topk_groups. per_group = 1 gives score_topk_groups' result; per_group >= k can not bind and is
+    answered by score_topk. Otherwise (DESIGN §4): the top-k documents, the per_group best pages of each
+    (vr_group_pages_topm), and the top-k of those k * per_group pages. stats: the searches', and with
+    stats={"stages": {}} the CUDA-event times of "documents", "pages" and "merge"."""
+    m = _check_per_group(per_group, "per_group")
+    k = _check_count(k, "k")
+    if m >= k:
+        q = _check_f32(queries, "queries")
+        s, p = score_topk(q, index, k, id_offset, force_exact, stats, doc_mask, mask_of, doc_lists, list_of)
+        with L.on_device(q.device):
+            gt = _group_table(doc_groups, index)
+            return s, p, torch.where(p >= 0, gt.groups[(p - id_offset).clamp(min=0)].long(), -1)
+    if m > GROUP_PAGES_MAX:
+        raise ValueError(f"per_group={m} must be >= k or lie in [1, {GROUP_PAGES_MAX}]")
+    _, _, g, ps, pp = score_topk_groups_pages(queries, index, k, doc_groups, m, id_offset, force_exact, stats, doc_mask,
+                                              mask_of, doc_lists, list_of)
+    ev = _Stages(stats)
+    with L.on_device(ps.device):
+        nq = ps.shape[0]
+        out = _capped_merge(ps.view(nq, k * m), pp.view(nq, k * m), g[:, :, None].expand(nq, k, m).reshape(nq, k * m), k)
+    ev.mark("merge")
+    return out
 
 
 # ------------------------------------------------------------------------------------------------------
@@ -1022,6 +1176,79 @@ def sharded_topk_groups(queries: torch.Tensor, index: CorpusIndex, k: int, doc_g
     gathered = _all_gather_rows(torch.stack([s.contiguous().view(torch.int32).to(torch.int64), p, g], dim=-1), group)
     ev.mark("all_gather_partials")
     out = merge_topk_groups(gathered[..., 0].to(torch.int32).view(torch.float32), gathered[..., 1], gathered[..., 2], k)
+    ev.mark("merge")
+    return out
+
+
+def _score_bits(s: torch.Tensor) -> torch.Tensor:
+    return s.contiguous().view(torch.int32).to(torch.int64)
+
+
+def _bits_score(b: torch.Tensor) -> torch.Tensor:
+    return b.to(torch.int32).view(torch.float32)
+
+
+def sharded_topk_groups_pages(queries: torch.Tensor, index: CorpusIndex, k: int, doc_groups: torch.Tensor, pages: int,
+                              id_offset: int, group=None, stats: Optional[dict] = None, doc_mask: Optional[torch.Tensor] = None,
+                              mask_of: Optional[torch.Tensor] = None,
+                              doc_lists: Optional[Tuple[torch.Tensor, torch.Tensor]] = None,
+                              list_of: Optional[torch.Tensor] = None):
+    """Inner hits over a corpus sharded by page (score_topk_groups_pages of the whole corpus): sharded_topk_groups gives
+    the global top-k documents on every rank; each rank takes the `pages` best of its own pages of each (global group
+    ids, as in sharded_topk_groups: a document this rank does not hold is empty); ONE all-gather of [nq, k, pages]
+    (score bits, page); and per (row, slot) the top-`pages` of the world * pages entries. That last step is exact because
+    a document's global top-m pages lie in the union of its ranks' local top-m lists (a page with m better pages on its
+    own rank has m better pages globally), and it may not be skipped: the capped top-k over the gathered lists directly
+    could take more than m pages of one document. Returns as score_topk_groups_pages."""
+    m = _check_pages(pages)
+    s, p, g = sharded_topk_groups(queries, index, k, doc_groups, id_offset, group, stats, doc_mask, mask_of, doc_lists,
+                                  list_of)
+    q = _check_f32(queries, "queries")
+    ev = _Stages(stats)
+    with L.on_device(q.device):
+        masks = _stage_masks(q, index, doc_mask, mask_of, doc_lists, list_of)
+        ps, pp = _group_pages_topm(q, index, g, _group_table(doc_groups, index), m, id_offset, masks)
+        ev.mark("pages")
+        world = _world(group)
+        if world == 1:
+            return s, p, g, ps, pp
+        nq = q.shape[0]
+        got = _all_gather_rows(torch.stack([_score_bits(ps), pp], dim=-1).view(nq, k * m, 2), group)  # [nq, world*k*m, 2]
+        ev.mark("all_gather_pages")
+        got = got.view(nq, world, k, m, 2).permute(0, 2, 1, 3, 4).reshape(nq * k, world * m, 2)
+        ms, mp = merge_topk(_bits_score(got[..., 0]), got[..., 1], m)
+        ev.mark("merge_pages")
+    return s, p, g, ms.view(nq, k, m), mp.view(nq, k, m)
+
+
+def sharded_topk_capped(queries: torch.Tensor, index: CorpusIndex, k: int, doc_groups: torch.Tensor, per_group: int,
+                        id_offset: int, group=None, stats: Optional[dict] = None, doc_mask: Optional[torch.Tensor] = None,
+                        mask_of: Optional[torch.Tensor] = None, doc_lists: Optional[Tuple[torch.Tensor, torch.Tensor]] = None,
+                        list_of: Optional[torch.Tensor] = None):
+    """score_topk_capped over a corpus sharded by page: the top-k of the k * per_group pages of sharded_topk_groups_pages
+    (per_group >= k: sharded_topk's pages, with their groups gathered alongside)."""
+    m = _check_per_group(per_group, "per_group")
+    k = _check_count(k, "k")
+    if m < k:
+        if m > GROUP_PAGES_MAX:
+            raise ValueError(f"per_group={m} must be >= k or lie in [1, {GROUP_PAGES_MAX}]")
+        _, _, g, ps, pp = sharded_topk_groups_pages(queries, index, k, doc_groups, m, id_offset, group, stats, doc_mask,
+                                                    mask_of, doc_lists, list_of)
+        nq = ps.shape[0]
+        ev = _Stages(stats)
+        with L.on_device(ps.device):
+            out = _capped_merge(ps.view(nq, k * m), pp.view(nq, k * m), g[:, :, None].expand(nq, k, m).reshape(nq, k * m), k)
+        ev.mark("merge")
+        return out
+    s, p, g = score_topk_capped(queries, index, k, doc_groups, m, id_offset, False, stats, doc_mask, mask_of, doc_lists,
+                                list_of)
+    if _world(group) == 1:
+        return s, p, g
+    ev = _Stages(stats)
+    got = _all_gather_rows(torch.stack([_score_bits(s), p, g], dim=-1), group)
+    ev.mark("all_gather_partials")
+    with L.on_device(s.device):
+        out = _capped_merge(_bits_score(got[..., 0]), got[..., 1], got[..., 2], k)
     ev.mark("merge")
     return out
 
