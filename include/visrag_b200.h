@@ -481,6 +481,28 @@ int vr_range_sort(const float* scores, const int32_t* ids, int64_t pitch, const 
                   const int32_t* row_of, const int64_t* out_offsets, int32_t max_count, int64_t id_offset, void* ws,
                   int64_t ws_bytes, float* out_scores, int64_t* out_ids, void* stream);
 
+/* vr_select_rows: the top-k of each row by a radix select, in passes over the row whose number does not depend on k
+ * (DESIGN §4, "Deep top-k"). The contract of vr_topk_rows / vr_topk_rows_masks / vr_topk_rows_chunked(_masks), with the
+ * same result bit for bit: out_scores / out_ids [rows, k] in (score desc, id asc) order (+0 = -0, the id decides; a
+ * repeated (score, id) pair emitted once; NaN never selected), ids + id_offset, then (-inf, -1). ids (optional, int64
+ * [rows, cols]; a negative id is skipped) and masks (the _masks forms: row r filtered by the mask of query r) are
+ * exclusive. The chunked forms spread each row over `chunks` blocks, each writing its chunk's top-k into ws_scores /
+ * ws_ids [rows, chunks, k], then select from those lists. Cost: about five reads of each row (four 8-bit digit passes,
+ * fewer when a bin settles the boundary, plus the gather; ties split at the boundary add one pass per id byte), and a
+ * bitonic sort of the k winners in shared memory (k * 16 bytes). No allocation and no synchronisation.
+ * Refused before any CUDA call: a NULL or misaligned pointer, rows < 1, cols outside [1, 2^31), k outside [1, 4096],
+ * chunks outside [1, 65535], ids with masks, and a bad mask set.
+ * Alignment (bytes) of the vr_select_rows arguments: scores 4, ids 8, ws_scores 4, ws_ids 8, out_scores 4, out_ids 8 */
+int vr_select_rows(const float* scores, const int64_t* ids, int32_t rows, int64_t cols, int32_t k, int64_t id_offset,
+                   float* out_scores, int64_t* out_ids, void* stream);
+int vr_select_rows_masks(const float* scores, const int64_t* ids, int32_t rows, int64_t cols, int32_t k, int64_t id_offset,
+                         float* out_scores, int64_t* out_ids, const vr_doc_masks* masks, void* stream);
+int vr_select_rows_chunked(const float* scores, int32_t rows, int64_t cols, int32_t k, int64_t id_offset, int32_t chunks,
+                           float* ws_scores, int64_t* ws_ids, float* out_scores, int64_t* out_ids, void* stream);
+int vr_select_rows_chunked_masks(const float* scores, int32_t rows, int64_t cols, int32_t k, int64_t id_offset,
+                                 int32_t chunks, float* ws_scores, int64_t* ws_ids, float* out_scores, int64_t* out_ids,
+                                 const vr_doc_masks* masks, void* stream);
+
 /* vr_mmr_select: maximal marginal relevance (DESIGN §4) over given candidates. Query row r has the candidates
  * cand_ids [nq, fetch] (local doc ids, row-major) with relevance scores cand_scores [nq, fetch], in (score desc, id asc)
  * order as vr_topk_rows returns them; the first id outside [0, nd) ends the row's candidates (F' of them) and is never

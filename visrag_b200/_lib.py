@@ -162,6 +162,14 @@ def _declare(lib: C.CDLL) -> None:
     lib.vr_topk_rows_masks.argtypes = [vp, vp, i32, i64, i32, i64, vp, vp, dm, vp]
     lib.vr_topk_rows_chunked_masks.restype = i32
     lib.vr_topk_rows_chunked_masks.argtypes = [vp, i32, i64, i32, i64, i32, vp, vp, vp, vp, dm, vp]
+    lib.vr_select_rows.restype = i32
+    lib.vr_select_rows.argtypes = [vp, vp, i32, i64, i32, i64, vp, vp, vp]
+    lib.vr_select_rows_masks.restype = i32
+    lib.vr_select_rows_masks.argtypes = [vp, vp, i32, i64, i32, i64, vp, vp, dm, vp]
+    lib.vr_select_rows_chunked.restype = i32
+    lib.vr_select_rows_chunked.argtypes = [vp, i32, i64, i32, i64, i32, vp, vp, vp, vp, vp]
+    lib.vr_select_rows_chunked_masks.restype = i32
+    lib.vr_select_rows_chunked_masks.argtypes = [vp, i32, i64, i32, i64, i32, vp, vp, vp, vp, dm, vp]
     lib.vr_group_topk_rows_masks.restype = i32
     lib.vr_group_topk_rows_masks.argtypes = [vp, i32, i64, vp, i32, dm, i32, i64, i32, vp, i64, vp, vp, vp, vp]
     lib.vr_score_lists.restype = i32

@@ -906,11 +906,12 @@ __device__ __forceinline__ bool col_eligible(const uint32_t* __restrict__ mask, 
 // top-k of each row of a dense [rows, cols] fp32 matrix (optionally with explicit ids per entry).
 // MASKED (ids == NULL only): row r's ineligible columns (by the mask of row r's query) are skipped like negative ids -
 // never represented by a -inf score, which would count as a valid entry.
+// The body of topk_rows_kernel, also the rerun of select_rows_kernel for rows that repeat a (score, id) pair.
 template <bool MASKED>
-__global__ void __launch_bounds__(256)
-topk_rows_kernel(const float* __restrict__ scores, const long long* __restrict__ ids, long long cols, int k,
-                 long long id_offset, long long chunk_cols, float* __restrict__ out_scores,
-                 long long* __restrict__ out_ids, const DocMasks masks) {
+__device__ __forceinline__ void topk_rows_block(const float* __restrict__ scores, const long long* __restrict__ ids,
+                                                long long cols, int k, long long id_offset, long long chunk_cols,
+                                                float* __restrict__ out_scores, long long* __restrict__ out_ids,
+                                                const DocMasks& masks) {
     // block (row, chunk): top-k of columns [chunk*chunk_cols, ...) of one row, written as list `row*gridDim.y + chunk`
     __shared__ float red_s[8];
     __shared__ long long red_i[8];
@@ -948,6 +949,14 @@ topk_rows_kernel(const float* __restrict__ scores, const long long* __restrict__
         }
         last_s = bs; last_i = bi;
     }
+}
+
+template <bool MASKED>
+__global__ void __launch_bounds__(256)
+topk_rows_kernel(const float* __restrict__ scores, const long long* __restrict__ ids, long long cols, int k,
+                 long long id_offset, long long chunk_cols, float* __restrict__ out_scores,
+                 long long* __restrict__ out_ids, const DocMasks masks) {
+    topk_rows_block<MASKED>(scores, ids, cols, k, id_offset, chunk_cols, out_scores, out_ids, masks);
 }
 
 // Short rows (cols <= 32*NPL): one WARP per row, the row lives in registers, k rounds of shuffle arg-max - no block barriers.
@@ -1547,11 +1556,16 @@ range_select_kernel(const float* __restrict__ scores, long long nd, const float*
 // of the score, inverted; -0 is canonicalised to +0 (they tie under before(), so the id decides). Low word: id << 1, and
 // bit 0 remembers a -0 so that the output keeps the score's own bits (it never decides an order: ids are distinct).
 // The all-ones key is the padding: it would need a NaN score, which no producer emits.
+// Order-preserving bits of a score (raw bits b): increasing in the score, -0 as +0 (NaNs land beyond +-inf).
+__device__ __forceinline__ uint32_t score_order(uint32_t b) {
+    if (b == 0x80000000u) b = 0u;
+    return (b & 0x80000000u) ? ~b : (b | 0x80000000u);
+}
+
 __device__ __forceinline__ unsigned long long range_key(float s, int id) {
-    uint32_t b = __float_as_uint(s);
+    const uint32_t b = __float_as_uint(s);
     const uint32_t negzero = b == 0x80000000u ? 1u : 0u;
-    if (negzero) b = 0u;
-    const uint32_t o = (b & 0x80000000u) ? ~b : (b | 0x80000000u);
+    const uint32_t o = score_order(b);
     return (static_cast<unsigned long long>(~o) << 32) | (static_cast<uint32_t>(id) << 1) | negzero;
 }
 
@@ -1676,6 +1690,208 @@ static long long range_sort_P(int max_count) {
 
 static long long range_sort_ws(int rows, int max_count) {
     return max_count <= RSORT_TILE ? 0 : static_cast<long long>(rows) * range_sort_P(max_count) * 8;
+}
+
+// ---------------------------------------------------------------------------------------------------- radix select
+// vr_select_rows: the top-k of each row with the bits and order of vr_topk_rows, in passes over the row whose number does
+// not grow with k (DESIGN §4, "Deep top-k"). An entry counts when its id is >= 0, its column is eligible under the row's
+// mask and its score is not NaN; its key is score_order(score) (-0 as +0, the tie rule of before()). Digit passes of 8
+// bits, each a shared-memory histogram of the entries that match the digits chosen so far, find the key B of the k-th
+// entry and how many entries of key B it takes; a pass whose chosen bin holds exactly that many ends the search early.
+// When the boundary splits the entries of key B, digit passes over their ids (from the top byte of the largest) find the
+// highest id taken. The winners - key > B, or key == B and id <= that id - are gathered in shared memory and sorted
+// bitonically by (key desc, id asc). vr_topk_rows emits a repeated (score, id) pair once: a block whose winners repeat a
+// pair (only an input that repeats one can) reruns its row through topk_rows_block, so the result is that kernel's in
+// every case.
+constexpr int SEL_THREADS = 256;
+constexpr int SEL_MAX_K = 4096;
+
+struct SelState {
+    int need;           // entries still to take from the matching bins
+    int total;          // entries counted by the last histogram
+    int bin_count;      // entries in the chosen bin
+    unsigned int bin;   // the chosen bin
+};
+
+// Warp 0 after a histogram: the bin holding the need-th entry, bins walked from 255 down (DESC) or from 0 up. Sets
+// st.bin and st.bin_count, lowers st.need by the entries of the bins walked past, and sets st.total.
+template <bool DESC>
+__device__ __forceinline__ void select_bin(const unsigned int* hist, SelState& st) {
+    const int lane = threadIdx.x;
+    int h[8], sum = 0;
+#pragma unroll
+    for (int j = 0; j < 8; ++j) {
+        const int b = lane * 8 + j;
+        h[j] = static_cast<int>(hist[DESC ? 255 - b : b]);
+        sum += h[j];
+    }
+    int incl = sum;
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) {
+        const int t = __shfl_up_sync(0xffffffffu, incl, o);
+        if (lane >= o) incl += t;
+    }
+    const int need = st.need;
+    __syncwarp();
+    int past = incl - sum;
+    bool found = !(past < need && need <= incl);
+#pragma unroll
+    for (int j = 0; j < 8; ++j) {
+        if (!found && past + h[j] >= need) {
+            found = true;
+            st.bin = DESC ? 255 - (lane * 8 + j) : lane * 8 + j;
+            st.bin_count = h[j];
+            st.need = need - past;
+        }
+        past += h[j];
+    }
+    if (lane == 31) st.total = incl;
+    __syncwarp();
+}
+
+template <bool MASKED>
+__global__ void __launch_bounds__(SEL_THREADS, 4)  // without the 4, ptxas caps the unmasked form at 48 registers and spills
+select_rows_kernel(const float* __restrict__ scores, const long long* __restrict__ ids, long long cols, int k,
+                   long long id_offset, long long chunk_cols, float* __restrict__ out_scores,
+                   long long* __restrict__ out_ids, const DocMasks masks) {
+    // block (row, chunk) as in topk_rows_kernel. Dynamic shared memory: [P] sort words (~key << 32 | score bits), then
+    // [P] ids, P = the power of two >= k.
+    extern __shared__ unsigned long long sel_words[];
+    __shared__ unsigned int hist[256];
+    __shared__ SelState st;
+    __shared__ unsigned long long id_max;
+    __shared__ int taken, repeat;
+    const long long c_lo = static_cast<long long>(blockIdx.y) * chunk_cols;
+    const long long c_hi = min(cols, c_lo + chunk_cols);
+    const float* srow = scores + static_cast<long long>(blockIdx.x) * cols;
+    const long long* irow = ids ? ids + static_cast<long long>(blockIdx.x) * cols : nullptr;
+    const long long row = static_cast<long long>(blockIdx.x) * gridDim.y + blockIdx.y;  // output list
+    const uint32_t* mask = MASKED ? mask_of_row(masks, blockIdx.x) : nullptr;
+    const int lane = threadIdx.x & 31;
+
+    // column c: false when it does not count, else its key, raw score bits and id
+    auto entry = [&](long long c, uint32_t& key, uint32_t& bits, long long& id) -> bool {
+        if (c >= c_hi) return false;
+        id = irow ? irow[c] : c;
+        if (id < 0 || (MASKED && !col_eligible(mask, c))) return false;
+        const float s = srow[c];
+        bits = __float_as_uint(s);
+        key = score_order(bits);
+        return !isnan(s);
+    };
+    // hist[d] = the entries whose digit_of is d (256: not counted), one shared atomic per distinct digit of a warp
+    auto histogram = [&](auto digit_of) {
+        for (int i = threadIdx.x; i < 256; i += SEL_THREADS) hist[i] = 0;
+        __syncthreads();
+        for (long long c0 = c_lo; c0 < c_hi; c0 += SEL_THREADS) {
+            const unsigned int d = digit_of(c0 + threadIdx.x);
+            const unsigned int peers = __match_any_sync(0xffffffffu, d);
+            if (d < 256 && lane == __ffs(peers) - 1) atomicAdd(hist + d, static_cast<unsigned int>(__popc(peers)));
+        }
+        __syncthreads();
+    };
+
+    // winners: key > thr, or key == thr and id <= id_hi
+    uint32_t thr = 0, pmask = 0;
+    long long id_hi = 0x7fffffffffffffffll;
+    bool split = true;  // the boundary splits the entries of key thr
+    if (threadIdx.x == 0) st.need = k;
+    for (int shift = 24; shift >= 0; shift -= 8) {
+        histogram([&](long long c) -> unsigned int {
+            uint32_t key, bits;
+            long long id;
+            if (!entry(c, key, bits, id) || (key & pmask) != thr) return 256u;
+            return (key >> shift) & 255u;
+        });
+        if (threadIdx.x < 32) select_bin<true>(hist, st);
+        __syncthreads();
+        if (shift == 24 && st.total <= k) {  // k or fewer entries: every one is a winner
+            split = false;
+            break;
+        }
+        thr |= st.bin << shift;
+        pmask |= 255u << shift;
+        if (st.bin_count == st.need) {  // the whole bin is taken: key >= thr
+            split = false;
+            break;
+        }
+    }
+    if (split) {  // the lowest st.need ids of key thr
+        if (threadIdx.x == 0) id_max = 0;
+        __syncthreads();
+        for (long long c = c_lo + threadIdx.x; c < c_hi; c += SEL_THREADS) {
+            uint32_t key, bits;
+            long long id;
+            if (entry(c, key, bits, id) && key == thr) atomicMax(&id_max, static_cast<unsigned long long>(id));
+        }
+        __syncthreads();
+        const unsigned long long top = id_max;
+        unsigned long long ip = 0, imask = 0;
+        int shift = top ? (63 - __clzll(static_cast<long long>(top))) & ~7 : 0;
+        for (;; shift -= 8) {
+            histogram([&](long long c) -> unsigned int {
+                uint32_t key, bits;
+                long long id;
+                if (!entry(c, key, bits, id) || key != thr || (static_cast<unsigned long long>(id) & imask) != ip) return 256u;
+                return static_cast<unsigned int>(id >> shift) & 255u;
+            });
+            if (threadIdx.x < 32) select_bin<false>(hist, st);
+            __syncthreads();
+            ip |= static_cast<unsigned long long>(st.bin) << shift;
+            imask |= 255ull << shift;
+            if (shift == 0 || st.bin_count == st.need) break;
+        }
+        id_hi = static_cast<long long>(ip | ((1ull << shift) - 1));  // ids of key thr sit below 2^(shift + 8)
+    }
+
+    int P = 1;
+    while (P < k) P <<= 1;
+    unsigned long long* wk = sel_words;
+    long long* wi = reinterpret_cast<long long*>(sel_words + P);
+    if (threadIdx.x == 0) { taken = 0; repeat = 0; }
+    __syncthreads();
+    for (long long c = c_lo + threadIdx.x; c < c_hi; c += SEL_THREADS) {
+        uint32_t key, bits;
+        long long id;
+        if (entry(c, key, bits, id) && (key > thr || (key == thr && id <= id_hi))) {
+            const int slot = atomicAdd(&taken, 1);
+            if (slot < k) {
+                wk[slot] = (static_cast<unsigned long long>(~key) << 32) | bits;
+                wi[slot] = id;
+            }
+        }
+    }
+    __syncthreads();
+    const int n = taken;
+    if (n <= k) {
+        int P2 = 1;
+        while (P2 < n) P2 <<= 1;
+        for (int j = n + threadIdx.x; j < P2; j += SEL_THREADS) { wk[j] = ~0ull; wi[j] = 0x7fffffffffffffffll; }
+        __syncthreads();
+        for (int kk = 2; kk <= P2; kk <<= 1) {
+            for (int j = kk >> 1; j > 0; j >>= 1) {
+                for (int t = threadIdx.x; t < P2 / 2; t += SEL_THREADS) {
+                    const int i = ((t & ~(j - 1)) << 1) | (t & (j - 1));
+                    const unsigned long long a = wk[i], b = wk[i + j];
+                    const long long ia = wi[i], ib = wi[i + j];
+                    const bool later = (a >> 32) > (b >> 32) || ((a >> 32) == (b >> 32) && ia > ib);
+                    if (later == ((i & kk) == 0)) { wk[i] = b; wk[i + j] = a; wi[i] = ib; wi[i + j] = ia; }
+                }
+                __syncthreads();
+            }
+        }
+        for (int j = threadIdx.x; j + 1 < n; j += SEL_THREADS)
+            if ((wk[j] >> 32) == (wk[j + 1] >> 32) && wi[j] == wi[j + 1]) repeat = 1;
+        __syncthreads();
+    }
+    if (n > k || repeat) {  // block-uniform
+        topk_rows_block<MASKED>(scores, ids, cols, k, id_offset, chunk_cols, out_scores, out_ids, masks);
+        return;
+    }
+    for (int j = threadIdx.x; j < k; j += SEL_THREADS) {
+        out_scores[row * k + j] = j < n ? __uint_as_float(static_cast<uint32_t>(wk[j])) : -INFINITY;
+        out_ids[row * k + j] = j < n ? wi[j] + id_offset : -1;
+    }
 }
 
 // ---------------------------------------------------------------------------------------------------- MMR selection
@@ -2451,6 +2667,96 @@ extern "C" int vr_range_sort(const float* scores, const int32_t* ids, int64_t pi
     range_emit_kernel<<<grid, 256, 0, st>>>(w, P, counts, row_of, oo, id_offset, out_scores, oi);
     VR_CHECK_CUDA(cudaGetLastError());
     return 0;
+}
+
+// vr_select_rows(_masks) and the chunked forms, after the mask checks: select_rows_kernel over (rows, chunks) blocks; with
+// chunks >= 2 each block writes its chunk's list (ids = column + id_offset) and a second launch selects from the
+// [rows, chunks * k] lists, as topk_rows_chunked does.
+static int select_rows(const char* fn, const float* scores, const int64_t* ids, int rows, long long cols, int k,
+                       long long id_offset, int chunks, float* ws_scores, int64_t* ws_ids, float* out_scores,
+                       int64_t* out_ids, const DocMasks* masks, void* stream) {
+    VR_REQUIRE(scores && out_scores && out_ids, "%s: null pointer", fn);
+    VR_REQUIRE(chunks < 2 || (ws_scores && ws_ids), "%s: null pointer", fn);
+    VR_REQUIRE(rows > 0 && cols > 0 && cols < 2147483647ll && k > 0 && chunks > 0 && chunks <= 65535, "%s: bad shape", fn);
+    VR_REQUIRE(k <= SEL_MAX_K, "%s: k=%d, needs k <= %d", fn, k, SEL_MAX_K);
+    static unsigned long long attr_set = 0;
+    if (first_use_on_device(&attr_set)) {
+        VR_CHECK_CUDA(cudaFuncSetAttribute(select_rows_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, SEL_MAX_K * 16));
+        VR_CHECK_CUDA(cudaFuncSetAttribute(select_rows_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, SEL_MAX_K * 16));
+    }
+    int P = 1;
+    while (P < k) P <<= 1;
+    const size_t smem = static_cast<size_t>(P) * 16;
+    cudaStream_t s = reinterpret_cast<cudaStream_t>(stream);
+    const long long* i = reinterpret_cast<const long long*>(ids);
+    const long long chunk_cols = (cols + chunks - 1) / chunks;
+    float* os = chunks >= 2 ? ws_scores : out_scores;
+    long long* oi = reinterpret_cast<long long*>(chunks >= 2 ? ws_ids : out_ids);
+    if (masks)
+        select_rows_kernel<true><<<dim3(rows, chunks), SEL_THREADS, smem, s>>>(scores, i, cols, k, id_offset, chunk_cols, os,
+                                                                               oi, *masks);
+    else
+        select_rows_kernel<false><<<dim3(rows, chunks), SEL_THREADS, smem, s>>>(scores, i, cols, k, id_offset, chunk_cols, os,
+                                                                                oi, kNoMasks);
+    VR_CHECK_CUDA(cudaGetLastError());
+    if (chunks >= 2) {
+        select_rows_kernel<false><<<rows, SEL_THREADS, smem, s>>>(ws_scores, oi, static_cast<long long>(chunks) * k, k, 0,
+                                                                  static_cast<long long>(chunks) * k, out_scores,
+                                                                  reinterpret_cast<long long*>(out_ids), kNoMasks);
+        VR_CHECK_CUDA(cudaGetLastError());
+    }
+    return 0;
+}
+
+extern "C" int vr_select_rows(const float* scores, const int64_t* ids, int32_t rows, int64_t cols, int32_t k,
+                              int64_t id_offset, float* out_scores, int64_t* out_ids, void* stream) {
+    const char* fn = "vr_select_rows";
+    VR_REQUIRE_ALIGNED(fn, "ids", ids, 8);  // optional
+    VR_REQUIRE_PTR(fn, "scores", scores, 4);
+    VR_REQUIRE_PTR(fn, "out_scores", out_scores, 4);
+    VR_REQUIRE_PTR(fn, "out_ids", out_ids, 8);
+    return select_rows(fn, scores, ids, rows, cols, k, id_offset, 1, nullptr, nullptr, out_scores, out_ids, nullptr, stream);
+}
+
+extern "C" int vr_select_rows_masks(const float* scores, const int64_t* ids, int32_t rows, int64_t cols, int32_t k,
+                                    int64_t id_offset, float* out_scores, int64_t* out_ids, const vr_doc_masks* masks,
+                                    void* stream) {
+    const char* fn = "vr_select_rows_masks";
+    VR_REQUIRE_MASKS(fn, masks, cols);
+    VR_REQUIRE(!ids, "%s: the masks index columns, so ids must be NULL", fn);
+    VR_REQUIRE_PTR(fn, "scores", scores, 4);
+    VR_REQUIRE_PTR(fn, "out_scores", out_scores, 4);
+    VR_REQUIRE_PTR(fn, "out_ids", out_ids, 8);
+    const DocMasks m = device_masks(masks);
+    return select_rows(fn, scores, nullptr, rows, cols, k, id_offset, 1, nullptr, nullptr, out_scores, out_ids, &m, stream);
+}
+
+extern "C" int vr_select_rows_chunked(const float* scores, int32_t rows, int64_t cols, int32_t k, int64_t id_offset,
+                                      int32_t chunks, float* ws_scores, int64_t* ws_ids, float* out_scores, int64_t* out_ids,
+                                      void* stream) {
+    const char* fn = "vr_select_rows_chunked";
+    VR_REQUIRE_PTR(fn, "scores", scores, 4);
+    VR_REQUIRE_PTR(fn, "ws_scores", ws_scores, 4);
+    VR_REQUIRE_PTR(fn, "ws_ids", ws_ids, 8);
+    VR_REQUIRE_PTR(fn, "out_scores", out_scores, 4);
+    VR_REQUIRE_PTR(fn, "out_ids", out_ids, 8);
+    return select_rows(fn, scores, nullptr, rows, cols, k, id_offset, chunks, ws_scores, ws_ids, out_scores, out_ids, nullptr,
+                       stream);
+}
+
+extern "C" int vr_select_rows_chunked_masks(const float* scores, int32_t rows, int64_t cols, int32_t k, int64_t id_offset,
+                                            int32_t chunks, float* ws_scores, int64_t* ws_ids, float* out_scores,
+                                            int64_t* out_ids, const vr_doc_masks* masks, void* stream) {
+    const char* fn = "vr_select_rows_chunked_masks";
+    VR_REQUIRE_MASKS(fn, masks, cols);
+    VR_REQUIRE_PTR(fn, "scores", scores, 4);
+    VR_REQUIRE_PTR(fn, "ws_scores", ws_scores, 4);
+    VR_REQUIRE_PTR(fn, "ws_ids", ws_ids, 8);
+    VR_REQUIRE_PTR(fn, "out_scores", out_scores, 4);
+    VR_REQUIRE_PTR(fn, "out_ids", out_ids, 8);
+    const DocMasks m = device_masks(masks);
+    return select_rows(fn, scores, nullptr, rows, cols, k, id_offset, chunks, ws_scores, ws_ids, out_scores, out_ids, &m,
+                       stream);
 }
 
 // ---------------------------------------------------------------------------------------------------- MMR selection

@@ -42,6 +42,12 @@ import torch
 from . import _lib as L
 
 SMALL_PROBLEM = 1 << 22  # nq*nd below this: plain fp32 scan (the GEMM pipeline would not even fill)
+SELECT_K_MIN = 32        # k above this (up to SELECT_K_MAX): the radix select vr_select_rows instead of the k-pass vr_topk_rows
+SELECT_K_MAX = 4096
+DEEP_K_MIN = 300         # k above this (up to DEEP_K_MAX): score_topk's deep route (DESIGN §4, "Deep top-k")
+DEEP_K_MAX = 1024
+DEEP_SAMPLE_RANK = 16    # the threshold is the sample's 16th exact score; a sample of every (k // 8)-th page puts it near
+                         # rank 2k of the whole index
 
 
 @dataclass
@@ -159,6 +165,13 @@ def _check_doc_mask(doc_mask: torch.Tensor, index: CorpusIndex, nq: int, mask_of
     return _MaskSet(pack_doc_mask(doc_mask), of_query)
 
 
+def _rows_fn(k: int, form: str = ""):
+    """The row selection of k for the entry point form ("", "_masks", "_chunked", "_chunked_masks"): vr_select_rows for
+    SELECT_K_MIN < k <= SELECT_K_MAX, else vr_topk_rows. Both take the same arguments and give the same bits."""
+    name = "vr_select_rows" if SELECT_K_MIN < k <= SELECT_K_MAX else "vr_topk_rows"
+    return getattr(L.lib(), name + form)
+
+
 def _exact_topk(q: torch.Tensor, index: CorpusIndex, k: int, id_offset: int, masks: Optional[_MaskSet]):
     """The plain fp32 scan: (scores, ids)."""
     nq, d = q.shape
@@ -176,10 +189,10 @@ def _exact_topk(q: torch.Tensor, index: CorpusIndex, k: int, id_offset: int, mas
         if chunks >= 2:
             ws_s = torch.empty((n, chunks, k), dtype=torch.float32, device=q.device)
             ws_i = torch.empty((n, chunks, k), dtype=torch.int64, device=q.device)
-            fn = lib.vr_topk_rows_chunked_masks if mw else lib.vr_topk_rows_chunked
+            fn = _rows_fn(k, "_chunked_masks" if mw else "_chunked")
             args = (scratch.data_ptr(), n, nd, k, id_offset, chunks, ws_s.data_ptr(), ws_i.data_ptr())
         else:
-            fn = lib.vr_topk_rows_masks if mw else lib.vr_topk_rows
+            fn = _rows_fn(k, "_masks" if mw else "")
             args = (scratch.data_ptr(), None, n, nd, k, id_offset)
         L.check(fn(*args, out_s[r0:].data_ptr(), out_i[r0:].data_ptr(), *mw, L.stream_ptr()))
     return out_s, out_i
@@ -199,7 +212,9 @@ def score_topk(queries: torch.Tensor, index: CorpusIndex, k: int, id_offset: int
     CSR form, list m = ids[offsets[m]:offsets[m+1]] (any order, repeats count once), and list_of int [nq] in [0, M) picks
     each query's list (default: list i for query i when M == nq, or the one list for every query when M == 1). Only the
     listed docs are read; each row equals this call with a doc_mask of exactly its list's docs. stats["path"] is "lists".
-    doc_lists cannot be combined with doc_mask or mask_of."""
+    doc_lists cannot be combined with doc_mask or mask_of.
+    For DEEP_K_MIN < k <= DEEP_K_MAX (without lists) the rows go the deep route (_deep_topk): stats path "deep",
+    sample_stride, candidates (rescored by the range filter) and fallback (rows rerun through the scan)."""
     if doc_lists is not None or list_of is not None:
         q, ls = _queries_and_lists(queries, index, doc_mask, mask_of, doc_lists, list_of)
         with L.on_device(q.device):
@@ -348,15 +363,15 @@ def _lists_topk(q: torch.Tensor, index: CorpusIndex, k: int, id_offset: int, ls:
         if grouped:
             _merge_group_levels(sc[:n], si[:n], sg[:n], k, [t[r0:r0 + n] for t in out])
         elif W <= LIST_CHUNK:
-            L.check(lib.vr_topk_rows(sc.data_ptr(), si.data_ptr(), n, W, k, id_offset, out[0][r0:].data_ptr(),
-                                     out[1][r0:].data_ptr(), sp))
+            L.check(_rows_fn(k)(sc.data_ptr(), si.data_ptr(), n, W, k, id_offset, out[0][r0:].data_ptr(),
+                                out[1][r0:].data_ptr(), sp))
         else:
             c = W // LIST_CHUNK
             ws_s = torch.empty((n * c, k), dtype=torch.float32, device=q.device)
             ws_i = torch.empty((n * c, k), dtype=torch.int64, device=q.device)
-            L.check(lib.vr_topk_rows(sc.data_ptr(), si.data_ptr(), n * c, LIST_CHUNK, k, 0, ws_s.data_ptr(), ws_i.data_ptr(), sp))
-            L.check(lib.vr_topk_rows(ws_s.data_ptr(), ws_i.data_ptr(), n, c * k, k, id_offset, out[0][r0:].data_ptr(),
-                                     out[1][r0:].data_ptr(), sp))
+            L.check(_rows_fn(k)(sc.data_ptr(), si.data_ptr(), n * c, LIST_CHUNK, k, 0, ws_s.data_ptr(), ws_i.data_ptr(), sp))
+            L.check(_rows_fn(k)(ws_s.data_ptr(), ws_i.data_ptr(), n, c * k, k, id_offset, out[0][r0:].data_ptr(),
+                                out[1][r0:].data_ptr(), sp))
     bad = int(status.item())  # host sync: the caller reads the result next anyway
     if bad:
         raise RuntimeError(f"vr_score_lists reported status {bad} (a list longer than its width, or a list index out of range)")
@@ -445,6 +460,8 @@ def _score_topk(q: torch.Tensor, index: CorpusIndex, k: int, id_offset: int, for
         if stats is not None:
             stats.update(path="exact", flagged=0)
         return exact(q, masks)
+    if gt is None and not page_lists and DEEP_K_MIN < k <= DEEP_K_MAX:
+        return _deep_topk(q, index, k, id_offset, stats, masks)
     lib = L.lib()
     ranges = lib.vr_score_ranges(nq, nd)
     lists = ranges * 2 * lib.vr_score_list_len()
@@ -482,8 +499,10 @@ def _score_topk(q: torch.Tensor, index: CorpusIndex, k: int, id_offset: int, for
     if stats is not None:
         stats.update(path="filter+rescore", flagged=int(bad.numel()), ranges=ranges)
     if bad.numel() > 0:
-        # each flagged row reruns with its own mask
-        for t, fix in zip(out, exact(q.index_select(0, bad), None if masks is None else masks.rows(bad))):
+        # each flagged row reruns with its own mask; many rows at a deep k take the deep route, which is exact as well
+        rows, m = q.index_select(0, bad), None if masks is None else masks.rows(bad)
+        deep = gt is None and not page_lists and SELECT_K_MIN < k <= DEEP_K_MAX and bad.numel() * nd > SMALL_PROBLEM
+        for t, fix in zip(out, _deep_topk(rows, index, k, id_offset, None, m) if deep else exact(rows, m)):
             t.index_copy_(0, bad, fix)
     return out
 
@@ -616,8 +635,8 @@ def merge_topk(scores: torch.Tensor, ids: torch.Tensor, k: int) -> Tuple[torch.T
     out_s = torch.empty((nq, k), dtype=torch.float32, device=scores.device)
     out_i = torch.empty((nq, k), dtype=torch.int64, device=scores.device)
     with L.on_device(scores.device):
-        L.check(L.lib().vr_topk_rows(scores.data_ptr(), ids.data_ptr(), nq, m, k, 0, out_s.data_ptr(), out_i.data_ptr(),
-                                     L.stream_ptr()))
+        L.check(_rows_fn(k)(scores.data_ptr(), ids.data_ptr(), nq, m, k, 0, out_s.data_ptr(), out_i.data_ptr(),
+                            L.stream_ptr()))
     return out_s, out_i
 
 
@@ -856,6 +875,28 @@ def _range_filter(q: torch.Tensor, index: CorpusIndex, t: torch.Tensor, masks: O
     """Query rows r0 .. r0 + n of the batch through the range filter and the candidate rescoring; rows that overflowed
     (or have no bound) rerun through the scan. Returns the CSR pieces of these rows."""
     n, d = q.shape
+    dev = q.device
+    counts, kept, rs, ri = _range_candidates(q, index, t, masks, r0, cap)
+    host = torch.stack([counts, kept]).cpu()  # host sync: the CSR sizes are needed to allocate the output
+    over = host[0] > cap
+    info["candidates"] += int(host[0][~over].sum())
+    ok = torch.nonzero(~over).flatten()
+    pieces = []
+    if ok.numel():
+        pieces.append(_range_sort(rs, ri, cap, kept, host[1], ok, rows, id_offset))
+    bad = torch.nonzero(over).flatten()
+    if bad.numel():
+        info["fallback"] += int(bad.numel())
+        sel = bad.to(dev)
+        m = None if masks is None else _MaskSet(masks.words, None if masks.of_query is None else masks.of_query[r0:r0 + n]).rows(sel)
+        pieces += _range_scan(q.index_select(0, sel), index, t.index_select(0, sel), m, rows[bad], id_offset)
+    return pieces
+
+
+def _range_candidates(q: torch.Tensor, index: CorpusIndex, t: torch.Tensor, masks: Optional[_MaskSet], r0: int, cap: int):
+    """The range filter and the candidate rescoring of query rows r0 .. r0 + n of the batch: (counts [n] (> cap: the row
+    overflowed), kept [n], the region scores / ids [n, cap] (row r's first kept[r] entries, in no order))."""
+    n, d = q.shape
     nd, dev = index.nd, q.device
     lib, sp = L.lib(), L.stream_ptr()
     q16 = torch.empty((n, d), dtype=torch.float16, device=dev)
@@ -872,21 +913,7 @@ def _range_filter(q: torch.Tensor, index: CorpusIndex, t: torch.Tensor, masks: O
     kept = torch.empty(n, dtype=torch.int32, device=dev)
     L.check(lib.vr_score_rescore_range(q.data_ptr(), n, index.emb.data_ptr(), nd, d, t.data_ptr(), cap, counts.data_ptr(),
                                        cand.data_ptr(), rs.data_ptr(), ri.data_ptr(), kept.data_ptr(), sp))
-    del cand
-    host = torch.stack([counts, kept]).cpu()  # host sync: the CSR sizes are needed to allocate the output
-    over = host[0] > cap
-    info["candidates"] += int(host[0][~over].sum())
-    ok = torch.nonzero(~over).flatten()
-    pieces = []
-    if ok.numel():
-        pieces.append(_range_sort(rs, ri, cap, kept, host[1], ok, rows, id_offset))
-    bad = torch.nonzero(over).flatten()
-    if bad.numel():
-        info["fallback"] += int(bad.numel())
-        sel = bad.to(dev)
-        m = None if masks is None else _MaskSet(masks.words, None if masks.of_query is None else masks.of_query[r0:r0 + n]).rows(sel)
-        pieces += _range_scan(q.index_select(0, sel), index, t.index_select(0, sel), m, rows[bad], id_offset)
-    return pieces
+    return counts, kept, rs, ri
 
 
 def _range_scan(q: torch.Tensor, index: CorpusIndex, t: torch.Tensor, masks: Optional[_MaskSet], rows: torch.Tensor,
@@ -967,6 +994,75 @@ def _range_assemble(nq: int, pieces, device) -> Tuple[torch.Tensor, torch.Tensor
         out_s[dst] = s
         out_i[dst] = i
     return offsets.to(device), out_s, out_i
+
+
+# ------------------------------------------------------------------------------------------------------
+# Deep top-k: a sampled threshold on the range filter (DESIGN §4, "Deep top-k")
+# ------------------------------------------------------------------------------------------------------
+def _sample_masks(masks: Optional[_MaskSet], nd: int, stride: int) -> Optional[_MaskSet]:
+    """The mask set over the sampled pages 0, stride, 2 stride, ... (each mask keeps its rows)."""
+    if masks is None:
+        return None
+    cols = torch.arange(0, nd, stride, device=masks.words.device)
+    w = masks.words.view(torch.int32).index_select(1, cols >> 5)
+    bits = ((w >> (cols & 31).to(torch.int32)) & 1).bool()
+    return _MaskSet(pack_doc_mask(bits), masks.of_query)
+
+
+def _deep_topk(q: torch.Tensor, index: CorpusIndex, k: int, id_offset: int, stats: Optional[dict],
+               masks: Optional[_MaskSet]):
+    """score_topk for DEEP_K_MIN < k <= DEEP_K_MAX. Every (k // 8)-th page forms a sample; t_q = the 16th best exact score
+    of query q over its eligible sampled pages. The range filter and rescoring give A = {eligible pages with exact s >=
+    t_q} with the scan's bits. When |A| >= k the top-k of q is the top-k of A (its k-th score is >= t_q, and every page
+    ranked above it has s >= t_q). Rows with |A| < k, rows that overflowed RANGE_CAP and rows
+    whose sample holds fewer than 16 eligible pages rerun through the fp32 scan. A poor threshold costs time, never bits.
+    The first k of A come from vr_select_rows over the rescored region."""
+    nq, d = q.shape
+    nd, dev = index.nd, q.device
+    ev = _Stages(stats)
+    stride = max(1, k // 8)
+    sample = CorpusIndex(index.emb[::stride].contiguous(), index.emb_f16[::stride].contiguous(), index.max_norm)
+    ss, si = _score_topk(q, sample, DEEP_SAMPLE_RANK, 0, False, None, _sample_masks(masks, nd, stride))
+    t = ss[:, DEEP_SAMPLE_RANK - 1].contiguous()
+    short = si[:, DEEP_SAMPLE_RANK - 1] < 0
+    del sample, ss, si
+    ev.mark("sample")
+    out_s = torch.empty((nq, k), dtype=torch.float32, device=dev)
+    out_i = torch.empty((nq, k), dtype=torch.int64, device=dev)
+    info = dict(path="deep", flagged=0, sample_stride=stride, candidates=0, fallback=0)
+    bad = [torch.nonzero(short).flatten().cpu()]
+    step = max(1, min(nq, RANGE_BUDGET // RANGE_CAP))
+    for r0 in range(0, nq, step):
+        n = min(step, nq - r0)
+        counts, kept, rs, ri = _range_candidates(q[r0:r0 + n], index, t[r0:r0 + n], masks, r0, RANGE_CAP)
+        host = torch.stack([counts, kept, short[r0:r0 + n].to(torch.int32)]).cpu()
+        ev.mark("range")
+        over = host[0] > RANGE_CAP
+        info["candidates"] += int(host[0][~over].sum())
+        ok = (~over) & (host[1] >= k) & (host[2] == 0)
+        bad.append(torch.nonzero(~ok & (host[2] == 0)).flatten() + r0)
+        sel = torch.nonzero(ok).flatten().to(dev)
+        if sel.numel():  # the top-k of each row's kept region: vr_select_rows with explicit ids (-1 past kept)
+            m = sel.numel()
+            ids = torch.where(torch.arange(RANGE_CAP, device=dev) < kept.index_select(0, sel)[:, None],
+                              ri.index_select(0, sel), -1).long()
+            sc = rs.index_select(0, sel)
+            ps = torch.empty((m, k), dtype=torch.float32, device=dev)
+            pi = torch.empty((m, k), dtype=torch.int64, device=dev)
+            L.check(L.lib().vr_select_rows(sc.data_ptr(), ids.data_ptr(), m, RANGE_CAP, k, id_offset, ps.data_ptr(),
+                                           pi.data_ptr(), L.stream_ptr()))
+            out_s[sel + r0], out_i[sel + r0] = ps, pi
+        ev.mark("pick")
+    bad = torch.cat(bad)
+    if bad.numel():
+        info["fallback"] = int(bad.numel())
+        sel = bad.to(dev)
+        fs, fi = _exact_topk(q.index_select(0, sel), index, k, id_offset, None if masks is None else masks.rows(sel))
+        out_s[sel], out_i[sel] = fs, fi
+        ev.mark("fallback")
+    if stats is not None:
+        stats.update(info)
+    return out_s, out_i
 
 
 # ------------------------------------------------------------------------------------------------------
