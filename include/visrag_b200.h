@@ -481,6 +481,26 @@ int vr_range_sort(const float* scores, const int32_t* ids, int64_t pitch, const 
                   const int32_t* row_of, const int64_t* out_offsets, int32_t max_count, int64_t id_offset, void* ws,
                   int64_t ws_bytes, float* out_scores, int64_t* out_ids, void* stream);
 
+/* vr_range_groups: the document form of a range region. scores / ids [rows, pitch] with counts[rows] is a region as
+ * vr_score_rescore_range and vr_range_rows write it (ids distinct within a row); doc_groups int32 [nd] gives each page its
+ * group (document). Row r of the output region (out_scores / out_ids [rows, pitch], first out_counts[r] entries, in no
+ * order) holds one entry per group present in row r: the group's first entry in (score desc, id asc) order (+0 = -0, the
+ * lower id wins), carrying that entry's own score bits. Entries with a NaN score, an id outside [0, nd) or a group outside
+ * [0, G) are dropped. vr_range_sort then orders the output region (its ids are distinct); the groups of the output come
+ * from doc_groups. The caller keeps every counts[r] <= max_count <= pitch (entries past max_count are not read). Two
+ * passes over each row against a hash table of P = 2^m >= 2 max_count slots: an atomicMax of the (score order, ~page)
+ * key per group, then the entry holding its group's key appends itself. Up to 4096 entries a row the table lives in
+ * shared memory (one block per row, 12 P bytes); longer rows need a workspace of vr_range_groups_ws_bytes(rows,
+ * max_count) bytes. No allocation and no synchronisation.
+ * Refused before any CUDA call, naming the argument: a NULL or misaligned pointer, rows outside [1, 65535], nd outside
+ * [1, 2^31 - 1), G < 1, max_count outside [0, pitch] and a workspace too small.
+ * Alignment (bytes) of the vr_range_groups arguments: scores 4, ids 4, counts 4, doc_groups 4, out_scores 4, out_ids 4,
+ * out_counts 4, ws 8 */
+int64_t vr_range_groups_ws_bytes(int32_t rows, int32_t max_count);
+int vr_range_groups(const float* scores, const int32_t* ids, int64_t pitch, const int32_t* counts, int32_t rows,
+                    int32_t max_count, const int32_t* doc_groups, int64_t nd, int32_t G, void* ws, int64_t ws_bytes,
+                    float* out_scores, int32_t* out_ids, int32_t* out_counts, void* stream);
+
 /* vr_select_rows: the top-k of each row by a radix select, in passes over the row whose number does not depend on k
  * (DESIGN §4, "Deep top-k"). The contract of vr_topk_rows / vr_topk_rows_masks / vr_topk_rows_chunked(_masks), with the
  * same result bit for bit: out_scores / out_ids [rows, k] in (score desc, id asc) order (+0 = -0, the id decides; a

@@ -184,6 +184,10 @@ def _declare(lib: C.CDLL) -> None:
     lib.vr_range_sort_ws_bytes.argtypes = [i32, i32]
     lib.vr_range_sort.restype = i32
     lib.vr_range_sort.argtypes = [vp, vp, i64, vp, i32, vp, vp, i32, i64, vp, i64, vp, vp, vp]
+    lib.vr_range_groups_ws_bytes.restype = i64
+    lib.vr_range_groups_ws_bytes.argtypes = [i32, i32]
+    lib.vr_range_groups.restype = i32
+    lib.vr_range_groups.argtypes = [vp, vp, i64, vp, i32, i32, vp, i64, i32, vp, i64, vp, vp, vp, vp]
     lib.vr_mmr_select.restype = i32
     lib.vr_mmr_select.argtypes = [vp, i64, i32, vp, vp, i32, i32, vp, i32, i64, vp, vp, vp]
     lib.vr_group_pages_topm.restype = i32

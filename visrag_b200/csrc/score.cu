@@ -1692,6 +1692,105 @@ static long long range_sort_ws(int rows, int max_count) {
     return max_count <= RSORT_TILE ? 0 : static_cast<long long>(rows) * range_sort_P(max_count) * 8;
 }
 
+// vr_range_groups: a region reduced to one entry per group (document) of each row, the group's first entry in the
+// before() order with that entry's own score bits, appended to the output region in no particular order. Pass 1 takes
+// the atomicMax of page_key per (row, group): the order bits of the score above ~page, so the largest key is the highest
+// score and then the lowest page (-0 as +0), whatever order the atomics run in. Pass 2: the entry whose key equals its
+// group's slot claims the slot (an atomicCAS back to 0, so a repeated entry is emitted once) and appends itself. The
+// per-row table is an open-addressing hash of P >= 2 * max_count slots (key u64, group int32; load <= 1/2): in shared
+// memory up to RGROUP_SMEM_MAX entries a row, one block per row, else in the caller's workspace [rows, P] with blocks
+// spread over each row. An entry counts when its score is not NaN, its id lies in [0, nd) and its group in [0, G).
+constexpr int RGROUP_SMEM_MAX = 4096;  // 8192 slots, 96 KB
+constexpr int RGROUP_THREADS = 512;
+
+__device__ __forceinline__ uint32_t rgroup_hash(uint32_t g) {  // the finaliser of MurmurHash3: spreads strided group ids
+    g ^= g >> 16; g *= 0x85ebca6bu; g ^= g >> 13; g *= 0xc2b2ae35u; g ^= g >> 16;
+    return g;
+}
+
+// One pass over entries [j0, n) (step `step`) of a region row (at `base`) against its table (keys tk, groups tg, P = mask + 1
+// slots). INSERT: atomicMax of each entry's key into its group's slot (taking an empty slot when the group has none).
+// Else: the entry holding its slot's key claims it and goes to the output row at `obase` (count in *emitted).
+template <bool INSERT>
+__device__ __forceinline__ void rgroup_pass(const float* __restrict__ scores, const int* __restrict__ ids, long long base,
+                                            int j0, int n, int step, long long nd, const int* __restrict__ doc_groups, int G,
+                                            unsigned long long* tk, int* tg, uint32_t mask, float* __restrict__ out_scores,
+                                            int* __restrict__ out_ids, long long obase, int* emitted) {
+    for (int j = j0; j < n; j += step) {
+        const float s = scores[base + j];
+        const int id = ids[base + j];
+        if (isnan(s) || id < 0 || id >= nd) continue;
+        const int g = __ldg(doc_groups + id);
+        if (g < 0 || g >= G) continue;
+        const unsigned long long key = page_key(s, id);
+        uint32_t h = rgroup_hash(static_cast<uint32_t>(g)) & mask;
+        for (;;) {  // the group's slot: pass 2 finds it before any empty slot
+            const int cur = INSERT ? atomicCAS(tg + h, -1, g) : tg[h];
+            if (cur == -1 || cur == g) break;
+            h = (h + 1) & mask;
+        }
+        if (INSERT) {
+            atomicMax(tk + h, key);
+        } else if (atomicCAS(tk + h, key, 0ull) == key) {
+            const int o = atomicAdd(emitted, 1);
+            out_scores[obase + o] = s;
+            out_ids[obase + o] = id;
+        }
+    }
+}
+
+__device__ __forceinline__ int rgroup_count(const int* counts, long long r, int max_count) {
+    return max(0, min(__ldg(counts + r), max_count));  // the caller keeps counts <= max_count; the table holds no more
+}
+
+__global__ void __launch_bounds__(RGROUP_THREADS)
+range_groups_smem_kernel(const float* __restrict__ scores, const int* __restrict__ ids, long long pitch,
+                         const int* __restrict__ counts, int max_count, long long nd, const int* __restrict__ doc_groups,
+                         int G, int P, float* __restrict__ out_scores, int* __restrict__ out_ids, int* __restrict__ out_counts) {
+    extern __shared__ unsigned long long rg_keys[];  // [P] keys, then [P] groups
+    int* rg_groups = reinterpret_cast<int*>(rg_keys + P);
+    __shared__ int emitted;
+    const long long r = blockIdx.x, base = r * pitch;
+    const int n = rgroup_count(counts, r, max_count);
+    for (int j = threadIdx.x; j < P; j += RGROUP_THREADS) { rg_keys[j] = 0; rg_groups[j] = -1; }
+    if (threadIdx.x == 0) emitted = 0;
+    __syncthreads();
+    rgroup_pass<true>(scores, ids, base, threadIdx.x, n, RGROUP_THREADS, nd, doc_groups, G, rg_keys, rg_groups, P - 1,
+                      nullptr, nullptr, 0, nullptr);
+    __syncthreads();
+    rgroup_pass<false>(scores, ids, base, threadIdx.x, n, RGROUP_THREADS, nd, doc_groups, G, rg_keys, rg_groups, P - 1,
+                       out_scores, out_ids, base, &emitted);
+    __syncthreads();
+    if (threadIdx.x == 0) out_counts[r] = emitted;
+}
+
+// The workspace form: block (x, y) takes entries 256 x, 256 (x + gridDim.x), ... of row y; one launch per pass (the
+// output counts are zeroed by the host).
+template <bool INSERT>
+__global__ void __launch_bounds__(256)
+range_groups_ws_kernel(const float* __restrict__ scores, const int* __restrict__ ids, long long pitch,
+                       const int* __restrict__ counts, int max_count, long long nd, const int* __restrict__ doc_groups, int G,
+                       long long P, unsigned long long* __restrict__ ws, float* __restrict__ out_scores,
+                       int* __restrict__ out_ids, int* __restrict__ out_counts) {
+    const long long r = blockIdx.y, base = r * pitch;
+    const int n = rgroup_count(counts, r, max_count);
+    unsigned long long* tk = ws + r * P;
+    int* tg = reinterpret_cast<int*>(ws + gridDim.y * P) + r * P;
+    rgroup_pass<INSERT>(scores, ids, base, blockIdx.x * 256 + threadIdx.x, n, gridDim.x * 256, nd, doc_groups, G, tk, tg,
+                        static_cast<uint32_t>(P - 1), out_scores, out_ids, base, out_counts + r);
+}
+
+static long long range_groups_P(int max_count) {
+    long long P = 2;
+    while (P < 2ll * max_count) P <<= 1;
+    return P;
+}
+
+// The workspace of vr_range_groups: none up to RGROUP_SMEM_MAX entries a row, else rows x P slots of 12 bytes.
+static long long range_groups_ws(int rows, int max_count) {
+    return max_count <= RGROUP_SMEM_MAX ? 0 : static_cast<long long>(rows) * range_groups_P(max_count) * 12;
+}
+
 // ---------------------------------------------------------------------------------------------------- radix select
 // vr_select_rows: the top-k of each row with the bits and order of vr_topk_rows, in passes over the row whose number does
 // not grow with k (DESIGN §4, "Deep top-k"). An entry counts when its id is >= 0, its column is eligible under the row's
@@ -1705,6 +1804,7 @@ static long long range_sort_ws(int rows, int max_count) {
 // every case.
 constexpr int SEL_THREADS = 256;
 constexpr int SEL_MAX_K = 4096;
+constexpr int SEL_K_MIN = 32;  // k above this: vr_group_topk_rows selects with the radix select (retriever.SELECT_K_MIN)
 
 struct SelState {
     int need;           // entries still to take from the matching bins
@@ -2377,6 +2477,10 @@ extern "C" int64_t vr_group_topk_ws_bytes(int32_t rows, int32_t G, int32_t k, in
     return rows > 0 && G > 0 && k > 0 ? group_topk_ws(rows, G, k, chunks) : -1;
 }
 
+static int select_rows(const char* fn, const float* scores, const int64_t* ids, int rows, long long cols, int k,
+                       long long id_offset, int chunks, float* ws_scores, int64_t* ws_ids, float* out_scores,
+                       int64_t* out_ids, const DocMasks* masks, void* stream);
+
 // vr_group_topk_rows(_masks)
 static int group_topk_rows(const char* fn, const float* scores, int rows, long long nd, const int* doc_groups, int G,
                            const uint32_t* doc_mask, const vr_doc_masks* set, int k, long long id_offset, int chunks, void* ws,
@@ -2408,9 +2512,14 @@ static int group_topk_rows(const char* fn, const float* scores, int rows, long l
     group_decode_kernel<<<static_cast<int>(blocks), 256, 0, st>>>(scores, rows, nd, G, gpages, gscores);
     VR_CHECK_CUDA(cudaGetLastError());
     long long* op = reinterpret_cast<long long*>(out_pages);
-    if (chunks >= 2) {  // few rows x many groups: spread each row over `chunks` blocks, then merge their lists
-        long long* ws_i = reinterpret_cast<long long*>(reinterpret_cast<char*>(ws) + ((n * 12 + 15) / 16) * 16);
-        float* ws_s = reinterpret_cast<float*>(ws_i + static_cast<long long>(rows) * chunks * k);
+    long long* ws_i = reinterpret_cast<long long*>(reinterpret_cast<char*>(ws) + ((n * 12 + 15) / 16) * 16);
+    float* ws_s = reinterpret_cast<float*>(ws_i + static_cast<long long>(rows) * chunks * k);
+    if (k > SEL_K_MIN && k <= SEL_MAX_K) {  // the radix select over the group rows, with the best pages as ids (same bits)
+        if (int rc = select_rows(fn, gscores, reinterpret_cast<const int64_t*>(gpages), rows, G, k, id_offset,
+                                 chunks >= 2 ? chunks : 1, ws_s, reinterpret_cast<int64_t*>(ws_i), out_scores, out_pages,
+                                 nullptr, stream))
+            return rc;
+    } else if (chunks >= 2) {  // few rows x many groups: spread each row over `chunks` blocks, then merge their lists
         topk_rows_kernel<false><<<dim3(rows, chunks), 256, 0, st>>>(gscores, gpages, G, k, id_offset, (G + chunks - 1) / chunks,
                                                                     ws_s, ws_i, kNoMasks);
         VR_CHECK_CUDA(cudaGetLastError());
@@ -2665,6 +2774,60 @@ extern "C" int vr_range_sort(const float* scores, const int32_t* ids, int64_t pi
         range_bitonic_tile_kernel<<<tiles, RSORT_THREADS, 0, st>>>(w, P, k);
     }
     range_emit_kernel<<<grid, 256, 0, st>>>(w, P, counts, row_of, oo, id_offset, out_scores, oi);
+    VR_CHECK_CUDA(cudaGetLastError());
+    return 0;
+}
+
+extern "C" int64_t vr_range_groups_ws_bytes(int32_t rows, int32_t max_count) {
+    return rows > 0 && max_count >= 0 ? range_groups_ws(rows, max_count) : -1;
+}
+
+extern "C" int vr_range_groups(const float* scores, const int32_t* ids, int64_t pitch, const int32_t* counts, int32_t rows,
+                               int32_t max_count, const int32_t* doc_groups, int64_t nd, int32_t G, void* ws, int64_t ws_bytes,
+                               float* out_scores, int32_t* out_ids, int32_t* out_counts, void* stream) {
+    const char* fn = "vr_range_groups";
+    VR_REQUIRE_PTR(fn, "scores", scores, 4);
+    VR_REQUIRE_PTR(fn, "ids", ids, 4);
+    VR_REQUIRE_PTR(fn, "counts", counts, 4);
+    VR_REQUIRE_PTR(fn, "doc_groups", doc_groups, 4);
+    VR_REQUIRE_PTR(fn, "out_scores", out_scores, 4);
+    VR_REQUIRE_PTR(fn, "out_ids", out_ids, 4);
+    VR_REQUIRE_PTR(fn, "out_counts", out_counts, 4);
+    VR_REQUIRE(rows > 0 && rows <= 65535, "%s: rows=%d, needs 0 < rows <= 65535", fn, rows);
+    VR_REQUIRE(nd > 0 && nd < 2147483647ll, "%s: nd=%lld beyond the int32 doc ids", fn, (long long)nd);
+    VR_REQUIRE(G > 0, "%s: G=%d, needs at least one group", fn, G);
+    VR_REQUIRE(max_count >= 0 && max_count <= pitch, "%s: max_count=%d, needs 0 <= max_count <= pitch=%lld", fn, max_count,
+               (long long)pitch);
+    const long long need = range_groups_ws(rows, max_count);
+    VR_REQUIRE(need == 0 || (ws && ws_bytes >= need), "%s: ws of %lld bytes, needs %lld (vr_range_groups_ws_bytes)", fn,
+               (long long)ws_bytes, need);
+    VR_REQUIRE_ALIGNED(fn, "ws", ws, 8);
+    cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+    if (need == 0) {
+        const int P = static_cast<int>(range_groups_P(max_count));
+        const size_t smem = static_cast<size_t>(P) * 12;
+        static unsigned long long attr_set = 0;
+        if (first_use_on_device(&attr_set))  // the static `emitted` counts too: set it whatever this call's size
+            VR_CHECK_CUDA(cudaFuncSetAttribute(range_groups_smem_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                               static_cast<int>(range_groups_P(RGROUP_SMEM_MAX)) * 12));
+        range_groups_smem_kernel<<<rows, RGROUP_THREADS, smem, st>>>(scores, ids, pitch, counts, max_count, nd, doc_groups, G,
+                                                                     P, out_scores, out_ids, out_counts);
+        VR_CHECK_CUDA(cudaGetLastError());
+        return 0;
+    }
+    const long long P = range_groups_P(max_count), slots = static_cast<long long>(rows) * P;
+    unsigned long long* w = reinterpret_cast<unsigned long long*>(ws);
+    VR_CHECK_CUDA(cudaMemsetAsync(w, 0, slots * 8, st));            // keys: 0 = no entry
+    VR_CHECK_CUDA(cudaMemsetAsync(w + slots, 0xff, slots * 4, st));  // groups: -1 = empty slot
+    VR_CHECK_CUDA(cudaMemsetAsync(out_counts, 0, static_cast<size_t>(rows) * sizeof(int), st));
+    long long gx = (max_count + 255) / 256;
+    const long long want = (8ll * num_sms() + rows - 1) / rows;
+    if (gx > want) gx = want;
+    const dim3 grid(static_cast<unsigned>(gx), rows);
+    range_groups_ws_kernel<true><<<grid, 256, 0, st>>>(scores, ids, pitch, counts, max_count, nd, doc_groups, G, P, w,
+                                                       out_scores, out_ids, out_counts);
+    range_groups_ws_kernel<false><<<grid, 256, 0, st>>>(scores, ids, pitch, counts, max_count, nd, doc_groups, G, P, w,
+                                                        out_scores, out_ids, out_counts);
     VR_CHECK_CUDA(cudaGetLastError());
     return 0;
 }

@@ -290,13 +290,32 @@ class KnowledgeBase:
         as CSR on the device: (offsets int64 [nq + 1], scores f32 [R], page indices int64 [R]); query i's pages are
         [offsets[i], offsets[i + 1]), by (score desc, page asc), with the exact fp32 scores (retriever.score_range).
         within / within_each: the pages searched, as in search (default: every live page); removed pages never appear."""
+        q, scope = self._range_scope(query_reps, within, within_each)
+        return retriever.score_range(q, self.index, min_score, **scope)
+
+    def search_documents_above(self, query_reps, min_score, within: Optional[Iterable[str]] = None,
+                               within_each: Optional[Sequence[Optional[Iterable[str]]]] = None
+                               ) -> Tuple[torch.Tensor, torch.Tensor, torch.Tensor, List[List[str]]]:
+        """Every document with a page scoring at least min_score (a float, or an f32 tensor [nq] on the device), each
+        scored by its best page: (offsets int64 [nq + 1], scores f32 [R], best page indices int64 [R] on the device,
+        document names [nq][*]); query i's documents are [offsets[i], offsets[i + 1]), by (score desc, best page asc) as
+        in search_documents (retriever.score_range_groups). within / within_each as in search_above: a document is
+        scored by its searched live pages only, and one whose searched pages all score below min_score is left out."""
+        q, scope = self._range_scope(query_reps, within, within_each)
+        offsets, s, p, g = retriever.score_range_groups(q, self.index, min_score, self._doc_groups, **scope)
+        groups, ends = g.tolist(), offsets.tolist()
+        names = [[self.documents[j] for j in groups[a:b]] for a, b in zip(ends[:-1], ends[1:])]
+        return offsets, s, p, names
+
+    def _range_scope(self, query_reps, within, within_each):
+        """(queries, the mask arguments of a range search over the scopes' live pages)."""
         if within_each is not None:
             q, keys, scope_of, _ = self._query_and_scopes(query_reps, within, within_each)
             if q.shape[0] == 0:
-                return retriever.score_range(q, self.index, min_score)
-            return retriever.score_range(q, self.index, min_score, doc_mask=self._scope_masks(keys), mask_of=scope_of)
+                return q, {}
+            return q, dict(doc_mask=self._scope_masks(keys), mask_of=scope_of)
         q, mask, _ = self._query_and_mask(query_reps, within)
-        return retriever.score_range(q, self.index, min_score, doc_mask=mask)
+        return q, dict(doc_mask=mask)
 
     NEAR_DUPLICATE_ROWS = 8192  # pages scored as queries per pass of near_duplicates
 

@@ -18,7 +18,9 @@ Candidate lists (`doc_lists=(offsets, ids)`, CSR, with `list_of`): each query sc
 no others; the result equals the masked call with a mask of exactly the listed pages, bit for bit.
 
 Document-level retrieval (`score_topk_groups`, `sharded_topk_groups`): `doc_groups` (int [nd]) gives every doc (page) its
-group (document); the top-k groups by their best page's exact fp32 score, ranked by (score desc, best page asc).
+group (document); the top-k groups by their best page's exact fp32 score, ranked by (score desc, best page asc). For
+300 < k <= 1024 they take the deep route over a sample of documents. `score_range_groups`: every document whose best
+page scores at least a threshold, in the same order (DESIGN §4).
 
 Per-document caps (`score_topk_capped`, `score_topk_groups_pages`, `group_pages_topm` and the sharded forms): k pages with
 at most m from any document, or the top-k documents each with its m best pages, with the bits of the fp32 scan (DESIGN §4).
@@ -460,8 +462,8 @@ def _score_topk(q: torch.Tensor, index: CorpusIndex, k: int, id_offset: int, for
         if stats is not None:
             stats.update(path="exact", flagged=0)
         return exact(q, masks)
-    if gt is None and not page_lists and DEEP_K_MIN < k <= DEEP_K_MAX:
-        return _deep_topk(q, index, k, id_offset, stats, masks)
+    if not page_lists and DEEP_K_MIN < k <= DEEP_K_MAX:
+        return _deep_topk(q, index, k, id_offset, stats, masks, gt)
     lib = L.lib()
     ranges = lib.vr_score_ranges(nq, nd)
     lists = ranges * 2 * lib.vr_score_list_len()
@@ -501,8 +503,8 @@ def _score_topk(q: torch.Tensor, index: CorpusIndex, k: int, id_offset: int, for
     if bad.numel() > 0:
         # each flagged row reruns with its own mask; many rows at a deep k take the deep route, which is exact as well
         rows, m = q.index_select(0, bad), None if masks is None else masks.rows(bad)
-        deep = gt is None and not page_lists and SELECT_K_MIN < k <= DEEP_K_MAX and bad.numel() * nd > SMALL_PROBLEM
-        for t, fix in zip(out, _deep_topk(rows, index, k, id_offset, None, m) if deep else exact(rows, m)):
+        deep = not page_lists and SELECT_K_MIN < k <= DEEP_K_MAX and bad.numel() * nd > SMALL_PROBLEM
+        for t, fix in zip(out, _deep_topk(rows, index, k, id_offset, None, m, gt) if deep else exact(rows, m)):
             t.index_copy_(0, bad, fix)
     return out
 
@@ -846,34 +848,62 @@ def score_range(queries: torch.Tensor, index: CorpusIndex, min_score, id_offset:
         return _score_range(q, index, t, id_offset, masks, force_exact, stats, cap)
 
 
+def score_range_groups(queries: torch.Tensor, index: CorpusIndex, min_score, doc_groups: torch.Tensor, id_offset: int = 0,
+                       doc_mask: Optional[torch.Tensor] = None, mask_of: Optional[torch.Tensor] = None,
+                       force_exact: bool = False, stats: Optional[dict] = None, cap: Optional[int] = None
+                       ) -> Tuple[torch.Tensor, torch.Tensor, torch.Tensor, torch.Tensor]:
+    """Document range search: for query i, every document (doc_groups as in score_topk_groups) with at least one eligible
+    page whose exact fp32 score is >= t_i. A document's score is the maximum over all its eligible pages, with that
+    page's bits; its best page the lowest page with it. Returns CSR on the index's device: (offsets int64 [nq + 1],
+    scores f32 [R], best pages int64 [R] = local page + id_offset, groups int64 [R]); row i is [offsets[i],
+    offsets[i + 1]), ordered by (score desc, best page asc) as in score_topk_groups. min_score, doc_mask / mask_of, cap,
+    force_exact and stats as in score_range (its pages s >= t, reduced to each document's first page in that order, are
+    exactly the documents scoring >= t: DESIGN §4); stats["documents"] = R."""
+    q, masks = _queries_and_mask(queries, index, doc_mask, mask_of)
+    t = _check_min_score(min_score, q.shape[0], index.emb.device)
+    cap = _check_cap(cap)
+    with L.on_device(q.device):
+        gt = _group_table(doc_groups, index)
+        offsets, s, p = _score_range(q, index, t, id_offset, masks, force_exact, stats, cap, gt)
+        g = gt.groups.index_select(0, p - id_offset).long()
+    if stats is not None:
+        stats["documents"] = p.numel()
+    return offsets, s, p, g
+
+
 def _score_range(q: torch.Tensor, index: CorpusIndex, t: torch.Tensor, id_offset: int, masks: Optional[_MaskSet],
-                 force_exact: bool, stats: Optional[dict], cap: int):
+                 force_exact: bool, stats: Optional[dict], cap: int, gt: Optional[_GroupTable] = None):
+    """score_range, and with the group table gt the documents of score_range_groups (the same paths, each region reduced
+    to the best page of every document before it is ordered)."""
     nq, d = q.shape
     nd = index.nd
     if d != index.emb.shape[1]:
         raise ValueError("query / corpus dim mismatch")
     rows = torch.arange(nq, dtype=torch.int64)
     info = dict(path="exact", candidates=0, fallback=0, cap=cap)
+    grouping = () if gt is None else (gt,)
     if nq == 0:
         pieces = []
     elif force_exact or nq * nd <= SMALL_PROBLEM or nd < 256:
-        pieces = _range_scan(q, index, t, masks, rows, id_offset)
+        pieces = _range_scan(q, index, t, masks, rows, id_offset, *grouping)
     else:
         info["path"] = "filter+rescore"
         pieces = []
         step = max(1, min(nq, RANGE_BUDGET // cap))
         for r0 in range(0, nq, step):
             n = min(step, nq - r0)
-            pieces += _range_filter(q[r0:r0 + n], index, t[r0:r0 + n], masks, r0, rows[r0:r0 + n], cap, id_offset, info)
+            pieces += _range_filter(q[r0:r0 + n], index, t[r0:r0 + n], masks, r0, rows[r0:r0 + n], cap, id_offset, info,
+                                    *grouping)
     if stats is not None:
         stats.update(info)
     return _range_assemble(nq, pieces, q.device)
 
 
 def _range_filter(q: torch.Tensor, index: CorpusIndex, t: torch.Tensor, masks: Optional[_MaskSet], r0: int,
-                  rows: torch.Tensor, cap: int, id_offset: int, info: dict):
-    """Query rows r0 .. r0 + n of the batch through the range filter and the candidate rescoring; rows that overflowed
-    (or have no bound) rerun through the scan. Returns the CSR pieces of these rows."""
+                  rows: torch.Tensor, cap: int, id_offset: int, info: dict, gt: Optional[_GroupTable] = None):
+    """Query rows r0 .. r0 + n of the batch through the range filter and the candidate rescoring (then, with gt, the
+    reduction to documents); rows that overflowed (or have no bound) rerun through the scan. Returns the CSR pieces of
+    these rows."""
     n, d = q.shape
     dev = q.device
     counts, kept, rs, ri = _range_candidates(q, index, t, masks, r0, cap)
@@ -883,14 +913,40 @@ def _range_filter(q: torch.Tensor, index: CorpusIndex, t: torch.Tensor, masks: O
     ok = torch.nonzero(~over).flatten()
     pieces = []
     if ok.numel():
-        pieces.append(_range_sort(rs, ri, cap, kept, host[1], ok, rows, id_offset))
+        kept_host = host[1]
+        if gt is not None:  # overflowed rows kept nothing, so every row of the region can be reduced
+            rs, ri, kept = _range_groups(rs, ri, kept, n, int(kept_host.max()), gt)
+            kept_host = kept.cpu()
+        pieces.append(_range_sort(rs, ri, cap, kept, kept_host, ok, rows, id_offset))
     bad = torch.nonzero(over).flatten()
     if bad.numel():
         info["fallback"] += int(bad.numel())
         sel = bad.to(dev)
         m = None if masks is None else _MaskSet(masks.words, None if masks.of_query is None else masks.of_query[r0:r0 + n]).rows(sel)
-        pieces += _range_scan(q.index_select(0, sel), index, t.index_select(0, sel), m, rows[bad], id_offset)
+        grouping = () if gt is None else (gt,)
+        pieces += _range_scan(q.index_select(0, sel), index, t.index_select(0, sel), m, rows[bad], id_offset, *grouping)
     return pieces
+
+
+def _range_groups(rs: torch.Tensor, ri: torch.Tensor, counts: torch.Tensor, n: int, most: int, gt: _GroupTable):
+    """Rows [0, n) of the region (rs, ri [*, pitch], counts) reduced by vr_range_groups to the first entry of each
+    document in (score desc, page asc) order, with its own bits: (scores, ids, counts) of a region of the same pitch.
+    most >= every counts[r]; rows longer than the shared-memory table go in chunks that bound the workspace."""
+    pitch, dev = rs.shape[1], rs.device
+    lib, sp = L.lib(), L.stream_ptr()
+    gs = torch.empty((n, pitch), dtype=torch.float32, device=dev)
+    gi = torch.empty((n, pitch), dtype=torch.int32, device=dev)
+    gc = torch.empty(n, dtype=torch.int32, device=dev)
+    row_ws = lib.vr_range_groups_ws_bytes(1, most)
+    per = 65535 if row_ws == 0 else max(1, min(65535, RANGE_BUDGET // (row_ws // 8)))
+    ws_bytes = lib.vr_range_groups_ws_bytes(min(per, n), most) if n else 0
+    ws = torch.empty(ws_bytes // 8, dtype=torch.int64, device=dev) if ws_bytes else None
+    for r0 in range(0, n, per):
+        m = min(per, n - r0)
+        L.check(lib.vr_range_groups(rs[r0:].data_ptr(), ri[r0:].data_ptr(), pitch, counts[r0:].data_ptr(), m, most,
+                                    gt.groups.data_ptr(), gt.groups.shape[0], gt.G, L.ptr(ws), ws_bytes, gs[r0:].data_ptr(),
+                                    gi[r0:].data_ptr(), gc[r0:].data_ptr(), sp))
+    return gs, gi, gc
 
 
 def _range_candidates(q: torch.Tensor, index: CorpusIndex, t: torch.Tensor, masks: Optional[_MaskSet], r0: int, cap: int):
@@ -917,9 +973,10 @@ def _range_candidates(q: torch.Tensor, index: CorpusIndex, t: torch.Tensor, mask
 
 
 def _range_scan(q: torch.Tensor, index: CorpusIndex, t: torch.Tensor, masks: Optional[_MaskSet], rows: torch.Tensor,
-                id_offset: int):
+                id_offset: int, gt: Optional[_GroupTable] = None):
     """The fp32 scan path over query rows q (global row ids `rows`): vr_score_exact, then vr_range_rows keeps the eligible
-    columns with s >= t, in chunks of rows that bound the [rows, nd] scratch. Returns the CSR pieces."""
+    columns with s >= t (with gt: reduced to documents), in chunks of rows that bound the [rows, nd] scratch. Returns the
+    CSR pieces."""
     n, d = q.shape
     nd, dev = index.nd, q.device
     lib, sp = L.lib(), L.stream_ptr()
@@ -934,7 +991,11 @@ def _range_scan(q: torch.Tensor, index: CorpusIndex, t: torch.Tensor, masks: Opt
         L.check(lib.vr_score_exact(q[r0:].data_ptr(), m, index.emb.data_ptr(), nd, d, scratch.data_ptr(), sp))
         L.check(lib.vr_range_rows(scratch.data_ptr(), m, nd, t[r0:].data_ptr(), None if masks is None else masks.arg(r0), nd,
                                   rs.data_ptr(), ri.data_ptr(), counts.data_ptr(), sp))
-        pieces.append(_range_sort(rs, ri, nd, counts, counts[:m].cpu(), torch.arange(m), rows[r0:r0 + m], id_offset))
+        region = (rs, ri, counts, counts[:m].cpu())
+        if gt is not None:
+            gs, gi, gc = _range_groups(rs, ri, counts, m, int(region[3].max()), gt)
+            region = (gs, gi, gc, gc.cpu())
+        pieces.append(_range_sort(*region[:2], nd, *region[2:], torch.arange(m), rows[r0:r0 + m], id_offset))
     return pieces
 
 
@@ -999,42 +1060,66 @@ def _range_assemble(nq: int, pieces, device) -> Tuple[torch.Tensor, torch.Tensor
 # ------------------------------------------------------------------------------------------------------
 # Deep top-k: a sampled threshold on the range filter (DESIGN §4, "Deep top-k")
 # ------------------------------------------------------------------------------------------------------
-def _sample_masks(masks: Optional[_MaskSet], nd: int, stride: int) -> Optional[_MaskSet]:
-    """The mask set over the sampled pages 0, stride, 2 stride, ... (each mask keeps its rows)."""
+def _sample_masks(masks: Optional[_MaskSet], cols: torch.Tensor) -> Optional[_MaskSet]:
+    """The mask set over the pages `cols` (int64, on the device), in that order (each mask keeps its rows)."""
     if masks is None:
         return None
-    cols = torch.arange(0, nd, stride, device=masks.words.device)
     w = masks.words.view(torch.int32).index_select(1, cols >> 5)
     bits = ((w >> (cols & 31).to(torch.int32)) & 1).bool()
     return _MaskSet(pack_doc_mask(bits), masks.of_query)
 
 
+def _sample_documents(gt: _GroupTable, stride: int) -> Tuple[torch.Tensor, torch.Tensor]:
+    """Every stride-th document by group id with all its pages, through the group CSR: (pages int64, their groups
+    renumbered as g // stride, int32)."""
+    g = torch.arange(0, gt.G, stride, device=gt.offsets.device)
+    starts = gt.offsets.index_select(0, g).long()
+    lens = gt.offsets.index_select(0, g + 1).long() - starts
+    shift = torch.repeat_interleave(starts - (torch.cumsum(lens, 0) - lens), lens)
+    cols = gt.pages.index_select(0, torch.arange(shift.numel(), device=g.device) + shift).long()
+    return cols, torch.div(gt.groups.index_select(0, cols), stride, rounding_mode="floor")
+
+
 def _deep_topk(q: torch.Tensor, index: CorpusIndex, k: int, id_offset: int, stats: Optional[dict],
-               masks: Optional[_MaskSet]):
+               masks: Optional[_MaskSet], gt: Optional[_GroupTable] = None):
     """score_topk for DEEP_K_MIN < k <= DEEP_K_MAX. Every (k // 8)-th page forms a sample; t_q = the 16th best exact score
     of query q over its eligible sampled pages. The range filter and rescoring give A = {eligible pages with exact s >=
     t_q} with the scan's bits. When |A| >= k the top-k of q is the top-k of A (its k-th score is >= t_q, and every page
     ranked above it has s >= t_q). Rows with |A| < k, rows that overflowed RANGE_CAP and rows
     whose sample holds fewer than 16 eligible pages rerun through the fp32 scan. A poor threshold costs time, never bits.
-    The first k of A come from vr_select_rows over the rescored region."""
+    The first k of A come from vr_select_rows over the rescored region.
+    Documents (gt, the group table): the sample is every (k // 8)-th document by group id with all its pages, t_q the
+    16th document score of that sample, and A is reduced to the best page of each document (vr_range_groups) before the
+    select; a row is answered when A holds at least k distinct documents (DESIGN §4)."""
     nq, d = q.shape
     nd, dev = index.nd, q.device
     ev = _Stages(stats)
     stride = max(1, k // 8)
-    sample = CorpusIndex(index.emb[::stride].contiguous(), index.emb_f16[::stride].contiguous(), index.max_norm)
-    ss, si = _score_topk(q, sample, DEEP_SAMPLE_RANK, 0, False, None, _sample_masks(masks, nd, stride))
-    t = ss[:, DEEP_SAMPLE_RANK - 1].contiguous()
-    short = si[:, DEEP_SAMPLE_RANK - 1] < 0
-    del sample, ss, si
+    if gt is None:
+        cols, sample_groups = torch.arange(0, nd, stride, device=dev), None
+    else:
+        cols, sample_groups = _sample_documents(gt, stride)
+    if cols.numel():
+        sample = CorpusIndex(index.emb.index_select(0, cols), index.emb_f16.index_select(0, cols), index.max_norm)
+        sample_gt = None if gt is None else _group_table(sample_groups, sample)
+        res = _score_topk(q, sample, DEEP_SAMPLE_RANK, 0, False, None, _sample_masks(masks, cols), sample_gt)
+        t = res[0][:, DEEP_SAMPLE_RANK - 1].contiguous()
+        short = res[1][:, DEEP_SAMPLE_RANK - 1] < 0
+        del sample, sample_gt, res
+    else:  # no sampled document has a page: every row reruns through the scan
+        t = torch.full((nq,), float("inf"), dtype=torch.float32, device=dev)
+        short = torch.ones(nq, dtype=torch.bool, device=dev)
     ev.mark("sample")
-    out_s = torch.empty((nq, k), dtype=torch.float32, device=dev)
-    out_i = torch.empty((nq, k), dtype=torch.int64, device=dev)
+    dtypes = (torch.float32, torch.int64) if gt is None else (torch.float32, torch.int64, torch.int64)
+    out = tuple(torch.empty((nq, k), dtype=dt, device=dev) for dt in dtypes)
     info = dict(path="deep", flagged=0, sample_stride=stride, candidates=0, fallback=0)
     bad = [torch.nonzero(short).flatten().cpu()]
     step = max(1, min(nq, RANGE_BUDGET // RANGE_CAP))
     for r0 in range(0, nq, step):
         n = min(step, nq - r0)
         counts, kept, rs, ri = _range_candidates(q[r0:r0 + n], index, t[r0:r0 + n], masks, r0, RANGE_CAP)
+        if gt is not None:  # A reduced to documents (overflowed rows kept nothing)
+            rs, ri, kept = _range_groups(rs, ri, kept, n, int(kept.max()), gt)
         host = torch.stack([counts, kept, short[r0:r0 + n].to(torch.int32)]).cpu()
         ev.mark("range")
         over = host[0] > RANGE_CAP
@@ -1051,18 +1136,23 @@ def _deep_topk(q: torch.Tensor, index: CorpusIndex, k: int, id_offset: int, stat
             pi = torch.empty((m, k), dtype=torch.int64, device=dev)
             L.check(L.lib().vr_select_rows(sc.data_ptr(), ids.data_ptr(), m, RANGE_CAP, k, id_offset, ps.data_ptr(),
                                            pi.data_ptr(), L.stream_ptr()))
-            out_s[sel + r0], out_i[sel + r0] = ps, pi
+            out[0][sel + r0], out[1][sel + r0] = ps, pi
+            if gt is not None:
+                out[2][sel + r0] = torch.where(pi >= 0, gt.groups.index_select(0, (pi - id_offset).clamp(min=0).flatten())
+                                               .view(m, k).long(), -1)
         ev.mark("pick")
     bad = torch.cat(bad)
     if bad.numel():
         info["fallback"] = int(bad.numel())
         sel = bad.to(dev)
-        fs, fi = _exact_topk(q.index_select(0, sel), index, k, id_offset, None if masks is None else masks.rows(sel))
-        out_s[sel], out_i[sel] = fs, fi
+        rows, m = q.index_select(0, sel), None if masks is None else masks.rows(sel)
+        fix = _exact_topk(rows, index, k, id_offset, m) if gt is None else _exact_topk_groups(rows, index, k, id_offset, m, gt)
+        for o, f in zip(out, fix):
+            o[sel] = f
         ev.mark("fallback")
     if stats is not None:
         stats.update(info)
-    return out_s, out_i
+    return out
 
 
 # ------------------------------------------------------------------------------------------------------
