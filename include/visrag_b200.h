@@ -568,6 +568,50 @@ int vr_group_pages_topm(const float* q_f32, int32_t nq, const float* d_f32, int6
                         const vr_doc_masks* masks, int32_t m, int32_t piece, int32_t pieces, int64_t id_offset,
                         float* out_scores, int64_t* out_pages, void* stream);
 
+/* Hybrid retrieval (DESIGN §4, "Hybrid retrieval"): the dense score fused with an external score v >= 0 per (query, page),
+ * e.g. BM25 over the pages' OCR text. A hit list is CSR over query rows: row r's hits are hit_ids (local pages, distinct
+ * within a row) / hit_values [hit_offsets[r], hit_offsets[r + 1]), hit_offsets int64 [rows + 1].
+ *
+ * vr_fuse_rows: the candidate row of each query, ready for vr_select_rows / vr_topk_rows (which give the (score desc,
+ * id asc) order and the k cut). dense_scores / dense_ids [rows, kd] are the dense top-kd of each row in (score desc,
+ * id asc) order as vr_select_rows writes it (local ids, a (-inf, -1) tail allowed). Row r of out_scores / out_ids
+ * [rows, width] holds slots [0, kd) the dense entries whose page is not a hit of row r ((-inf, -1) for the others), slot
+ * kd + i hit i, then (-inf, -1). mode VR_FUSE_SUM: hit i scores fl(hit_dense[r * hit_pitch + i] + fl(weight * v)), with
+ * hit_dense the hits' exact dense scores (vr_score_lists' out_scores, hit i at column i), and a dense entry keeps its
+ * score; the top-k of the row is the exact top-k of the fused score over the whole index when kd >= k (every listed page
+ * scores at least its dense score). mode VR_FUSE_RRF: reciprocal rank fusion, fl(1/fl(c + rank_dense) + 1/fl(c + rank_ext))
+ * with c = rrf_c, rank_dense = slot + 1 in the dense window and rank_ext = i + 1 (the caller orders each row's hits by
+ * (value desc, id asc)); a missing rank contributes 0; hit_values and hit_dense are not read (may be NULL). The dense
+ * entries are hashed in shared memory (2^m >= 2 kd slots), so any hit list length takes the same path. A row with more
+ * than width - kd hits keeps its first width - kd and ORs 1 into *status. Repeated hits, negative or non-finite values
+ * are the caller's to refuse (visrag_b200.retriever.score_topk_hybrid does, on the host). No allocation and no
+ * synchronisation.
+ * Refused before any CUDA call, naming the argument: a NULL or misaligned pointer, a mode other than VR_FUSE_SUM /
+ * VR_FUSE_RRF, rows < 1, kd outside [1, 4096], width outside [kd, 2^31), hit_pitch < 1 (SUM), weight negative, NaN or
+ * infinite (SUM), rrf_c < 0 (RRF).
+ * Alignment (bytes) of the vr_fuse_rows arguments: dense_scores 4, dense_ids 8, hit_offsets 8, hit_ids 4, hit_values 4,
+ * hit_dense 4, out_scores 4, out_ids 8, status 4
+ *
+ * vr_group_pages_fused: the document form. vr_group_pages_topm with m = 1 (same traversal, same arguments, same output
+ * layout [nq, kg, pieces, 1]) where an eligible page p that is a hit of row r is ranked by fl(s + fl(weight * v)): each
+ * (row, slot, piece) gets its best page by fused score (score desc, page asc). Row r's hits must be sorted by id (each
+ * page is looked up by a binary search). Reducing the pieces with vr_topk_rows (k = 1) gives each document's fused score
+ * and best page. Refused before any CUDA call as vr_group_pages_topm, plus NULL or misaligned hit pointers and a weight
+ * that is negative, NaN or infinite.
+ * Alignment (bytes) of the vr_group_pages_fused arguments: q_f32 4, d_f32 16, groups 8, group_offsets 4, group_pages 4,
+ * hit_offsets 8, hit_ids 4, hit_values 4, out_scores 4, out_pages 8 */
+#define VR_FUSE_SUM 0
+#define VR_FUSE_RRF 1
+int vr_fuse_rows(const float* dense_scores, const int64_t* dense_ids, int32_t rows, int32_t kd, const int64_t* hit_offsets,
+                 const int32_t* hit_ids, const float* hit_values, const float* hit_dense, int64_t hit_pitch, int32_t mode,
+                 float weight, int32_t rrf_c, int64_t width, float* out_scores, int64_t* out_ids, int32_t* status,
+                 void* stream);
+int vr_group_pages_fused(const float* q_f32, int32_t nq, const float* d_f32, int64_t nd, int32_t dim, const int64_t* groups,
+                         int32_t kg, const int32_t* group_offsets, const int32_t* group_pages, int32_t G,
+                         const vr_doc_masks* masks, const int64_t* hit_offsets, const int32_t* hit_ids,
+                         const float* hit_values, float weight, int32_t piece, int32_t pieces, int64_t id_offset,
+                         float* out_scores, int64_t* out_pages, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

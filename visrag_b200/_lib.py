@@ -79,6 +79,7 @@ class DocLists(C.Structure):
 
 VR_ATTN_V_ONES_COLUMN = 1
 VR_ATTN_F16 = 2  # q / k / v / out are fp16
+VR_FUSE_SUM, VR_FUSE_RRF = 0, 1  # vr_fuse_rows modes
 
 _lib: Optional[C.CDLL] = None
 
@@ -192,6 +193,11 @@ def _declare(lib: C.CDLL) -> None:
     lib.vr_mmr_select.argtypes = [vp, i64, i32, vp, vp, i32, i32, vp, i32, i64, vp, vp, vp]
     lib.vr_group_pages_topm.restype = i32
     lib.vr_group_pages_topm.argtypes = [vp, i32, vp, i64, i32, vp, i32, vp, vp, i32, dm, i32, i32, i32, i64, vp, vp, vp]
+    lib.vr_fuse_rows.restype = i32
+    lib.vr_fuse_rows.argtypes = [vp, vp, i32, i32, vp, vp, vp, vp, i64, i32, f32, i32, i64, vp, vp, vp, vp]
+    lib.vr_group_pages_fused.restype = i32
+    lib.vr_group_pages_fused.argtypes = [vp, i32, vp, i64, i32, vp, i32, vp, vp, i32, dm, vp, vp, vp, f32, i32, i32, i64, vp, vp,
+                                         vp]
     lib.vr_pool_norm.restype = i32
     lib.vr_pool_norm.argtypes = [vp, i64, vp, f32, vp, i32, i32, i32, i32, vp, vp]
     lib.vr_prefix_rows.restype = i32

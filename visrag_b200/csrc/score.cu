@@ -2137,14 +2137,17 @@ constexpr int GROUP_PIECE_MAX = 4096;  // pages of one group a block scores
 // Block (row * kg + slot, piece) scores pages [piece * y, piece * (y + 1)) of group g = groups[row, slot] through the
 // CSR, one warp per page (warp_dot_row: the lane loop of exact_scores_kernel, so every score has the bits
 // vr_score_exact gives that pair), with the query row in shared memory. An ineligible page is never read and counts as
-// NaN, which is never selected. Page keys are distinct, so each entry's rank in (score desc, page asc) order is the
-// number of entries before it: the entries of rank < m go straight to their slot, and the rest of the m slots get
-// (-inf, -1). A group outside [0, G) is empty: padding, and nothing is read.
-__global__ void __launch_bounds__(256)
-group_pages_topm_kernel(const float* __restrict__ Q, const float* __restrict__ D, int dim, const long long* __restrict__ groups,
-                        int kg, const int* __restrict__ offsets, const int* __restrict__ pages, int G, const DocMasks masks,
-                        int m, int piece, long long id_offset, float* __restrict__ out_scores,
-                        long long* __restrict__ out_pages) {
+// NaN, which is never selected. fuse(row, page, s) turns each eligible page's score into the score it is ranked by
+// (NoFuse: s itself). Page keys are distinct, so each entry's rank in (score desc, page asc) order is the number of
+// entries before it: the entries of rank < m go straight to their slot, and the rest of the m slots get (-inf, -1). A
+// group outside [0, G) is empty: padding, and nothing is read. The body of group_pages_topm_kernel and
+// group_pages_fused_kernel.
+template <class Fuse>
+__device__ __forceinline__ void group_pages_block(const float* __restrict__ Q, const float* __restrict__ D, int dim,
+                                                  const long long* __restrict__ groups, int kg, const int* __restrict__ offsets,
+                                                  const int* __restrict__ pages, int G, const DocMasks& masks, int m,
+                                                  int piece, long long id_offset, const Fuse& fuse,
+                                                  float* __restrict__ out_scores, long long* __restrict__ out_pages) {
     extern __shared__ float gsm[];  // [dim] query row, then [piece] scores and [piece] pages
     float* qs = gsm;
     float* ps = gsm + dim;
@@ -2171,8 +2174,9 @@ group_pages_topm_kernel(const float* __restrict__ Q, const float* __restrict__ D
     const uint32_t* mask = masks.words ? mask_of_row(masks, row) : nullptr;
     for (int j = warp; j < n; j += warps) {
         const int p = __ldg(pages + lo + j);
-        const float s = !mask || col_eligible(mask, p) ? warp_dot_row(qs, D + static_cast<long long>(p) * dim, dim, lane) : NAN;
-        if (lane == 0) { ps[j] = s; pp[j] = p; }
+        const bool eligible = !mask || col_eligible(mask, p);
+        const float s = eligible ? warp_dot_row(qs, D + static_cast<long long>(p) * dim, dim, lane) : NAN;
+        if (lane == 0) { ps[j] = eligible ? fuse(row, p, s) : s; pp[j] = p; }
     }
     __syncthreads();
     int valid = 0;
@@ -2194,6 +2198,127 @@ group_pages_topm_kernel(const float* __restrict__ Q, const float* __restrict__ D
     for (int t = min(valid, m) + threadIdx.x; t < m; t += blockDim.x) {
         out_scores[o + t] = -INFINITY;
         out_pages[o + t] = -1;
+    }
+}
+
+struct NoFuse {
+    __device__ __forceinline__ float operator()(long long, int, float s) const { return s; }
+};
+
+__global__ void __launch_bounds__(256)
+group_pages_topm_kernel(const float* __restrict__ Q, const float* __restrict__ D, int dim, const long long* __restrict__ groups,
+                        int kg, const int* __restrict__ offsets, const int* __restrict__ pages, int G, const DocMasks masks,
+                        int m, int piece, long long id_offset, float* __restrict__ out_scores,
+                        long long* __restrict__ out_pages) {
+    group_pages_block(Q, D, dim, groups, kg, offsets, pages, G, masks, m, piece, id_offset, NoFuse{}, out_scores, out_pages);
+}
+
+// ---------------------------------------------------------------------------------------------
+// Hybrid retrieval: the dense score fused with an external score per (query, page) (DESIGN §4, "Hybrid retrieval").
+// A hit list is CSR over query rows: row r's hits are ids / values [offsets[r], offsets[r + 1]).
+// ---------------------------------------------------------------------------------------------
+constexpr int FUSE_DENSE_MAX = 4096;  // dense entries per row vr_fuse_rows hashes (k of score_topk, or the RRF window)
+constexpr int FUSE_THREADS = 256;
+
+// The weighted sum with the two roundings of fp32 torch, fl(s + fl(w * v)): no contraction into an FMA.
+__device__ __forceinline__ float fuse_sum(float s, float w, float v) { return __fadd_rn(s, __fmul_rn(w, v)); }
+
+// The RRF term of a rank (from 1): fl(1 / fl(c + rank)), rounded to nearest.
+__device__ __forceinline__ float rrf_term(int c, long long rank) {
+    return __frcp_rn(static_cast<float>(static_cast<long long>(c) + rank));
+}
+
+// The weighted-sum fusion of vr_group_pages_fused: row r's hits sorted by id, looked up by a binary search.
+struct HitsFuse {
+    const long long* offsets;
+    const int* ids;
+    const float* values;
+    float w;
+    __device__ __forceinline__ float operator()(long long row, int p, float s) const {
+        long long a = __ldg(offsets + row), b = __ldg(offsets + row + 1);
+        while (a < b) {
+            const long long mid = (a + b) >> 1;
+            if (__ldg(ids + mid) < p) a = mid + 1;
+            else b = mid;
+        }
+        return a < __ldg(offsets + row + 1) && __ldg(ids + a) == p ? fuse_sum(s, w, __ldg(values + a)) : s;
+    }
+};
+
+__global__ void __launch_bounds__(256)
+group_pages_fused_kernel(const float* __restrict__ Q, const float* __restrict__ D, int dim, const long long* __restrict__ groups,
+                         int kg, const int* __restrict__ offsets, const int* __restrict__ pages, int G, const DocMasks masks,
+                         const HitsFuse fuse, int piece, long long id_offset, float* __restrict__ out_scores,
+                         long long* __restrict__ out_pages) {
+    group_pages_block(Q, D, dim, groups, kg, offsets, pages, G, masks, 1, piece, id_offset, fuse, out_scores, out_pages);
+}
+
+// One block per query row. The row's dense entries (ids distinct, a negative id is empty) go into an open-addressing
+// hash of P = 2^m >= 2 kd slots in shared memory (id -> slot; load <= 1/2), so the table fits whatever the length of the
+// hit list. Each hit probes it: a hit whose page is a dense entry retires that entry and carries both scores. Output
+// row r of [rows, width]: slots [0, kd) the dense entries that are not hits, then slot kd + i for hit i, then (-inf, -1).
+// SUM: a hit scores fuse_sum(dense, w, v), a dense entry its own score. RRF: the dense rank of slot j is j + 1 and the
+// external rank of hit i is i + 1 (the caller orders each row by (value desc, id asc)); a score is
+// fl(rrf_term(dense rank) + rrf_term(external rank)), a missing rank contributing 0.
+__global__ void __launch_bounds__(FUSE_THREADS)
+fuse_rows_kernel(const float* __restrict__ dense_scores, const long long* __restrict__ dense_ids, int kd,
+                 const long long* __restrict__ hit_offsets, const int* __restrict__ hit_ids,
+                 const float* __restrict__ hit_values, const float* __restrict__ hit_dense, long long hit_pitch, bool rrf,
+                 float w, int c, long long width, int P, float* __restrict__ out_scores, long long* __restrict__ out_ids,
+                 int* __restrict__ status) {
+    extern __shared__ int fsm[];  // [P] keys (page id, -1 empty), [P] dense slot, [kd] retired flags
+    int* tk = fsm;
+    int* tj = fsm + P;
+    int* gone = fsm + 2 * P;
+    const long long r = blockIdx.x;
+    const uint32_t mask = static_cast<uint32_t>(P - 1);
+    for (int i = threadIdx.x; i < P; i += blockDim.x) tk[i] = -1;
+    for (int j = threadIdx.x; j < kd; j += blockDim.x) gone[j] = 0;
+    __syncthreads();
+    const long long* di = dense_ids + r * kd;
+    for (int j = threadIdx.x; j < kd; j += blockDim.x) {
+        const long long id = di[j];
+        if (id < 0 || id > 0x7fffffffll) continue;
+        const int key = static_cast<int>(id);
+        for (uint32_t h = rgroup_hash(static_cast<uint32_t>(key)) & mask;; h = (h + 1) & mask) {
+            const int prev = atomicCAS(tk + h, -1, key);
+            if (prev == -1) { tj[h] = j; break; }
+            if (prev == key) break;  // a repeated dense id keeps its first slot
+        }
+    }
+    __syncthreads();
+    const long long off = __ldg(hit_offsets + r);
+    const long long len = __ldg(hit_offsets + r + 1) - off;
+    const long long n = min(len, width - kd);
+    if (len > n && threadIdx.x == 0) atomicOr(status, 1);
+    float* os = out_scores + r * width;
+    long long* oi = out_ids + r * width;
+    for (long long i = threadIdx.x; i < n; i += blockDim.x) {
+        const int p = __ldg(hit_ids + off + i);
+        int j = -1;
+        for (uint32_t h = rgroup_hash(static_cast<uint32_t>(p)) & mask;; h = (h + 1) & mask) {
+            const int key = tk[h];
+            if (key == -1) break;
+            if (key == p) { j = tj[h]; break; }
+        }
+        if (j >= 0) gone[j] = 1;
+        float s;
+        if (rrf) s = __fadd_rn(j >= 0 ? rrf_term(c, j + 1) : 0.f, rrf_term(c, i + 1));
+        else s = fuse_sum(__ldg(hit_dense + r * hit_pitch + i), w, __ldg(hit_values + off + i));
+        os[kd + i] = s;
+        oi[kd + i] = p;
+    }
+    __syncthreads();
+    const float* ds = dense_scores + r * kd;
+    for (int j = threadIdx.x; j < kd; j += blockDim.x) {
+        const long long id = di[j];
+        const bool live = id >= 0 && !gone[j];
+        os[j] = live ? (rrf ? rrf_term(c, j + 1) : ds[j]) : -INFINITY;
+        oi[j] = live ? id : -1;
+    }
+    for (long long t = kd + n + threadIdx.x; t < width; t += blockDim.x) {
+        os[t] = -INFINITY;
+        oi[t] = -1;
     }
 }
 
@@ -2998,6 +3123,90 @@ extern "C" int vr_group_pages_topm(const float* q_f32, int32_t nq, const float* 
     group_pages_topm_kernel<<<dim3(static_cast<unsigned>(nq * kg), static_cast<unsigned>(pieces)), threads, smem,
                               reinterpret_cast<cudaStream_t>(stream)>>>(
         q_f32, d_f32, dim, reinterpret_cast<const long long*>(groups), kg, group_offsets, group_pages, G, dm, m, piece,
+        static_cast<long long>(id_offset), out_scores, reinterpret_cast<long long*>(out_pages));
+    VR_CHECK_CUDA(cudaGetLastError());
+    return 0;
+}
+
+// ---------------------------------------------------------------------------------------------------- hybrid retrieval
+extern "C" int vr_fuse_rows(const float* dense_scores, const int64_t* dense_ids, int32_t rows, int32_t kd,
+                            const int64_t* hit_offsets, const int32_t* hit_ids, const float* hit_values,
+                            const float* hit_dense, int64_t hit_pitch, int32_t mode, float weight, int32_t rrf_c,
+                            int64_t width, float* out_scores, int64_t* out_ids, int32_t* status, void* stream) {
+    const char* fn = "vr_fuse_rows";
+    VR_REQUIRE(mode == VR_FUSE_SUM || mode == VR_FUSE_RRF, "%s: mode=%d, needs VR_FUSE_SUM (0) or VR_FUSE_RRF (1)", fn, mode);
+    const bool rrf = mode == VR_FUSE_RRF;
+    VR_REQUIRE_PTR(fn, "dense_scores", dense_scores, 4);
+    VR_REQUIRE_PTR(fn, "dense_ids", dense_ids, 8);
+    VR_REQUIRE_PTR(fn, "hit_offsets", hit_offsets, 8);
+    VR_REQUIRE_PTR(fn, "hit_ids", hit_ids, 4);
+    if (!rrf) {  // RRF reads neither the values nor the dense scores of the hits, only their order
+        VR_REQUIRE_PTR(fn, "hit_values", hit_values, 4);
+        VR_REQUIRE_PTR(fn, "hit_dense", hit_dense, 4);
+    }
+    VR_REQUIRE_PTR(fn, "out_scores", out_scores, 4);
+    VR_REQUIRE_PTR(fn, "out_ids", out_ids, 8);
+    VR_REQUIRE_PTR(fn, "status", status, 4);
+    VR_REQUIRE(rows >= 1, "%s: rows=%d, needs at least 1", fn, rows);
+    VR_REQUIRE(kd >= 1 && kd <= FUSE_DENSE_MAX, "%s: kd=%d, needs 1 <= kd <= %d", fn, kd, FUSE_DENSE_MAX);
+    VR_REQUIRE(width >= kd && width < 2147483647ll, "%s: width=%lld, needs kd=%d <= width < 2^31", fn, (long long)width, kd);
+    VR_REQUIRE(rrf || hit_pitch >= 1, "%s: hit_pitch=%lld, needs at least 1", fn, (long long)hit_pitch);
+    VR_REQUIRE(rrf || (weight >= 0.f && weight <= 3.4028234663852886e38f),
+               "%s: weight=%g, needs a finite weight >= 0", fn, static_cast<double>(weight));
+    VR_REQUIRE(!rrf || rrf_c >= 0, "%s: rrf_c=%d, needs rrf_c >= 0", fn, rrf_c);
+    int P = 2;
+    while (P < 2 * kd) P <<= 1;
+    const size_t smem = (2 * static_cast<size_t>(P) + kd) * sizeof(int);
+    static unsigned long long attr_set = 0;
+    if (smem > 48 * 1024 && first_use_on_device(&attr_set))
+        VR_CHECK_CUDA(cudaFuncSetAttribute(fuse_rows_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 80 * 1024));
+    fuse_rows_kernel<<<rows, FUSE_THREADS, smem, reinterpret_cast<cudaStream_t>(stream)>>>(
+        dense_scores, reinterpret_cast<const long long*>(dense_ids), kd, reinterpret_cast<const long long*>(hit_offsets),
+        hit_ids, hit_values, hit_dense, static_cast<long long>(hit_pitch), rrf, weight, rrf_c, static_cast<long long>(width), P,
+        out_scores, reinterpret_cast<long long*>(out_ids), status);
+    VR_CHECK_CUDA(cudaGetLastError());
+    return 0;
+}
+
+extern "C" int vr_group_pages_fused(const float* q_f32, int32_t nq, const float* d_f32, int64_t nd, int32_t dim,
+                                    const int64_t* groups, int32_t kg, const int32_t* group_offsets,
+                                    const int32_t* group_pages, int32_t G, const vr_doc_masks* masks,
+                                    const int64_t* hit_offsets, const int32_t* hit_ids, const float* hit_values, float weight,
+                                    int32_t piece, int32_t pieces, int64_t id_offset, float* out_scores, int64_t* out_pages,
+                                    void* stream) {
+    const char* fn = "vr_group_pages_fused";
+    if (masks) VR_REQUIRE_MASKS(fn, masks, nd);
+    VR_REQUIRE_PTR(fn, "q_f32", q_f32, 4);
+    VR_REQUIRE_PTR(fn, "d_f32", d_f32, 16);  // float4 rows (dim % 4 == 0 keeps every row aligned)
+    VR_REQUIRE_PTR(fn, "groups", groups, 8);
+    VR_REQUIRE_PTR(fn, "group_offsets", group_offsets, 4);
+    VR_REQUIRE_PTR(fn, "group_pages", group_pages, 4);
+    VR_REQUIRE_PTR(fn, "hit_offsets", hit_offsets, 8);
+    VR_REQUIRE_PTR(fn, "hit_ids", hit_ids, 4);
+    VR_REQUIRE_PTR(fn, "hit_values", hit_values, 4);
+    VR_REQUIRE_PTR(fn, "out_scores", out_scores, 4);
+    VR_REQUIRE_PTR(fn, "out_pages", out_pages, 8);
+    VR_REQUIRE(nq > 0, "%s: nq=%d, needs at least 1", fn, nq);
+    VR_REQUIRE(nd > 0 && nd < 2147483647ll, "%s: nd=%lld beyond the int32 doc ids", fn, (long long)nd);
+    VR_REQUIRE(dim > 0 && dim % 4 == 0, "%s: dim=%d, needs a positive multiple of 4", fn, dim);
+    VR_REQUIRE(kg >= 1, "%s: kg=%d, needs at least 1", fn, kg);
+    VR_REQUIRE(static_cast<long long>(nq) * kg < 2147483647ll, "%s: nq=%d x kg=%d rows, needs fewer than 2^31", fn, nq, kg);
+    VR_REQUIRE(G >= 1, "%s: G=%d, needs at least 1", fn, G);
+    VR_REQUIRE(weight >= 0.f && weight <= 3.4028234663852886e38f, "%s: weight=%g, needs a finite weight >= 0", fn,
+               static_cast<double>(weight));
+    VR_REQUIRE(piece >= 1 && piece <= GROUP_PIECE_MAX, "%s: piece=%d, needs 1 <= piece <= %d", fn, piece, GROUP_PIECE_MAX);
+    VR_REQUIRE(pieces >= 1 && pieces <= 65535, "%s: pieces=%d, needs 1 <= pieces <= 65535", fn, pieces);
+    const size_t smem = static_cast<size_t>(dim) * sizeof(float) + static_cast<size_t>(piece) * 8;
+    VR_REQUIRE(smem <= 200 * 1024, "%s: dim=%d with piece=%d too large for shared memory", fn, dim, piece);
+    static unsigned long long attr_set = 0;
+    if (smem > 48 * 1024 && first_use_on_device(&attr_set))
+        VR_CHECK_CUDA(cudaFuncSetAttribute(group_pages_fused_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
+    const int threads = 32 * (piece < 8 ? piece : 8);  // a warp per page, as vr_group_pages_topm
+    const DocMasks dm = masks ? device_masks(masks) : kNoMasks;
+    const HitsFuse fuse = {reinterpret_cast<const long long*>(hit_offsets), hit_ids, hit_values, weight};
+    group_pages_fused_kernel<<<dim3(static_cast<unsigned>(nq * kg), static_cast<unsigned>(pieces)), threads, smem,
+                               reinterpret_cast<cudaStream_t>(stream)>>>(
+        q_f32, d_f32, dim, reinterpret_cast<const long long*>(groups), kg, group_offsets, group_pages, G, dm, fuse, piece,
         static_cast<long long>(id_offset), out_scores, reinterpret_cast<long long*>(out_pages));
     VR_CHECK_CUDA(cudaGetLastError());
     return 0;

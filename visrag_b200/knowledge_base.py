@@ -20,7 +20,8 @@ Documents: `build_index.py` stores page i of `report.pdf` as `report.pdf_i.png`,
 the last `_` when the rest is `<digits>.png` (any other filename is its own document). `search_documents` returns the
 top-k documents by their best page (`retriever.score_topk_groups`), so one long document cannot fill every slot.
 `search(…, per_document=m)` caps the pages of any one document at m, and `search_document_pages` returns the top-k
-documents each with its m best pages. `search_diverse` / `retrieve_diverse` pick pages by maximal marginal relevance (`retriever.mmr_select`), so near-copies
+documents each with its m best pages. `search_hybrid` / `search_documents_hybrid` fuse the dense score with another
+retriever's score of each page (e.g. BM25 over OCR text). `search_diverse` / `retrieve_diverse` pick pages by maximal marginal relevance (`retriever.mmr_select`), so near-copies
 of one page, in one document or several, do not fill every slot either.
 """
 from __future__ import annotations
@@ -408,6 +409,68 @@ class KnowledgeBase:
         """Full `retrieve(knowledge_base_path, query, topk)`: instruction + query -> embedding (B2 wrapper) -> top-k."""
         out = model(query={"text": [DEMO_QUERY_PREFIX + query], "image": [None]}, tokenizer=tokenizer)
         return self.retrieve(out.q_reps, topk, within, per_document)
+
+    def _hits(self, hits: Sequence[dict], nq: int) -> Tuple[torch.Tensor, torch.Tensor, torch.Tensor]:
+        """One {filename: external score} mapping per query -> the retriever's hit CSR (offsets, page rows, values) on
+        the device. Unknown and removed filenames are dropped."""
+        hits = list(hits)
+        if len(hits) != nq:
+            raise ValueError(f"hits has {len(hits)} entries for {nq} queries (one {{filename: score}} mapping per query)")
+        rows, vals, offsets = [], [], [0]
+        for h in hits:
+            live = [(self._row[f], v) for f, v in h.items() if f in self._row]
+            rows.extend(r for r, _ in live)
+            vals.extend(v for _, v in live)
+            offsets.append(len(rows))
+        dev = self.index.emb.device
+        return (torch.tensor(offsets, dtype=torch.int64, device=dev), torch.tensor(rows, dtype=torch.int32, device=dev),
+                torch.tensor(vals, dtype=torch.float32, device=dev))
+
+    def search_hybrid(self, query_reps, topk: int, hits: Sequence[dict], weight=1.0, fusion: str = "sum",
+                      window: Optional[int] = None, within: Optional[Iterable[str]] = None,
+                      within_each: Optional[Sequence[Optional[Iterable[str]]]] = None) -> Tuple[torch.Tensor, torch.Tensor]:
+        """Hybrid top-k pages (retriever.score_topk_hybrid): the dense score fused with an external score of each page,
+        e.g. BM25 over its OCR text. hits: one {filename: score >= 0} mapping per query (unknown or removed filenames
+        are dropped; an unlisted page scores 0). fusion="sum": dense + weight * score; fusion="rrf": reciprocal rank
+        fusion of the dense top-`window` (default k) and the hits ranked by score. Returns (fused scores [nq,k] f32, page
+        indices [nq,k] i64) on the device. within / within_each and k as in search; hits outside a query's scope are
+        dropped."""
+        q, keys, scope_of, rows_of = self._scopes(query_reps, within, within_each)
+        h = self._hits(hits, q.shape[0])
+        if keys is None:
+            k = min(topk, len(self))
+        else:
+            k = min(topk, max(len(rows) for rows in rows_of)) if rows_of else 0
+        if k == 0:
+            return (torch.empty((q.shape[0], 0), dtype=torch.float32, device=q.device),
+                    torch.empty((q.shape[0], 0), dtype=torch.int64, device=q.device))
+        return retriever.score_topk_hybrid(q, self.index, k, h, weight, fusion, window,
+                                           **self._scope_args(q, keys, rows_of, scope_of, k, False))
+
+    def search_documents_hybrid(self, query_reps, topk: int, hits: Sequence[dict], weight=1.0, fusion: str = "sum",
+                                within: Optional[Iterable[str]] = None,
+                                within_each: Optional[Sequence[Optional[Iterable[str]]]] = None
+                                ) -> Tuple[torch.Tensor, torch.Tensor, List[List[str]]]:
+        """Hybrid top-k documents (retriever.score_topk_groups_hybrid): each document scored by its best page under
+        dense + weight * score, hits as in search_hybrid (weighted sum only). Returns (scores [nq,k] f32, best page
+        indices [nq,k] i64 on the device, document names [nq][k]); within / within_each and k as in search_documents."""
+        q, keys, scope_of, rows_of = self._scopes(query_reps, within, within_each)
+        h = self._hits(hits, q.shape[0])
+        k = min(topk, self._n_documents(q, keys, rows_of)) if rows_of != [] else 0
+        if k == 0:
+            return (torch.empty((q.shape[0], 0), dtype=torch.float32, device=q.device),
+                    torch.empty((q.shape[0], 0), dtype=torch.int64, device=q.device), [[] for _ in range(q.shape[0])])
+        s, p, g = retriever.score_topk_groups_hybrid(q, self.index, k, self._doc_groups, h, weight, fusion,
+                                                     **self._scope_args(q, keys, rows_of, scope_of, k, True))
+        return s, p, self._names(g)
+
+    def retrieve_hybrid_text(self, model, tokenizer, query: str, topk: int, hits: dict, weight=1.0, fusion: str = "sum",
+                             window: Optional[int] = None, within: Optional[Iterable[str]] = None) -> List[str]:
+        """retrieve_text with hybrid ranking: instruction + query -> embedding -> search_hybrid with the query's
+        {filename: score} hits -> paths of the top-k page images, best first."""
+        out = model(query={"text": [DEMO_QUERY_PREFIX + query], "image": [None]}, tokenizer=tokenizer)
+        _, ids = self.search_hybrid(out.q_reps, topk, [hits], weight, fusion, window, within)
+        return [os.path.join(self.path, self.filenames[i]) for i in ids[0].tolist() if i >= 0]
 
     def remove(self, filenames: Iterable[str]) -> None:
         """Mark pages dead: no search returns them again. The other pages keep their indices, and the index's max row norm

@@ -27,6 +27,9 @@ at most m from any document, or the top-k documents each with its m best pages, 
 
 Diverse retrieval (`score_mmr`, `mmr_select`): maximal marginal relevance over each query's top fetch_k pages, picked
 on the GPU (vr_mmr_select) with the bits fixed by the definition in DESIGN §4.
+
+Hybrid retrieval (`score_topk_hybrid`, `score_topk_groups_hybrid`): the dense score fused with an external score per
+page (e.g. BM25 over OCR text), by weighted sum or reciprocal rank fusion, exactly over the whole index (DESIGN §4).
 """
 from __future__ import annotations
 
@@ -1284,6 +1287,298 @@ def score_mmr(queries: torch.Tensor, index: CorpusIndex, k: int, lambda_mult=0.5
         ev.mark("select")
     if stats is not None:
         stats["fetch_k"] = fetch
+    return out
+
+
+# ------------------------------------------------------------------------------------------------------
+# Hybrid retrieval: the dense score fused with an external score (DESIGN §4, "Hybrid retrieval")
+# ------------------------------------------------------------------------------------------------------
+FUSIONS = {"sum": L.VR_FUSE_SUM, "rrf": L.VR_FUSE_RRF}
+FUSE_K_MAX = 4096          # dense entries per row vr_fuse_rows takes (k of the sum, the window of RRF)
+FUSE_BUDGET = 1 << 27      # fused candidate entries per pass: query rows go in chunks
+
+
+@dataclass
+class _Hits:
+    """A validated hit list on the index's device, CSR over query rows: offsets int64 [nq + 1], ids int32 (local pages),
+    values f32, width = the longest row, n = offsets[-1] (ids / values may hold unused entries after it). Each row is in
+    (id asc) order, or (value desc, id asc) for RRF."""
+    offsets: torch.Tensor
+    ids: torch.Tensor
+    values: torch.Tensor
+    width: int
+    n: int
+
+
+def _check_weight(weight) -> float:
+    if isinstance(weight, bool) or not isinstance(weight, (int, float, np.floating, np.integer)):
+        raise ValueError(f"weight must be a float, got {type(weight).__name__}")
+    w = float(np.float32(weight))
+    if not np.isfinite(w) or w < 0:
+        raise ValueError(f"weight must be finite and >= 0 (in fp32), got {weight}")
+    return w
+
+
+def _check_fusion(fusion, k, window, rrf_c) -> Tuple[int, int, int]:
+    """(k, dense entries per row, rrf_c) of a hybrid page search."""
+    if fusion not in FUSIONS:
+        raise ValueError(f"fusion must be one of {sorted(FUSIONS)}, got {fusion!r}")
+    k = _check_count(k, "k")
+    if not 1 <= k <= FUSE_K_MAX:
+        raise ValueError(f"k={k} must lie in [1, {FUSE_K_MAX}]")
+    if fusion == "sum":
+        if window is not None:
+            raise ValueError('window is the dense window of fusion="rrf"; the weighted sum needs none')
+        return k, k, 0
+    window = k if window is None else _check_count(window, "window")
+    if not 1 <= window <= FUSE_K_MAX:
+        raise ValueError(f"window={window} must lie in [1, {FUSE_K_MAX}]")
+    rrf_c = _check_count(rrf_c, "rrf_c")
+    if not 0 <= rrf_c < 1 << 24:
+        raise ValueError(f"rrf_c={rrf_c} must lie in [0, 2^24)")
+    return k, window, rrf_c
+
+
+def _hits_in_scope(row: torch.Tensor, ids: torch.Tensor, nd: int, masks: Optional[_MaskSet], ls: Optional[_ListSet]):
+    """bool [N]: hit (row, id) lies in the scope of its query row (masks, or lists; neither: every page). ids must lie in
+    [0, nd). No host read."""
+    if masks is not None:
+        m = row.new_zeros(row.shape) if masks.of_query is None else masks.of_query.long().index_select(0, row)
+        w = masks.words.view(torch.int32)[m, ids >> 5]
+        return ((w >> (ids & 31).to(torch.int32)) & 1).bool()
+    if ls is not None:
+        # every (list, page) of the list set as a sorted key; the placeholder id of an empty set gets list M (no query's)
+        pos = torch.arange(ls.ids.shape[0], device=ids.device)
+        listed = torch.searchsorted(ls.offsets[1:], pos, right=True) * nd + ls.ids.long()
+        listed = torch.sort(listed).values
+        m = row.new_zeros(row.shape) if ls.of_query is None else ls.of_query.long().index_select(0, row)
+        key = m * nd + ids
+        at = torch.searchsorted(listed, key).clamp(max=listed.numel() - 1)
+        return listed[at] == key
+    return torch.ones_like(ids, dtype=torch.bool)
+
+
+def _check_hits(hits, nq: int, nd: int, device, masks: Optional[_MaskSet] = None, ls: Optional[_ListSet] = None,
+                rank_order: bool = False) -> _Hits:
+    """Validate hits = (offsets int [nq + 1], ids int (local pages), values f32) on `device`, drop the hits outside each
+    query's scope, and order each row by id (rank_order: by (value desc, id asc), the external ranks of RRF). One host
+    read serves every value check (offsets from 0 to len(ids) and non-decreasing, ids in [0, nd), values finite and
+    >= 0, no page twice in a row) and the sizes of the result; nothing before it can index out of bounds. A value of -0.0
+    is a zero score and becomes +0.0."""
+    if not isinstance(hits, (tuple, list)) or len(hits) != 3:
+        raise ValueError("hits must be a triple (offsets, ids, values) of tensors")
+    offsets, ids, values = hits
+    _int_tensor(offsets, "hits offsets", nq + 1, device)
+    _int_tensor(ids, "hits ids", None, device)
+    if not isinstance(values, torch.Tensor) or values.dtype != torch.float32 or values.dim() != 1:
+        raise ValueError("hits values must be a 1-D torch.float32 tensor")
+    if values.shape[0] != ids.shape[0]:
+        raise ValueError(f"hits values has {values.shape[0]} entries for {ids.shape[0]} ids")
+    if values.device != device:
+        raise ValueError(f"hits values live on {values.device}, the index on {device}")
+    offsets, ids = offsets.to(torch.int64), ids.to(torch.int64)
+    values = values + 0.0  # -0.0 -> +0.0: the sign bit would break the rank key below
+    n = ids.shape[0]
+    z = offsets.new_zeros(())
+    # the row of each entry, by search (no host read; any offsets give rows in [0, nq), checked below)
+    row = torch.searchsorted(offsets[1:], torch.arange(n, device=device), right=True).clamp(max=max(nq - 1, 0))
+    safe = ids.clamp(0, nd - 1)
+    key = row * nd + safe                       # (row, id): distinct keys unless a page repeats in a row
+    order = torch.argsort(key)
+    srt = key.index_select(0, order)
+    keep = _hits_in_scope(row, safe, nd, masks, ls)
+    counts = offsets.new_zeros(max(nq, 1)).scatter_add_(0, row, keep.long())[:nq]
+    checks = torch.stack([offsets[0], offsets[-1], (offsets[1:] - offsets[:-1]).min() if nq else z,
+                          ids.min() if n else z, ids.max() if n else z,
+                          (~torch.isfinite(values)).sum() if n else z, (values < 0).sum() if n else z,
+                          (srt[1:] == srt[:-1]).sum() if n > 1 else z, counts.max() if nq else z, counts.sum()]).tolist()
+    first, last, min_len, lo, hi, bad_values, negative, repeats, width, kept = checks
+    if first != 0:
+        raise ValueError(f"hits offsets must start at 0, got {first}")
+    if min_len < 0:
+        raise ValueError("hits offsets must be non-decreasing")
+    if last != n:
+        raise ValueError(f"hits offsets must end at len(ids) = {n}, got {last}")
+    if n and (lo < 0 or hi >= nd):
+        raise ValueError(f"hits ids must lie in [0, {nd}) (local pages of the index), got [{lo}, {hi}]")
+    if bad_values:
+        raise ValueError(f"hits values must be finite: {bad_values} are NaN or infinite")
+    if negative:
+        raise ValueError(f"hits values must be >= 0 (a negative external score needs a deeper dense top-k): {negative} are not")
+    if repeats:
+        raise ValueError(f"a page appears more than once in one query's hits ({repeats} repeats)")
+    out_off = torch.zeros(nq + 1, dtype=torch.int64, device=device)
+    out_off[1:] = torch.cumsum(counts, 0)
+    if not n:
+        return _Hits(out_off, torch.zeros(1, dtype=torch.int32, device=device),
+                     torch.zeros(1, dtype=torch.float32, device=device), 0, 0)
+    # kept entries first, by (row, id) or (row, value desc, id asc); a stable sort keeps id order within equal keys
+    outside = (~keep).long().index_select(0, order)
+    if rank_order:  # values >= 0 here: their bits order like the values
+        vkey = (outside << 62) | (row.index_select(0, order) << 31) | (0x7FFFFFFF - values.index_select(0, order).view(torch.int32).long())
+    else:
+        vkey = outside
+    order = order.index_select(0, torch.sort(vkey, stable=True).indices)
+    return _Hits(out_off, ids.index_select(0, order).to(torch.int32), values.index_select(0, order).contiguous(), width,
+                 kept)
+
+
+def score_topk_hybrid(queries: torch.Tensor, index: CorpusIndex, k: int, hits, weight=1.0, fusion: str = "sum",
+                      window: Optional[int] = None, rrf_c: int = 60, id_offset: int = 0,
+                      doc_mask: Optional[torch.Tensor] = None, mask_of: Optional[torch.Tensor] = None,
+                      doc_lists: Optional[Tuple[torch.Tensor, torch.Tensor]] = None, list_of: Optional[torch.Tensor] = None,
+                      stats: Optional[dict] = None) -> Tuple[torch.Tensor, torch.Tensor]:
+    """Exact hybrid top-k pages: (fused scores [nq, k] f32, ids [nq, k] i64 = local page + id_offset) in (fused score
+    desc, id asc) order, ending in (-inf, -1) when fewer pages have a score. hits = (offsets int [nq + 1], ids int local
+    pages, values f32 >= 0) on the index's device: query i's external scores are values[offsets[i]:offsets[i + 1]]
+    (CSR), an unlisted page having v = 0. A page may appear once per query; negative, NaN or infinite values are refused.
+    fusion="sum": fl(dense + fl(weight * v)), dense the exact fp32 score (the bits of the fp32 scan). The answer lies in
+    score_topk(k) plus the query's hits (DESIGN §4), whose dense scores come from vr_score_lists.
+    fusion="rrf": reciprocal rank fusion in fp32, fl(1/(rrf_c + rank_dense) + 1/(rrf_c + rank_ext)), ranks from 1: the
+    dense rank within score_topk(window) (default window = k, at most 4096), the external rank within the query's hits
+    by (value desc, id asc); a missing rank contributes 0 and weight is not used.
+    Scopes (doc_mask / mask_of, doc_lists / list_of, as in score_topk) apply to both sides: a hit outside its query's
+    scope is dropped. stats: score_topk's, candidates (int64 [nq]: fused candidates of each row), and with
+    stats={"stages": {}} the CUDA-event times of "dense", "lists", "fuse" and "select"."""
+    k, kd, rrf_c = _check_fusion(fusion, k, window, rrf_c)
+    w = _check_weight(weight)
+    q = _check_f32(queries, "queries")
+    nq = q.shape[0]
+    ls = masks = None
+    if doc_lists is not None or list_of is not None:
+        q, ls = _queries_and_lists(q, index, doc_mask, mask_of, doc_lists, list_of)
+    else:
+        q, masks = _queries_and_mask(q, index, doc_mask, mask_of)
+    rrf = fusion == "rrf"
+    with L.on_device(q.device):
+        h = _check_hits(hits, nq, index.nd, q.device, masks, ls, rank_order=rrf)
+        ev = _Stages(stats)
+        ds, di = score_topk(q, index, kd, 0, False, stats, doc_mask, mask_of, doc_lists, list_of)
+        ev.mark("dense")
+        out_s = torch.empty((nq, k), dtype=torch.float32, device=q.device)
+        out_i = torch.empty((nq, k), dtype=torch.int64, device=q.device)
+        cands = torch.zeros(nq, dtype=torch.int64, device=q.device) if stats is not None else None
+        if nq == 0:
+            if stats is not None:
+                stats["candidates"] = cands
+            return out_s, out_i
+        lib, sp = L.lib(), L.stream_ptr()
+        hw = max(1, h.width)
+        W = kd + h.width
+        rows_per = max(1, min(nq, FUSE_BUDGET // (W + hw)))
+        hs = torch.empty((rows_per, hw), dtype=torch.float32, device=q.device) if not rrf else None
+        hi = torch.empty((rows_per, hw), dtype=torch.int64, device=q.device) if not rrf else None
+        fs = torch.empty((rows_per, W), dtype=torch.float32, device=q.device)
+        fi = torch.empty((rows_per, W), dtype=torch.int64, device=q.device)
+        status = torch.zeros(1, dtype=torch.int32, device=q.device)
+        of = torch.arange(nq, dtype=torch.int32, device=q.device)
+        lists = _ListSet(h.offsets, h.ids, of if nq > 1 else None, hw, False)
+        for r0 in range(0, nq, rows_per):
+            n = min(rows_per, nq - r0)
+            if hs is not None and h.width:  # the exact dense scores of the hits, hit j of a row at column j
+                L.check(lib.vr_score_lists(q[r0:].data_ptr(), n, index.emb.data_ptr(), index.nd, q.shape[1],
+                                           lists.arg(lists.of_query, r0), hw, None, hs.data_ptr(), hi.data_ptr(), None,
+                                           status.data_ptr(), sp))
+            ev.mark("lists")
+            L.check(lib.vr_fuse_rows(ds[r0:].data_ptr(), di[r0:].data_ptr(), n, kd, h.offsets[r0:].data_ptr(),
+                                     h.ids.data_ptr(), h.values.data_ptr(), L.ptr(hs), hw, FUSIONS[fusion], w, rrf_c, W,
+                                     fs.data_ptr(), fi.data_ptr(), status.data_ptr(), sp))
+            ev.mark("fuse")
+            L.check(_rows_fn(k)(fs.data_ptr(), fi.data_ptr(), n, W, k, id_offset, out_s[r0:].data_ptr(),
+                                out_i[r0:].data_ptr(), sp))
+            ev.mark("select")
+            if cands is not None:
+                cands[r0:r0 + n] = (fi[:n] >= 0).sum(1)
+    # status is not read: the width is the longest row, so neither call can truncate a list
+    if stats is not None:
+        stats["candidates"] = cands
+    return out_s, out_i
+
+
+def _group_pages_fused(q: torch.Tensor, index: CorpusIndex, groups: torch.Tensor, gt: _GroupTable, h: _Hits, w: float,
+                       masks: Optional[_MaskSet]) -> Tuple[torch.Tensor, torch.Tensor]:
+    """vr_group_pages_fused over every (row, slot) of groups [nq, kg] (int64), the pieces of long documents reduced by
+    vr_topk_rows: (fused scores [nq, kg], best pages [nq, kg], local)."""
+    nq, kg = groups.shape
+    dev = q.device
+    out_s = torch.empty((nq, kg), dtype=torch.float32, device=dev)
+    out_p = torch.empty((nq, kg), dtype=torch.int64, device=dev)
+    piece = max(1, min(GROUP_PIECE, gt.max_pages))
+    pieces = max(1, -(-gt.max_pages // piece))
+    lib, sp = L.lib(), L.stream_ptr()
+    rows_per = max(1, min(nq, GROUP_STAGE_BUDGET // (kg * pieces)))
+    ws_s = torch.empty((rows_per, kg, pieces), dtype=torch.float32, device=dev) if pieces > 1 else None
+    ws_p = torch.empty((rows_per, kg, pieces), dtype=torch.int64, device=dev) if pieces > 1 else None
+    for r0 in range(0, nq, rows_per):
+        n = min(rows_per, nq - r0)
+        s, p = (out_s[r0:], out_p[r0:]) if pieces == 1 else (ws_s, ws_p)
+        L.check(lib.vr_group_pages_fused(q[r0:].data_ptr(), n, index.emb.data_ptr(), index.nd, q.shape[1],
+                                         groups[r0:].data_ptr(), kg, gt.offsets.data_ptr(), gt.pages.data_ptr(), gt.G,
+                                         None if masks is None else masks.arg(r0), h.offsets[r0:].data_ptr(),
+                                         h.ids.data_ptr(), h.values.data_ptr(), w, piece, pieces, 0, s.data_ptr(),
+                                         p.data_ptr(), sp))
+        if pieces > 1:
+            L.check(lib.vr_topk_rows(ws_s.data_ptr(), ws_p.data_ptr(), n * kg, pieces, 1, 0, out_s[r0:].data_ptr(),
+                                     out_p[r0:].data_ptr(), sp))
+    return out_s, out_p
+
+
+def score_topk_groups_hybrid(queries: torch.Tensor, index: CorpusIndex, k: int, doc_groups: torch.Tensor, hits,
+                             weight=1.0, fusion: str = "sum", id_offset: int = 0, doc_mask: Optional[torch.Tensor] = None,
+                             mask_of: Optional[torch.Tensor] = None,
+                             doc_lists: Optional[Tuple[torch.Tensor, torch.Tensor]] = None,
+                             list_of: Optional[torch.Tensor] = None, stats: Optional[dict] = None
+                             ) -> Tuple[torch.Tensor, torch.Tensor, torch.Tensor]:
+    """Exact hybrid top-k documents (doc_groups as in score_topk_groups): a document's fused score is the maximum over
+    its eligible pages of fl(dense + fl(weight * v)) (hits and v as in score_topk_hybrid), its best page the lowest page
+    with it; documents rank by (score desc, best page asc). Returns (scores [nq, k] f32, best pages [nq, k] i64 = local
+    page + id_offset, groups [nq, k] i64), ending in (-inf, -1, -1). The candidates are the dense top-k documents
+    (score_topk_groups) and the documents of the query's hits; every page of each is scored exactly
+    (vr_group_pages_fused), since a document's best page need not be a hit. Only fusion="sum": RRF over documents needs
+    the external retriever's document ranks, which page hits do not give. Scopes and stats as in score_topk_hybrid
+    (stages "dense", "lists" (the candidate documents), "fuse" and "select"; candidates: documents scored per row)."""
+    if fusion != "sum":
+        raise ValueError(f'score_topk_groups_hybrid fuses by weighted sum only (fusion="sum"), got {fusion!r}: reciprocal '
+                         "rank fusion of documents needs the external retriever's document ranks, not page hits")
+    k = _check_count(k, "k")
+    if not 1 <= k <= FUSE_K_MAX:
+        raise ValueError(f"k={k} must lie in [1, {FUSE_K_MAX}]")
+    w = _check_weight(weight)
+    q = _check_f32(queries, "queries")
+    nq = q.shape[0]
+    ls = masks = None
+    if doc_lists is not None or list_of is not None:
+        q, ls = _queries_and_lists(q, index, doc_mask, mask_of, doc_lists, list_of)
+    else:
+        q, masks = _queries_and_mask(q, index, doc_mask, mask_of)
+    with L.on_device(q.device):
+        gt = _group_table(doc_groups, index)
+        h = _check_hits(hits, nq, index.nd, q.device, masks, ls)
+        ev = _Stages(stats)
+        _, _, dg = score_topk_groups(q, index, k, doc_groups, 0, False, stats, doc_mask, mask_of, doc_lists, list_of)
+        ev.mark("dense")
+        out = tuple(torch.empty((nq, k), dtype=t, device=q.device) for t in (torch.float32, torch.int64, torch.int64))
+        if nq == 0:
+            return out
+        # candidate documents: the dense top-k and the documents of the hits, each once per row (-1: empty)
+        hg = torch.full((nq, max(1, h.width)), -1, dtype=torch.int64, device=q.device)
+        if h.n:
+            pos = torch.arange(h.n, device=q.device)
+            row = torch.searchsorted(h.offsets[1:], pos, right=True)
+            hg[row, pos - h.offsets[row]] = gt.groups.index_select(0, h.ids[:h.n].long()).long()
+        cand = torch.sort(torch.cat([dg, hg], 1), dim=1).values
+        cand[:, 1:].masked_fill_(cand[:, 1:] == cand[:, :-1], -1)
+        masks = _stage_masks(q, index, doc_mask, mask_of, doc_lists, list_of) if ls is not None else masks
+        ev.mark("lists")
+        fs, fp = _group_pages_fused(q, index, cand.contiguous(), gt, h, w, masks)
+        ev.mark("fuse")
+        L.check(_rows_fn(k)(fs.data_ptr(), fp.data_ptr(), nq, fs.shape[1], k, id_offset, out[0].data_ptr(),
+                            out[1].data_ptr(), L.stream_ptr()))
+        out[2].copy_(torch.where(out[1] >= 0, gt.groups.index_select(0, (out[1] - id_offset).clamp(min=0).flatten())
+                                 .view(nq, k).long(), -1))
+        ev.mark("select")
+        if stats is not None:
+            stats["candidates"] = (cand >= 0).sum(1)
     return out
 
 
