@@ -30,6 +30,10 @@ on the GPU (vr_mmr_select) with the bits fixed by the definition in DESIGN §4.
 
 Hybrid retrieval (`score_topk_hybrid`, `score_topk_groups_hybrid`): the dense score fused with an external score per
 page (e.g. BM25 over OCR text), by weighted sum or reciprocal rank fusion, exactly over the whole index (DESIGN §4).
+
+Sharded forms of range search, document range search, hybrid retrieval and MMR (`sharded_range`,
+`sharded_range_groups`, `sharded_topk_hybrid`, `sharded_topk_groups_hybrid`, `sharded_mmr`): the bits of the plain call
+over the shards concatenated in rank order, from each rank's local call, a few collectives and a merge (DESIGN §4).
 """
 from __future__ import annotations
 
@@ -918,7 +922,7 @@ def _range_filter(q: torch.Tensor, index: CorpusIndex, t: torch.Tensor, masks: O
     if ok.numel():
         kept_host = host[1]
         if gt is not None:  # overflowed rows kept nothing, so every row of the region can be reduced
-            rs, ri, kept = _range_groups(rs, ri, kept, n, int(kept_host.max()), gt)
+            rs, ri, kept = _range_groups(rs, ri, kept, n, int(kept_host.max()), gt.groups, gt.G)
             kept_host = kept.cpu()
         pieces.append(_range_sort(rs, ri, cap, kept, kept_host, ok, rows, id_offset))
     bad = torch.nonzero(over).flatten()
@@ -931,10 +935,11 @@ def _range_filter(q: torch.Tensor, index: CorpusIndex, t: torch.Tensor, masks: O
     return pieces
 
 
-def _range_groups(rs: torch.Tensor, ri: torch.Tensor, counts: torch.Tensor, n: int, most: int, gt: _GroupTable):
+def _range_groups(rs: torch.Tensor, ri: torch.Tensor, counts: torch.Tensor, n: int, most: int, groups: torch.Tensor, G: int):
     """Rows [0, n) of the region (rs, ri [*, pitch], counts) reduced by vr_range_groups to the first entry of each
     document in (score desc, page asc) order, with its own bits: (scores, ids, counts) of a region of the same pitch.
-    most >= every counts[r]; rows longer than the shared-memory table go in chunks that bound the workspace."""
+    groups (int32, indexed by the region's ids) and G as vr_range_groups takes them. most >= every counts[r]; rows
+    longer than the shared-memory table go in chunks that bound the workspace."""
     pitch, dev = rs.shape[1], rs.device
     lib, sp = L.lib(), L.stream_ptr()
     gs = torch.empty((n, pitch), dtype=torch.float32, device=dev)
@@ -947,7 +952,7 @@ def _range_groups(rs: torch.Tensor, ri: torch.Tensor, counts: torch.Tensor, n: i
     for r0 in range(0, n, per):
         m = min(per, n - r0)
         L.check(lib.vr_range_groups(rs[r0:].data_ptr(), ri[r0:].data_ptr(), pitch, counts[r0:].data_ptr(), m, most,
-                                    gt.groups.data_ptr(), gt.groups.shape[0], gt.G, L.ptr(ws), ws_bytes, gs[r0:].data_ptr(),
+                                    groups.data_ptr(), groups.shape[0], G, L.ptr(ws), ws_bytes, gs[r0:].data_ptr(),
                                     gi[r0:].data_ptr(), gc[r0:].data_ptr(), sp))
     return gs, gi, gc
 
@@ -996,7 +1001,7 @@ def _range_scan(q: torch.Tensor, index: CorpusIndex, t: torch.Tensor, masks: Opt
                                   rs.data_ptr(), ri.data_ptr(), counts.data_ptr(), sp))
         region = (rs, ri, counts, counts[:m].cpu())
         if gt is not None:
-            gs, gi, gc = _range_groups(rs, ri, counts, m, int(region[3].max()), gt)
+            gs, gi, gc = _range_groups(rs, ri, counts, m, int(region[3].max()), gt.groups, gt.G)
             region = (gs, gi, gc, gc.cpu())
         pieces.append(_range_sort(*region[:2], nd, *region[2:], torch.arange(m), rows[r0:r0 + m], id_offset))
     return pieces
@@ -1122,7 +1127,7 @@ def _deep_topk(q: torch.Tensor, index: CorpusIndex, k: int, id_offset: int, stat
         n = min(step, nq - r0)
         counts, kept, rs, ri = _range_candidates(q[r0:r0 + n], index, t[r0:r0 + n], masks, r0, RANGE_CAP)
         if gt is not None:  # A reduced to documents (overflowed rows kept nothing)
-            rs, ri, kept = _range_groups(rs, ri, kept, n, int(kept.max()), gt)
+            rs, ri, kept = _range_groups(rs, ri, kept, n, int(kept.max()), gt.groups, gt.G)
         host = torch.stack([counts, kept, short[r0:r0 + n].to(torch.int32)]).cpu()
         ev.mark("range")
         over = host[0] > RANGE_CAP
@@ -1358,13 +1363,13 @@ def _hits_in_scope(row: torch.Tensor, ids: torch.Tensor, nd: int, masks: Optiona
     return torch.ones_like(ids, dtype=torch.bool)
 
 
-def _check_hits(hits, nq: int, nd: int, device, masks: Optional[_MaskSet] = None, ls: Optional[_ListSet] = None,
-                rank_order: bool = False) -> _Hits:
-    """Validate hits = (offsets int [nq + 1], ids int (local pages), values f32) on `device`, drop the hits outside each
-    query's scope, and order each row by id (rank_order: by (value desc, id asc), the external ranks of RRF). One host
-    read serves every value check (offsets from 0 to len(ids) and non-decreasing, ids in [0, nd), values finite and
-    >= 0, no page twice in a row) and the sizes of the result; nothing before it can index out of bounds. A value of -0.0
-    is a zero score and becomes +0.0."""
+def _hit_rows(offsets: torch.Tensor, n: int, nq: int) -> torch.Tensor:
+    """The query row of each of the n hit entries, by search (no host read; any offsets give rows in [0, nq))."""
+    return torch.searchsorted(offsets[1:], torch.arange(n, device=offsets.device), right=True).clamp(max=max(nq - 1, 0))
+
+
+def _hit_tensors(hits, nq: int, device) -> Tuple[torch.Tensor, torch.Tensor, torch.Tensor]:
+    """The shape, dtype and device checks of a hit list: (offsets int64, ids int64, values f32)."""
     if not isinstance(hits, (tuple, list)) or len(hits) != 3:
         raise ValueError("hits must be a triple (offsets, ids, values) of tensors")
     offsets, ids, values = hits
@@ -1376,17 +1381,28 @@ def _check_hits(hits, nq: int, nd: int, device, masks: Optional[_MaskSet] = None
         raise ValueError(f"hits values has {values.shape[0]} entries for {ids.shape[0]} ids")
     if values.device != device:
         raise ValueError(f"hits values live on {values.device}, the index on {device}")
-    offsets, ids = offsets.to(torch.int64), ids.to(torch.int64)
+    return offsets.to(torch.int64), ids.to(torch.int64), values
+
+
+def _check_hits(hits, nq: int, nd: int, device, masks: Optional[_MaskSet] = None, ls: Optional[_ListSet] = None,
+                rank_order: bool = False, keep: Optional[torch.Tensor] = None) -> _Hits:
+    """Validate hits = (offsets int [nq + 1], ids int (local pages), values f32) on `device`, drop the hits outside each
+    query's scope, and order each row by id (rank_order: by (value desc, id asc), the external ranks of RRF). One host
+    read serves every value check (offsets from 0 to len(ids) and non-decreasing, ids in [0, nd), values finite and
+    >= 0, no page twice in a row) and the sizes of the result; nothing before it can index out of bounds. A value of -0.0
+    is a zero score and becomes +0.0. keep (bool [len(ids)], optional) replaces the scope test: the hits to keep."""
+    offsets, ids, values = _hit_tensors(hits, nq, device)
     values = values + 0.0  # -0.0 -> +0.0: the sign bit would break the rank key below
     n = ids.shape[0]
     z = offsets.new_zeros(())
-    # the row of each entry, by search (no host read; any offsets give rows in [0, nq), checked below)
-    row = torch.searchsorted(offsets[1:], torch.arange(n, device=device), right=True).clamp(max=max(nq - 1, 0))
+    # the row of each entry (any offsets give rows in [0, nq); they are checked below)
+    row = _hit_rows(offsets, n, nq)
     safe = ids.clamp(0, nd - 1)
     key = row * nd + safe                       # (row, id): distinct keys unless a page repeats in a row
     order = torch.argsort(key)
     srt = key.index_select(0, order)
-    keep = _hits_in_scope(row, safe, nd, masks, ls)
+    if keep is None:
+        keep = _hits_in_scope(row, safe, nd, masks, ls)
     counts = offsets.new_zeros(max(nq, 1)).scatter_add_(0, row, keep.long())[:nq]
     checks = torch.stack([offsets[0], offsets[-1], (offsets[1:] - offsets[:-1]).min() if nq else z,
                           ids.min() if n else z, ids.max() if n else z,
@@ -1455,40 +1471,49 @@ def score_topk_hybrid(queries: torch.Tensor, index: CorpusIndex, k: int, hits, w
         ev = _Stages(stats)
         ds, di = score_topk(q, index, kd, 0, False, stats, doc_mask, mask_of, doc_lists, list_of)
         ev.mark("dense")
-        out_s = torch.empty((nq, k), dtype=torch.float32, device=q.device)
-        out_i = torch.empty((nq, k), dtype=torch.int64, device=q.device)
-        cands = torch.zeros(nq, dtype=torch.int64, device=q.device) if stats is not None else None
-        if nq == 0:
-            if stats is not None:
-                stats["candidates"] = cands
-            return out_s, out_i
-        lib, sp = L.lib(), L.stream_ptr()
-        hw = max(1, h.width)
-        W = kd + h.width
-        rows_per = max(1, min(nq, FUSE_BUDGET // (W + hw)))
-        hs = torch.empty((rows_per, hw), dtype=torch.float32, device=q.device) if not rrf else None
-        hi = torch.empty((rows_per, hw), dtype=torch.int64, device=q.device) if not rrf else None
-        fs = torch.empty((rows_per, W), dtype=torch.float32, device=q.device)
-        fi = torch.empty((rows_per, W), dtype=torch.int64, device=q.device)
-        status = torch.zeros(1, dtype=torch.int32, device=q.device)
-        of = torch.arange(nq, dtype=torch.int32, device=q.device)
-        lists = _ListSet(h.offsets, h.ids, of if nq > 1 else None, hw, False)
-        for r0 in range(0, nq, rows_per):
-            n = min(rows_per, nq - r0)
-            if hs is not None and h.width:  # the exact dense scores of the hits, hit j of a row at column j
-                L.check(lib.vr_score_lists(q[r0:].data_ptr(), n, index.emb.data_ptr(), index.nd, q.shape[1],
-                                           lists.arg(lists.of_query, r0), hw, None, hs.data_ptr(), hi.data_ptr(), None,
-                                           status.data_ptr(), sp))
-            ev.mark("lists")
-            L.check(lib.vr_fuse_rows(ds[r0:].data_ptr(), di[r0:].data_ptr(), n, kd, h.offsets[r0:].data_ptr(),
-                                     h.ids.data_ptr(), h.values.data_ptr(), L.ptr(hs), hw, FUSIONS[fusion], w, rrf_c, W,
-                                     fs.data_ptr(), fi.data_ptr(), status.data_ptr(), sp))
-            ev.mark("fuse")
-            L.check(_rows_fn(k)(fs.data_ptr(), fi.data_ptr(), n, W, k, id_offset, out_s[r0:].data_ptr(),
-                                out_i[r0:].data_ptr(), sp))
-            ev.mark("select")
-            if cands is not None:
-                cands[r0:r0 + n] = (fi[:n] >= 0).sum(1)
+        return _fuse_select(q, index, ds, di, h, k, fusion, w, rrf_c, id_offset, stats, ev)
+
+
+def _fuse_select(q: torch.Tensor, index: CorpusIndex, ds: torch.Tensor, di: torch.Tensor, h: _Hits, k: int, fusion: str,
+                 w: float, rrf_c: int, id_offset: int, stats: Optional[dict], ev: _Stages):
+    """The stages of score_topk_hybrid after the dense top-kd (ds, di [nq, kd], ids in the hits' id space): the hits'
+    dense scores (sum), vr_fuse_rows and the select of k, ids + id_offset. RRF reads no index rows."""
+    nq, kd = ds.shape
+    rrf = fusion == "rrf"
+    out_s = torch.empty((nq, k), dtype=torch.float32, device=q.device)
+    out_i = torch.empty((nq, k), dtype=torch.int64, device=q.device)
+    cands = torch.zeros(nq, dtype=torch.int64, device=q.device) if stats is not None else None
+    if nq == 0:
+        if stats is not None:
+            stats["candidates"] = cands
+        return out_s, out_i
+    lib, sp = L.lib(), L.stream_ptr()
+    hw = max(1, h.width)
+    W = kd + h.width
+    rows_per = max(1, min(nq, FUSE_BUDGET // (W + hw)))
+    hs = torch.empty((rows_per, hw), dtype=torch.float32, device=q.device) if not rrf else None
+    hi = torch.empty((rows_per, hw), dtype=torch.int64, device=q.device) if not rrf else None
+    fs = torch.empty((rows_per, W), dtype=torch.float32, device=q.device)
+    fi = torch.empty((rows_per, W), dtype=torch.int64, device=q.device)
+    status = torch.zeros(1, dtype=torch.int32, device=q.device)
+    of = torch.arange(nq, dtype=torch.int32, device=q.device)
+    lists = _ListSet(h.offsets, h.ids, of if nq > 1 else None, hw, False)
+    for r0 in range(0, nq, rows_per):
+        n = min(rows_per, nq - r0)
+        if hs is not None and h.width:  # the exact dense scores of the hits, hit j of a row at column j
+            L.check(lib.vr_score_lists(q[r0:].data_ptr(), n, index.emb.data_ptr(), index.nd, q.shape[1],
+                                       lists.arg(lists.of_query, r0), hw, None, hs.data_ptr(), hi.data_ptr(), None,
+                                       status.data_ptr(), sp))
+        ev.mark("lists")
+        L.check(lib.vr_fuse_rows(ds[r0:].data_ptr(), di[r0:].data_ptr(), n, kd, h.offsets[r0:].data_ptr(),
+                                 h.ids.data_ptr(), h.values.data_ptr(), L.ptr(hs), hw, FUSIONS[fusion], w, rrf_c, W,
+                                 fs.data_ptr(), fi.data_ptr(), status.data_ptr(), sp))
+        ev.mark("fuse")
+        L.check(_rows_fn(k)(fs.data_ptr(), fi.data_ptr(), n, W, k, id_offset, out_s[r0:].data_ptr(),
+                            out_i[r0:].data_ptr(), sp))
+        ev.mark("select")
+        if cands is not None:
+            cands[r0:r0 + n] = (fi[:n] >= 0).sum(1)
     # status is not read: the width is the longest row, so neither call can truncate a list
     if stats is not None:
         stats["candidates"] = cands
@@ -1523,6 +1548,12 @@ def _group_pages_fused(q: torch.Tensor, index: CorpusIndex, groups: torch.Tensor
     return out_s, out_p
 
 
+def _check_group_fusion(fusion, name: str) -> None:
+    if fusion != "sum":
+        raise ValueError(f'{name} fuses by weighted sum only (fusion="sum"), got {fusion!r}: reciprocal '
+                         "rank fusion of documents needs the external retriever's document ranks, not page hits")
+
+
 def score_topk_groups_hybrid(queries: torch.Tensor, index: CorpusIndex, k: int, doc_groups: torch.Tensor, hits,
                              weight=1.0, fusion: str = "sum", id_offset: int = 0, doc_mask: Optional[torch.Tensor] = None,
                              mask_of: Optional[torch.Tensor] = None,
@@ -1537,9 +1568,7 @@ def score_topk_groups_hybrid(queries: torch.Tensor, index: CorpusIndex, k: int, 
     (vr_group_pages_fused), since a document's best page need not be a hit. Only fusion="sum": RRF over documents needs
     the external retriever's document ranks, which page hits do not give. Scopes and stats as in score_topk_hybrid
     (stages "dense", "lists" (the candidate documents), "fuse" and "select"; candidates: documents scored per row)."""
-    if fusion != "sum":
-        raise ValueError(f'score_topk_groups_hybrid fuses by weighted sum only (fusion="sum"), got {fusion!r}: reciprocal '
-                         "rank fusion of documents needs the external retriever's document ranks, not page hits")
+    _check_group_fusion(fusion, "score_topk_groups_hybrid")
     k = _check_count(k, "k")
     if not 1 <= k <= FUSE_K_MAX:
         raise ValueError(f"k={k} must lie in [1, {FUSE_K_MAX}]")
@@ -1754,6 +1783,449 @@ def gather_queries(local: torch.Tensor, n_total: int, group=None) -> torch.Tenso
         lo, hi = shard_range(n_total, r, world)
         parts.append(flat[r * per: r * per + (hi - lo)])
     return torch.cat(parts)
+
+
+# ------------------------------------------------------------------------------------------------------
+# Sharded range search, document range search, hybrid retrieval and MMR (DESIGN §4, "Sharded retrieval")
+# ------------------------------------------------------------------------------------------------------
+# Each sharded_* function below is three stages: the rank's local stage, an exchange (collectives only) and a merge that
+# every rank runs on identical inputs. The local stages and merges are the functions named here, so that a test on one
+# process can run every rank's local stage, replace the exchange by concatenation in rank order, and run the merge.
+def _check_spans(spans: torch.Tensor) -> torch.Tensor:
+    """spans int64 [world, 2] on the host: every rank's (id_offset, nd). The ranks' page ranges must follow each other
+    in rank order from page 0 (rank r starts where rank r - 1 ends), so that the shards in rank order are one index and
+    every page has one owner; overlapping, out-of-order and gapped ranges are refused. Returns the range ends [world]."""
+    lo, nd = spans[:, 0], spans[:, 1]
+    hi = lo + nd
+    if bool((nd < 0).any()) or int(lo[0]) != 0 or bool((lo[1:] != hi[:-1]).any()):
+        raise ValueError("sharded retrieval needs the ranks' page ranges [id_offset, id_offset + nd) to follow each other "
+                         f"in rank order from page 0 (one contiguous range per rank), got {spans.tolist()}")
+    if int(hi[-1]) >= 1 << 31:
+        raise ValueError(f"sharded retrieval takes fewer than 2^31 pages in all, got {int(hi[-1])}")
+    return hi
+
+
+def _gather_spans(id_offset: int, nd: int, device, group) -> torch.Tensor:
+    """One all-gather of every rank's (id_offset, nd): int64 [world, 2] on the host, checked by _check_spans."""
+    import torch.distributed as dist
+
+    mine = torch.tensor([id_offset, nd], dtype=torch.int64, device=device)
+    got = torch.empty(dist.get_world_size(group) * 2, dtype=torch.int64, device=device)  # rank-major concatenation
+    dist.all_gather_into_tensor(got, mine, group=group)
+    spans = got.view(-1, 2).cpu()
+    _check_spans(spans)
+    return spans
+
+
+def concat_csr(parts) -> Tuple[torch.Tensor, torch.Tensor]:
+    """CSR arrays over the same nq rows -> one CSR array whose row r is the parts' rows r one after the other, in part
+    order. parts: (offsets int64 [nq + 1] from 0, entries [n, c]) on one device (entries past offsets[-1] are ignored).
+    The merge step of gather_csr, and on one process the exchange itself. Returns (offsets int64 [nq + 1], entries)."""
+    offs = [o.to(torch.int64) for o, _ in parts]
+    counts = torch.stack([o[1:] - o[:-1] for o in offs])           # [parts, nq]
+    nq, dev = counts.shape[1], counts.device
+    offsets = torch.zeros(nq + 1, dtype=torch.int64, device=dev)
+    offsets[1:] = torch.cumsum(counts.sum(0), 0)
+    base = offsets[:-1] + torch.cumsum(counts, 0) - counts         # where part p's row r starts
+    sizes = torch.cat([offsets[-1:], counts.sum(1)]).tolist()      # host read: the sizes of the output and of each part
+    first = parts[0][1]
+    out = torch.empty((sizes[0],) + tuple(first.shape[1:]), dtype=first.dtype, device=dev)
+    rows = torch.arange(nq, device=dev)
+    for p, ((_, e), o, n) in enumerate(zip(parts, offs, sizes[1:])):
+        if n:
+            row = torch.repeat_interleave(rows, counts[p], output_size=n)
+            out[base[p].index_select(0, row) + torch.arange(n, device=dev) - o.index_select(0, row)] = e[:n]
+    return offsets, out
+
+
+def gather_csr(offsets: torch.Tensor, entries: torch.Tensor, group=None, head: Optional[torch.Tensor] = None):
+    """Variable-length rows across ranks: every rank holds a CSR array over the same nq rows (offsets int64 [nq + 1] from
+    0, entries int64 [n, c]); every rank gets concat_csr of all ranks' arrays in rank order. Two all-gathers: the per-row
+    counts [nq] (after `head`, an optional int64 [h] of per-rank values such as (id_offset, nd)), then the entries
+    padded to the largest rank's n. Returns (offsets, entries, heads int64 [world, h] on the host)."""
+    import torch.distributed as dist
+
+    world = dist.get_world_size(group)
+    dev, nq, c = entries.device, offsets.shape[0] - 1, entries.shape[1]
+    offsets = offsets.to(torch.int64)
+    head = torch.zeros(0, dtype=torch.int64, device=dev) if head is None else head.to(device=dev, dtype=torch.int64)
+    h = head.shape[0]
+    got = torch.empty(world * (h + nq), dtype=torch.int64, device=dev)  # rank-major concatenation
+    dist.all_gather_into_tensor(got, torch.cat([head, offsets[1:] - offsets[:-1]]), group=group)
+    got = got.view(world, h + nq)
+    info = torch.cat([got[:, :h], got[:, h:].sum(1, keepdim=True)], 1).cpu()  # host read: heads and each rank's n
+    pad = max(1, int(info[:, h].max()))
+    mine = torch.zeros((pad, c), dtype=torch.int64, device=dev)
+    n = int(offsets[-1])
+    mine[:n] = entries[:n]
+    flat = torch.empty((world * pad, c), dtype=torch.int64, device=dev)
+    dist.all_gather_into_tensor(flat, mine, group=group)
+    parts = []
+    for r in range(world):
+        o = torch.zeros(nq + 1, dtype=torch.int64, device=dev)
+        o[1:] = torch.cumsum(got[r, h:], 0)
+        parts.append((o, flat[r * pad:(r + 1) * pad]))
+    return (*concat_csr(parts), info[:, :h])
+
+
+def _range_entries(offsets: torch.Tensor, s: torch.Tensor, p: torch.Tensor, g: Optional[torch.Tensor] = None):
+    """A rank's range CSR as (offsets, entries int64 [R, 2 or 3] = (score bits, page[, group]))."""
+    cols = [_score_bits(s), p] + ([] if g is None else [g])
+    return offsets, torch.stack(cols, 1)
+
+
+def _merge_range(offsets: torch.Tensor, entries: torch.Tensor, groups: bool = False):
+    """The merge of sharded_range (groups False) and sharded_range_groups: the ranks' local results, each row the ranks'
+    rows in rank order (concat_csr's layout; entries from _range_entries, global pages) -> score_range's CSR (offsets,
+    scores, pages), or score_range_groups' (offsets, scores, best pages, groups).
+    Pages: each row's region is ordered by vr_range_sort with the global pages as ids. Documents: the region's ids are
+    the entries' positions and its groups the entries' groups; vr_range_groups keeps each document's first entry in
+    (score desc, position asc) order, and vr_range_sort orders the kept ones the same way. Within a rank's row, equal
+    scores are in page order, and the ranks hold increasing page ranges: position order is page order (DESIGN §4)."""
+    dev, nq = entries.device, offsets.shape[0] - 1
+    off_h = offsets.cpu()
+    tot = off_h[1:] - off_h[:-1]
+    total = int(off_h[-1])
+    rows = torch.arange(nq, dtype=torch.int64)
+    scores = _bits_score(entries[:, 0]).contiguous()
+    if total == 0:
+        pieces = [(rows, tot, scores, entries[:, 1].contiguous())]
+    else:
+        if groups:
+            if total >= 1 << 31:
+                raise ValueError(f"the document merge takes fewer than 2^31 entries, got {total}")
+            ids = torch.arange(total, dtype=torch.int32, device=dev)
+            grp = entries[:, 2].to(torch.int32).contiguous()
+            G = int(grp.max()) + 1
+        else:
+            ids = entries[:, 1].to(torch.int32)
+        step = max(1, min(nq, RANGE_BUDGET // int(tot.max())))
+        pieces = []
+        for r0 in range(0, nq, step):
+            n = min(step, nq - r0)
+            c_h = tot[r0:r0 + n]
+            pitch = max(1, int(c_h.max()))
+            a, b = int(off_h[r0]), int(off_h[r0 + n])
+            rs = torch.empty((n, pitch), dtype=torch.float32, device=dev)
+            ri = torch.empty((n, pitch), dtype=torch.int32, device=dev)
+            counts = c_h.to(torch.int32).to(dev)
+            if b > a:  # row r0 + j of the merged CSR -> region row j, its entries from column 0
+                row = torch.repeat_interleave(torch.arange(n, device=dev), counts, output_size=b - a)
+                at = row * pitch + torch.arange(a, b, device=dev) - offsets[r0:r0 + n].index_select(0, row)
+                rs.view(-1)[at] = scores[a:b]
+                ri.view(-1)[at] = ids[a:b]
+                if groups:
+                    rs, ri, counts = _range_groups(rs, ri, counts, n, int(c_h.max()), grp, G)
+                    c_h = counts.cpu()
+            pieces.append(_range_sort(rs, ri, pitch, counts, c_h, torch.arange(n), rows[r0:r0 + n], 0))
+    offsets, s, i = _range_assemble(nq, pieces, dev)
+    if not groups:
+        return offsets, s, i
+    return offsets, s, entries[:, 1].index_select(0, i), entries[:, 2].index_select(0, i)
+
+
+def sharded_range(queries: torch.Tensor, index: CorpusIndex, min_score, id_offset: int, group=None,
+                  doc_mask: Optional[torch.Tensor] = None, mask_of: Optional[torch.Tensor] = None, force_exact: bool = False,
+                  stats: Optional[dict] = None, cap: Optional[int] = None):
+    """score_range over a corpus sharded by page (every rank holds the same queries; rank r's shard holds pages
+    [id_offset, id_offset + nd), the ranks' ranges following each other in rank order from page 0). Each rank runs
+    score_range on its shard with global ids; gather_csr moves the rows (an all-gather of the per-row counts, then one
+    of the (score bits, page) int64 entries padded to the largest rank's total: 16 bytes an entry from every rank to
+    every rank); vr_range_sort orders each row. A page lives on one rank and its score bits depend only on its query and
+    page rows, so the union of the ranks' rows is the whole-index answer: the result equals score_range over the shards
+    concatenated in rank order, bit for bit. min_score must be the same on every rank (it is not checked: that would
+    take another collective). doc_mask / mask_of: this rank's part of its own shard, as in sharded_topk. stats: the local
+    call's, and with stats={"stages": {}} the times of "local", "exchange" and "merge"."""
+    ev = _Stages(stats)
+    offsets, s, i = score_range(queries, index, min_score, id_offset, doc_mask, mask_of, force_exact, stats, cap)
+    if _world(group) == 1:
+        return offsets, s, i
+    ev.mark("local")
+    head = torch.tensor([id_offset, index.nd], dtype=torch.int64)
+    offsets, entries, spans = gather_csr(*_range_entries(offsets, s, i), group, head)
+    _check_spans(spans)
+    ev.mark("exchange")
+    with L.on_device(entries.device):
+        out = _merge_range(offsets, entries)
+    ev.mark("merge")
+    return out
+
+
+def sharded_range_groups(queries: torch.Tensor, index: CorpusIndex, min_score, doc_groups: torch.Tensor, id_offset: int,
+                         group=None, doc_mask: Optional[torch.Tensor] = None, mask_of: Optional[torch.Tensor] = None,
+                         force_exact: bool = False, stats: Optional[dict] = None, cap: Optional[int] = None):
+    """score_range_groups over a corpus sharded by page: doc_groups holds this shard's pages' GLOBAL group ids (a
+    document may span ranks). Each rank runs score_range_groups on its shard (each document's best page on that rank);
+    gather_csr moves the rows as in sharded_range, with the groups (24 bytes an entry); then each (row, document) keeps
+    the first of the ranks' entries in (score desc, page asc) order, and the rows are ordered (_merge_range). A
+    document's best page is the best of its ranks' best pages, so the result equals score_range_groups over the shards
+    concatenated in rank order, bit for bit. Arguments, stats and the page ranges as in sharded_range."""
+    ev = _Stages(stats)
+    offsets, s, p, g = score_range_groups(queries, index, min_score, doc_groups, id_offset, doc_mask, mask_of, force_exact,
+                                          stats, cap)
+    if _world(group) == 1:
+        return offsets, s, p, g
+    ev.mark("local")
+    head = torch.tensor([id_offset, index.nd], dtype=torch.int64)
+    offsets, entries, spans = gather_csr(*_range_entries(offsets, s, p, g), group, head)
+    _check_spans(spans)
+    ev.mark("exchange")
+    with L.on_device(entries.device):
+        out = _merge_range(offsets, entries, groups=True)
+    ev.mark("merge")
+    if stats is not None:
+        stats["documents"] = out[1].numel()
+    return out
+
+
+def _scope(queries, index: CorpusIndex, doc_mask, mask_of, doc_lists, list_of):
+    """(queries, mask set, list set) of a search's scope, validated as the plain calls do (at most one set is given)."""
+    q = _check_f32(queries, "queries")
+    if doc_lists is not None or list_of is not None:
+        q, ls = _queries_and_lists(q, index, doc_mask, mask_of, doc_lists, list_of)
+        return q, None, ls
+    q, masks = _queries_and_mask(q, index, doc_mask, mask_of)
+    return q, masks, None
+
+
+def _hit_marks(hits, nq: int, id_offset: int, index: CorpusIndex, masks: Optional[_MaskSet], ls: Optional[_ListSet]
+               ) -> torch.Tensor:
+    """int32 [len(ids)]: 1 for each hit (a global page) that this rank holds (id_offset <= id < id_offset + nd) and that
+    lies in its query's scope on this rank, else 0. Only the owner can apply the scope. No host read."""
+    offsets, ids, _ = _hit_tensors(hits, nq, index.emb.device)
+    local = ids - id_offset
+    if index.nd == 0 or ids.numel() == 0:
+        return torch.zeros(ids.shape[0], dtype=torch.int32, device=ids.device)
+    inside = _hits_in_scope(_hit_rows(offsets, ids.shape[0], nq), local.clamp(0, index.nd - 1), index.nd, masks, ls)
+    return ((local >= 0) & (local < index.nd) & inside).to(torch.int32)
+
+
+def _combine_marks(marks: torch.Tensor, group) -> torch.Tensor:
+    """The exchange of the sharded RRF: every rank's _hit_marks summed by one int32 all-reduce (a hit has one owner, so
+    the sum is 0 or 1 and exact) -> bool, the same on every rank."""
+    import torch.distributed as dist
+
+    marks = marks.clone()
+    dist.all_reduce(marks, group=group)
+    return marks > 0
+
+
+def _local_hits(hits, nq: int, spans: torch.Tensor, rank: int, index: CorpusIndex, masks: Optional[_MaskSet],
+                ls: Optional[_ListSet]):
+    """The local stage's hits of the sharded weighted sum: hits in global pages, checked against the whole corpus as the
+    plain call checks them (every rank refuses the same lists), reduced to the ones rank `rank` holds and keeps, in local
+    ids: an (offsets, ids, values) triple for score_topk_hybrid on the rank's shard."""
+    total = int(_check_spans(spans)[-1])
+    lo = int(spans[rank, 0])
+    keep = _hit_marks(hits, nq, lo, index, masks, ls) > 0
+    h = _check_hits(hits, nq, total, index.emb.device, keep=keep)
+    return h.offsets, (h.ids[:h.n] - lo).to(torch.int32), h.values[:h.n]
+
+
+def _rrf_merge(q: torch.Tensor, ds: torch.Tensor, di: torch.Tensor, hits, keep: torch.Tensor, k: int, rrf_c: int,
+               total: int, stats: Optional[dict]):
+    """The merge of the sharded RRF, the same on every rank: the global dense top-window (ds, di: global pages) and the
+    kept hits (global pages) fused by vr_fuse_rows and selected, as score_topk_hybrid does on one index."""
+    h = _check_hits(hits, q.shape[0], total, q.device, rank_order=True, keep=keep)
+    return _fuse_select(q, None, ds, di, h, k, "rrf", 0.0, rrf_c, 0, stats, _Stages(None))
+
+
+def _shift_hits(hits, id_offset: int):
+    """hits in global pages -> in this index's local pages (world 1: the plain call's argument)."""
+    if id_offset == 0 or not isinstance(hits, (tuple, list)) or len(hits) != 3 or not isinstance(hits[1], torch.Tensor):
+        return hits
+    return hits[0], hits[1] - id_offset, hits[2]
+
+
+def sharded_topk_hybrid(queries: torch.Tensor, index: CorpusIndex, k: int, hits, id_offset: int, group=None, weight=1.0,
+                        fusion: str = "sum", window: Optional[int] = None, rrf_c: int = 60,
+                        doc_mask: Optional[torch.Tensor] = None, mask_of: Optional[torch.Tensor] = None,
+                        doc_lists: Optional[Tuple[torch.Tensor, torch.Tensor]] = None, list_of: Optional[torch.Tensor] = None,
+                        stats: Optional[dict] = None):
+    """score_topk_hybrid over a corpus sharded by page (page ranges as in sharded_range). hits are in GLOBAL pages and
+    the same on every rank; they are checked against the whole corpus on every rank, with the plain call's refusals.
+    Scopes (doc_mask / mask_of, doc_lists / list_of) are this rank's part of its own shard, in local ids; only a hit's
+    owner applies its query's scope. One all-gather of (id_offset, nd) first.
+    fusion="sum": each rank runs score_topk_hybrid on its shard with the hits it holds (local ids) and global ids out;
+    then gather_partials ([nq, k] pairs) and merge_topk. A page's fused score does not depend on the shard, so the
+    global top-k lies in the union of the local top-k's.
+    fusion="rrf": the dense ranks must be global. sharded_topk(window) gives every rank the global dense top-window;
+    each rank marks the hits it holds and keeps, and one int32 all-reduce over the hits combines the marks; every rank
+    then fuses and selects on identical inputs (RRF reads no index rows). The result equals score_topk_hybrid over the
+    shards concatenated in rank order, bit for bit. stats: with stats={"stages": {}} the times of "local" ("dense" for
+    RRF: the whole sharded_topk), "exchange" and "merge"; sum also gives the local call's stats."""
+    k, kd, rrf_c = _check_fusion(fusion, k, window, rrf_c)
+    w = _check_weight(weight)
+    if _world(group) == 1:
+        return score_topk_hybrid(queries, index, k, _shift_hits(hits, id_offset), w, fusion, window, rrf_c, id_offset,
+                                 doc_mask, mask_of, doc_lists, list_of, stats)
+    import torch.distributed as dist
+
+    q, masks, ls = _scope(queries, index, doc_mask, mask_of, doc_lists, list_of)
+    nq = q.shape[0]
+    _hit_tensors(hits, nq, q.device)  # a malformed triple is refused before any collective
+    with L.on_device(q.device):
+        ev = _Stages(stats)
+        spans = _gather_spans(id_offset, index.nd, q.device, group)
+        if fusion == "sum":
+            local = _local_hits(hits, nq, spans, dist.get_rank(group), index, masks, ls)
+            s, i = score_topk_hybrid(q, index, k, local, w, "sum", None, rrf_c, id_offset, doc_mask, mask_of, doc_lists,
+                                     list_of, stats)
+            ev.mark("local")
+            gs, gi = gather_partials(s, i, group)
+            ev.mark("exchange")
+            out = merge_topk(gs, gi, k)
+            ev.mark("merge")
+            return out
+        ds, di = sharded_topk(q, index, kd, id_offset, group, None, doc_mask, mask_of, doc_lists, list_of)
+        marks = _hit_marks(hits, nq, id_offset, index, masks, ls)
+        ev.mark("dense")
+        keep = _combine_marks(marks, group)
+        ev.mark("exchange")
+        out = _rrf_merge(q, ds, di, hits, keep, k, rrf_c, int(_check_spans(spans)[-1]), stats)
+        ev.mark("merge")
+        return out
+
+
+def sharded_topk_groups_hybrid(queries: torch.Tensor, index: CorpusIndex, k: int, doc_groups: torch.Tensor, hits,
+                               id_offset: int, group=None, weight=1.0, fusion: str = "sum",
+                               doc_mask: Optional[torch.Tensor] = None, mask_of: Optional[torch.Tensor] = None,
+                               doc_lists: Optional[Tuple[torch.Tensor, torch.Tensor]] = None,
+                               list_of: Optional[torch.Tensor] = None, stats: Optional[dict] = None):
+    """score_topk_groups_hybrid over a corpus sharded by page: doc_groups holds this shard's pages' GLOBAL group ids,
+    hits and scopes as in sharded_topk_hybrid. Each rank runs score_topk_groups_hybrid on its shard with the hits it
+    holds, then one all-gather of [nq, k, 3] int64 (score bits, page, group) and merge_topk_groups. A document's fused
+    score is the best of its ranks' local fused scores, and the rank holding its best page ranks it in its local top-k
+    whenever it is in the global top-k (the argument of sharded_topk_groups), so the result equals the plain call over
+    the shards concatenated in rank order. Only fusion="sum"; with world > 1, world * k must be <= MERGE_GROUPS_MAX
+    (512). Both are checked before any work. stats: the local call's, and with stats={"stages": {}} the times of "local", "exchange", "merge"."""
+    _check_group_fusion(fusion, "sharded_topk_groups_hybrid")
+    k = _check_count(k, "k")
+    world = _world(group)
+    if world > 1 and world * k > MERGE_GROUPS_MAX:
+        raise ValueError(f"sharded_topk_groups_hybrid: world * k = {world * k} > {MERGE_GROUPS_MAX}")
+    w = _check_weight(weight)
+    if world == 1:
+        return score_topk_groups_hybrid(queries, index, k, doc_groups, _shift_hits(hits, id_offset), w, "sum", id_offset,
+                                        doc_mask, mask_of, doc_lists, list_of, stats)
+    import torch.distributed as dist
+
+    q, masks, ls = _scope(queries, index, doc_mask, mask_of, doc_lists, list_of)
+    nq = q.shape[0]
+    _hit_tensors(hits, nq, q.device)  # a malformed triple is refused before any collective
+    with L.on_device(q.device):
+        ev = _Stages(stats)
+        spans = _gather_spans(id_offset, index.nd, q.device, group)
+        local = _local_hits(hits, nq, spans, dist.get_rank(group), index, masks, ls)
+        s, p, g = score_topk_groups_hybrid(q, index, k, doc_groups, local, w, "sum", id_offset, doc_mask, mask_of,
+                                           doc_lists, list_of, stats)
+        ev.mark("local")
+        got = _all_gather_rows(torch.stack([_score_bits(s), p, g], dim=-1), group)
+        ev.mark("exchange")
+        out = merge_topk_groups(_bits_score(got[..., 0]), got[..., 1], got[..., 2], k)
+        ev.mark("merge")
+    return out
+
+
+def _mmr_routes(ids: torch.Tensor, spans: torch.Tensor, world: int) -> torch.Tensor:
+    """int64 [world, world] on the host: entry (r, s) counts the candidates (global ids [nq, fetch], -1 = none) of rank
+    r's queries (shard_range(nq, r, world)) that rank s holds; the sizes of sharded_mmr's all-to-all, computed alike on
+    every rank."""
+    nq, fetch = ids.shape
+    dev = ids.device
+    q_ends = torch.tensor([shard_range(nq, r, world)[1] for r in range(world)], dtype=torch.int64, device=dev)
+    receiver = torch.searchsorted(q_ends, torch.arange(nq, device=dev), right=True)[:, None].expand(nq, fetch)
+    owner = torch.searchsorted(_check_spans(spans).to(dev), ids, right=True)
+    owner = torch.where(ids >= 0, owner, world)
+    n = torch.bincount((receiver * (world + 1) + owner).flatten(), minlength=world * (world + 1))
+    return n.view(world, world + 1)[:, :world].cpu()
+
+
+def _mmr_send(index: CorpusIndex, ids: torch.Tensor, spans: torch.Tensor, rank: int) -> torch.Tensor:
+    """The rows rank `rank` sends in sharded_mmr's all-to-all: the fp32 rows of the candidates it holds, in (query, slot)
+    order over all queries, which is receiver order (_mmr_routes' column `rank` gives each receiver's share)."""
+    lo = int(spans[rank, 0])
+    flat = ids.flatten()
+    local = flat[(flat >= lo) & (flat < lo + index.nd)] - lo
+    return index.emb.index_select(0, local)
+
+
+def _all_to_all_rows(send: torch.Tensor, send_sizes: List[int], recv_sizes: List[int], group) -> torch.Tensor:
+    """The exchange of sharded_mmr: one all_to_all_single of rows [n, dim]; rank r receives every rank's share for it,
+    in rank order."""
+    import torch.distributed as dist
+
+    recv = torch.empty((sum(recv_sizes),) + tuple(send.shape[1:]), dtype=send.dtype, device=send.device)
+    dist.all_to_all_single(recv, send.contiguous(), recv_sizes, send_sizes, group=group)
+    return recv
+
+
+def _mmr_place(ids: torch.Tensor, recv: torch.Tensor, spans: torch.Tensor) -> Tuple[torch.Tensor, torch.Tensor]:
+    """A rank's query block: ids [n, fetch] (global candidates, -1 = none) and recv, the candidates' rows in owner order,
+    each owner's in (query, slot) order -> (buf [n * fetch, dim] with candidate (i, j)'s row at i * fetch + j, the ids
+    remapped to those rows [n, fetch], -1 kept). Rows of missing candidates are not written."""
+    n, fetch = ids.shape
+    flat = ids.flatten()
+    owner = torch.searchsorted(_check_spans(spans).to(ids.device), flat, right=True)
+    owner = torch.where(flat >= 0, owner, spans.shape[0])
+    order = torch.sort(owner, stable=True).indices[:recv.shape[0]]
+    buf = torch.empty((n * fetch, recv.shape[1]), dtype=torch.float32, device=ids.device)
+    buf[order] = recv
+    return buf, torch.where(flat >= 0, torch.arange(n * fetch, device=ids.device), -1).view(n, fetch)
+
+
+def _mmr_block(scores: torch.Tensor, ids: torch.Tensor, recv: torch.Tensor, spans: torch.Tensor, k: int,
+               lam: torch.Tensor) -> Tuple[torch.Tensor, torch.Tensor]:
+    """The selection of a rank's query block: scores / ids [n, fetch] (global candidates) and recv (as _mmr_place
+    takes it) -> (scores, global ids) [n, k] of vr_mmr_select over the placed rows. The picks depend only on the
+    candidates' scores, rows and order, so they are the picks over the whole index."""
+    buf, pos = _mmr_place(ids, recv, spans)
+    s, p = _mmr_select(CorpusIndex(buf, None, None), scores.contiguous(), pos, k, lam.contiguous(), 0)
+    flat = ids.flatten()
+    return s, torch.where(p >= 0, flat.index_select(0, p.clamp(min=0).flatten()).view(p.shape), -1)
+
+
+def sharded_mmr(queries: torch.Tensor, index: CorpusIndex, k: int, lambda_mult=0.5, fetch_k: Optional[int] = None,
+                id_offset: int = 0, group=None, doc_mask: Optional[torch.Tensor] = None,
+                mask_of: Optional[torch.Tensor] = None, doc_lists: Optional[Tuple[torch.Tensor, torch.Tensor]] = None,
+                list_of: Optional[torch.Tensor] = None, stats: Optional[dict] = None):
+    """score_mmr over a corpus sharded by page (page ranges as in sharded_range; scopes as in sharded_topk).
+    sharded_topk(fetch_k) gives every rank the global candidates (bit-identical to score_topk over the whole index).
+    Rank r runs the selection for its queries shard_range(nq, r, world) and needs the candidates' rows that other ranks
+    hold: one all_to_all_single routes them, rank s sending the rows of the candidates it holds among rank r's queries
+    in (query, slot) order; every rank computes the split sizes from the candidate ids and the all-gathered
+    (id_offset, nd) of each rank. The selection (vr_mmr_select) runs on a buffer of those rows. One all-gather of the
+    [ceil(nq / world), k] picks gives every rank every row. The picks depend only on the candidates' scores, rows and
+    order (and the cluster size on fetch_k and dim), so the result equals score_mmr over the shards concatenated in rank
+    order, bit for bit. Each rank receives about nq / world * fetch_k * dim * 4 bytes: 0.46 GB at 10 k queries, 8
+    ranks, fetch_k = 40 and dim 2304. stats: fetch_k, and with stats={"stages": {}} the times of "candidates",
+    "exchange", "select" and "gather"."""
+    k, fetch = _check_fetch(k, fetch_k, index.emb.shape[1])
+    world = _world(group)
+    if world == 1:
+        return score_mmr(queries, index, k, lambda_mult, fetch, id_offset, doc_mask, mask_of, doc_lists, list_of, stats)
+    import torch.distributed as dist
+
+    q = _check_f32(queries, "queries")
+    nq, dev = q.shape[0], q.device
+    lam = _check_lambda(lambda_mult, nq, index.emb.device)
+    rank = dist.get_rank(group)
+    with L.on_device(dev):
+        ev = _Stages(stats)
+        spans = _gather_spans(id_offset, index.nd, dev, group)
+        s, i = sharded_topk(q, index, fetch, id_offset, group, None, doc_mask, mask_of, doc_lists, list_of)
+        routes = _mmr_routes(i, spans, world)
+        ev.mark("candidates")
+        recv = _all_to_all_rows(_mmr_send(index, i, spans, rank), routes[:, rank].tolist(), routes[rank].tolist(), group)
+        ev.mark("exchange")
+        lo, hi = shard_range(nq, rank, world)
+        ps, pi = _mmr_block(s[lo:hi], i[lo:hi], recv, spans, k, lam[lo:hi])
+        ev.mark("select")
+        got = gather_queries(torch.stack([_score_bits(ps), pi], -1).view(hi - lo, 2 * k), nq, group).view(nq, k, 2)
+        ev.mark("gather")
+    if stats is not None:
+        stats["fetch_k"] = fetch
+    return _bits_score(got[..., 0]).contiguous(), got[..., 1].contiguous()
 
 
 # ------------------------------------------------------------------------------------------------------
